@@ -1,7 +1,8 @@
 #!/usr/bin/env python
-"""bench.py -- decode tokens/s of Llama-3.1-8B GPTQ-int4 (g128) on B200, the BASELINE.json metric.
+"""bench.py -- decode tokens/s of Llama-3.1-8B GPTQ-int4 (g128) on H100, the BASELINE.json metric.
 
     python bench.py --gpus N --steps K --warmup W [--batch B] [--prompt P] [--impl reference] [--model NAME]
+                    [--dump-outputs DIR]
 
 A "step" is one decode step of the whole batch through the hot path (32 layers of W4A16 Linear +
 decode attention + RMSNorm/RoPE fusions, lm_head, greedy pick).  Random-init weights of the named
@@ -12,9 +13,15 @@ architecture in HF-GPTQ layout, synthetic prompt token ids ("data": "synthetic")
   e2e     the same step through the public host-buffer API (zl_llama_decode): pinned-host token ids and
           positions are copied H2D and the picked tokens are read back D2H inside every timed step.
   roofline  the dominant kernel (W4A16 GEMM): all 128 GEMM launches of a step replayed on their own real
-          weights between CUDA events; achieved = algorithmic bytes / time against MEASURED_PEAKS.json.
+          weights between CUDA events; achieved = algorithmic bytes / time against the H100 SXM data-sheet HBM3
+          bandwidth (3.35 TB/s), or MEASURED_PEAKS.json where it exists.
   cpu_baseline  the oracle's dequant-to-bf16 torch CPU path on a bounded sample (1 of 32 layers + lm_head),
           a reported baseline, not a target.
+
+--dump-outputs DIR writes what the last timed step computed -- the picked tokens (tokens.npy, float64) and its fp32
+logits (logits.npy; rank 0's vocabulary shard under tensor parallelism; a fixed seeded column sample when the files
+would exceed 64 MB in all) -- so that two builds can be compared output for output:
+weights, prompts and positions are seeded, so the same arguments give the same inputs.
 
 --impl reference times that CPU path as the whole arm (the reference has no CPU implementation of its own;
 SURVEY.md section 8d names this torch dequant path as the side-by-side baseline).
@@ -41,11 +48,11 @@ def read_peaks():
         with open(p) as f:
             d = json.load(f)
         return float(d["hbm_gbs"]), "measured"
-    return 6650.0, "fallback"
+    return 3350.0, "datasheet (H100 SXM HBM3)"
 
 
 class ClockSampler(threading.Thread):
-    """nvidia-smi clocks / throttle reasons sampled during the timed region (B200_PROFILING.md)."""
+    """nvidia-smi clocks / throttle reasons sampled during the timed region."""
     Q = ("index,clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.active,clocks_event_reasons.hw_slowdown,"
          "clocks_event_reasons.hw_thermal_slowdown,clocks_event_reasons.sw_thermal_slowdown,"
          "clocks_event_reasons.sw_power_cap")
@@ -325,6 +332,28 @@ def ingest_prompt(dec, B, prompt_len, vocab, rng):
     dec.sync()
 
 
+DUMP_LIMIT_BYTES = 64 << 20
+
+
+def dump_outputs(out_dir, dec, B):
+    """The arrays the timed path handed back in its last step: next tokens (B) and fp32 logits (B, V/tp) -- under tensor
+    parallelism rank 0's vocabulary shard, the first V/tp columns.  When all files would exceed the limit, the logits are
+    reduced to a fixed seeded sample of columns (logits_columns.npy holds their indices) sized so that everything
+    written stays within it."""
+    import numpy as np
+    os.makedirs(out_dir, exist_ok=True)
+    tok, _ = dec.get_state(B)
+    logits = dec.get_logits(B)
+    np.save(os.path.join(out_dir, "tokens.npy"), tok.astype(np.float64))
+    header = 4096                                   # .npy headers of the files, generously
+    if 8 * B + logits.nbytes + header > DUMP_LIMIT_BYTES:
+        n_cols = (DUMP_LIMIT_BYTES - 8 * B - header) // (4 * B + 8)   # float32 logits + float64 column index
+        cols = np.sort(np.random.default_rng(0).choice(logits.shape[1], size=n_cols, replace=False))
+        logits = logits[:, cols]
+        np.save(os.path.join(out_dir, "logits_columns.npy"), cols.astype(np.float64))
+    np.save(os.path.join(out_dir, "logits.npy"), np.ascontiguousarray(logits, dtype=np.float32))
+
+
 def step_bytes_of(cfg, weight_bytes, B, ctx):
     return weight_bytes + B * ctx * cfg["num_layers"] * 2 * cfg["num_kv_heads"] * cfg["dim_head"] * 2
 
@@ -351,6 +380,8 @@ def main():
                     help="default: the model's BASELINE quantisation (GPTQ int4 for 8B, bf16 for 1B); int8 / fp8: W8A8 Linear rows")
     ap.add_argument("--prefill-chunk", type=int, default=128, help="tokens per chunked-prefill pass of the TTFT measurement")
     ap.add_argument("--fuse", type=int, default=2, help="0: one kernel per reference op; 1: +RMSNorm fused; 2: +qkv RoPE/KV epilogue")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write the picked tokens and logits of the last timed step as DIR/<name>.npy")
     args = ap.parse_args()
 
     cfg = model_cfg(args.model)
@@ -419,6 +450,8 @@ def main():
     launches0 = dec.lib.zl_launch_count(0)
     ms_dev, clocks = measure_decode(dec, B, args.steps, W, stream, barrier, sampler_gpu=local_rank)
     weight_bytes, kernels_per_step = dec.stats(B)
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, dec, B)
 
     # sanity of the synthetic model: the logits of the last timed step must be finite (a NaN step costs the same time)
     tok, pos = dec.get_state(B)
@@ -458,7 +491,7 @@ def main():
             args.quant, "bf16" if dense else "f16 (W4A16: int4 weights, fp16 activations, fp32 accumulate)"),
         "data": "synthetic (random-init HF-GPTQ tensors: uniform nibbles recentred on the symmetric zero point, scales 0.002-0.006)",
         "config": {"workload": workload, "parallelism": "single GPU" if world == 1 else "tp%d (NVLink peer-memory exchange fused into the GEMMs, %s payload)" % (world, "int8-g32 (stand-alone kernel)" if args.tp_int8 else "fp16"),
-                   "l2": "weights per step (%.2f GB) exceed L2 (126 MB); no explicit flush" % (weight_bytes / 1e9),
+                   "l2": "weights per step (%.2f GB) exceed L2 (50 MB); no explicit flush" % (weight_bytes / 1e9),
                    "pdl": not args.no_pdl, "cuda_graph": not args.no_graph, "fuse": args.fuse},
         "clocks": clocks,
         "e2e": {"value": e2e_value, "unit": "tokens/s", "h2d_bytes_per_step": 8 * B, "d2h_bytes_per_step": 4 * B,
@@ -494,7 +527,7 @@ def main():
             tpot.append((t2 - t1) * 1e3 / (n_out - 1))
         out["latency"] = {"ttft_ms_p50": float(np.median(ttft)), "tpot_ms_p50": float(np.median(tpot)),
                           "requests": args.requests, "prompt_tokens": plen, "new_tokens": n_out, "batch": 1,
-                          "prefill": "chunked, %d tokens per pass (tcgen05 GEMMs)" % args.prefill_chunk}
+                          "prefill": "chunked, %d tokens per pass (wgmma GEMMs)" % args.prefill_chunk}
 
     # ---- extras of the N = 1 line: BASELINE config 3 batch sizes and config 2, through the same harness ----
     if sweep:
@@ -518,11 +551,11 @@ def main():
         "bound": "hbm",
         "kernel": ("k_w8a8_skinny (+ activation quant)" if args.quant != "default" else "k_dense_skinny") if dense
         else ("k_w4a16_v3 (integer IMMA, fused norm / RoPE / SwiGLU / residual variants as in the step)" if B <= 7
-              else "k_w4a16_ts (tcgen05, A operand in TMEM, tensor-TMA)"),
+              else "k_w4a16_ts (wgmma, A operand in registers, tensor-TMA)"),
         "achieved": achieved, "peak": peak, "unit": "GB/s", "frac": achieved / peak, "peak_kind": peak_kind,
         "bytes_per_launch": g_bytes / g_launches, "us_per_launch": g_ms * 1e3 / iters / g_launches,
         "traffic": None,
-        "traffic_note": "dram bytes are not observable from inside the run; ncu --set full captures: profiles/r01_w4a16_traffic.json (integer kernel: dram reads = algorithmic bytes within 0.1 %), profiles/r02_w4a16_ts_ncu_full.txt (tcgen05 kernel: 61.4 MB read for 61.0 MB algorithmic)",
+        "traffic_note": "dram bytes are not observable from inside the run",
     }
 
     if extras:
@@ -539,7 +572,7 @@ def main():
                                     "kernels_per_step": kps1,
                                     "step_roofline_frac": step_bytes_of(c1, wb1, 1, args.prompt + 40) / (ms1 / 64 * 1e-3) / 1e9 / peak}
         d1.close()
-        # the reference's own decode kernels (recompiled for sm_100, oracle/_ref) chained for one 8B layer + lm_head on
+        # the reference's own decode kernels (recompiled for sm_90a, oracle/_ref) chained for one 8B layer + lm_head on
         # this GPU, in a separate process: a reported side-by-side, not an arm
         ref_tool = os.path.join(ROOT, "tools", "ref_layer_bench.py")
         if os.path.exists(os.path.join(ROOT, "oracle", "_ref", "libzl_ref.so")):

@@ -1,7 +1,7 @@
 /*
- * zhilight_b200 -- C-ABI of the B200-native (sm_100a) quantized-decode hot path of ZhiLight.
+ * zhilight_b200 -- C-ABI of the H100-native (sm_90a) quantized-decode hot path of ZhiLight.
  *
- * Every entry point replaces one reference operator (cited as file:line under /root/reference).
+ * Every entry point replaces one reference operator (cited as file:line inside the reference checkout).
  * Conventions (SURVEY.md section 8b):
  *   - plain pointers + sizes, no C++/torch types; all data pointers are DEVICE pointers unless
  *     the name ends in _host;
@@ -78,7 +78,7 @@ int zl_gptq_dequant_k_major(const uint32_t* qweight_km, const uint8_t* qzeros_km
                             void* out_f16, int N, int K, int group_size, zl_stream_t stream);
 
 /* ------------------------------------------------------------------------------------------ *
- * ZLW4: the B200 tile-packed W4 layout consumed by zl_w4a16_gemm (DESIGN.md section 3).
+ * ZLW4: the tile-packed W4 layout consumed by zl_w4a16_gemm (DESIGN.md section 3).
  * Built once at load from the reference k-major tensors
  * (Int4GPTQ::preprocess_weight, src/nn/linear/linear.cpp:1139-1160).
  * ------------------------------------------------------------------------------------------ */
@@ -141,22 +141,19 @@ typedef struct zl_w4_fused_args {
 int zl_w4a16_gemm_fused(const zl_w4_fused_args_t* args, zl_stream_t stream);
 /* 1 if the exact-integer kernel (variant 1, M <= 16) can run this shape: its staged activations must fit shared memory. */
 int zl_w4_int_kernel_fits(int M, int N, int K);
-/* which kernel serves (M, N, K) on the ZLW4I layout (variant 1): 3 = exact-integer mma.sync kernel, 4 = tcgen05 / TMEM /
- * TMA kernel (any M, N % 128 == 0, no fused RMSNorm prologue), 0 = neither (pack variant 0 and use the fp16 mma.sync kernel). */
+/* which kernel serves (M, N, K) on the ZLW4I layout (variant 1): 3 = exact-integer mma.sync kernel, 4 = wgmma / TMA
+ * kernel (any M, N % 128 == 0, no fused RMSNorm prologue), 0 = neither (pack variant 0 and use the fp16 mma.sync kernel). */
 int zl_w4_int_layout_route(int M, int N, int K);
-/* last watchdog code published by a tcgen05 kernel on the current device (0 = none); a bounded mbarrier wait that expires
+/* last watchdog code published by a tensor-core kernel on the current device (0 = none); a bounded mbarrier wait that expires
  * records which pipeline barrier starved and traps instead of hanging the GPU. */
 unsigned zl_w4_tc_watchdog(void);
-/* debug / tests: at least `splits` pieces per weight-row tile in the tcgen05 kernel's stream-k schedule (0 = automatic; also
+/* debug / tests: at least `splits` pieces per weight-row tile in the wgmma kernel's stream-k schedule (0 = automatic; also
  * ZL_TC_SPLITS). */
 int zl_w4_tc_set_splits(int splits);
-/* tests: host view of the tcgen05 kernel's stream-k schedule (the kernel's own scheduling code): pieces of CTA `cta` of `ctas`
+/* tests: host view of the wgmma kernel's stream-k schedule (the kernel's own scheduling code): pieces of CTA `cta` of `ctas`
  * for n_tiles x G (tile, group) units; out[5 i ..] = tile, g0, g1, pieces of that tile, workspace slot (-1: whole tile);
  * returns the number of pieces. */
 int zl_w4_tc_schedule(int n_tiles, int G, int ctas, int cta, int* out, int max_pieces);
-/* debug: with ZL_TC_DBG & 16, CTA 0 of the tcgen05 kernel stamps its pipeline hand-overs with clock64; copies
- * [11 roles][64 stages][4 events] of the last launch to `out` (n <= 2816 values). */
-int zl_w4_tc_read_trace(long long* out, int n);
 /* debug: device buffer of grid*16 uint64 globaltimer samples written by the integer kernel (NULL = off). */
 int zl_w4_set_trace(void* buf);
 /* row_map (n_heads_total*dim_head) for zl_w4_pack so that RoPE partners (c, c+d/2) share an MMA tile. */
@@ -350,7 +347,7 @@ typedef struct zl_llama_config {
     int use_pdl, use_graph;
     int tp_int8; /* TP all-reduce payload: 0 = activation dtype, 1 = int8 group-32 (REDUCE_TP_INT8 of the reference) */
     int fuse; /* 0: one kernel per reference operator; 1: RMSNorm folded into the W4 GEMMs; 2 (3 is accepted as 2):
-               * + qkv RoPE/KV-append epilogue.  Launches with more than 16 tokens run zl_rmsnorm + the tcgen05 GEMM. */
+               * + qkv RoPE/KV-append epilogue.  Launches with more than 16 tokens run zl_rmsnorm + the wgmma GEMM. */
     int prefill_chunk; /* 0: decode only.  1..2048: zl_llama_prefill processes a prompt in chunks of this many tokens
                         * (chunked prefill, zhilight/config/adapter.py:47-48) */
     int qkv_bias; /* zl_llama_init_synthetic: also create q/k/v biases (Qwen2: attention.cpp:105-109); loaded checkpoints
@@ -380,6 +377,8 @@ int zl_llama_set_state(zl_llama_t* m, const int32_t* tokens_host, const int32_t*
 int zl_llama_step_device(zl_llama_t* m, int B);
 /* read back the device-resident (token, position) state; synchronous. */
 int zl_llama_get_state(zl_llama_t* m, int32_t* tokens_host, int32_t* positions_host, int B);
+/* fp32 logits (B, vocab/tp) of the last step (device-resident or host-API), this rank's vocabulary shard.  Synchronous. */
+int zl_llama_get_logits(zl_llama_t* m, float* logits_host, int B);
 int zl_llama_sync(zl_llama_t* m);
 /* Chunked prefill of ONE task (SearchTask prompt, src/generator/batch_generator.cpp:1576): appends tokens_host[0..n) at
  * positions pos0.. to the task's KV buffers through the same kernels (M = chunk GEMMs, causal len_q = chunk attention)

@@ -1,7 +1,7 @@
 // Drop-in definitions of the reference's hot-path operator symbols (namespaces nn, nn::gptq, nn::fp8, int8_op) on top of
 // the C-ABI of libzhilight_b200.so -- the file a ZhiLight maintainer adds to the `backend` target in place of the
-// corresponding .cu files (INTEGRATION.md).  It is compiled HERE against the reference's own headers where they lie
-// under /root/reference (integration/Makefile.dropin) and linked with bmengine's core + oracle/ref_shim.cu into
+// corresponding .cu files (INTEGRATION.md).  It is compiled against the reference's own headers where they lie
+// in a reference checkout (integration/Makefile.dropin) and linked with bmengine's core + oracle/ref_shim.cu into
 // oracle/_ref/libzl_dropin.so, so that tests/test_dropin_gpu.py can drive the reference-signature functions and
 // compare them with the reference's own kernels (oracle/_ref/libzl_ref.so) call for call.
 //
@@ -124,7 +124,7 @@ Tensor gptq_gemm_k_major(const core::Context& ctx, const Tensor& a, const Tensor
     (void)precomputed_w8;
     BM_ASSERT_EQ(a.dtype(), DataType::kHalf, "A must be half");             // q_gemm_k_major.cu:989
     BM_ASSERT(qzeros.dtype() == DataType::kInt8, "qzeros must be int8");     // :990
-    BM_ASSERT_EQ(q_perm.numel(), 0, "act-order is not supported on the B200 path");
+    BM_ASSERT_EQ(q_perm.numel(), 0, "act-order is not supported on the H100 path");
     const int K = (int)a.size(-1), M = (int)(a.numel() / K), N = (int)q_weight.size(-2);
     BM_ASSERT_EQ((size_t)K, q_weight.size(-1) * 8, "K mismatch");
     if (cache_only) return Tensor();

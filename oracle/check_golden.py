@@ -1,8 +1,9 @@
 """Compare the CPU oracle with the golden outputs of the reference's own kernels (TEST INFRASTRUCTURE).
 
-tests/golden/ref_<case>.npz were produced by oracle/gen_ref_golden.py on a B200 from the reference kernels
-recompiled for sm_100.  Integer stages must match bit for bit; float stages within the stated tolerance
+tests/golden/ref_<case>.npz were produced by oracle/gen_ref_golden.py on a GPU from the reference kernels
+recompiled for that GPU.  Integer stages must match bit for bit; float stages within the stated tolerance
 (the reference's fp16 8-wide partial sums are emulated where that matters)."""
+import hashlib
 import os
 
 import numpy as np
@@ -152,8 +153,10 @@ def check_kv8(g):
     for i, (k, v) in enumerate(zip(c["ks"], c["vs"])):
         kq, sk = ops.int8_quant_per_token(k.reshape(-1, c["d"]))        # same absmax / 127 rounding, codes offset by 128
         vq, sv = ops.int8_quant_per_token(v.reshape(-1, c["d"]))
-        np.testing.assert_array_equal(g["kq%d" % i].reshape(-1, c["d"]).astype(np.int32) - 128, kq.astype(np.int32))
-        np.testing.assert_array_equal(g["vq%d" % i].reshape(-1, c["d"]).astype(np.int32) - 128, vq.astype(np.int32))
+        for name, codes in (("kq", kq), ("vq", vq)):   # the reference's uint8 codes = ours + 128, bit for bit
+            u8 = (codes.astype(np.int32) + 128).astype(np.uint8).reshape(-1)
+            digest = np.frombuffer(hashlib.sha256(u8.tobytes()).digest(), np.uint8)
+            np.testing.assert_array_equal(g["%s%d_sha256" % (name, i)], digest)
         np.testing.assert_array_equal(g["sk%d" % i].reshape(-1), sk)
         np.testing.assert_array_equal(g["sv%d" % i].reshape(-1), sv)
         kd.append((kq.astype(np.float32) * sk[:, None]).reshape(k.shape))

@@ -1,6 +1,6 @@
 #!/usr/bin/env python
-"""Run the REFERENCE's own kernels (oracle/_ref/libzl_ref.so, built by oracle/Makefile.ref from /root/reference
-sources, recompiled for sm_100) on the seeded inputs of oracle/golden_cases.py and store their outputs as
+"""Run the REFERENCE's own kernels (oracle/_ref/libzl_ref.so, built by oracle/Makefile.ref from the reference
+checkout's sources, recompiled for sm_90a) on the seeded inputs of oracle/golden_cases.py and store their outputs as
 tests/golden/ref_<case>.npz.  TEST INFRASTRUCTURE; needs a GPU (run through gpurun):
 
     python -m oracle.gen_ref_golden gpurun_out/golden      # then copy *.npz into tests/golden/
@@ -8,6 +8,7 @@ tests/golden/ref_<case>.npz.  TEST INFRASTRUCTURE; needs a GPU (run through gpur
 The fixtures are small (a few hundred KB) and are committed together with this script.
 """
 import ctypes
+import hashlib
 import os
 import sys
 
@@ -18,6 +19,11 @@ from . import golden_cases as gc
 
 HERE = os.path.dirname(os.path.abspath(__file__))
 LIB = os.path.join(HERE, "_ref", "libzl_ref.so")
+
+
+def codes_digest(a):
+    """SHA-256 of a uint8 array's bytes (C order), as a uint8 array"""
+    return np.frombuffer(hashlib.sha256(np.ascontiguousarray(a, dtype=np.uint8).tobytes()).digest(), np.uint8).copy()
 
 
 class Ref:
@@ -378,7 +384,9 @@ def main(out_dir, lib_path=None):
         kq.append(a.view(k.shape)); sk.append(s.view(k.shape[0], c["hkv"]))
         b, s2 = ref.quant_u8(ref.t(v.reshape(-1, c["d"])))
         vq.append(b.view(v.shape)); sv.append(s2.view(v.shape[0], c["hkv"]))
-        outs["kq%d" % i], outs["sk%d" % i], outs["vq%d" % i], outs["sv%d" % i] = n(kq[-1]), n(sk[-1]), n(vq[-1]), n(sv[-1])
+        # the uint8 codes are compared bit for bit: their SHA-256 digests keep the fixture small
+        outs["kq%d_sha256" % i], outs["vq%d_sha256" % i] = codes_digest(n(kq[-1])), codes_digest(n(vq[-1]))
+        outs["sk%d" % i], outs["sv%d" % i] = n(sk[-1]), n(sv[-1])
     mask = ref.t(np.concatenate([m.reshape(-1) for m in c["masks"]]))
     outs["out"] = n(ref.attention_kv8(ref.t(c["q"]), ref.t(c["lens"]), kq, vq, sk, sv, mask, c["scale"], c["hkv"]).float())
     np.savez(os.path.join(out_dir, "ref_kv8.npz"), **outs)

@@ -1,6 +1,6 @@
 """Seeded inputs of the golden cases (TEST INFRASTRUCTURE).
 
-`oracle/gen_ref_golden.py` feeds them to the REFERENCE's own kernels (oracle/_ref/libzl_ref.so, on the B200 box)
+`oracle/gen_ref_golden.py` feeds them to the REFERENCE's own kernels (oracle/_ref/libzl_ref.so, on a GPU)
 and stores the outputs in tests/golden/ref_<case>.npz; `oracle/check_golden.py` regenerates the same inputs on
 the CPU, runs the oracle and compares -- that is what pins the oracle to the reference.
 """

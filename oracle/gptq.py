@@ -3,7 +3,7 @@
 TEST INFRASTRUCTURE -- see oracle/__init__.py.  Integer stages are bit-exact
 restatements of the reference's load pipeline; float stages are fp32.
 
-Reference files followed (all under /root/reference):
+Reference files followed (paths inside the reference checkout):
   * nibble shuffle            src/nn/quant/gptq/qdq_4.cuh:16-35, q_gemm.cu:778-791
   * act-order gather          src/nn/quant/gptq/q_gemm.cu:794-829, linear.cpp:1010-1028
   * zero +1 with 4-bit wrap   src/nn/quant/gptq/utils.cu:61-88

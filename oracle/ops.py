@@ -3,7 +3,7 @@ int8 TP all-reduce (numpy, fp32 math).
 
 TEST INFRASTRUCTURE -- see oracle/__init__.py.
 
-Reference files followed (all under /root/reference):
+Reference files followed (paths inside the reference checkout):
   * RMSNorm (+fused add)      src/nn/layernorm/layernorm.cu:9-42
   * residual add              src/nn/block/block_kernel.cu:7-17
   * RoPE                      src/nn/position/rope_common.cuh:3-34, rope_preparer.cu:49-161,

@@ -1,8 +1,8 @@
 // TEST INFRASTRUCTURE (oracle/_ref): a thin extern "C" shim over the REFERENCE's own hot-path kernels.
 //
-// Built by oracle/Makefile.ref from the sources where they lie under /root/reference (never copied into
+// Built by oracle/Makefile.ref from the sources where they lie in a reference checkout (never copied into
 // this repo) into oracle/_ref/libzl_ref.so.  It lets the GPU parity tests and oracle/gen_ref_golden.py run
-// the reference's kernels (recompiled for sm_100) on the same device buffers as ours.  Only tests/,
+// the reference's kernels (recompiled for sm_90a) on the same device buffers as ours.  Only tests/,
 // __graft_entry__ and bench tooling may load it; the product library never links or dlopens it.
 //
 // All pointers are device pointers; every call runs on the shim's private bmengine Context/stream and

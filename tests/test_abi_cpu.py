@@ -65,7 +65,7 @@ def test_missing_library_fails_loudly(monkeypatch, tmp_path):
 @pytest.mark.parametrize("n_tiles,G,ctas", [(224, 32, 148), (48, 32, 148), (32, 32, 128), (32, 112, 148), (1, 8, 4), (7, 5, 3),
                                             (300, 3, 148), (16, 128, 148)])
 def test_tcgen05_stream_k_schedule_covers_every_unit_once(n_tiles, G, ctas):
-    """The tcgen05 W4 kernel's scheduling code (TcSched in w4a16_tc.cu, exported as zl_w4_tc_schedule): every
+    """The wgmma W4 kernel's scheduling code (TcSched in w4a16_tc.cu, exported as zl_w4_tc_schedule): every
     (128-row tile, 128-k group) unit belongs to exactly one piece, a tile's pieces are contiguous in k and counted correctly,
     partial pieces come first in a CTA's order (at most two) and never share a workspace slot."""
     import ctypes

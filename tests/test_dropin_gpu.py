@@ -1,14 +1,15 @@
 """Drop-in proof: the SAME reference-signature calls (nn::gptq::gptq_gemm_k_major, nn::multi_query_attention_rag_buffer,
 nn::LayerNorm, int8_op::*, nn::fp8::dynamic_scaled_quant ... driven by oracle/ref_shim.cu over every case of
-oracle/golden_cases.py) are executed twice on the B200:
+oracle/golden_cases.py) are executed twice on the GPU:
 
   * oracle/_ref/libzl_ref.so     -- the reference's own kernels,
   * oracle/_ref/libzl_dropin.so  -- integration/zl_nn_dropin.cpp, i.e. OUR definitions of those symbols on top of
                                     libzhilight_b200.so (none of the reference's hot-path kernel files is linked),
 
 each in its own process, and the outputs are compared: integer / index work bit-exact, fp16 within the tolerances of
-north_star (1e-3 rel; 2e-3 where the reference itself accumulates 8 products in fp16).  Skipped when the two
-libraries were not built (they need /root/reference at build time; the built files travel to the GPU box)."""
+north_star (1e-3 rel; 2e-3 where the reference itself accumulates 8 products in fp16).  Both libraries link the
+reference's own engine core and are compiled against its headers, so they exist only where build() ran with
+ZHILIGHT_REFERENCE naming a ZhiLight checkout; elsewhere this test is skipped."""
 import os
 import subprocess
 import sys

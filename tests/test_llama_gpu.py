@@ -126,7 +126,7 @@ LAYER8B = dict(num_layers=3, dim_model=4096, num_heads=32, num_kv_heads=8, dim_h
                eps=1e-5, rope_theta=500000.0, rope_llama3=dict(factor=8.0, low=1.0, high=4.0, orig=8192.0))
 
 
-# W4: chunks of more than 16 tokens run the tcgen05 kernel (w rounded to fp16 once, fp32 accumulate in TMEM) behind a
+# W4: chunks of more than 16 tokens run the wgmma kernel (w rounded to fp16 once, fp32 accumulate) behind a
 # stand-alone RMSNorm, not the exact-integer M <= 16 kernel with the fused norm
 @pytest.mark.parametrize("chunk", [32, 64])
 @pytest.mark.parametrize("quant,dtype,tol,cfg", [(5, "f16", 5e-3, TINY128), (5, "f16", 5e-3, TINY), (0, "f16", 3e-3, TINY),
@@ -208,7 +208,7 @@ def test_dual_stream_prefill_matches_single_stream(lib, cuda, monkeypatch, cfg):
         outs.append(steps)
     for a, b in zip(*outs):
         assert np.isfinite(a).all()
-        # M = 32 chunks (tcgen05 kernel: weights rounded to fp16, stand-alone RMSNorm) vs two M = 16 halves (exact-integer
+        # M = 32 chunks (wgmma kernel: weights rounded to fp16, stand-alone RMSNorm) vs two M = 16 halves (exact-integer
         # kernel, fused norm): fp16-level agreement
         assert rel_l2(b, a) <= 5e-3
     orc = omodel.OracleLlama(cfg, sd, 5, 128, False, "f16", fuse_norm=True)
@@ -268,7 +268,7 @@ LAYERS8B_SMALLV = dict(num_layers=2, dim_model=4096, num_heads=32, num_kv_heads=
 
 @pytest.mark.parametrize("b,graph,pdl", [(20, True, True), (32, True, True), (32, False, True), (32, False, False), (17, True, False)])
 def test_large_batch_decode_on_8b_shapes_matches_batch_1(lib, cuda, b, graph, pdl):
-    """Batch 17..32 decode runs the tcgen05 GEMMs (split-k, qkv-RoPE / SwiGLU / residual epilogues) inside the CUDA graph
+    """Batch 17..32 decode runs the wgmma GEMMs (split-k, qkv-RoPE / SwiGLU / residual epilogues) inside the CUDA graph
     with programmatic dependent launch on Llama-3.1-8B layer shapes: every task of a batch of identical tokens must
     reproduce the batch-1 logits (exact-integer kernel) to fp16 accuracy, with and without graph / PDL."""
     from zhilight_b200.llama import LlamaDecoder

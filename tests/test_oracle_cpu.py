@@ -200,7 +200,7 @@ def test_e4m3_rounding_grid():
 
 @pytest.mark.parametrize("path", sorted(glob.glob(os.path.join(GOLDEN, "ref_*.npz"))) or [None])
 def test_oracle_against_reference_goldens(path):
-    """Goldens are outputs of the reference's own kernels (oracle/_ref, built from /root/reference sources)
+    """Goldens are outputs of the reference's own kernels (oracle/_ref, built from the reference checkout's sources)
     on seeded inputs; they pin the oracle.  Absent -> parity is 'unpinned' and this test is skipped."""
     if path is None:
         pytest.skip("no reference goldens committed yet (parity unpinned)")

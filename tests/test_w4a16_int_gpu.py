@@ -57,12 +57,12 @@ def test_config1_1x4096x4096_int(lib, cuda, sym):
 def test_shapes_and_batches_int(lib, cuda, m, k, n):
     from zhilight_b200 import ops, _lib
     route = _lib.load().zl_w4_int_layout_route(m, n, k)
-    if route == 0:     # neither the integer kernel (staging too large) nor the tcgen05 kernel (N % 128): variant 0 territory
+    if route == 0:     # neither the integer kernel (staging too large) nor the wgmma kernel (N % 128): variant 0 territory
         with pytest.raises(_lib.ZLError):
             w, packed_i, _, _ = _setup(cuda, k, n, False, 5)
             ops.w4a16_gemm_fused(torch.zeros(m, k, dtype=torch.float16, device=cuda), packed_i, n, k, variant=1)
         return
-    # route 3: exact-integer kernel; route 4: the same ZLW4I weights through the tcgen05 kernel (fp16-rounded weights)
+    # route 3: exact-integer kernel; route 4: the same ZLW4I weights through the wgmma kernel (fp16-rounded weights)
     w, packed_i, _, _ = _setup(cuda, k, n, False, 5)
     g = torch.Generator().manual_seed(m)
     x = (torch.randn(m, k, generator=g) * torch.logspace(-2, 1, k)[torch.randperm(k, generator=g)]).half()

@@ -1,7 +1,7 @@
-"""GPU parity: the tcgen05 W4A16 kernel (k_w4a16_ts: A operand in TMEM, ZLW4I layout) vs the CPU oracle.
+"""GPU parity: the wgmma W4A16 kernel (k_w4a16_ts: A operand in registers, ZLW4I layout) vs the CPU oracle.
 
 The kernel rounds w = (q - z) * s to fp16 once (what the reference's M > 40 dequant + cuBLASLt route does,
-q_gemm_k_major.cu:843-905, 1083-1100), multiplies fp16 x fp16 exactly and accumulates all of K in fp32 in TMEM.
+q_gemm_k_major.cu:843-905, 1083-1100), multiplies fp16 x fp16 exactly and accumulates all of K in fp32.
 Tolerance (north_star): relative L2 <= 1e-3 against the fp32 oracle for fp16 outputs."""
 import numpy as np
 import pytest
@@ -43,7 +43,7 @@ def test_route_selects_tcgen05(lib):
     assert lib.zl_w4_int_layout_route(4, 4096, 4096) == 3
     assert lib.zl_w4_int_layout_route(16, 512, 1024) == 3
     assert lib.zl_w4_int_layout_route(16, 4096, 4096) == 4      # 16 staged token rows of K = 4096 do not fit beside the rings
-    assert lib.zl_w4_int_layout_route(17, 4096, 4096) == 4      # tcgen05
+    assert lib.zl_w4_int_layout_route(17, 4096, 4096) == 4      # wgmma
     assert lib.zl_w4_int_layout_route(32, 4096, 14336) == 4
     assert lib.zl_w4_int_layout_route(8, 4096, 14336) == 4      # staged activations of the integer kernel do not fit
     assert lib.zl_w4_int_layout_route(2048, 6144, 4096) == 4

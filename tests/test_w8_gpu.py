@@ -41,7 +41,7 @@ def test_int8_quant_per_token_bit_exact(lib, cuda, tag, m, k):
     (1, 4096, 4096, False, False), (3, 1000, 512, True, False), (8, 6144, 4096, False, True),
     (9, 4096, 14336, False, False), (16, 64, 64, False, True), (17, 2048, 2048, True, True),
     (32, 28672, 4096, False, False), (33, 1024, 1024, False, False), (70, 512, 256, False, True),
-    # M > 32: the tcgen05 kind::i8 kernel (both operands through tensor-TMA, s32 accumulators in TMEM, split-k)
+    # M > 32: the wgmma s8 kernel (both operands through tensor-TMA, s32 register accumulators, split-k)
     (64, 6144, 4096, False, True), (128, 4096, 14336, True, False), (300, 1000, 1024, False, True)])
 def test_int8_linear_bit_exact(lib, cuda, tag, m, n, k, f32_scale, with_bias):
     from zhilight_b200 import ops
@@ -87,7 +87,7 @@ def test_fp8_quant_codes_bit_exact(lib, cuda, tag, m, k):
 @pytest.mark.parametrize("tag", ["f16", "bf16"])
 @pytest.mark.parametrize("m,n,k,with_bias", [(1, 4096, 4096, False), (4, 1000, 512, True), (16, 6144, 4096, False),
                                              (32, 4096, 14336, True), (35, 256, 128, False),
-                                             # M > 32: the tcgen05 kind::f8f6f4 kernel
+                                             # M > 32: the wgmma e4m3 kernel
                                              (64, 6144, 4096, True), (130, 4096, 4096, False)])
 def test_fp8_linear(lib, cuda, tag, m, n, k, with_bias):
     from zhilight_b200 import ops

@@ -1,6 +1,6 @@
 #!/usr/bin/env python
 """Decode attention timings (fp16 KV and int8 KV) at Llama-3.1-8B head shapes: CUDA events, KV buffers of all tasks
-exceed L2 at the larger settings.  One JSON object per line; engineering probe (profiles/)."""
+exceed L2 at the larger settings.  One JSON object per line; engineering probe."""
 import json
 import os
 import sys

@@ -1,6 +1,6 @@
 #!/usr/bin/env python
-"""Kernel-level timings on one B200 (CUDA events, L2-cold by rotating through weight copies > L2).
-Writes one JSON object per line.  Not the bench contract -- an engineering probe (see profiles/)."""
+"""Kernel-level timings on one H100 (CUDA events, L2-cold by rotating through weight copies > L2).
+Writes one JSON object per line.  Not the bench contract -- an engineering probe."""
 import json
 import os
 import sys

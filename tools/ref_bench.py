@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""Reference kernels (recompiled for sm_100, oracle/_ref) vs ours on the same B200: W4A16 GEMV at the
+"""Reference kernels (recompiled for sm_90a, oracle/_ref) vs ours on the same H100: W4A16 GEMV at the
 Llama-3.1-8B shapes.  CUDA events, weights rotated through > L2 worth of copies.  One JSON object per line."""
 import ctypes
 import json

@@ -1,6 +1,6 @@
 #!/usr/bin/env python
-"""The reference's default decode chain for one Llama-3.1-8B GPTQ layer (+ lm_head), timed on the same B200 through
-oracle/_ref (the reference's kernels recompiled for sm_100; SURVEY.md 8d "reference side-by-side (i)", 9.8 row 2), next to
+"""The reference's default decode chain for one Llama-3.1-8B GPTQ layer (+ lm_head), timed on the same H100 through
+oracle/_ref (the reference's kernels recompiled for sm_90a; SURVEY.md 8d "reference side-by-side (i)", 9.8 row 2), next to
 the Marlin GEMM at the layer's shapes.  TEST / MEASUREMENT INFRASTRUCTURE.  One JSON object per line."""
 import ctypes
 import json

@@ -1,6 +1,6 @@
 #!/usr/bin/env python
-"""tcgen05 W4A16 kernel (k_w4a16_tc) timings at the Llama-3.1-8B projection shapes, M = 32..256, weights rotated through
-> L2 worth of copies, CUDA events.  One JSON object per line; engineering probe (profiles/)."""
+"""wgmma W4A16 kernel (k_w4a16_ts) timings at the Llama-3.1-8B projection shapes, M = 32..256, weights rotated through
+> L2 worth of copies, CUDA events.  One JSON object per line; engineering probe."""
 import json
 import os
 import sys

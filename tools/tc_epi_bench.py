@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""tcgen05 W4A16 kernel with its fused epilogues (none / residual / SwiGLU) and with / without programmatic dependent launch,
+"""wgmma W4A16 kernel with its fused epilogues (none / residual / SwiGLU) and with / without programmatic dependent launch,
 CUDA-graph timing of 20 back-to-back launches on rotating weights.  Engineering probe: explains the gap between the plain
 GEMM microbench and the in-chain prefill GEMMs."""
 import json

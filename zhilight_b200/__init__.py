@@ -1,4 +1,4 @@
-"""zhilight_b200 -- B200-native (sm_100a) quantized-decode hot path of ZhiLight.
+"""zhilight_b200 -- H100-native (sm_90a) quantized-decode hot path of ZhiLight.
 
 Only what the hot path needs: `csrc/` (CUDA kernels + the C-ABI of include/zhilight_b200.h),
 `ops` (torch-tensor front end), `layers` (mirror of the reference's test-facing operator API,

@@ -1,4 +1,4 @@
-"""In-tree build of libzhilight_b200.so (sm_100a only).  nvcc cross-compiles without a GPU.
+"""In-tree build of libzhilight_b200.so (sm_90a only: H100).  nvcc cross-compiles without a GPU.
 
     python -m zhilight_b200.build [--force] [--verbose]
 """
@@ -15,7 +15,7 @@ OBJ_DIR = os.path.join(HERE, "build")
 LIB_PATH = os.path.join(HERE, "libzhilight_b200.so")
 
 NVCC_FLAGS = [
-    "-gencode", "arch=compute_100a,code=sm_100a",
+    "-gencode", "arch=compute_90a,code=sm_90a",
     "-O3", "-lineinfo", "-std=c++17",
     "--expt-relaxed-constexpr",
     "-Xcompiler", "-fPIC",
@@ -51,7 +51,7 @@ def _digest(paths):
 
 
 def build(force=False, verbose=False):
-    # fast path: the shipped .so already matches the sources (e.g. on the GPU box, where build/ is not shipped)
+    # fast path: the library already matches the sources
     all_digest = _digest(_sources() + _headers())
     dig_path = LIB_PATH + ".digest"
     if not force and os.path.exists(LIB_PATH) and os.path.exists(dig_path) and open(dig_path).read() == all_digest:
@@ -90,7 +90,7 @@ def build(force=False, verbose=False):
                 if verbose:
                     print("== %s\n%s" % (os.path.basename(src), log))
     if jobs or force or not os.path.exists(LIB_PATH):
-        cmd = [nvcc, "-shared", "-o", LIB_PATH] + objs + ["-gencode", "arch=compute_100a,code=sm_100a",
+        cmd = [nvcc, "-shared", "-o", LIB_PATH] + objs + ["-gencode", "arch=compute_90a,code=sm_90a",
                                                           "-lcudart", "-Xlinker", "--no-undefined"]
         r = subprocess.run(cmd, capture_output=True, text=True)
         if r.returncode != 0:

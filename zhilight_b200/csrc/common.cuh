@@ -1,4 +1,4 @@
-// Shared device helpers for the sm_100a kernels (mbarrier, bulk-TMA, PDL, mma.sync, packing).
+// Shared device helpers for the sm_90a kernels (mbarrier, bulk-TMA, PDL, mma.sync, packing).
 #pragma once
 #include <cuda_runtime.h>
 #include <cuda_fp16.h>
@@ -52,7 +52,7 @@ inline int device_sm_count() {
     if (dev >= 0 && dev < 64 && cache[dev] > 0) return cache[dev];
     int n = 0;
     cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev);
-    if (n <= 0) n = 148;
+    if (n <= 0) n = 132;
     if (dev >= 0 && dev < 64) cache[dev] = n;
     return n;
 }
@@ -130,7 +130,7 @@ __device__ __forceinline__ void bulk_g2s(void* smem_dst, const void* gsrc, uint3
 }
 
 // same copy, tagged evict-first in L2: a weight stream is read exactly once per step and must not push the
-// prefetched weights of the NEXT kernel (l2_prefetch below) out of the 126 MB L2
+// prefetched weights of the NEXT kernel (l2_prefetch below) out of the 50 MB L2
 __device__ __forceinline__ uint64_t l2_evict_first_policy() {
     uint64_t pol;
     asm volatile("createpolicy.fractional.L2::evict_first.b64 %0, 1.0;" : "=l"(pol));
@@ -191,7 +191,7 @@ __device__ __forceinline__ uint4 ld_nc_na_u4(const void* p) {
 }
 
 // ---------------------------------------------------------------------------------------------
-// warp-level tensor-core MMA (legacy path; the tcgen05 kernels live in w4a16_tc.cu)
+// warp-level tensor-core MMA (the wgmma kernels live in w4a16_tc.cu and w8_tc.cu)
 // D(16x8,f32) += A(16x16,f16,row) * B(16x8,f16,col)
 // ---------------------------------------------------------------------------------------------
 __device__ __forceinline__ void mma_16816_f16(float (&d)[4], const uint32_t (&a)[4], uint32_t b0, uint32_t b1,

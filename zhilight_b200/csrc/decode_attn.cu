@@ -284,8 +284,8 @@ k_decode_attn(const T* __restrict__ q, const int32_t* __restrict__ buf_lens, T* 
 
 
 // ---------------------------------------------------------------------------------------------------------
-// Latency-optimised variant for the small-batch / short-context regime (B200: 148 SMs, a B=1 decode step has
-// 8 kv-heads of work): 512 threads, at most 256 keys per CTA, and EVERY global load of the CTA (q, its K tile,
+// Latency-optimised variant for the small-batch / short-context regime (a B=1 decode step has 8 kv-heads of
+// work for 132 SMs): 512 threads, at most 256 keys per CTA, and EVERY global load of the CTA (q, its K tile,
 // its V rows) is issued before the first dependent instruction, so the whole CTA costs one memory round trip
 // instead of one per loop iteration.  Same math and split/combine contract as k_decode_attn.
 // ---------------------------------------------------------------------------------------------------------
@@ -338,7 +338,7 @@ static int attn_num_splits(int B, int len_q, int num_kv_heads, int m_query, int 
     const int hgroups = (m_query + 7) / 8;
     const int base = B * len_q * num_kv_heads * hgroups;
     const int min_splits = cdiv(max_len_buf, kAttnMaxRange);
-    const int want = cdiv(2 * 148, base);
+    const int want = cdiv(2 * device_sm_count(), base);
     const int max_useful = cdiv(max_len_buf, 256) > 0 ? cdiv(max_len_buf, 256) : 1;   // >= 256 keys per split
     int s = want < max_useful ? want : max_useful;
     if (s > kAttnMaxSplits) s = kAttnMaxSplits;
@@ -383,7 +383,7 @@ extern "C" int zl_decode_attention(const void* q, const int32_t* buf_lens, void*
     const int hg0 = (m_query + 7) / 8;
     const int short_splits = cdiv(max_len_buf, kShortRange);
     const bool use_short = short_splits <= kAttnMaxSplits &&
-                           (long long)B * len_q * num_kv_heads * hg0 * short_splits <= 4 * 148;
+                           (long long)B * len_q * num_kv_heads * hg0 * short_splits <= 4 * device_sm_count();
     if (use_short) splits = short_splits;
     const size_t vheads = (size_t)B * len_q * num_heads;
     float* part_o = nullptr;

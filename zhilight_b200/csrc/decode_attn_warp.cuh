@@ -1,4 +1,4 @@
-// Latency-optimised decode attention for the small-batch regime (B200: a batch-1 step has H_kv CTAs of work and sits
+// Latency-optimised decode attention for the small-batch regime (a batch-1 step has H_kv CTAs of work and sits
 // between two GEMMs that each take a few microseconds): one WARP owns 32 keys of one kv-head group end to end --
 // S = K.Q^T on the tensor cores, its own softmax statistics with shuffles only, P.V in fp32 -- so a CTA (<= 8 warps =
 // 256 keys) has exactly ONE __syncthreads: the log-sum-exp merge of its warps.  Every global load of a warp (q, 32 K rows,

@@ -32,7 +32,7 @@ __device__ __forceinline__ void mma_t<__nv_bfloat16>(float (&d)[4], const uint32
 
 // Persistent: a CTA walks tile groups blockIdx.x, blockIdx.x + gridDim.x, ... (lm_head: 8016 tiles on 296 CTAs) so that
 // one wave of CTAs with UNROLL k-steps in flight per warp (>= 13 MB chip-wide) streams the whole matrix without the
-// wave tails of a tile-per-warp grid (measured in the decode chain: 282 us -> see profiles/).
+// wave tails of a tile-per-warp grid.
 template <typename T, typename TO, int NT, int KS, int UNROLL>
 __global__ void __launch_bounds__(kDenseWarps * 32, 2)
 k_dense_skinny(const T* __restrict__ x, int ldx, const T* __restrict__ w, const T* __restrict__ bias,
@@ -171,7 +171,7 @@ static cudaError_t launch_dense_ks(const T* x, int ldx, const T* w, const T* bia
         int dev = 0;
         cudaGetDevice(&dev);
         cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
-        if (sms <= 0) sms = 148;
+        if (sms <= 0) sms = 132;
     }
     const int steps = K / 32;
     constexpr int UNROLL = NT == 1 ? 8 : 4;   // k-steps (2 x 16 B per lane each) in flight per warp

@@ -329,7 +329,7 @@ int build_w4(zl_llama* m, const std::vector<std::string>& prefixes, const std::v
     }
     const size_t pbytes = zl_w4_packed_bytes(N, K, m->cfg.group_size);
     ZL_CHECK_SUPPORTED(pbytes > 0);
-    // the ZLW4I layout serves the exact-integer kernel (M <= 16 when its staged activations fit) and the tcgen05 kernel
+    // the ZLW4I layout serves the exact-integer kernel (M <= 16 when its staged activations fit) and the wgmma kernel
     // (any M, N % 128 == 0); the fp16 mma.sync layout is only materialised when some launch size has neither
     const int m_max = m->cfg.prefill_chunk > m->cfg.max_batch ? m->cfg.prefill_chunk : m->cfg.max_batch;
     bool need_half = getenv("ZL_W4_FORCE_HALF") != nullptr;
@@ -624,7 +624,7 @@ static size_t prefetch_cap() {
     static long v = -1;
     if (v < 0) {
         const char* e = getenv("ZL_L2_PREFETCH_MB");
-        v = e ? atol(e) : 0;   // measured on B200: bulk L2 prefetch competes with the ring's TMA traffic; off by default
+        v = e ? atol(e) : 0;   // bulk L2 prefetch competes with the ring's TMA traffic; off by default
     }
     return (size_t)v << 20;
 }
@@ -688,7 +688,7 @@ int w4_gemm(zl_llama* m, const void* x, int ldx, const W4Lin& w, const void* res
     a.packed = use_int ? w.packed_i : w.packed;
     a.variant = use_int ? 1 : 0;
     if (route == 4 && ln_w) {
-        // the tcgen05 kernel reads x through the TMA engine: the RMSNorm runs as its own kernel (reference order,
+        // the wgmma kernel reads x through the TMA engine: the RMSNorm runs as its own kernel (reference order,
         // block.cpp:125,131) into the matching rows of xn
         const size_t off = (const char*)x - (const char*)m->h;
         void* xn = (char*)m->xn + off;
@@ -1342,6 +1342,13 @@ extern "C" int zl_llama_get_state(zl_llama_t* m, int32_t* tokens_host, int32_t* 
         tokens_host[i] = m->h_stage[i];
         positions_host[i] = m->h_stage[B + i];
     }
+    return ZL_OK;
+}
+
+extern "C" int zl_llama_get_logits(zl_llama_t* m, float* logits_host, int B) {
+    ZL_CHECK_ARG(m && logits_host && B > 0 && B <= m->cfg.max_batch);
+    ZL_CHECK_CUDA(cudaMemcpyAsync(logits_host, m->logits, (size_t)B * m->vshard * 4, cudaMemcpyDeviceToHost, m->stream));
+    ZL_CHECK_CUDA(cudaStreamSynchronize(m->stream));
     return ZL_OK;
 }
 

@@ -1,13 +1,14 @@
-// tcgen05 / TMEM / TMA building blocks shared by the tensor-core kernels (w4a16_tc.cu, w8_tc.cu): bounded mbarrier waits,
-// tensor-TMA loads, shared-memory matrix descriptors, TMEM loads, and the host-side tensor-map encoder.
+// wgmma / TMA building blocks shared by the tensor-core kernels (w4a16_tc.cu, w8_tc.cu): bounded mbarrier waits,
+// tensor-TMA loads, shared-memory matrix descriptors, wgmma fences, and the host-side tensor-map encoder.
 #pragma once
 #include "common.cuh"
+#include "wgmma.cuh"
 
 #include <cuda.h>
 
 namespace zl {
 
-constexpr int kTcRows = 128;   // rows per tile = UMMA M = TMEM lanes
+constexpr int kTcRows = 128;   // weight rows per tile: two consumer warpgroups of wgmma M = 64
 
 // ---- PTX wrappers -------------------------------------------------------------------------------------------------
 __device__ __forceinline__ void mbar_arrive(uint64_t* bar) {
@@ -51,14 +52,6 @@ __device__ __forceinline__ void tma_load_4d_hint(void* smem_dst, const CUtensorM
         "l"(reinterpret_cast<uint64_t>(map)), "r"(c0), "r"(c1), "r"(c2), "r"(c3), "r"(smem_u32(bar)), "l"(policy)
         : "memory");
 }
-// registers -> TMEM: lane i of the warp writes r[0..15] to columns taddr.col .. +15 of TMEM lane (taddr.lane + i)
-__device__ __forceinline__ void tc_st16(uint32_t taddr, const uint32_t (&r)[16]) {
-    asm volatile(
-        "tcgen05.st.sync.aligned.32x32b.x16.b32 [%0], {%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16};" ::"r"(taddr),
-        "r"(r[0]), "r"(r[1]), "r"(r[2]), "r"(r[3]), "r"(r[4]), "r"(r[5]), "r"(r[6]), "r"(r[7]), "r"(r[8]), "r"(r[9]),
-        "r"(r[10]), "r"(r[11]), "r"(r[12]), "r"(r[13]), "r"(r[14]), "r"(r[15])
-        : "memory");
-}
 // tagged 8-byte words of the partial-tile exchange: {payload, tag}, one atomic store / load each
 __device__ __forceinline__ void tc_st_tag(uint2* p, uint32_t data, uint32_t tag) {
     asm volatile("st.volatile.global.v2.u32 [%0], {%1, %2};" ::"l"(p), "r"(data), "r"(tag) : "memory");
@@ -68,46 +61,21 @@ __device__ __forceinline__ uint2 tc_ld_tag(const uint2* p) {
     asm volatile("ld.volatile.global.v2.u32 {%0, %1}, [%2];" : "=r"(v.x), "=r"(v.y) : "l"(p) : "memory");
     return v;
 }
-__device__ __forceinline__ void tc_wait_st() { asm volatile("tcgen05.wait::st.sync.aligned;" ::: "memory"); }
-// true in exactly one lane of a converged warp (elect.sync): ptxas then knows the guarded region is single-threaded and passes
-// the tcgen05 operands through plain R2UR moves instead of a per-instruction ELECT / R2UR.BROADCAST waterfall loop
-__device__ __forceinline__ bool tc_elect_one() {
-    uint32_t pred;
-    asm volatile(
-        "{\n\t.reg .pred p;\n\t"
-        "elect.sync _|p, 0xffffffff;\n\t"
-        "selp.u32 %0, 1, 0, p;\n\t}"
-        : "=r"(pred));
-    return pred != 0;
-}
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_commit(uint64_t* bar) {
-    asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar))
-                 : "memory");
-}
-// K-major, SWIZZLE_128B shared-memory matrix descriptor (cute/arch/mma_sm100_desc.hpp SmemDescriptor): start address
-// >> 4, LBO (unused for swizzled K-major, canonical value 1), SBO = 1024 B between 8-row groups, version 1, layout 2.
-__device__ __forceinline__ uint64_t tc_desc_sw128(uint32_t saddr) {
+// K-major, 128-byte-swizzled shared-memory matrix descriptor of wgmma: start address >> 4, LBO (unused for swizzled K-major,
+// canonical value 1), SBO = 1024 B between 8-row groups, layout type 1 (SWIZZLE_128B).  The tile must be 1024-byte aligned;
+// +2 on the descriptor advances K by 32 bytes inside the swizzle atom.
+__device__ __forceinline__ uint64_t wg_desc_sw128(uint32_t saddr) {
     uint64_t d = (uint64_t)((saddr >> 4) & 0x3FFF);
     d |= (uint64_t)1 << 16;
     d |= (uint64_t)(1024 >> 4) << 32;
-    d |= (uint64_t)1 << 46;
-    d |= (uint64_t)2 << 61;
+    d |= (uint64_t)1 << 62;
     return d;
 }
-__device__ __forceinline__ void tc_ld16(uint32_t taddr, float (&v)[16]) {
-    uint32_t r[16];
-    asm volatile(
-        "tcgen05.ld.sync.aligned.32x32b.x16.b32 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15}, [%16];"
-        : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),
-          "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15])
-        : "r"(taddr));
-    asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-#pragma unroll
-    for (int i = 0; i < 16; ++i) v[i] = __uint_as_float(r[i]);
-}
-__device__ __forceinline__ void epi_bar() { asm volatile("bar.sync 1, 128;" ::: "memory"); }
+__device__ __forceinline__ void wg_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wg_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wg_wait_all() { asm volatile("wgmma.wait_group.sync.aligned 0;" ::: "memory"); }
+// named barrier of the two consumer warpgroups (the producer warp does not take part)
+__device__ __forceinline__ void consumer_bar() { asm volatile("bar.sync 1, 256;" ::: "memory"); }
 
 // ---- host: cuTensorMapEncodeTiled through the runtime's driver entry point (no -lcuda) ----
 typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*,
@@ -127,7 +95,7 @@ inline EncodeTiledFn tc_encode_fn() {
 }
 
 // 2-D row-major tensor (rows, cols) of `elem_bytes`-byte elements, row pitch ld_bytes; box = 128 bytes of a row x box_rows
-// rows, 128-byte swizzle (the K-major UMMA operand layout), out-of-bounds rows / columns read as zero
+// rows, 128-byte swizzle (the K-major wgmma operand layout), out-of-bounds rows / columns read as zero
 inline bool tc_make_map_2d(CUtensorMap* map, const void* base, CUtensorMapDataType dt, int elem_bytes, uint64_t rows,
                            uint64_t cols, uint64_t ld_bytes, uint32_t box_rows) {
     EncodeTiledFn enc = tc_encode_fn();
@@ -166,8 +134,8 @@ struct TcDeviceState {
     unsigned* err = nullptr;
     size_t ws_bytes = 0;
 };
-constexpr size_t kTcWsLlBytes = 80ull << 20;   // >= 2 slots x 148 CTAs x 256 tokens x 128 rows x 8 B
-constexpr size_t kTcWsBytes = 64ull << 20;   // >= 2 x 148 items x 256 tokens x 128 rows x 4 B
+constexpr size_t kTcWsLlBytes = 80ull << 20;   // >= 2 slots x 132 CTAs x 256 tokens x 128 rows x 8 B
+constexpr size_t kTcWsBytes = 64ull << 20;   // >= 2 x 132 items x 256 tokens x 128 rows x 4 B
 constexpr int kTcMaxTiles = 8192;
 TcDeviceState* tc_state();                   // w4a16_tc.cu; nullptr before prepare_w4_tc() ran on the current device
 

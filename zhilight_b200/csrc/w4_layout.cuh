@@ -1,4 +1,4 @@
-// ZLW4: tile-packed int4 weight layout for the B200 W4A16 kernels (DESIGN.md section 3).
+// ZLW4: tile-packed int4 weight layout for the W4A16 kernels (DESIGN.md section 3).
 //
 // The matrix W (N rows = output features, K cols) is cut into blocks of 32 rows x 128 k
 // (= one quantization group of the g128 checkpoints).  Blocks are stored [N/32][K/128], each

@@ -47,7 +47,7 @@ cudaError_t prepare_w4_v2();
 bool launch_w4_v3(const W4Params& p, bool pdl, cudaStream_t stream, cudaError_t* err);
 bool w4_v3_fits(int mc, int N, int K);
 cudaError_t prepare_w4_v3();
-// tcgen05 / TMEM / TMA kernel on the ZLW4I layout (w4a16_tc.cu): up to 256 tokens per launch, N % 128 == 0, no fused
+// wgmma / TMA kernel on the ZLW4I layout (w4a16_tc.cu): up to 256 tokens per launch, N % 128 == 0, no fused
 // RMSNorm prologue (ln_w is ignored)
 cudaError_t launch_w4_tc(const W4Params& p, bool pdl, cudaStream_t stream);
 bool w4_tc_supports(int mc, int N, int K);

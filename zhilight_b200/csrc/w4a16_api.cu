@@ -3,7 +3,7 @@
 // Stands in for nn::gptq::gptq_gemm_k_major's router (reference src/nn/quant/gptq/q_gemm_k_major.cu:957-1116:
 // M <= 40 GEMV, else dequant + cuBLASLt) and for GPTQMarlin::forward (src/nn/linear/linear.cpp:1247-1451):
 //   M <= 16 and the staged activations fit shared memory -> k_w4a16_v3  (exact-integer mma.sync kernel, ZLW4I layout)
-//   otherwise, N % 128 == 0                              -> k_w4a16_ts  (tcgen05 kernel, A operand in TMEM, ZLW4I layout)
+//   otherwise, N % 128 == 0                              -> k_w4a16_ts  (wgmma kernel, A operand in registers, ZLW4I layout)
 //   otherwise                                            -> k_w4a16_v2  (fp16 mma.sync kernel, ZLW4 layout, 32-row passes)
 #include "common.cuh"
 #include "w4_layout.cuh"
@@ -15,7 +15,7 @@
 using namespace zl;
 
 extern "C" int zl_prepare(void) {
-    // opt-in shared memory sizes and the per-device split-k workspace of the tcgen05 kernel must be set up outside of
+    // opt-in shared memory sizes and the per-device split-k workspace of the wgmma kernel must be set up outside of
     // stream capture; idempotent per device
     ZL_CHECK_CUDA(prepare_w4_v2());
     ZL_CHECK_CUDA(prepare_w4_v3());
@@ -24,14 +24,14 @@ extern "C" int zl_prepare(void) {
     return ZL_OK;
 }
 
-// ZL_W4_NO_TC=1 (experiments): never route to the tcgen05 kernel
+// ZL_W4_NO_TC=1 (experiments): never route to the wgmma kernel
 static bool tc_disabled() {
     static int v = -1;
     if (v < 0) v = getenv("ZL_W4_NO_TC") ? 1 : 0;
     return v != 0;
 }
 
-// which kernel serves (M, N, K) on the ZLW4I layout: 3 = exact-integer mma.sync, 4 = tcgen05, 0 = neither
+// which kernel serves (M, N, K) on the ZLW4I layout: 3 = exact-integer mma.sync, 4 = wgmma, 0 = neither
 static int int_layout_route(int M, int N, int K) {
     if (M <= 16 && w4_v3_fits(M, N, K)) return 3;
     if (!tc_disabled() && w4_tc_supports(M < 256 ? M : 256, N, K)) return 4;
@@ -134,10 +134,10 @@ extern "C" int zl_w4a16_gemm_fused(const zl_w4_fused_args_t* a, zl_stream_t stre
         }
     }
     const int n_out = a->epilogue == ZL_EPI_SWIGLU ? a->N / 2 : a->N;
-    // rows per pass: the tcgen05 kernel takes up to 256 tokens at once, the mma.sync kernels 32 (v2) / 16 (v3)
+    // rows per pass: the wgmma kernel takes up to 256 tokens at once, the mma.sync kernels 32 (v2) / 16 (v3)
     const int route = a->variant == kW4VariantInt ? int_layout_route(a->M, a->N, a->K) : 2;
     ZL_CHECK_SUPPORTED(route != 0 && "ZLW4I layout: M > 16 (or staged activations too large) and N % 128 != 0: use variant 0");
-    ZL_CHECK_SUPPORTED(!(route == 4 && a->ln_weight) && "the tcgen05 kernel has no fused RMSNorm prologue: run zl_rmsnorm first");
+    ZL_CHECK_SUPPORTED(!(route == 4 && a->ln_weight) && "the wgmma kernel has no fused RMSNorm prologue: run zl_rmsnorm first");
     const int step = route == 4 ? 256 : 32;
     for (int m0 = 0; m0 < a->M; m0 += step) {
         W4Params p;

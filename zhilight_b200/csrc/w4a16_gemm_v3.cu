@@ -1,9 +1,9 @@
 // W4A16 skinny GEMM, exact-integer variant (ZLW4I layout): the default for small M.
 //
-// Why: on B200 a decode GEMM must consume ~23 weight bytes per cycle per SM to keep up with HBM.  The classic
+// Why: a decode GEMM must consume ~14 weight bytes per cycle per SM to keep up with an H100's HBM3.  The classic
 // "dequantise int4 -> fp16 on the CUDA cores, then HMMA" recipe (our v1/v2 kernels, Marlin, the reference's
 // GEMV) costs ~10 issue slots per packed word, which makes the kernel ISSUE-bound before it is HBM-bound
-// (profiles/r01b_w4a16_v2.txt: 48 % issue utilisation at 32 % of HBM peak).  Here the int4 weights never
+// (measured on the previous target).  Here the int4 weights never
 // become floating point:
 //   * activations are decomposed once per CTA into a block-floating-point integer  x_k = 2^e_g * m_k,
 //     m_k a 16-bit integer per 128-group (error <= 2^-16 of the group maximum, far below fp16's own 2^-11),
@@ -708,7 +708,7 @@ static bool v3_try(const W4Params& p, bool pdl, cudaStream_t stream, cudaError_t
 static int v3_max_stages() {
     static int v = -1;
     if (v < 0) {
-        // measured on B200 (Llama-3.1-8B B=1): 5 stages 600 tok/s, 6 stages 568 tok/s -- deeper rings only add HBM
+        // deeper rings only add HBM
         // queueing, so the 6-stage variants stay opt-in
         const char* e = getenv("ZL_W4_STAGES");
         v = e ? atoi(e) : 4;

@@ -1,6 +1,6 @@
-// W4A16 GEMM on the 5th-generation tensor cores: tcgen05.mma (kind::f16) with the dequantised weights as the A operand in
-// TENSOR MEMORY, activations through tensor-TMA, TMEM accumulators.  Serves every M the exact-integer mma.sync kernel
-// (w4a16_gemm_v3.cu) cannot stage: batch 17..256 decode and chunked prefill.
+// W4A16 GEMM on the Hopper tensor cores: wgmma.mma_async (f16 x f16 -> f32) with the dequantised weights as the A operand
+// in REGISTERS, activations through tensor-TMA as the shared-memory B operand, register accumulators.  Serves every M the
+// exact-integer mma.sync kernel (w4a16_gemm_v3.cu) cannot stage: batch 17..256 decode and chunked prefill.
 //
 // Replaces the reference's Marlin kernel (src/nn/quant/marlin/gptq_marlin.cu:425-1620), the M <= 40 GEMV tiles of
 // KERNEL_gemm_warp_reduce (src/nn/quant/gptq/q_gemm_k_major.cu:176-237, 580-686: the weight matrix is streamed
@@ -10,29 +10,23 @@
 //
 // One CTA per SM.  The work is the list of (128-row tile, 128-k group) units in tile-major order, cut into one contiguous
 // range per CTA ("stream-k"): a tile that lies inside one range is finished by that CTA alone, a tile cut by a range
-// boundary is shared by the CTAs that own its pieces -- each writes its fp32 partial tile to a per-CTA slot, the last
-// arriver (one atomic per piece) adds the pieces in k order (deterministic) and runs the epilogue.  Every CTA does its
-// (at most two) partial pieces FIRST, so the exchange overlaps the full tiles that follow.
+// boundary is shared by the CTAs that own its pieces -- each writes its fp32 partial tile to a per-CTA slot as tagged words,
+// the owners then split the tile's tokens among themselves and add the pieces in k order (deterministic).  Every CTA does
+// its (at most two) partial pieces FIRST, so the exchange overlaps the full tiles that follow.
 //
-//   warps 0-3          epilogue     : tcgen05.ld 32x32b of their TMEM lane quadrant; bias / residual / SwiGLU / qkv-RoPE-KV
-//   warps 4 .. 4+4KQ-1 dequant      : quadrant = warp % 4 = 32-row block of the tile, k-slice = (warp - 4) / 4 of KQ;
-//                                     the lane owns ONE weight row: nibbles -> fp16 (PRMT 0x64xx / 0x54xx magic, exact
-//                                     q - z, one HMUL2 by the group scale) in registers, tcgen05.st into the A columns
-//   then               raw producer : tensor-TMA (UTMALDG.4D / .3D) of the 4 ZLW4I records of a stage
-//                      x producer   : cp.async.bulk.tensor.2d, box 64 k x NTOK tokens, SWIZZLE_128B, OOB rows = 0
-//                      MMA issuer   : one thread, 8 x tcgen05.mma 128 x NTOK x 16 per stage (A from TMEM, B from smem),
-//                                     tcgen05.commit frees the stage; also owns the TMEM allocation
+//   warps 0-7  consumers : two warpgroups; warpgroup r owns weight rows 64 r .. 64 r + 63 of the tile (two ZLW4I 32-row
+//                          blocks).  Per 128-k group each thread converts its A fragments (rows g and g + 8 of its warp's
+//                          16-row slab: PRMT 0x64xx / 0x54xx magic, exact q - z, one HMUL2 by the group scale), issues
+//                          8 x wgmma m64 x NTOK x 16, and at the end of a piece runs the bias / residual / SwiGLU /
+//                          qkv-RoPE-KV epilogue from its accumulators
+//   warp 8     producer  : tensor-TMA (4-D / 3-D maps) of the 4 ZLW4I records of a stage and of the x tile
+//                          (box 64 k x NTOK tokens, SWIZZLE_128B, OOB rows = 0)
 //
-// Why A in TMEM (measured on the first version, which wrote a swizzled fp16 A tile to shared memory; profiles/r02_w4a16_tc_*):
-// a 128 x 128 fp16 A stage is 32 KB written and read back through shared memory per 8.5 KB of HBM traffic, plus a
-// generic->async proxy fence per hand-over and ~10 address / store instructions per converted word.  With TMEM lane =
-// weight row and 32-bit column = two consecutive k the conversion stays in registers.
-//
-// A ZLW4I word holds 4 k of row g (low nibbles) and of row g + 8 (high nibbles); the thread of row g masks the low
-// nibbles, the thread of row g + 8 the high ones (same words, a shared-memory broadcast).  Lanes g = 0..7 of a
-// quarter-warp read 16-byte chunks 64 B apart -- a 4-way bank conflict in the plain record layout -- so the nibble words
-// arrive through a tensor map with 64-byte swizzle (chunk ^= (row >> 1) & 3): conflict-free, the HBM format is unchanged.
-// The 80-byte scale / zero trailers of the four records of a stage come through a second (unswizzled) map.
+// A ZLW4I word holds 4 k of row g (low nibbles) and of row g + 8 (high nibbles), which is exactly the row pair of a wgmma
+// A fragment: one 16-bit half of a word gives a thread both rows for its two consecutive k.  The 8 row groups g of a warp
+// read 16-byte chunks 64 B apart -- a 4-way bank conflict in the plain record layout -- so the nibble words arrive through a
+// tensor map with 64-byte swizzle (chunk ^= (row >> 1) & 3): conflict-free, the HBM format is unchanged.  The 80-byte
+// scale / zero trailers of the four records of a stage come through a second (unswizzled) map.
 #include "common.cuh"
 #include "w4_layout.cuh"
 #include "w4_params.h"
@@ -54,11 +48,8 @@ struct alignas(64) W4TcParams {
     const __half* residual;
     __half* y;
     int M, N, K, epi;
-    int dbg;                    // ZL_TC_DBG timing ablations (results are wrong): 1 no x loads, 2 no dequant, 4 no MMA, 8 no weight loads
     uint2* ws;                  // [2 * CTA + slot][M][128] tagged words {fp32 partial sum, tag}: all zero between launches
-    float* ws_f32;              // plain scratch (its last MB carries the ZL_TC_DBG trace)
     unsigned* err;              // watchdog code
-    long long* trace;           // ZL_TC_DBG & 16: clock64 stamps of CTA 0, [role][64 stages][8]
     const float* cos;
     const float* sin;
     __half* q_out;
@@ -69,118 +60,72 @@ struct alignas(64) W4TcParams {
     int num_heads, num_kv_heads, dim_head;
 };
 
-// instruction descriptor, kind::f16: D f32 (bits 4-5 = 1), A/B f16 (0), both K-major, N >> 3 at bit 17, M >> 4 at bit 24
-__host__ __device__ constexpr uint32_t tc_idesc_f16(int n) {
-    return (1u << 4) | ((uint32_t)(n >> 3) << 17) | ((uint32_t)(kTcRows >> 4) << 24);
-}
-__device__ __forceinline__ void tc_mma_f16_ts(uint32_t d_tmem, uint32_t a_tmem, uint64_t bdesc, uint32_t idesc, uint32_t accum) {
-    asm volatile(
-        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %4, 0;\n\t"
-        "tcgen05.mma.cta_group::1.kind::f16 [%0], [%1], %2, %3, p;\n\t}" ::"r"(d_tmem),
-        "r"(a_tmem), "l"(bdesc), "r"(idesc), "r"(accum)
-        : "memory");
-}
-
-// ---- epilogue of 16 tokens (c0 .. c0+15) for the weight row owned by this lane -----------------------------------------
-// Packed row p = tile * 128 + 32 * quadrant + lane.  Inside a 32-row block, rows (16 tt + g) and (16 tt + g + 8) are
-// partners (gate / up, RoPE low / high half): lane and lane + 8.
-// the epilogue warps share their schedulers with the dequant warps, which are issue-bound: SiLU through the fast exp / divide
-// (2 ulp of fp32, invisible after the fp16 rounding of the product)
+// ---- epilogue of one token for one row pair -----------------------------------------------------------------------------
+// Packed rows blk * 32 + 16 tt + g (lo) and + 8 (hi) are partners (gate / up, RoPE low / high half); a wgmma accumulator
+// fragment holds both for the same token.
 __device__ __forceinline__ float tc_silu(float x) { return __fdividef(x, 1.0f + __expf(-x)); }
 
-__device__ __forceinline__ void tc_epilogue16(const W4TcParams& p, int prow, int lane, int c0, float (&v)[16],
-                                              const uint32_t* rpre = nullptr) {   // rpre: 16 residual halves, packed in pairs
-    const float b = p.bias ? __half2float(p.bias[prow]) : 0.f;
+__device__ __forceinline__ void tc_epilogue_pair(const W4TcParams& p, int blk, int tt, int g, int tok, float vlo, float vhi) {
+    if (tok >= p.M) return;
+    const int plo = blk * 32 + tt * 16 + g, phi = plo + 8;
+    const float lo = __half2float(__float2half_rn(vlo + (p.bias ? __half2float(p.bias[plo]) : 0.f)));
+    const float hi = __half2float(__float2half_rn(vhi + (p.bias ? __half2float(p.bias[phi]) : 0.f)));
     if (p.epi == ZL_EPI_SWIGLU) {
-        const int n_out = p.N / 2;
-        const int col = (prow >> 5) * 16 + ((lane >> 4) << 3) + (lane & 7);
-#pragma unroll
-        for (int i = 0; i < 16; ++i) {
-            const float mine = __half2float(__float2half_rn(v[i] + b));
-            const float up = __shfl_down_sync(0xffffffffu, mine, 8);
-            const int tok = c0 + i;
-            if (!(lane & 8) && tok < p.M) p.y[(size_t)tok * n_out + col] = __float2half_rn(tc_silu(mine) * up);
-        }
+        p.y[(size_t)tok * (p.N / 2) + blk * 16 + tt * 8 + g] = __float2half_rn(tc_silu(lo) * hi);
     } else if (p.epi == ZL_EPI_QKV_ROPE) {
         const int d = p.dim_head, half_dim = d / 2, tiles_per_head = d / 32;
-        const int st = prow >> 5, head = st / tiles_per_head, jt = st % tiles_per_head;
-        const int c = jt * 16 + ((lane >> 4) << 3) + (lane & 7);
+        const int head = blk / tiles_per_head, jt = blk % tiles_per_head;
+        const int c = jt * 16 + tt * 8 + g;
         const bool is_v = head >= p.num_heads + p.num_kv_heads;
-#pragma unroll
-        for (int i = 0; i < 16; ++i) {
-            const float lo = __half2float(__float2half_rn(v[i] + b));
-            const float hi = __shfl_down_sync(0xffffffffu, lo, 8);
-            const int tok = c0 + i;
-            if ((lane & 8) || tok >= p.M) continue;
-            __half olo, ohi;
-            if (is_v) {
-                olo = __float2half_rn(lo);
-                ohi = __float2half_rn(hi);
-            } else {
-                const float* cs = p.cos + (size_t)tok * d;
-                const float* sn = p.sin + (size_t)tok * d;
-                olo = __float2half_rn(lo * cs[c] - hi * sn[c]);
-                ohi = __float2half_rn(hi * cs[c + half_dim] + lo * sn[c + half_dim]);
-            }
-            if (head < p.num_heads) {
-                __half* dst = p.q_out + ((size_t)tok * p.num_heads + head) * d;
+        __half olo, ohi;
+        if (is_v) {
+            olo = __float2half_rn(lo);
+            ohi = __float2half_rn(hi);
+        } else {
+            const float* cs = p.cos + (size_t)tok * d;
+            const float* sn = p.sin + (size_t)tok * d;
+            olo = __float2half_rn(lo * cs[c] - hi * sn[c]);
+            ohi = __float2half_rn(hi * cs[c + half_dim] + lo * sn[c + half_dim]);
+        }
+        if (head < p.num_heads) {
+            __half* dst = p.q_out + ((size_t)tok * p.num_heads + head) * d;
+            dst[c] = olo;
+            dst[c + half_dim] = ohi;
+        } else {
+            const int pl = p.placement[tok];
+            if (pl >= 0) {
+                const bool is_k = !is_v;
+                const int hk = is_k ? head - p.num_heads : head - p.num_heads - p.num_kv_heads;
+                __half* base = (is_k ? p.k_addrs : p.v_addrs)[p.token_batch[tok]];
+                __half* dst = base + ((size_t)pl * p.num_kv_heads + hk) * d;
                 dst[c] = olo;
                 dst[c + half_dim] = ohi;
-            } else {
-                const int pl = p.placement[tok];
-                if (pl >= 0) {
-                    const bool is_k = !is_v;
-                    const int hk = is_k ? head - p.num_heads : head - p.num_heads - p.num_kv_heads;
-                    __half* base = (is_k ? p.k_addrs : p.v_addrs)[p.token_batch[tok]];
-                    __half* dst = base + ((size_t)pl * p.num_kv_heads + hk) * d;
-                    dst[c] = olo;
-                    dst[c + half_dim] = ohi;
-                }
             }
         }
     } else {
-#pragma unroll
-        for (int i = 0; i < 16; ++i) {
-            const int tok = c0 + i;
-            if (tok >= p.M) continue;
-            __half h = __float2half_rn(v[i] + b);
-            if (p.epi == ZL_EPI_RESIDUAL) {
-                const __half r = rpre ? __ushort_as_half((unsigned short)(rpre[i >> 1] >> ((i & 1) * 16)))
-                                      : p.residual[(size_t)tok * p.N + prow];
-                h = __float2half_rn(__half2float(h) + __half2float(r));
-            }
-            p.y[(size_t)tok * p.N + prow] = h;
+        __half hlo = __float2half_rn(lo), hhi = __float2half_rn(hi);
+        if (p.epi == ZL_EPI_RESIDUAL) {
+            hlo = __float2half_rn(lo + __half2float(p.residual[(size_t)tok * p.N + plo]));
+            hhi = __float2half_rn(hi + __half2float(p.residual[(size_t)tok * p.N + phi]));
         }
+        p.y[(size_t)tok * p.N + plo] = hlo;
+        p.y[(size_t)tok * p.N + phi] = hhi;
     }
 }
 
-
 template <int NTOK>
 struct TsCfg {
-    static constexpr int KQ = 2;                                        // k-slices per quadrant
-    static constexpr int GW = 4 * KQ;                                   // dequant warps per group (one group converts one stage)
-    static constexpr int NG = 2;                                        // groups take the stages alternately
-    static constexpr int DQ = NG * GW;
-    static constexpr int kWarpDq0 = 4, kWarpRaw = 4 + DQ, kWarpX = kWarpRaw + 1, kWarpMma = kWarpRaw + 2;
-    static constexpr int kThreads = (kWarpMma + 1) * 32;
-    // A pipeline stage is KG quantisation groups (KG x 128 k): every hand-over (mbarrier wait, fence, commit) costs the
-    // single MMA-issuing warp 60-150 cycles, ~700 per stage (measured with the clock64 trace, profiles/r02_tc_trace_*),
-    // against 128 cycles of tensor work per group at 32 tokens -- two groups per stage halve that overhead per byte.
-    static constexpr int KG = NTOK <= 128 ? 2 : 1;
-    static constexpr int AS = NTOK <= 64 ? 3 : (NTOK <= 128 ? 2 : 3);   // A (TMEM) / x (smem) stages
-    static constexpr int RS = NTOK <= 64 ? 4 : 3;                       // raw weight stages
-    static constexpr int NACC = NTOK <= 128 ? 2 : 1;                    // accumulator buffers in TMEM
-    static constexpr int kACol0 = NACC * NTOK;                          // first A column; 64 columns per group
+    static constexpr int kThreads = 9 * 32;                             // 2 consumer warpgroups + 1 producer warp
+    static constexpr int kWarpProducer = 8;
+    static constexpr int ST = NTOK <= 64 ? 8 : (NTOK <= 128 ? 5 : 3);   // stages of one 128-k group
     static constexpr int kXGroup = 2 * NTOK * 128;                      // [k atom (64 k)][token][128 B]
     static constexpr int kNibGroup = 4 * 2048, kTrGroup = 384;          // 4 x 80 B trailers, padded to the TMA alignment
     static constexpr int kXOff = 0;
-    static constexpr int kNibOff = kXOff + AS * KG * kXGroup;
-    static constexpr int kTrOff = kNibOff + RS * KG * kNibGroup;
-    static constexpr int kBarOff = kTrOff + RS * KG * kTrGroup;
-    static constexpr int kNumBars = 2 * RS + 2 * AS + 4;
-    static constexpr int kMiscOff = kBarOff + kNumBars * 8;
-    static constexpr int kBytes = kMiscOff + 16 + 1024;                 // + slack for the manual 1024-byte alignment
-    static_assert(kACol0 + AS * KG * 64 <= 512, "TMEM columns");
+    static constexpr int kNibOff = kXOff + ST * kXGroup;
+    static constexpr int kTrOff = kNibOff + ST * kNibGroup;
+    static constexpr int kBarOff = kTrOff + ST * kTrGroup;
+    static constexpr int kNumBars = 2 * ST;
+    static constexpr int kBytes = kBarOff + kNumBars * 8 + 1024;        // + slack for the manual 1024-byte alignment
     static_assert(kBytes <= 232448, "shared memory");
 };
 
@@ -237,367 +182,179 @@ struct TcSched {
     }
 };
 
+// dequantised fp16 pair (q - z) * s of two 4-bit codes picked from `w` by the PRMT selector
+__device__ __forceinline__ uint32_t tc_dq2(uint32_t w, uint32_t magic, uint32_t sel, __half2 cz, __half2 s2) {
+    uint32_t a = __byte_perm(w, magic, sel);
+    __half2 v = __hmul2(__hsub2(*reinterpret_cast<__half2*>(&a), cz), s2);
+    return *reinterpret_cast<uint32_t*>(&v);
+}
+
 template <int NTOK>
 __global__ void __launch_bounds__(TsCfg<NTOK>::kThreads, 1) k_w4a16_ts(const __grid_constant__ W4TcParams p) {
     using C = TsCfg<NTOK>;
-    constexpr int KG = C::KG, NG = C::NG;
     extern __shared__ uint8_t smem_dyn[];
     uint8_t* smem = smem_dyn + ((1024u - (smem_u32(smem_dyn) & 1023u)) & 1023u);
-    uint64_t* bars = reinterpret_cast<uint64_t*>(smem + C::kBarOff);
-    uint64_t* raw_full = bars;
-    uint64_t* raw_empty = raw_full + C::RS;
-    uint64_t* a_full = raw_empty + C::RS;      // dequant warps of the stage's group + the x producer (carries the x bytes)
-    uint64_t* ax_empty = a_full + C::AS;
-    uint64_t* acc_full = ax_empty + C::AS;
-    uint64_t* acc_empty = acc_full + 2;
-    uint32_t* s_tmem = reinterpret_cast<uint32_t*>(smem + C::kMiscOff);
+    uint64_t* full = reinterpret_cast<uint64_t*>(smem + C::kBarOff);
+    uint64_t* empty = full + C::ST;
 
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     const int G = p.K / kW4GroupK, n_tiles = p.N / kTcRows;
     const TcSched sch(n_tiles, G, (int)gridDim.x, (int)blockIdx.x);
-    const bool tracing = (p.dbg & 16) && blockIdx.x == 0 && p.trace;
-    auto stamp = [&](int role, int stage, int ev) {
-        if (tracing && stage < 64) p.trace[(role * 64 + stage) * 8 + ev] = clock64();
-    };
 
     if (threadIdx.x == 0) {
-        for (int i = 0; i < C::RS; ++i) {
-            mbar_init(&raw_full[i], 1);
-            mbar_init(&raw_empty[i], C::GW);
-        }
-        for (int i = 0; i < C::AS; ++i) {
-            mbar_init(&a_full[i], C::GW + 1);
-            mbar_init(&ax_empty[i], 1);
-        }
-        for (int i = 0; i < 2; ++i) {
-            mbar_init(&acc_full[i], 1);
-            mbar_init(&acc_empty[i], 4);
+        for (int i = 0; i < C::ST; ++i) {
+            mbar_init(&full[i], 1);
+            mbar_init(&empty[i], 8);             // one arrival per consumer warp
         }
         mbar_fence_init();
     }
-    if (warp == C::kWarpMma) {
-        asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(s_tmem)), "n"(512));
-        asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;");
-    }
     pdl_trigger();
-    tc_fence_before();
     __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem_base = *s_tmem;
 
-    if (warp == C::kWarpRaw) {
-        // ---------------- weight stream: constants, may run ahead of the predecessor kernel (PDL) ----------------
-        const uint64_t pol = l2_evict_first_policy();
-        int rs = 0, st_i = 0;
-        uint32_t ph = 0;
-        for (int si = 0; si < sch.n_segs; ++si) {
-            int tile, g0, g1;
-            sch.seg(si, tile, g0, g1);
-            for (int gi = g0; gi < g1; gi += KG, ++st_i) {
-                const int ng = min(KG, g1 - gi);
-                mbar_wait_wd(&raw_empty[rs], ph ^ 1u, p.err, 0x100 + rs);
-                if (lane == 0) stamp(0, st_i, 1);
-                if (tc_elect_one()) {
-                    if (p.dbg & 8) {
-                        mbar_arrive(&raw_full[rs]);
-                    } else {
-                        mbar_expect_tx(&raw_full[rs], (uint32_t)ng * (C::kNibGroup + 4 * 80));
-#pragma unroll
-                        for (int j = 0; j < KG; ++j)
-                            if (j < ng) {
-                                tma_load_4d_hint(smem + C::kNibOff + (rs * KG + j) * C::kNibGroup, &p.wmap, 0, 0, gi + j, tile * 4,
-                                                 &raw_full[rs], pol);
-                                tma_load_3d_hint(smem + C::kTrOff + (rs * KG + j) * C::kTrGroup, &p.tmap, 0, gi + j, tile * 4,
-                                                 &raw_full[rs], pol);
-                            }
+    if (warp == C::kWarpProducer) {
+        // weights are constants and may be requested before the predecessor kernel has finished (PDL); x may not
+        if (lane == 0) {
+            const uint64_t pol = l2_evict_first_policy();
+            int st = 0;
+            uint32_t ph = 0;
+            bool waited = false;
+            for (int si = 0; si < sch.n_segs; ++si) {
+                int tile, g0, g1;
+                sch.seg(si, tile, g0, g1);
+                for (int gi = g0; gi < g1; ++gi) {
+                    mbar_wait_wd(&empty[st], ph ^ 1u, p.err, 0x100 + st);
+                    mbar_expect_tx(&full[st], (uint32_t)(C::kNibGroup + 4 * 80 + C::kXGroup));
+                    tma_load_4d_hint(smem + C::kNibOff + st * C::kNibGroup, &p.wmap, 0, 0, gi, tile * 4, &full[st], pol);
+                    tma_load_3d_hint(smem + C::kTrOff + st * C::kTrGroup, &p.tmap, 0, gi, tile * 4, &full[st], pol);
+                    if (!waited) {
+                        pdl_wait();
+                        waited = true;
                     }
-                }
-                __syncwarp();
-                if (++rs == C::RS) {
-                    rs = 0;
-                    ph ^= 1u;
+                    uint8_t* dst = smem + C::kXOff + st * C::kXGroup;
+                    tma_load_2d(dst, &p.xmap, gi * kW4GroupK, 0, &full[st]);
+                    tma_load_2d(dst + NTOK * 128, &p.xmap, gi * kW4GroupK + 64, 0, &full[st]);
+                    if (++st == C::ST) {
+                        st = 0;
+                        ph ^= 1u;
+                    }
                 }
             }
         }
-    } else if (warp == C::kWarpX) {
-        // ---------------- activations: produced by the predecessor kernel ----------------
-        pdl_wait();
-        int as = 0, st_i = 0;
-        uint32_t ph = 0;
-        for (int si = 0; si < sch.n_segs; ++si) {
-            int tile, g0, g1;
-            sch.seg(si, tile, g0, g1);
-            for (int gi = g0; gi < g1; gi += KG, ++st_i) {
-                const int ng = min(KG, g1 - gi);
-                mbar_wait_wd(&ax_empty[as], ph ^ 1u, p.err, 0x200 + as);
-                if (lane == 0) stamp(1, st_i, 1);
-                if (tc_elect_one()) {
-                    if (p.dbg & 1) {
-                        mbar_arrive(&a_full[as]);
-                    } else {
-                        mbar_expect_tx(&a_full[as], (uint32_t)ng * C::kXGroup);
+        return;
+    }
+
+    // ---------------- consumers ----------------
+    // warp w of warpgroup wr covers rows 64 wr + 16 (w % 4) .. + 15 of the tile = ZLW4I block b = 2 wr + (w % 4) / 2 of the
+    // tile, 16-row tile tt = w % 2 of that block; the thread holds rows g and g + 8 for k 2 tig, 2 tig + 1 (+ 8)
+    const int b = warp >> 1, tt = warp & 1, g = lane >> 2, tig = lane & 3;
+    const int m_lo = b * 32 + tt * 16 + g;                         // row in the tile; its partner is m_lo + 8
+    const uint32_t sw = (uint32_t)(g >> 1) & 3u;                   // the map's 64-byte swizzle: chunk ^= (row >> 1) & 3
+    const uint32_t sel = (tig & 1) ? 0x4342u : 0x4140u;            // bytes 2 tig % 4 and + 1 of a word
+    const int wsel = tig >> 1;                                     // word of k 2 tig (word wsel + 2: k 2 tig + 8)
+    pdl_wait();
+    int st = 0;
+    uint32_t ph = 0;
+    for (int si = 0; si < sch.n_segs; ++si) {
+        int tile, g0, g1;
+        sch.seg(si, tile, g0, g1);
+        float acc[NTOK / 2];
+        for (int gi = g0; gi < g1; ++gi) {
+            mbar_wait_wd(&full[st], ph, p.err, 0x400 + st);
+            const uint8_t* nib = smem + C::kNibOff + st * C::kNibGroup + b * 2048;
+            const uint8_t* tr = smem + C::kTrOff + st * C::kTrGroup + b * 80;
+            const __half2 sc2 = *reinterpret_cast<const __half2*>(tr + (tt * 8 + g) * 4);
+            const int zz = tr[64 + tt * 8 + g];
+            const __half2 cz_lo = __float2half2_rn((float)(1024 + (zz & 0xF))), cz_hi = __float2half2_rn((float)(64 + (zz >> 4)));
+            const __half2 s_lo = __half2half2(__low2half(sc2)), s_hi = __half2half2(__high2half(sc2));
+            uint32_t a[8][4];
 #pragma unroll
-                        for (int j = 0; j < KG; ++j)
-                            if (j < ng) {
-                                uint8_t* dst = smem + C::kXOff + (as * KG + j) * C::kXGroup;
-                                tma_load_2d(dst, &p.xmap, (gi + j) * kW4GroupK, 0, &a_full[as]);
-                                tma_load_2d(dst + NTOK * 128, &p.xmap, (gi + j) * kW4GroupK + 64, 0, &a_full[as]);
-                            }
-                    }
-                }
-                __syncwarp();
-                if (++as == C::AS) {
-                    as = 0;
-                    ph ^= 1u;
-                }
+            for (int s = 0; s < 8; ++s) {
+                // 16-k step s = 2 t + hh of the group: record row (2 tt + hh) * 8 + g, 16-byte chunk t
+                const int t = s >> 1, hh = s & 1;
+                const uint4 wv = *reinterpret_cast<const uint4*>(nib + ((tt * 2 + hh) * 8 + g) * 64 + (((uint32_t)t ^ sw) << 4));
+                const uint32_t w0 = wsel ? wv.y : wv.x, w1 = wsel ? wv.w : wv.z;
+                a[s][0] = tc_dq2(w0 & 0x0f0f0f0fu, 0x64646464u, sel, cz_lo, s_lo);   // row g,     k 2 tig, 2 tig + 1
+                a[s][1] = tc_dq2(w0 & 0xf0f0f0f0u, 0x54545454u, sel, cz_hi, s_hi);   // row g + 8
+                a[s][2] = tc_dq2(w1 & 0x0f0f0f0fu, 0x64646464u, sel, cz_lo, s_lo);   // row g,     k 2 tig + 8, + 9
+                a[s][3] = tc_dq2(w1 & 0xf0f0f0f0u, 0x54545454u, sel, cz_hi, s_hi);   // row g + 8
             }
-        }
-    } else if (warp == C::kWarpMma) {
-        // ---------------- MMA issue: the warp stays converged (uniform operands), one elected lane issues ----------------
-        constexpr uint32_t idesc = tc_idesc_f16(NTOK);
-        int as = 0, acc = 0, st_i = 0;
-        uint32_t ph = 0, acc_ph = 0;
-        for (int si = 0; si < sch.n_segs; ++si) {
-            int tile, g0, g1;
-            sch.seg(si, tile, g0, g1);
-            mbar_wait_wd(&acc_empty[acc], acc_ph ^ 1u, p.err, 0x300 + acc);
-            tc_fence_after();
-            const uint32_t d_tmem = tmem_base + (uint32_t)(acc * NTOK);
-            for (int gi = g0; gi < g1; gi += KG, ++st_i) {
-                const int ng = min(KG, g1 - gi);
-                if (lane == 0) stamp(2, st_i, 0);
-                mbar_wait_wd(&a_full[as], ph, p.err, 0x400 + as);   // dequant arrivals + the x tiles' bytes
-                if (lane == 0) stamp(2, st_i, 1);
-                tc_fence_after();
-                if (tc_elect_one()) {
+            const uint64_t xd0 = wg_desc_sw128(smem_u32(smem + C::kXOff + st * C::kXGroup));
+            wg_fence();
 #pragma unroll
-                    for (int j = 0; j < KG; ++j) {
-                        if (j < ng && (!(p.dbg & 4) || gi + j == g0)) {
-                            const uint32_t a_col = tmem_base + (uint32_t)(C::kACol0 + (as * KG + j) * 64);
-                            const uint64_t xd0 = tc_desc_sw128(smem_u32(smem + C::kXOff + (as * KG + j) * C::kXGroup));
-#pragma unroll
-                            for (int jj = 0; jj < 8; ++jj)   // 16 k = 8 TMEM columns of A; x: 64-k atom jj / 4, 32 bytes per step
-                                tc_mma_f16_ts(d_tmem, a_col + (uint32_t)(jj * 8),
-                                              xd0 + (uint64_t)((jj >> 2) * ((NTOK * 128) >> 4) + (jj & 3) * 2), idesc,
-                                              (gi + j > g0 || jj > 0) ? 1u : 0u);
-                        }
-                    }
-                    tc_commit(&ax_empty[as]);   // frees the A columns and the x tiles once the MMAs above have read them
-                    if (gi + KG >= g1) tc_commit(&acc_full[acc]);
-                }
-                if (lane == 0) stamp(2, st_i, 3);
-                if (++as == C::AS) {
-                    as = 0;
-                    ph ^= 1u;
-                }
-            }
-            if (++acc == C::NACC) {
-                acc = 0;
-                acc_ph ^= 1u;
-            }
-        }
-    } else if (warp >= C::kWarpDq0) {
-        // ---------------- dequant: the lane owns packed row 32 q + lane of the tile, k-slice ks of each group; the two warp
-        // groups take the stages alternately, so that while one sits in its barrier / TMEM-store round trip the other converts
-        const int dw = warp - C::kWarpDq0;
-        const int grp = dw / C::GW, q = warp & 3, ks = (dw % C::GW) >> 2;
-        const int tt = lane >> 4, hi = (lane >> 3) & 1, g = lane & 7;
-        constexpr int KW = kW4GroupK / C::KQ;            // k per warp and group: 64
-        constexpr int NCH = KW / 16;                     // 16-k chunks (one uint4 each) per lane and group
-        const uint32_t mask = hi ? 0xf0f0f0f0u : 0x0f0f0f0fu;
-        const uint32_t magic = hi ? 0x54545454u : 0x64646464u;   // 64 + n / 16 for a high nibble n, 1024 + n for a low one
-        const uint32_t sw = (uint32_t)(g >> 1) & 3u;     // the map's 64-byte swizzle: chunk ^= (row >> 1) & 3, row % 8 = g
-        const uint32_t lane_taddr = tmem_base + ((uint32_t)(q * 32) << 16) + (uint32_t)(C::kACol0 + ks * (KW / 2));
-        const int trole = 3 + (dw % C::GW);              // trace roles 3..10: the warps of group 0
-        int st_i = 0;
-        for (int si = 0; si < sch.n_segs; ++si) {
-            int tile, g0, g1;
-            sch.seg(si, tile, g0, g1);
-            for (int gi = g0; gi < g1; gi += KG, ++st_i) {
-                if (st_i % NG != grp) continue;
-                const int ng = min(KG, g1 - gi);
-                const int rs = st_i % C::RS, as = st_i % C::AS;
-                const uint32_t rph = (uint32_t)(st_i / C::RS) & 1u, aph = (uint32_t)(st_i / C::AS) & 1u;
-                if (lane == 0) {
-                    if (grp == 0) stamp(trole, st_i, 0);
-                    mbar_wait_wd(&raw_full[rs], rph, p.err, 0x600 + rs);
-                    if (grp == 0) stamp(trole, st_i, 1);
-                }
-                __syncwarp();
-#pragma unroll
-                for (int j = 0; j < KG; ++j) {
-                    if (j < ng) {
-                        const uint8_t* nib = smem + C::kNibOff + (rs * KG + j) * C::kNibGroup + q * 2048;
-                        const uint8_t* tr = smem + C::kTrOff + (rs * KG + j) * C::kTrGroup + q * 80;
-                        uint4 wv[NCH];
-#pragma unroll
-                        for (int c = 0; c < NCH; ++c) {
-                            // 16-k chunk kc of the group: k = 32 t + 16 hh + ..., record row (2 tt + hh) * 8 + g, chunk t
-                            const int kc = ks * NCH + c, t = kc >> 1, hh = kc & 1;
-                            wv[c] = *reinterpret_cast<const uint4*>(nib + ((tt * 2 + hh) * 8 + g) * 64 + (((uint32_t)t ^ sw) << 4));
-                        }
-                        const __half2 sc2 = *reinterpret_cast<const __half2*>(tr + (tt * 8 + g) * 4);
-                        const int zz = tr[64 + tt * 8 + g];
-                        if (j == ng - 1) {
-                            __syncwarp();               // every lane's shared-memory reads of the stage have returned
-                            if (lane == 0) mbar_arrive(&raw_empty[rs]);
-                        }
-                        const __half2 cz = __float2half2_rn(hi ? (float)(64 + (zz >> 4)) : (float)(1024 + (zz & 0xF)));
-                        const __half2 s2 = hi ? __half2half2(__high2half(sc2)) : __half2half2(__low2half(sc2));
-                        if (j == 0) {
-                            if (lane == 0) {
-                                mbar_wait_wd(&ax_empty[as], aph ^ 1u, p.err, 0x700 + as);
-                                if (grp == 0) stamp(trole, st_i, 2);
-                            }
-                            __syncwarp();
-                            tc_fence_after();
-                        }
-                        if (!(p.dbg & 2)) {
-#pragma unroll
-                            for (int c2 = 0; c2 < NCH; c2 += 2) {   // 32 k = 16 columns per tcgen05.st
-                                uint32_t r[16];
-#pragma unroll
-                                for (int c = 0; c < 2; ++c) {
-                                    const uint32_t words[4] = {wv[c2 + c].x, wv[c2 + c].y, wv[c2 + c].z, wv[c2 + c].w};
-#pragma unroll
-                                    for (int wq = 0; wq < 4; ++wq) {
-                                        const uint32_t wm = words[wq] & mask;
-                                        uint32_t a0 = __byte_perm(wm, magic, 0x4140), a1 = __byte_perm(wm, magic, 0x4342);
-                                        __half2 v0 = __hmul2(__hsub2(*reinterpret_cast<__half2*>(&a0), cz), s2);
-                                        __half2 v1 = __hmul2(__hsub2(*reinterpret_cast<__half2*>(&a1), cz), s2);
-                                        r[c * 8 + wq * 2] = *reinterpret_cast<uint32_t*>(&v0);
-                                        r[c * 8 + wq * 2 + 1] = *reinterpret_cast<uint32_t*>(&v1);
-                                    }
-                                }
-                                tc_st16(lane_taddr + (uint32_t)((as * KG + j) * 64 + c2 * 8), r);
-                            }
-                        }
-                    }
-                }
-                tc_wait_st();
-                tc_fence_before();
-                __syncwarp();                       // one arrival per warp
-                if (lane == 0) {
-                    mbar_arrive(&a_full[as]);
-                    if (grp == 0) stamp(trole, st_i, 3);
-                }
-            }
-        }
-    } else {
-        // ---------------- epilogue: TMEM -> registers -> global ----------------
-        const int q = warp;                      // TMEM lane quadrant this warp may read
-        const int m = q * 32 + lane;             // row inside the tile
-        pdl_wait();
-        int acc = 0;
-        uint32_t acc_ph = 0;
-        for (int si = 0; si < sch.n_segs; ++si) {
-            int tile, g0, g1;
-            sch.seg(si, tile, g0, g1);
-            const bool whole = g0 == 0 && g1 == G;
-            const int prow = tile * kTcRows + m;
-            if (lane == 0) mbar_wait_wd(&acc_full[acc], acc_ph, p.err, 0x800 + acc);
+            for (int s = 0; s < 8; ++s)   // x: 64-k atom s / 4, 32 bytes per 16-k step
+                wg_f16_rs<NTOK>(acc, a[s], xd0 + (uint64_t)((s >> 2) * ((NTOK * 128) >> 4) + (s & 3) * 2),
+                                (gi > g0 || s > 0) ? 1u : 0u);
+            wg_commit();
+            wg_wait_all();
             __syncwarp();
-            tc_fence_after();
-            const uint32_t taddr = tmem_base + ((uint32_t)(q * 32) << 16) + (uint32_t)(acc * NTOK);
-            uint2* wsp = whole ? nullptr : p.ws + ((size_t)sch.slot((int)blockIdx.x, tile) * p.M) * kTcRows + m;
-            // residual rows are one L2 round trip per 16-token chunk away: fetch the next chunk's while this one is processed
-            const bool pre = whole && p.epi == ZL_EPI_RESIDUAL;
-            uint32_t rnext[8];
-            auto fetch_res = [&](int c0) {
-#pragma unroll
-                for (int i = 0; i < 8; ++i) {
-                    const uint32_t lo = (c0 + 2 * i < p.M) ? __half_as_ushort(p.residual[(size_t)(c0 + 2 * i) * p.N + prow]) : 0u;
-                    const uint32_t hi = (c0 + 2 * i + 1 < p.M) ? __half_as_ushort(p.residual[(size_t)(c0 + 2 * i + 1) * p.N + prow]) : 0u;
-                    rnext[i] = lo | (hi << 16);
-                }
-            };
-            if (pre) fetch_res(0);
-#pragma unroll 1
-            for (int c0 = 0; c0 < NTOK; c0 += 16) {
-                if (c0 >= p.M) break;
-                float v[16];
-                tc_ld16(taddr + (uint32_t)c0, v);
-                if (!whole) {
-                    // a piece of a shared tile: tagged words, valid on arrival (no fence, no counter)
-#pragma unroll
-                    for (int i = 0; i < 16; ++i)
-                        if (c0 + i < p.M) tc_st_tag(wsp + (size_t)(c0 + i) * kTcRows, __float_as_uint(v[i]), 1u);
-                } else if (pre) {
-                    uint32_t rcur[8];
-#pragma unroll
-                    for (int i = 0; i < 8; ++i) rcur[i] = rnext[i];
-                    if (c0 + 16 < NTOK && c0 + 16 < p.M) fetch_res(c0 + 16);
-                    tc_epilogue16(p, prow, lane, c0, v, rcur);
-                } else {
-                    tc_epilogue16(p, prow, lane, c0, v);
-                }
-            }
-            tc_fence_before();
-            __syncwarp();                           // one arrival per epilogue warp
-            if (lane == 0) mbar_arrive(&acc_empty[acc]);
-            if (++acc == C::NACC) {
-                acc = 0;
-                acc_ph ^= 1u;
+            if (lane == 0) mbar_arrive(&empty[st]);
+            if (++st == C::ST) {
+                st = 0;
+                ph ^= 1u;
             }
         }
-        // ---- shared tiles: the owners of a tile's pieces split its 16-token chunks among themselves (chunk c goes to piece
-        // c mod nparts); each adds the pieces of its chunks in k order (deterministic), polling the tagged words, zeroes them for
-        // the next launch and runs the epilogue.  A CTA gets here only after it has written ALL its own pieces, so nobody ever
-        // waits for somebody who waits. ----
-        for (int si = 0; si < sch.n_segs && si < 2; ++si) {
-            int tile, g0, g1;
-            sch.seg(si, tile, g0, g1);
-            if (g0 == 0 && g1 == G) continue;
-            const int prow = tile * kTcRows + m;
-            const int c_first = sch.owner((long long)tile * G), c_last = sch.owner((long long)(tile + 1) * G - 1);
-            const int nparts = c_last - c_first + 1, part = (int)blockIdx.x - c_first;
-#pragma unroll 1
-            for (int c0 = part * 16; c0 < p.M; c0 += nparts * 16) {
-                float v[16];
+        if (g0 == 0 && g1 == G) {
 #pragma unroll
-                for (int i = 0; i < 16; ++i) v[i] = 0.f;
+            for (int j = 0; j < NTOK / 8; ++j)
+#pragma unroll
+                for (int e = 0; e < 2; ++e)
+                    tc_epilogue_pair(p, tile * 4 + b, tt, g, 8 * j + 2 * tig + e, acc[4 * j + e], acc[4 * j + 2 + e]);
+        } else {
+            // a piece of a shared tile: tagged words, valid on arrival (no fence, no counter)
+            uint2* wsp = p.ws + (size_t)sch.slot((int)blockIdx.x, tile) * p.M * kTcRows;
+#pragma unroll
+            for (int j = 0; j < NTOK / 8; ++j)
+#pragma unroll
+                for (int e = 0; e < 4; ++e) {
+                    const int tok = 8 * j + 2 * tig + (e & 1);
+                    if (tok < p.M) tc_st_tag(wsp + (size_t)tok * kTcRows + m_lo + (e >> 1) * 8, __float_as_uint(acc[4 * j + e]), 1u);
+                }
+        }
+    }
+    // ---- shared tiles: the owners of a tile's pieces split its 16-token chunks among themselves (chunk c goes to piece
+    // c mod nparts); each adds the pieces of its chunks in k order (deterministic), polling the tagged words, zeroes them for
+    // the next launch and runs the epilogue.  A CTA gets here only after it has written ALL its own pieces, so nobody ever
+    // waits for somebody who waits. ----
+    const int ct = threadIdx.x;                                  // 0 .. 255: (token of the chunk, row pair) items
+    for (int si = 0; si < sch.n_segs && si < 2; ++si) {
+        int tile, g0, g1;
+        sch.seg(si, tile, g0, g1);
+        if (g0 == 0 && g1 == G) continue;
+        const int c_first = sch.owner((long long)tile * G), c_last = sch.owner((long long)(tile + 1) * G - 1);
+        const int nparts = c_last - c_first + 1, part = (int)blockIdx.x - c_first;
+#pragma unroll 1
+        for (int c0 = part * 16; c0 < p.M; c0 += nparts * 16) {
+#pragma unroll 1
+            for (int idx = ct; idx < 16 * 64; idx += 256) {
+                const int tok = c0 + (idx >> 6), pr = idx & 63;
+                if (tok >= p.M) continue;
+                const int rb = pr >> 4, rtt = (pr >> 3) & 1, rg = pr & 7;
+                const int m = rb * 32 + rtt * 16 + rg;
+                float v[2] = {0.f, 0.f};
 #pragma unroll 1
                 for (int pp = 0; pp < nparts; ++pp) {
-                    uint2* src = p.ws + ((size_t)sch.slot(c_first + pp, tile) * p.M + c0) * kTcRows + m;
-                    uint2 t[16];
-                    bool ok = true;
-#pragma unroll
-                    for (int i = 0; i < 16; ++i) {
-                        t[i] = (c0 + i < p.M) ? tc_ld_tag(src + (size_t)i * kTcRows) : make_uint2(0u, 1u);
-                        ok = ok && t[i].y == 1u;
-                    }
-                    if (!ok) {                       // not all there yet: poll (bounded: a lost piece must not hang the GPU)
+                    uint2* src = p.ws + ((size_t)sch.slot(c_first + pp, tile) * p.M + tok) * kTcRows + m;
+                    uint2 t[2] = {tc_ld_tag(src), tc_ld_tag(src + 8)};
+                    if (t[0].y != 1u || t[1].y != 1u) {   // not there yet: poll (bounded: a lost piece must not hang the GPU)
                         const long long t_start = clock64();
-                        do {
-                            ok = true;
-#pragma unroll
-                            for (int i = 0; i < 16; ++i) {
-                                if (t[i].y != 1u) t[i] = tc_ld_tag(src + (size_t)i * kTcRows);
-                                ok = ok && t[i].y == 1u;
-                            }
+                        while (t[0].y != 1u || t[1].y != 1u) {
+                            if (t[0].y != 1u) t[0] = tc_ld_tag(src);
+                            if (t[1].y != 1u) t[1] = tc_ld_tag(src + 8);
                             if (clock64() - t_start > 4000000000ll) {
                                 if (p.err) atomicExch(p.err, 0x900u + (unsigned)pp);
                                 __threadfence_system();
                                 __trap();
                             }
-                        } while (!ok);
+                        }
                     }
-#pragma unroll
-                    for (int i = 0; i < 16; ++i) {
-                        v[i] += __uint_as_float(t[i].x);
-                        if (c0 + i < p.M) tc_st_tag(src + (size_t)i * kTcRows, 0u, 0u);   // consumed: back to "empty"
-                    }
+                    v[0] += __uint_as_float(t[0].x);
+                    v[1] += __uint_as_float(t[1].x);
+                    tc_st_tag(src, 0u, 0u);              // consumed: back to "empty"
+                    tc_st_tag(src + 8, 0u, 0u);
                 }
-                tc_epilogue16(p, prow, lane, c0, v);
+                tc_epilogue_pair(p, tile * 4 + rb, rtt, rg, tok, v[0], v[1]);
             }
         }
-    }
-
-    tc_fence_before();
-    __syncthreads();
-    if (warp == C::kWarpMma) {
-        tc_fence_after();
-        asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "n"(512));
     }
 }
 
@@ -638,7 +395,7 @@ bool w4_tc_supports(int mc, int N, int K) {
     return mc >= 1 && mc <= 256 && N % kTcRows == 0 && K % kW4GroupK == 0 && N / kTcRows <= kTcMaxTiles;
 }
 
-// last watchdog code published by a tcgen05 kernel on this device (0 = none); debugging aid
+// last watchdog code published by a tensor-core kernel on this device (0 = none); debugging aid
 extern "C" unsigned zl_w4_tc_watchdog(void) {
     TcDeviceState* st = tc_state();
     unsigned v = 0;
@@ -646,18 +403,7 @@ extern "C" unsigned zl_w4_tc_watchdog(void) {
     return v;
 }
 
-// copies the ZL_TC_DBG & 16 stamps of the last launch ([11 roles][64 stages][4] clock64 values) to the host; debugging aid
-extern "C" int zl_w4_tc_read_trace(long long* out, int n) {
-    TcDeviceState* st = tc_state();
-    if (!st || !st->ws || n > (1 << 17)) return ZL_ERR_INVALID_ARG;
-    cudaDeviceSynchronize();
-    return cudaMemcpy(out, reinterpret_cast<uint8_t*>(st->ws) + st->ws_bytes - (1 << 20), (size_t)n * 8, cudaMemcpyDeviceToHost) ==
-                   cudaSuccess
-               ? ZL_OK
-               : ZL_ERR_CUDA;
-}
-
-// host view of the stream-k schedule of the tcgen05 kernel (the same TcSched the kernel uses), for tests: the pieces of CTA
+// host view of the stream-k schedule of the wgmma kernel (the same TcSched the kernel uses), for tests: the pieces of CTA
 // `cta` out of `ctas` for n_tiles x G units.  out[5 * i + 0..4] = tile, g0, g1, number of pieces of that tile, workspace slot
 // of this piece (-1 for a whole tile); returns the number of pieces (<= max_pieces) or a negative error code.
 extern "C" int zl_w4_tc_schedule(int n_tiles, int G, int ctas, int cta, int* out, int max_pieces) {
@@ -760,14 +506,8 @@ cudaError_t launch_w4_tc(const W4Params& p, bool pdl, cudaStream_t stream) {
     q.N = p.N;
     q.K = p.K;
     q.epi = p.epi;
-    {
-        static const int tc_dbg = getenv("ZL_TC_DBG") ? atoi(getenv("ZL_TC_DBG")) : 0;
-        q.dbg = tc_dbg;
-    }
     q.ws = st->ws_ll;
-    q.ws_f32 = st->ws;
     q.err = st->err;
-    q.trace = reinterpret_cast<long long*>(reinterpret_cast<uint8_t*>(st->ws) + st->ws_bytes - (1 << 20));   // last MB of the workspace
     q.cos = p.cos;
     q.sin = p.sin;
     q.q_out = p.q_out;

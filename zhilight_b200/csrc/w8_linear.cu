@@ -18,7 +18,7 @@
 #include <cstdlib>
 
 namespace zl {
-// tcgen05 W8A8 kernel (w8_tc.cu)
+// wgmma W8A8 kernel (w8_tc.cu)
 bool w8_tc_supports(int N, int K);
 template <typename T, bool FP8>
 cudaError_t launch_w8_tc(const uint8_t* xq, const float* sx, const uint8_t* w, const void* sw, int sw_mode, const T* bias, T* y,
@@ -330,7 +330,7 @@ static cudaError_t launch_w8_ks(const uint8_t* xq, const float* sx, const uint8_
                                 const T* bias, T* y, int mc, int N, int K, bool pdl, cudaStream_t st) {
     const int tiles = cdiv(N, 16);
     // enough warps to keep ~13 MB of loads in flight chip-wide: aim for >= 16 warps per SM
-    int dev = 0, sms = 148;
+    int dev = 0, sms = 132;
     cudaGetDevice(&dev);
     cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
     const int steps = K / 64;
@@ -442,12 +442,12 @@ extern "C" int zl_w8a8_gemm(const void* xq, const float* x_scale, const void* w,
     const uint8_t* xq8 = static_cast<const uint8_t*>(xq);
     const uint8_t* w8 = static_cast<const uint8_t*>(w);
     const int sw_f32 = kind == ZL_W8_FP8_ROWS ? 2 : (w_scale_dtype == ZL_F32 ? 1 : 0);
-    // measured on B200 (tools/w8_bench.py): with the reference's row-major (N, K) layout every 128-byte row segment of a TMA
-    // box comes from a different DRAM page, and the mma.sync kernel's 16-byte row-contiguous loads stream faster at decode
-    // sizes; the tcgen05 kernel takes over where the mma.sync kernel would re-stream the weights (M > 32: prefill chunks)
+    // with the reference's row-major (N, K) layout every 128-byte row segment of a TMA box comes from a different DRAM page,
+    // so at decode sizes the mma.sync kernel's 16-byte row-contiguous loads are used; the wgmma kernel takes over where the
+    // mma.sync kernel would re-stream the weights (M > 32: prefill chunks).  The crossover was not measured on H100.
     static const int tc_min_m = getenv("ZL_W8_TC_MIN_M") ? atoi(getenv("ZL_W8_TC_MIN_M")) : 33;
     if (M >= tc_min_m && w8_tc_supports(N, K)) {
-        // tcgen05 path (w8_tc.cu): both operands through the TMA engine, s32 / f32 accumulators in TMEM
+        // wgmma path (w8_tc.cu): both operands through the TMA engine, s32 / f32 register accumulators
         {
             static bool prepared[64] = {};
             int dev = 0;

@@ -1,25 +1,27 @@
-// W8A8 Linear on the 5th-generation tensor cores: tcgen05.mma kind::i8 (s8 x s8 -> s32, exact) and kind::f8f6f4
-// (e4m3 x e4m3 -> f32) with TMEM accumulators; BOTH operands arrive through the TMA engine (cp.async.bulk.tensor.2d,
-// SWIZZLE_128B) straight from the reference's parameter layout, so no CUDA-core instruction touches a weight byte.
+// W8A8 Linear on the Hopper tensor cores: wgmma.mma_async s8 x s8 -> s32 (exact) and e4m3 x e4m3 -> f32 with register
+// accumulators; BOTH operands arrive through the TMA engine (cp.async.bulk.tensor.2d, SWIZZLE_128B) straight from the
+// reference's parameter layout and are read by wgmma from shared memory, so no CUDA-core instruction touches a weight byte.
 //
 // Replaces Int8Linear::forward = quant_calc_scale + cuBLASLt s32 GEMM (M padded to 32) + quant_scale_back
 // (reference src/nn/linear/linear.cpp:560-636, src/nn/quant/int8/quant_kernel.cu:231-306) and Fp8Linear::forward's
 // cuBLASLt fp8 GEMM (linear.cpp:1660-1695) for every M (decode and prefill chunks); the mma.sync kernel k_w8a8_skinny
 // (w8_linear.cu) stays as the fallback for K % 128 != 0 and as the A/B baseline (ZL_W8_NO_TC=1).
 //
-// One CTA per SM, persistent over work items (128 weight rows x a k-slice); 6 warps:
-//   warp 0     producer : per 128-byte k-stage one weight box (128 rows x 128 B) + one activation box (NTOK x 128 B)
-//   warp 1     MMA      : one thread, 4 x tcgen05.mma 128 x NTOK x 32 per stage; tcgen05.commit frees the stage
-//   warps 2-5  epilogue : tcgen05.ld of their TMEM lane quadrant, scale-back (+bias), or split-k partials + last-CTA reduce
+// One CTA per SM, persistent over work items (128 weight rows x a k-slice); 9 warps:
+//   warps 0-7  consumers : two warpgroups, warpgroup r owns weight rows 64 r .. 64 r + 63 of the tile and all NTOK tokens:
+//                          4 x wgmma m64 x NTOK x 32 per stage, then scale-back (+bias), or split-k partials + last-CTA reduce
+//   warp 8     producer  : per 128-byte k-stage one weight box (128 rows x 128 B) + one activation box (NTOK x 128 B)
 // INT8 results are bit-identical to the reference's three-kernel path (s32 accumulation is exact in any order).
 #include "common.cuh"
 #include "tc_common.cuh"
 
 #include <cstdlib>
+#include <type_traits>
 
 namespace zl {
 
-constexpr int kW8TcThreads = 6 * 32;
+constexpr int kW8TcThreads = 9 * 32;
+constexpr int kW8WarpProducer = 8;
 
 template <int NTOK>
 struct W8TcCfg {
@@ -29,10 +31,10 @@ struct W8TcCfg {
     static constexpr int kAOff = 0;
     static constexpr int kXOff = ST * kAStage;
     static constexpr int kBarOff = kXOff + ST * kXStage;
-    static constexpr int kNumBars = 2 * ST + 4;      // full[ST], empty[ST], acc_full[2], acc_empty[2]
+    static constexpr int kNumBars = 2 * ST;          // full[ST], empty[ST]
     static constexpr int kMiscOff = kBarOff + kNumBars * 8;
     static constexpr int kBytes = kMiscOff + 16 + 1024;
-    static constexpr int kTmemCols = 2 * NTOK < 32 ? 32 : 2 * NTOK;
+    static_assert(kBytes <= 232448, "shared memory");
 };
 
 struct alignas(64) W8TcParams {
@@ -49,65 +51,36 @@ struct alignas(64) W8TcParams {
     unsigned* err;
 };
 
-__host__ __device__ constexpr uint32_t w8_idesc(bool fp8, int n) {
-    // kind::i8: D s32 (2), A / B signed 8 bit (1); kind::f8f6f4: D f32 (1), A / B e4m3 (0); both K-major
-    return (fp8 ? (1u << 4) : ((2u << 4) | (1u << 7) | (1u << 10))) | ((uint32_t)(n >> 3) << 17) | ((uint32_t)(kTcRows >> 4) << 24);
-}
-template <bool FP8>
-__device__ __forceinline__ void w8_mma(uint32_t d_tmem, uint64_t adesc, uint64_t bdesc, uint32_t idesc, uint32_t accum) {
-    if constexpr (FP8)
-        asm volatile(
-            "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %4, 0;\n\t"
-            "tcgen05.mma.cta_group::1.kind::f8f6f4 [%0], %1, %2, %3, p;\n\t}" ::"r"(d_tmem),
-            "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accum)
-            : "memory");
-    else
-        asm volatile(
-            "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %4, 0;\n\t"
-            "tcgen05.mma.cta_group::1.kind::i8 [%0], %1, %2, %3, p;\n\t}" ::"r"(d_tmem),
-            "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accum)
-            : "memory");
-}
-
+// one output element: acc is the s32 sum (int8) or the f32 sum (fp8)
 template <typename T, bool FP8>
-__device__ __forceinline__ void w8_epilogue16(const W8TcParams& p, int row, int c0, const float (&v)[16]) {
-    if (row >= p.N) return;
+__device__ __forceinline__ void w8_epilogue1(const W8TcParams& p, int row, int tok, float acc) {
+    if (row >= p.N || tok >= p.M) return;
     const T* bias = static_cast<const T*>(p.bias);
-    T* y = static_cast<T*>(p.y);
     float s_w;
     if (p.sw_mode == 0) s_w = to_f32<T>(static_cast<const T*>(p.sw)[row]);
     else if (p.sw_mode == 3) s_w = *static_cast<const float*>(p.sw);
     else s_w = static_cast<const float*>(p.sw)[row];
-    const float b = bias ? to_f32<T>(bias[row]) : 0.f;
-#pragma unroll
-    for (int i = 0; i < 16; ++i) {
-        const int tok = c0 + i;
-        if (tok >= p.M) continue;
-        float r;
-        if constexpr (FP8) {
-            r = v[i] * (p.sx[0] * s_w);                       // cuBLASLt fp8: D = (scaleA * scaleB) * acc (+ bias)
-            if (bias) r += b;
-        } else {
-            // quant_scale_back (quant_kernel.cu:231-246): T(float(acc) * sx[m] * sw[n]), then add_bias in T
-            r = __fmul_rn(__fmul_rn((float)__float_as_int(v[i]), p.sx[tok]), s_w);
-            if (bias) r = to_f32<T>(from_f32<T>(r)) + b;
-        }
-        y[(size_t)tok * p.N + row] = from_f32<T>(r);
+    float r;
+    if constexpr (FP8) {
+        r = acc * (p.sx[0] * s_w);                       // cuBLASLt fp8: D = (scaleA * scaleB) * acc (+ bias)
+        if (bias) r += to_f32<T>(bias[row]);
+    } else {
+        // quant_scale_back (quant_kernel.cu:231-246): T(float(acc) * sx[m] * sw[n]), then add_bias in T
+        r = __fmul_rn(__fmul_rn(acc, p.sx[tok]), s_w);
+        if (bias) r = to_f32<T>(from_f32<T>(r)) + to_f32<T>(bias[row]);
     }
+    static_cast<T*>(p.y)[(size_t)tok * p.N + row] = from_f32<T>(r);
 }
 
 template <typename T, bool FP8, int NTOK>
 __global__ void __launch_bounds__(kW8TcThreads, 1) k_w8a8_tc(const __grid_constant__ W8TcParams p) {
     using C = W8TcCfg<NTOK>;
+    using Acc = typename std::conditional<FP8, float, int>::type;
     extern __shared__ uint8_t smem_dyn[];
     uint8_t* smem = smem_dyn + ((1024u - (smem_u32(smem_dyn) & 1023u)) & 1023u);
-    uint64_t* bars = reinterpret_cast<uint64_t*>(smem + C::kBarOff);
-    uint64_t* full = bars;
+    uint64_t* full = reinterpret_cast<uint64_t*>(smem + C::kBarOff);
     uint64_t* empty = full + C::ST;
-    uint64_t* acc_full = empty + C::ST;
-    uint64_t* acc_empty = acc_full + 2;
-    uint32_t* s_tmem = reinterpret_cast<uint32_t*>(smem + C::kMiscOff);
-    uint32_t* s_last = s_tmem + 1;
+    uint32_t* s_last = reinterpret_cast<uint32_t*>(smem + C::kMiscOff);
 
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     const int KS = p.K / 128;                      // 128-byte k-stages
@@ -117,26 +90,14 @@ __global__ void __launch_bounds__(kW8TcThreads, 1) k_w8a8_tc(const __grid_consta
     if (threadIdx.x == 0) {
         for (int i = 0; i < C::ST; ++i) {
             mbar_init(&full[i], 1);
-            mbar_init(&empty[i], 1);
-        }
-        for (int i = 0; i < 2; ++i) {
-            mbar_init(&acc_full[i], 1);
-            mbar_init(&acc_empty[i], 4);
+            mbar_init(&empty[i], 8);             // one arrival per consumer warp
         }
         mbar_fence_init();
     }
-    if (warp == 1) {
-        asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(s_tmem)),
-                     "n"(C::kTmemCols));
-        asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;");
-    }
     pdl_trigger();
-    tc_fence_before();
     __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem_base = *s_tmem;
 
-    if (warp == 0) {
+    if (warp == kW8WarpProducer) {
         if (lane == 0) {
             int st = 0;
             uint32_t ph = 0;
@@ -161,117 +122,97 @@ __global__ void __launch_bounds__(kW8TcThreads, 1) k_w8a8_tc(const __grid_consta
                 }
             }
         }
-    } else if (warp == 1) {
-        if (lane == 0) {
-            constexpr uint32_t idesc = w8_idesc(FP8, NTOK);
-            int st = 0, acc = 0;
-            uint32_t ph = 0, acc_ph = 0;
-            for (int it = blockIdx.x; it < n_items; it += gridDim.x) {
-                const int split = it % S;
-                const int s0 = (split * KS) / S, s1 = ((split + 1) * KS) / S;
-                mbar_wait_wd(&acc_empty[acc], acc_ph ^ 1u, p.err, 0x1300 + acc);
-                tc_fence_after();
-                const uint32_t d_tmem = tmem_base + (uint32_t)(acc * NTOK);
-                for (int ks = s0; ks < s1; ++ks) {
-                    mbar_wait_wd(&full[st], ph, p.err, 0x1400 + st);
-                    tc_fence_after();
-                    const uint64_t ad = tc_desc_sw128(smem_u32(smem + C::kAOff + st * C::kAStage));
-                    const uint64_t xd = tc_desc_sw128(smem_u32(smem + C::kXOff + st * C::kXStage));
-#pragma unroll
-                    for (int k32 = 0; k32 < 4; ++k32)   // 32 bytes along K per MMA inside the 128-byte swizzle atom
-                        w8_mma<FP8>(d_tmem, ad + (uint64_t)(k32 * 2), xd + (uint64_t)(k32 * 2), idesc, (ks > s0 || k32 > 0) ? 1u : 0u);
-                    tc_commit(&empty[st]);
-                    if (++st == C::ST) {
-                        st = 0;
-                        ph ^= 1u;
-                    }
-                }
-                tc_commit(&acc_full[acc]);
-                if (++acc == 2) {
-                    acc = 0;
-                    acc_ph ^= 1u;
-                }
-            }
-        }
-    } else {
-        const int q = warp & 3;
-        const int m = q * 32 + lane;
-        const int et = (warp - 2) * 32 + lane;
-        pdl_wait();
-        int acc = 0;
-        uint32_t acc_ph = 0;
-        for (int it = blockIdx.x; it < n_items; it += gridDim.x) {
-            const int tile = it / S, split = it % S;
-            const int row = tile * kTcRows + m;
-            if (lane == 0) mbar_wait_wd(&acc_full[acc], acc_ph, p.err, 0x1800 + acc);
-            __syncwarp();
-            tc_fence_after();
-            const uint32_t taddr = tmem_base + ((uint32_t)(q * 32) << 16) + (uint32_t)(acc * NTOK);
-            float* wsp = (S > 1) ? p.ws + ((size_t)(tile * S + split) * p.M) * kTcRows + m : nullptr;
-#pragma unroll 1
-            for (int c0 = 0; c0 < NTOK; c0 += 16) {
-                if (c0 >= p.M) break;
-                float v[16];
-                tc_ld16(taddr + (uint32_t)c0, v);    // raw 32-bit lanes: s32 for kind::i8, f32 for kind::f8f6f4
-                if (S > 1) {
-#pragma unroll
-                    for (int i = 0; i < 16; ++i)
-                        if (c0 + i < p.M) __stcg(wsp + (size_t)(c0 + i) * kTcRows, v[i]);
-                } else {
-                    w8_epilogue16<T, FP8>(p, row, c0, v);
-                }
-            }
-            tc_fence_before();
-            __syncwarp();                           // one arrival per epilogue warp
-            if (lane == 0) mbar_arrive(&acc_empty[acc]);
-            if (++acc == 2) {
-                acc = 0;
-                acc_ph ^= 1u;
-            }
-            if (S > 1) {
-                __threadfence();
-                epi_bar();
-                if (et == 0) *s_last = (atomicAdd(&p.counters[tile], 1u) == (unsigned)(S - 1)) ? 1u : 0u;
-                epi_bar();
-                const bool last = *s_last != 0u;
-                epi_bar();
-                if (last) {
-                    __threadfence();
-                    const float* base = p.ws + ((size_t)tile * S * p.M) * kTcRows + m;
-#pragma unroll 1
-                    for (int c0 = 0; c0 < p.M; c0 += 16) {
-                        float v[16];
-                        if constexpr (FP8) {
-#pragma unroll
-                            for (int i = 0; i < 16; ++i) v[i] = 0.f;
-                            for (int s = 0; s < S; ++s)
-#pragma unroll
-                                for (int i = 0; i < 16; ++i)
-                                    if (c0 + i < p.M) v[i] += __ldcg(base + ((size_t)s * p.M + c0 + i) * kTcRows);
-                        } else {
-                            int a[16];
-#pragma unroll
-                            for (int i = 0; i < 16; ++i) a[i] = 0;
-                            for (int s = 0; s < S; ++s)
-#pragma unroll
-                                for (int i = 0; i < 16; ++i)
-                                    if (c0 + i < p.M) a[i] += __float_as_int(__ldcg(base + ((size_t)s * p.M + c0 + i) * kTcRows));
-#pragma unroll
-                            for (int i = 0; i < 16; ++i) v[i] = __int_as_float(a[i]);
-                        }
-                        w8_epilogue16<T, FP8>(p, row, c0, v);
-                    }
-                    if (et == 0) p.counters[tile] = 0u;
-                }
-            }
-        }
+        return;
     }
 
-    tc_fence_before();
-    __syncthreads();
-    if (warp == 1) {
-        tc_fence_after();
-        asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "n"(C::kTmemCols));
+    // ---------------- consumers: warpgroup wr, rows 64 wr + 16 (warp % 4) + g (+ 8) of the tile ----------------
+    const int wr = warp >> 2, g = lane >> 2, tig = lane & 3;
+    const int m0 = wr * 64 + (warp & 3) * 16 + g;   // rows m0 and m0 + 8; tokens 8 j + 2 tig + e
+    const int ct = threadIdx.x;                     // 0 .. 255
+    pdl_wait();
+    int st = 0;
+    uint32_t ph = 0;
+    for (int it = blockIdx.x; it < n_items; it += gridDim.x) {
+        const int tile = it / S, split = it % S;
+        const int s0 = (split * KS) / S, s1 = ((split + 1) * KS) / S;
+        Acc acc[NTOK / 2];
+        // fp8: wgmma accumulates e4m3 products with less than fp32 precision, so each 128-byte k-stage starts a fresh
+        // accumulator that is then added into an fp32 one (int8 sums are exact and accumulate in place)
+        float accf[FP8 ? NTOK / 2 : 1];
+        if constexpr (FP8) {
+#pragma unroll
+            for (int i = 0; i < NTOK / 2; ++i) accf[i] = 0.f;
+        }
+        for (int ks = s0; ks < s1; ++ks) {
+            mbar_wait_wd(&full[st], ph, p.err, 0x1400 + st);
+            const uint64_t ad = wg_desc_sw128(smem_u32(smem + C::kAOff + st * C::kAStage + wr * 64 * 128));
+            const uint64_t xd = wg_desc_sw128(smem_u32(smem + C::kXOff + st * C::kXStage));
+            wg_fence();
+#pragma unroll
+            for (int k32 = 0; k32 < 4; ++k32) {   // 32 bytes along K per wgmma inside the 128-byte swizzle atom
+                const uint32_t accum = ((!FP8 && ks > s0) || k32 > 0) ? 1u : 0u;
+                if constexpr (FP8) wg_e4m3_ss<NTOK>(acc, ad + (uint64_t)(k32 * 2), xd + (uint64_t)(k32 * 2), accum);
+                else wg_s8_ss<NTOK>(acc, ad + (uint64_t)(k32 * 2), xd + (uint64_t)(k32 * 2), accum);
+            }
+            wg_commit();
+            wg_wait_all();
+            if constexpr (FP8) {
+#pragma unroll
+                for (int i = 0; i < NTOK / 2; ++i) accf[i] += acc[i];
+            }
+            __syncwarp();
+            if (lane == 0) mbar_arrive(&empty[st]);
+            if (++st == C::ST) {
+                st = 0;
+                ph ^= 1u;
+            }
+        }
+        if (S == 1) {
+#pragma unroll
+            for (int j = 0; j < NTOK / 8; ++j)
+#pragma unroll
+                for (int e = 0; e < 4; ++e)
+                    w8_epilogue1<T, FP8>(p, tile * kTcRows + m0 + (e >> 1) * 8, 8 * j + 2 * tig + (e & 1),
+                                        FP8 ? (float)accf[FP8 ? 4 * j + e : 0] : (float)acc[4 * j + e]);
+            continue;
+        }
+        float* wsp = p.ws + ((size_t)(tile * S + split) * p.M) * kTcRows;
+#pragma unroll
+        for (int j = 0; j < NTOK / 8; ++j)
+#pragma unroll
+            for (int e = 0; e < 4; ++e) {
+                const int tok = 8 * j + 2 * tig + (e & 1);
+                float v;
+                if constexpr (FP8) v = accf[4 * j + e];
+                else v = __int_as_float(acc[4 * j + e]);
+                if (tok < p.M) __stcg(wsp + (size_t)tok * kTcRows + m0 + (e >> 1) * 8, v);
+            }
+        __threadfence();
+        consumer_bar();
+        if (ct == 0) *s_last = (atomicAdd(&p.counters[tile], 1u) == (unsigned)(S - 1)) ? 1u : 0u;
+        consumer_bar();
+        const bool last = *s_last != 0u;
+        consumer_bar();
+        if (last) {
+            // the last arriver adds the k-slices in split order (deterministic) and runs the epilogue
+            __threadfence();
+            const float* base = p.ws + ((size_t)tile * S * p.M) * kTcRows;
+#pragma unroll 1
+            for (int idx = ct; idx < p.M * kTcRows; idx += 256) {
+                const int tok = idx / kTcRows, m = idx % kTcRows;
+                float v;
+                if constexpr (FP8) {
+                    v = 0.f;
+                    for (int s = 0; s < S; ++s) v += __ldcg(base + (size_t)s * p.M * kTcRows + idx);
+                } else {
+                    int a = 0;
+                    for (int s = 0; s < S; ++s) a += __float_as_int(__ldcg(base + (size_t)s * p.M * kTcRows + idx));
+                    v = (float)a;
+                }
+                w8_epilogue1<T, FP8>(p, tile * kTcRows + m, tok, v);
+            }
+            if (ct == 0) p.counters[tile] = 0u;
+        }
     }
 }
 
@@ -303,12 +244,22 @@ static cudaError_t launch_w8_tc_t(const W8TcParams& q, dim3 grid, bool pdl, cuda
     return launch(k_w8a8_tc<T, FP8, NTOK>, grid, dim3(kW8TcThreads), (size_t)W8TcCfg<NTOK>::kBytes, stream, pdl, q);
 }
 
-// mc <= 256 rows of one pass.  zl_prepare() must have run on this device (split-k workspace, opt-in shared memory).
+// mc <= 256 rows of one pass (fp8: passes of <= 128 rows, its promoted accumulators take twice the registers).
+// zl_prepare() must have run on this device (split-k workspace, opt-in shared memory).
 template <typename T, bool FP8>
 cudaError_t launch_w8_tc(const uint8_t* xq, const float* sx, const uint8_t* w, const void* sw, int sw_mode, const T* bias, T* y,
                          int mc, int N, int K, bool pdl, cudaStream_t stream) {
     TcDeviceState* st = tc_state();
     if (!st || !st->ws) return cudaErrorNotSupported;
+    if (FP8 && mc > 128) {
+        for (int r0 = 0; r0 < mc; r0 += 128) {   // one scale for all tokens: only x and y move
+            const int rows = mc - r0 < 128 ? mc - r0 : 128;
+            const cudaError_t e = launch_w8_tc<T, FP8>(xq + (size_t)r0 * K, sx, w, sw, sw_mode, bias, y + (size_t)r0 * N, rows,
+                                                       N, K, pdl, stream);
+            if (e != cudaSuccess) return e;
+        }
+        return cudaSuccess;
+    }
     const int ntok = mc <= 32 ? 32 : mc <= 64 ? 64 : mc <= 128 ? 128 : 256;
     W8TcParams q;
     if (!tc_make_map_2d(&q.wmap, w, CU_TENSOR_MAP_DATA_TYPE_UINT8, 1, (uint64_t)N, (uint64_t)K, (uint64_t)K, kTcRows) ||
@@ -333,7 +284,9 @@ cudaError_t launch_w8_tc(const uint8_t* xq, const float* sx, const uint8_t* w, c
         case 32: return launch_w8_tc_t<T, FP8, 32>(q, grid, pdl, stream);
         case 64: return launch_w8_tc_t<T, FP8, 64>(q, grid, pdl, stream);
         case 128: return launch_w8_tc_t<T, FP8, 128>(q, grid, pdl, stream);
-        default: return launch_w8_tc_t<T, FP8, 256>(q, grid, pdl, stream);
+        default:
+            if constexpr (FP8) return cudaErrorInvalidValue;
+            else return launch_w8_tc_t<T, FP8, 256>(q, grid, pdl, stream);
     }
 }
 
@@ -353,8 +306,9 @@ cudaError_t prepare_w8_tc() {
     if ((e = cudaFuncSetAttribute(k_w8a8_tc<TT, F8, NT>, cudaFuncAttributeMaxDynamicSharedMemorySize,               \
                                   W8TcCfg<NT>::kBytes)) != cudaSuccess)                                            \
         return e;
-#define ZL_W8TC_ALL(TT, F8) ZL_W8TC_SET(TT, F8, 32) ZL_W8TC_SET(TT, F8, 64) ZL_W8TC_SET(TT, F8, 128) ZL_W8TC_SET(TT, F8, 256)
+#define ZL_W8TC_ALL(TT, F8) ZL_W8TC_SET(TT, F8, 32) ZL_W8TC_SET(TT, F8, 64) ZL_W8TC_SET(TT, F8, 128)
     ZL_W8TC_ALL(__half, false) ZL_W8TC_ALL(__half, true) ZL_W8TC_ALL(__nv_bfloat16, false) ZL_W8TC_ALL(__nv_bfloat16, true)
+    ZL_W8TC_SET(__half, false, 256) ZL_W8TC_SET(__nv_bfloat16, false, 256)
 #undef ZL_W8TC_ALL
 #undef ZL_W8TC_SET
     return cudaSuccess;

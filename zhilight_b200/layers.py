@@ -60,7 +60,7 @@ class Linear:
             g_idx = sd.get("g_idx")
             if g_idx is not None and not torch.equal(g_idx.cpu().int(),
                                                      (torch.arange(k) // self.group_size).int()):
-                raise _lib.ZLError(-3, "act-order (desc_act) checkpoints are not supported on the B200 path")
+                raise _lib.ZLError(-3, "act-order (desc_act) checkpoints are not supported on the H100 path")
             qw, qz, sc = ops.gptq_to_k_major(sd["qweight"].int(), sd["qzeros"].int(), sd["scales"].half(), is_awq)
             self._p = {"qweight": qw, "qzeros": qz, "scales": sc}
             variant = 1 if _lib.load().zl_w4_int_kernel_fits(32, n, k) else 0

@@ -154,6 +154,15 @@ int zl_w4_tc_set_splits(int splits);
  * for n_tiles x G (tile, group) units; out[5 i ..] = tile, g0, g1, pieces of that tile, workspace slot (-1: whole tile);
  * returns the number of pieces. */
 int zl_w4_tc_schedule(int n_tiles, int G, int ctas, int cta, int* out, int max_pieces);
+/* host view of the variant the exact-integer kernel runs for (M <= 16 rows, N, K, tp_mode) on sm_count SMs: out[0..8] = NT,
+ * warps per sub-CTA, sub-CTAs per CTA, ring stages, reduction rows, PACK, grid, dynamic shared memory bytes, sub-major tile
+ * order (sub-CTA s of CTA b starts at tile s * grid + b instead of b * sub-CTAs + s); returns 0, or
+ * ZL_ERR_UNSUPPORTED when none fits. */
+int zl_w4_v3_plan(int mc, int N, int K, int tp_mode, int sm_count, int* out);
+/* host view of the L2 head a predecessor GEMM prefetches for such a launch: the first H weight records each of its warps
+ * requests, as out[3 i ..] = warp, byte offset, bytes; returns the number of ranges (<= max_ranges) or
+ * a negative error code. */
+int zl_w4_v3_l2_head(int mc, int N, int K, int tp_mode, int sm_count, int H, long long* out, int max_ranges);
 /* debug: device buffer of grid*16 uint64 globaltimer samples written by the integer kernel (NULL = off). */
 int zl_w4_set_trace(void* buf);
 /* row_map (n_heads_total*dim_head) for zl_w4_pack so that RoPE partners (c, c+d/2) share an MMA tile. */

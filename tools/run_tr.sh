@@ -6,4 +6,4 @@ for l in sys.stdin:
     except Exception: print(l.strip()[:300]); continue
     print('$1', {k:round(d[k],4) if isinstance(d[k],float) else d[k] for k in ('value','ms_per_step','kernels_per_step')}, 'gemm us/launch', round(d['roofline']['us_per_launch'],2), 'frac', round(d['roofline']['frac'],3))
 "; }
-for mb in 0 8 16 24 40 64; do ZL_L2_PREFETCH_MB=$mb run "prefetch=$mb" ""; done
+for h in 0 1 2 4 5; do ZL_W4_L2_HEAD=$h run "l2_head=$h" ""; done

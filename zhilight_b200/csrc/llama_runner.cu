@@ -9,6 +9,7 @@
 #include "common.cuh"
 #include "w4_layout.cuh"
 #include "comm_dev.cuh"
+#include "w4_params.h"
 
 #include <cstdlib>
 #include <cstring>
@@ -619,51 +620,57 @@ int alloc_runtime(zl_llama* m) {
 // The decode-step kernel chain (captured into a graph by run_step).
 // cfg.fuse: 0 = one kernel per reference operator; 1 = RMSNorm folded into the following W4 GEMM;
 //           2 = additionally qkv split + RoPE + KV append folded into the qkv GEMM epilogue.
-// cap of the L2 prefetch a kernel issues for its successor (bytes); ZL_L2_PREFETCH_MB overrides, 0 disables
-static size_t prefetch_cap() {
+// L2 head of the successor GEMM (w4a16_gemm_v3.cu): as an exact-integer GEMM's weight stream drains, it can prefetch the
+// first ZL_W4_L2_HEAD ring items of every warp of the next W4 GEMM of the decode chain, or the whole successor when it is
+// at most ZL_W4_L2_WHOLE_MB.  Both default to 0 (off): on an H100 at 400 W every setting measured slower than none
+// (profiles/l2_head_ab.txt).  Read once per process, so graphs capture a fixed plan.
+static int l2_head_depth() {
+    static int v = -1;
+    if (v < 0) {
+        const char* e = getenv("ZL_W4_L2_HEAD");
+        v = e ? atoi(e) : 0;
+        if (v < 0) v = 0;
+    }
+    return v;
+}
+static size_t l2_whole_max() {
     static long v = -1;
     if (v < 0) {
-        const char* e = getenv("ZL_L2_PREFETCH_MB");
-        v = e ? atol(e) : 0;   // bulk L2 prefetch competes with the ring's TMA traffic; off by default
+        const char* e = getenv("ZL_W4_L2_WHOLE_MB");
+        v = e ? atol(e) : 0;
+        if (v < 0) v = 0;
     }
     return (size_t)v << 20;
 }
-// which blob each kernel of a layer prefetches (ZL_L2_PREFETCH_PLAN, 5 digits for qkv,attn(unused),o,gate_up,down ->
-// 0 none, 1 o, 2 gate_up, 3 down, 4 next qkv); experiment knob, only read when ZL_L2_PREFETCH_MB > 0
-static int prefetch_plan(int slot) {
-    static int plan[5] = {-1, 0, 0, 0, 0};
-    if (plan[0] < 0) {
-        const char* e = getenv("ZL_L2_PREFETCH_PLAN");
-        const char* d = (e && strlen(e) == 5) ? e : "10234";
-        for (int i = 0; i < 5; ++i) plan[i] = d[i] - '0';
-    }
-    return plan[slot];
+
+static bool w4_routes_v3(const W4Lin& w, int B) {
+    return w.packed_i && !getenv("ZL_W4_FORCE_HALF") && zl_w4_int_layout_route(B, w.N, w.K) == 3;
 }
 
-// resolve the plan entry of kernel `slot` (0 qkv, 1 attention, 2 o, 3 gate_up, 4 down) of layer l to a packed blob
-static void prefetch_target(zl_llama* m, int l, int slot, int B, const void** ptr, size_t* bytes) {
-    *ptr = nullptr;
-    *bytes = 0;
-    const auto& c = m->cfg;
-    if (!(c.quant_type == 5 || c.quant_type == 6) || prefetch_cap() == 0) return;
-    const int what = prefetch_plan(slot);
-    const W4Lin* t = nullptr;
+// the successor of GEMM `slot` (0 qkv, 2 o, 3 gate_up, 4 down) of layer l in the decode chain -- qkv -> o -> gate_up -> down
+// -> next layer's qkv -- and its tensor-parallel mode given this GEMM's (the fused exchange alternates push / reduce-in; the
+// last layer's down keeps the stand-alone all-reduce).  The lm_head boundary is left out.
+static const W4Lin* w4_successor(zl_llama* m, int l, int slot, int tp_mode, int* succ_tp) {
     Layer& L = m->layers[l];
-    if (what == 1) t = &L.q_o;
-    else if (what == 2) t = &L.q_gu;
-    else if (what == 3) t = &L.q_down;
-    else if (what == 4 && l + 1 < c.num_layers) t = &m->layers[l + 1].q_qkv;
-    if (!t) return;
-    const bool t_int = t->packed_i && !getenv("ZL_W4_FORCE_HALF") && zl_w4_int_layout_route(B, t->N, t->K) != 0;
-    *ptr = t_int ? t->packed_i : t->packed;
-    const size_t nb = zl_w4_packed_bytes(t->N, t->K, c.group_size);
-    *bytes = nb < prefetch_cap() ? nb : prefetch_cap();
+    const bool last = l + 1 >= m->cfg.num_layers;
+    *succ_tp = 0;
+    switch (slot) {
+        case 0: *succ_tp = tp_mode ? 2 : 0; return &L.q_o;
+        case 2: *succ_tp = tp_mode ? 1 : 0; return &L.q_gu;
+        case 3: *succ_tp = tp_mode && !last ? 2 : 0; return &L.q_down;
+        case 4: *succ_tp = tp_mode ? 1 : 0; return last ? nullptr : &m->layers[l + 1].q_qkv;
+        default: return nullptr;
+    }
 }
 
 // ZL_NO_PDL_MASK (experiments): launch these kernels with a full dependency instead of a programmatic one.
 // 1 qkv GEMM, 2 attention, 4 o GEMM, 8 gate_up GEMM, 16 down GEMM, 32 final norm, 64 lm_head, 128 argmax.
-// Default 70 = lm_head + o GEMM + attention: a PDL-launched lm_head measured 128 us slower per step than a normally
-// launched one (tools/gpu_tail.sh); early-launched o GEMM / attention CTAs cost another ~1 % each.
+// Single GPU, default 66 = lm_head + attention (a PDL-launched lm_head measured much slower, tools/gpu_tail.sh): on an
+// H100 80GB HBM3 at 400 W, Llama-3.1-8B batch-1 decode measured 425.8 tok/s (425.6-426.2 over 5 runs) against 413.2
+// (412.5-415.2) with the o GEMM also fully dependent (70), 420 with attention PDL-launched too (64), and 400-405 with
+// lm_head PDL-launched (2, 0)
+// (profiles/l2_head_ab.txt): an o GEMM launched early stages its ring fill while attention runs.
+// Tensor parallel (exchange inside the GEMMs): 68, a PDL-launched attention kernel measured faster there.
 static int no_pdl_mask(bool tensor_parallel = false) {
     static int v = -2;
     if (v == -2) {
@@ -671,9 +678,7 @@ static int no_pdl_mask(bool tensor_parallel = false) {
         v = e ? atoi(e) : -1;
     }
     if (v >= 0) return v;
-    // single GPU: lm_head, o GEMM, attention with full dependencies measured best (tools/gpu_pdlmask.sh: 640 -> 710 tok/s);
-    // tensor parallel (exchange inside the GEMMs): a PDL-launched attention kernel wins (N = 2: 783 vs 754 tok/s, r2s)
-    return tensor_parallel ? 68 : 70;
+    return tensor_parallel ? 68 : 66;
 }
 
 int w4_gemm(zl_llama* m, const void* x, int ldx, const W4Lin& w, const void* residual, void* y, int B, int epi,
@@ -696,10 +701,12 @@ int w4_gemm(zl_llama* m, const void* x, int ldx, const W4Lin& w, const void* res
         a.x = xn;
         ln_w = nullptr;
     }
-    if (layer >= 0) {
-        size_t nb = 0;
-        prefetch_target(m, layer, slot, B, &a.prefetch_ptr, &nb);
-        a.prefetch_bytes = nb;
+    W4L2Head l2;
+    if (layer >= 0 && route == 3 && (l2_head_depth() > 0 || l2_whole_max() > 0)) {
+        int succ_tp = 0;
+        const W4Lin* nx = w4_successor(m, layer, slot, tp_mode, &succ_tp);
+        if (nx && w4_routes_v3(*nx, B))
+            w4_v3_l2_head(nx->packed_i, B, nx->N, nx->K, succ_tp, device_sm_count(), l2_head_depth(), l2_whole_max(), &l2);
     }
     if (!a.packed) {
         zl_set_last_error(__FILE__, __LINE__, "no packed weight variant for this batch size");
@@ -739,7 +746,7 @@ int w4_gemm(zl_llama* m, const void* x, int ldx, const W4Lin& w, const void* res
         a.tp_h_out = tp_h_out;
         a.tp_index = tp_index;
     }
-    return zl_w4a16_gemm_fused(&a, m->stream);
+    return w4a16_gemm_fused_l2(&a, &l2, m->stream);
 }
 
 static int num_sms() { return device_sm_count(); }
@@ -944,12 +951,6 @@ int enqueue_step(zl_llama* m, int n_tasks, int len_bucket, const PrefillChunk* p
         if (!(w4 && c.fuse >= 2) && !(skip & 64))
             RCHECK(zl_qkv_rope_append(m->cosb, m->sinb, m->qkv, m->q, m->cur_tb, m->cur_pos, L.k_addrs, L.v_addrs, B,
                                       m->hq, m->hkv, d, 1, 1, m->d_lens, dt, pdl, st));
-        if (!(skip & 1)) {
-            const void* pfp = nullptr;
-            size_t pfb = 0;
-            prefetch_target(m, l, 1, B, &pfp, &pfb);
-            zl_decode_attention_set_prefetch(pfp, pfb);
-        }
         if (pf) {
             // one task, len_q = chunk, causal int8 mask (Attention::dynamic_batch_forward with len_q > 1, attention.cpp:846-964)
             RCHECK(zl_decode_attention(m->q, m->d_lens + pf->task, L.k_addrs + pf->task, L.v_addrs + pf->task, m->d_mask,

@@ -4,7 +4,19 @@
 #include <cuda_runtime.h>
 #include <stdint.h>
 
+#include "../../include/zhilight_b200.h"
+
 namespace zl {
+
+// L2 prefetch of the NEXT GEMM's first weight bytes, issued by a v3 kernel as its weight stream drains (a hint: results
+// never depend on it).  whole_bytes > 0: the whole range [base, base + whole_bytes).  Otherwise, h > 0: the first h ring
+// items of every warp of the successor's v3 launch (grid x subs x warps warps over an n_tiles x G blob of ZLW4I
+// records), in the order that warp's producer will request them -- see v3_head_ranges.
+struct W4L2Head {
+    const uint8_t* base = nullptr;
+    int n_tiles = 0, G = 0, grid = 0, subs = 0, warps = 0, h = 0, sub_major = 0;
+    unsigned long long whole_bytes = 0;
+};
 
 struct W4Params {
     const __half* x;
@@ -26,10 +38,10 @@ struct W4Params {
     __half* const* k_addrs;
     __half* const* v_addrs;
     int num_heads, num_kv_heads, dim_head;
-    // weights of the NEXT kernel in the chain: prefetched into L2 when this CTA runs out of work (may be null)
-    const uint8_t* pf_ptr;
-    unsigned long long pf_bytes;
+    // weights of the NEXT kernel in the chain: prefetched into L2 as this kernel's weight stream drains (v3 only)
+    W4L2Head l2;
     unsigned long long* trace;   // debug: per-CTA globaltimer samples [grid][16] (zl_w4_set_trace)
+    int sub_major = 0;   // v3 tile order: sub-CTA s of CTA b starts at tile s * grid + b (else b * SUBS + s)
     int dbg;   // ZL_W4_DEBUG: 1 = skip dequant/MMA (pure weight-stream probe; results are garbage)
     // tensor-parallel exchange inside the GEMM (integer kernel only; comm_dev.cuh).  tp_mode 1 (reduce-in): the
     // activation row is  T(T(sum over ranks of the partial sums pushed by the previous row-parallel GEMM) + x)  -- x is the
@@ -41,11 +53,23 @@ struct W4Params {
     __half* tp_h_out = nullptr;
 };
 
+// zl_w4a16_gemm_fused with the L2 head of the successor GEMM as a descriptor (l2 == nullptr: the public whole-range
+// prefetch_ptr / prefetch_bytes).  Only the exact-integer kernel issues it, at the tail of its weight stream.
+int w4a16_gemm_fused_l2(const zl_w4_fused_args_t* a, const W4L2Head* l2, zl_stream_t stream);
 cudaError_t launch_w4_v2(const W4Params& p, bool pdl, cudaStream_t stream);
 cudaError_t prepare_w4_v2();
 // exact-integer kernel on the ZLW4I layout; false = staged activations do not fit shared memory
 bool launch_w4_v3(const W4Params& p, bool pdl, cudaStream_t stream, cudaError_t* err);
 bool w4_v3_fits(int mc, int N, int K);
+// the variant launch_w4_v3 runs for (mc, N, K, tp_mode) on sm_count SMs; false = none fits
+struct V3Plan {
+    int nt, warps, subs, stages, rt, pack, grid, smem, sub_major;
+};
+bool w4_v3_plan(int mc, int N, int K, int tp_mode, int sm_count, V3Plan* plan);
+// descriptor of the L2 head of a successor v3 launch with weights `packed`: its first h ring items per warp, or the
+// whole blob when it is at most whole_max bytes; false = the successor does not run the v3 kernel
+bool w4_v3_l2_head(const void* packed, int mc, int N, int K, int tp_mode, int sm_count, int h, size_t whole_max,
+                   W4L2Head* out);
 cudaError_t prepare_w4_v3();
 // wgmma / TMA kernel on the ZLW4I layout (w4a16_tc.cu): up to 256 tokens per launch, N % 128 == 0, no fused
 // RMSNorm prologue (ln_w is ignored)

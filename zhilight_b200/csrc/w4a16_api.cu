@@ -88,6 +88,10 @@ extern "C" int zl_gather_rows_16(const void* src, const int32_t* map, void* dst,
 }
 
 extern "C" int zl_w4a16_gemm_fused(const zl_w4_fused_args_t* a, zl_stream_t stream) {
+    return zl::w4a16_gemm_fused_l2(a, nullptr, stream);
+}
+
+int zl::w4a16_gemm_fused_l2(const zl_w4_fused_args_t* a, const W4L2Head* l2, zl_stream_t stream) {
     {
         static bool prepared[64] = {};
         int dev = 0;
@@ -108,6 +112,7 @@ extern "C" int zl_w4a16_gemm_fused(const zl_w4_fused_args_t* a, zl_stream_t stre
     ZL_CHECK_ARG(a->epilogue != ZL_EPI_RESIDUAL || a->residual != nullptr);
     ZL_CHECK_ARG(a->epilogue == ZL_EPI_QKV_ROPE || a->y != nullptr || a->tp_mode == 2);
     ZL_CHECK_ARG(a->ln_weight == nullptr || (reinterpret_cast<uintptr_t>(a->ln_weight) & 15) == 0);
+    ZL_CHECK_ARG((reinterpret_cast<uintptr_t>(a->prefetch_ptr) & 15) == 0);
     if (a->epilogue == ZL_EPI_QKV_ROPE) {
         ZL_CHECK_ARG(a->cos && a->sin && a->q_out && a->token_batch && a->placement && a->k_addrs && a->v_addrs);
         ZL_CHECK_ARG(a->num_heads > 0 && a->num_kv_heads > 0 && a->dim_head > 0);
@@ -177,8 +182,12 @@ extern "C" int zl_w4a16_gemm_fused(const zl_w4_fused_args_t* a, zl_stream_t stre
         p.tp_mode = a->tp_mode;
         p.tp_index = a->tp_index;
         p.tp_h_out = static_cast<__half*>(a->tp_h_out);
-        p.pf_ptr = static_cast<const uint8_t*>(a->prefetch_ptr);
-        p.pf_bytes = a->prefetch_bytes;
+        if (l2) {
+            p.l2 = *l2;
+        } else if (a->prefetch_ptr && a->prefetch_bytes) {
+            p.l2.base = static_cast<const uint8_t*>(a->prefetch_ptr);
+            p.l2.whole_bytes = a->prefetch_bytes;
+        }
         if (route == 4) {
             ZL_CHECK_CUDA(launch_w4_tc(p, a->pdl != 0 && m0 == 0, stream));
         } else if (route == 3) {

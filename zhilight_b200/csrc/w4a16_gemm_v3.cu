@@ -44,6 +44,10 @@ __device__ __forceinline__ void imma_u8u8(int (&d)[4], const uint32_t (&a)[4], u
 //   tall : SUBS=1 x 16 warps, 4-stage rings (N/32 <= #SMs: o_proj, down) -- k split 16 ways
 // RT = token rows kept in the split-k reduction buffers (even, >= mc): small batches shrink them to make room for
 // deeper rings -- the tile loop is latency-bound on ring depth (4 -> 5 stages is worth ~25 %).
+__host__ __device__ constexpr int v3_smem_fixed(int NT, int WARPS, int SUBS, int STAGES, int RT) {
+    return (WARPS * SUBS * STAGES * (kW4BlockBytes + 8) + SUBS * ((NT == 1) ? 2 : 1) * WARPS * RT * 32 * 4 +
+            2 * WARPS * SUBS * NT * 8 * 4 + 2 * NT * 8 * 4 + 127) & ~127;
+}
 template <int NT, int WARPS, int SUBS, int STAGES, int RT = NT * 8>
 struct V3Smem {
     static constexpr int kWarpsTotal = WARPS * SUBS;
@@ -56,11 +60,40 @@ struct V3Smem {
     static constexpr int kRstdOff = kSsOff + 2 * kWarpsTotal * NT * 8 * 4;      // [NT*8] rstd | [NT*8] poison
     static constexpr int kXOff = (kRstdOff + 2 * NT * 8 * 4 + 127) & ~127;
     static constexpr int kBytes = kXOff;
+    static_assert(kBytes == v3_smem_fixed(NT, WARPS, SUBS, STAGES, RT), "w4_v3_plan sizes shared memory with v3_smem_fixed");
 };
 // staged activations (whole K): mc rows of hi bytes, mc rows of lo bytes, then the group table
 __host__ __device__ inline int v3_row_bytes(int K) { return K + 16; }   // +16: conflict-free LDS.128 across tokens
 __host__ __device__ inline int v3_stage_bytes(int mc, int K) {
     return 2 * mc * v3_row_bytes(K) + (K / kW4GroupK) * mc * 8;
+}
+
+// The first hd.h ring items of warp `sw` (CTA sw / (subs*warps), then sub-CTA, then warp) of a successor v3 launch, in the
+// order its producer requests them (issue_next below: groups g_begin..g_end-1 of tile0, then of tile0 + stride, ...), as
+// emit(byte offset, bytes) per contiguous range.  Host (zl_w4_v3_l2_head) and device share this code.
+template <class F>
+__host__ __device__ inline void v3_head_ranges(const W4L2Head& hd, int sw, F&& emit) {
+    const int per_cta = hd.subs * hd.warps;
+    const int r = sw % per_cta, sub = r / hd.warps, wl = r % hd.warps;
+    const int g_begin = (wl * hd.G) / hd.warps, ng = ((wl + 1) * hd.G) / hd.warps - g_begin;
+    const int cta = sw / per_cta;
+    int left = hd.h;
+    for (int tile = hd.sub_major ? sub * hd.grid + cta : cta * hd.subs + sub; left > 0 && ng > 0 && tile < hd.n_tiles; tile += hd.grid * hd.subs) {
+        const int k = left < ng ? left : ng;
+        emit(((size_t)tile * hd.G + g_begin) * kW4BlockBytes, (size_t)k * kW4BlockBytes);
+        left -= k;
+    }
+}
+
+// this (cta, warp)'s strided share (part of parts) of the successor's L2 head; call from lane 0
+__device__ __forceinline__ void v3_l2_prefetch(const W4L2Head& hd, int part, int parts) {
+    if (hd.whole_bytes) {
+        l2_prefetch_share(hd.base, (size_t)hd.whole_bytes, part, parts);
+        return;
+    }
+    const int n = hd.grid * hd.subs * hd.warps;
+    for (int sw = part; sw < n; sw += parts)
+        v3_head_ranges(hd, sw, [&](size_t off, size_t bytes) { l2_prefetch(hd.base + off, (uint32_t)bytes); });
 }
 
 __device__ __forceinline__ void sub_barrier(int id, int nthreads) {
@@ -164,7 +197,9 @@ __global__ void __launch_bounds__(WARPS * SUBS * 32, 1) k_w4a16_v3(const W4Param
     const int g_end = ((wl + 1) * G) / WARPS;
     const int ng = g_end - g_begin;
     const int n_tiles = p.N / 32;
-    const int tile0 = (int)blockIdx.x * SUBS + sub;
+    // sub_major: sub-CTA s of CTA b starts at tile s * grid + b, so that with more tiles than sub-CTAs the extra ones land
+    // on different SMs instead of on both sub-CTAs of the first CTAs
+    const int tile0 = p.sub_major ? sub * (int)gridDim.x + (int)blockIdx.x : (int)blockIdx.x * SUBS + sub;
     const int tile_stride = (int)gridDim.x * SUBS;
     const int my_tiles = tile0 < n_tiles ? (n_tiles - tile0 + tile_stride - 1) / tile_stride : 0;
     const int total = my_tiles * ng;
@@ -214,6 +249,13 @@ __global__ void __launch_bounds__(WARPS * SUBS * 32, 1) k_w4a16_v3(const W4Param
     auto stamp = [&]() {
         if (tr && threadIdx.x == 0 && tr_n < 16) tr[tr_n++] = globaltimer_ns();
     };
+    // L2 head of the successor GEMM: once this warp's producer has requested its last weight block, its share of the
+    // successor's first ring items goes to L2, so that HBM streams them while this GEMM drains (last IMMAs, split-k
+    // reduction, epilogue, CTA exit, the successor's launch) and the successor's ring fill hits L2.  The ring loads are
+    // evict-first, so this GEMM's own stream does not push the head back out.  dbg & 4: issue it after the warp's last
+    // block has landed instead.
+    const bool pf_tail = p.l2.base != nullptr && !(p.dbg & 4);
+    auto l2_head = [&]() { v3_l2_prefetch(p.l2, (int)blockIdx.x * WT + warp, (int)gridDim.x * WT); };
     stamp();
     pdl_trigger();
     if (lane == 0) {
@@ -223,13 +265,8 @@ __global__ void __launch_bounds__(WARPS * SUBS * 32, 1) k_w4a16_v3(const W4Param
 #pragma unroll
         for (int s = 0; s < STAGES; ++s)
             if (s < total) issue_next();
-        // software-managed L2: start pulling the weights of a LATER kernel of the chain into the 126 MB L2 now, so
-        // that HBM keeps streaming while this kernel and its neighbours sit in their latency-bound phases
-        if (p.pf_ptr && !(p.dbg & 4))
-            l2_prefetch_share(p.pf_ptr, (size_t)p.pf_bytes, (int)blockIdx.x * WT + warp, (int)gridDim.x * WT);
+        if (pf_tail && p_issued == total) l2_head();
     }
-    if (p.pf_ptr && (p.dbg & 4))
-        l2_prefetch_lines(p.pf_ptr, (size_t)p.pf_bytes, (int)blockIdx.x * WT + warp, (int)gridDim.x * WT, lane);
     // staging assignment: group gi -> warp gi % WT.  RMSNorm weights are constants: fetch them before the wait.
     constexpr int kMaxNg = 8;   // groups per warp kept in registers during staging (K <= 8*WT*128)
     uint2 lnw[kMaxNg];
@@ -419,9 +456,10 @@ __global__ void __launch_bounds__(WARPS * SUBS * 32, 1) k_w4a16_v3(const W4Param
                 }
                 pack_blocks<2>(p, ring, bars, xs_hi, xs_lo, xs_tab, row_b, ss, pp, gg, g, t, lane, acc);
                 __syncwarp();
-                if (lane == 0) {
+                if (lane == 0 && p_issued < total) {
+                    issue_next();
                     if (p_issued < total) issue_next();
-                    if (p_issued < total) issue_next();
+                    if (pf_tail && p_issued == total) l2_head();
                 }
             }
         }
@@ -518,8 +556,12 @@ __global__ void __launch_bounds__(WARPS * SUBS * 32, 1) k_w4a16_v3(const W4Param
                 }
             }
             __syncwarp();
-            if (lane == 0 && p_issued < total) issue_next();   // refills the slot just drained (p_slot == s)
+            if (lane == 0 && p_issued < total) {   // refills the slot just drained (p_slot == s)
+                issue_next();
+                if (pf_tail && p_issued == total) l2_head();
+            }
         }
+        if ((p.dbg & 4) && p.l2.base && lane == 0 && ti == my_tiles - 1) l2_head();
 
         // ---- split-k reduction across the warps of this sub-CTA + epilogue ----
         float* rbuf = red + (S::kRedBufs == 2 ? (ti & 1) * S::kRedFloats : 0);
@@ -669,40 +711,33 @@ static int v3_num_sms() { return device_sm_count(); }
 constexpr int kV3Budget = 231000;   // one CTA per SM (227 KB usable + 1 KB reserved)
 
 template <int NT, bool NORM, int WARPS, int SUBS, int STAGES, int RT, bool PACK>
-static cudaError_t launch_v3_t(const W4Params& p, int smem, bool pdl, cudaStream_t stream) {
-    const int tiles = p.N / 32;
-    const int want = (tiles + SUBS - 1) / SUBS;
-    const int grid = want < v3_num_sms() ? want : v3_num_sms();
+static cudaError_t launch_v3_t(const W4Params& params, const V3Plan& pl, bool pdl, cudaStream_t stream) {
+    const dim3 grid(pl.grid), block(WARPS * SUBS * 32);
+    W4Params p = params;
+    p.sub_major = pl.sub_major;
     if (p.tp_mode != 0) {
-        // exchange variants exist for the 4-stage rings only (launch_w4_v3 routes tensor-parallel launches there)
+        // exchange variants exist for the 4-stage rings only (w4_v3_plan routes tensor-parallel launches there)
         if constexpr (STAGES == 4 && RT == NT * 8) {
             if (p.tp_mode == 1)
-                return launch(k_w4a16_v3<NT, NORM, WARPS, SUBS, STAGES, RT, PACK, 1>, dim3(grid), dim3(WARPS * SUBS * 32),
-                              (size_t)smem, stream, pdl, p);
-            return launch(k_w4a16_v3<NT, NORM, WARPS, SUBS, STAGES, RT, PACK, 2>, dim3(grid), dim3(WARPS * SUBS * 32),
-                          (size_t)smem, stream, pdl, p);
+                return launch(k_w4a16_v3<NT, NORM, WARPS, SUBS, STAGES, RT, PACK, 1>, grid, block, (size_t)pl.smem, stream,
+                              pdl, p);
+            return launch(k_w4a16_v3<NT, NORM, WARPS, SUBS, STAGES, RT, PACK, 2>, grid, block, (size_t)pl.smem, stream, pdl,
+                          p);
         } else {
             return cudaErrorNotSupported;
         }
     }
-    return launch(k_w4a16_v3<NT, NORM, WARPS, SUBS, STAGES, RT, PACK>, dim3(grid), dim3(WARPS * SUBS * 32), (size_t)smem, stream,
-                  pdl, p);
+    return launch(k_w4a16_v3<NT, NORM, WARPS, SUBS, STAGES, RT, PACK>, grid, block, (size_t)pl.smem, stream, pdl, p);
 }
 
-template <int NT, int WARPS, int SUBS, int STAGES, int RT = NT * 8>
-static bool v3_try(const W4Params& p, bool pdl, cudaStream_t stream, cudaError_t* err) {
-    const int G = p.K / kW4GroupK;
-    const int smem = V3Smem<NT, WARPS, SUBS, STAGES, RT>::kBytes + v3_stage_bytes(p.mc, p.K);
-    if (G > 8 * WARPS * SUBS || smem > kV3Budget || p.mc > RT) return false;   // 8 = kMaxNg
-    static const bool no_one = getenv("ZL_W4_NO_ONE") != nullptr;
-    if (NT == 1 && RT == NT * 8 && p.mc <= 4 && !no_one) {
-        *err = p.ln_w ? launch_v3_t<NT, true, WARPS, SUBS, STAGES, RT, NT == 1 && RT == NT * 8>(p, smem, pdl, stream)
-                      : launch_v3_t<NT, false, WARPS, SUBS, STAGES, RT, NT == 1 && RT == NT * 8>(p, smem, pdl, stream);
-        return true;
-    }
-    *err = p.ln_w ? launch_v3_t<NT, true, WARPS, SUBS, STAGES, RT, false>(p, smem, pdl, stream)
-                  : launch_v3_t<NT, false, WARPS, SUBS, STAGES, RT, false>(p, smem, pdl, stream);
-    return true;
+template <int NT, int WARPS, int SUBS, int STAGES, int RT>
+static cudaError_t v3_run(const W4Params& p, const V3Plan& pl, bool pdl, cudaStream_t stream) {
+    constexpr bool kPack = NT == 1 && RT == NT * 8;
+    if (kPack && pl.pack)
+        return p.ln_w ? launch_v3_t<NT, true, WARPS, SUBS, STAGES, RT, kPack>(p, pl, pdl, stream)
+                      : launch_v3_t<NT, false, WARPS, SUBS, STAGES, RT, kPack>(p, pl, pdl, stream);
+    return p.ln_w ? launch_v3_t<NT, true, WARPS, SUBS, STAGES, RT, false>(p, pl, pdl, stream)
+                  : launch_v3_t<NT, false, WARPS, SUBS, STAGES, RT, false>(p, pl, pdl, stream);
 }
 
 static int v3_max_stages() {
@@ -716,51 +751,137 @@ static int v3_max_stages() {
     return v;
 }
 
-static bool v3_is_tall(const W4Params& p) {
+static bool v3_sub_major() {
+    static int v = -1;
+    if (v < 0) {
+        const char* e = getenv("ZL_W4_SUB_MAJOR");
+        v = e ? atoi(e) != 0 : 1;
+    }
+    return v != 0;
+}
+
+static bool v3_is_tall(int N, int G, int sm_count) {
     static int force = -1;
     if (force < 0) {
         const char* e = getenv("ZL_W4_TALL");
         force = e ? atoi(e) : 0;
     }
-    if (force == 1) return p.K / kW4GroupK >= 32;
+    if (force == 1) return G >= 32;
     if (force == 2) return false;
-    return p.N / 32 <= v3_num_sms() && p.K / kW4GroupK >= 32;
+    return N / 32 <= sm_count && G >= 32;
+}
+
+// The one place that picks the v3 variant: launch_w4_v3 runs exactly this plan, and the L2 head of a successor launch
+// (w4_v3_l2_head) is computed from it.
+bool w4_v3_plan(int mc, int N, int K, int tp_mode, int sm_count, V3Plan* plan) {
+    if (mc < 1 || N <= 0 || K <= 0 || N % 32 || K % kW4GroupK || sm_count < 1) return false;
+    const int G = K / kW4GroupK;
+    const bool tall = v3_is_tall(N, G, sm_count);
+    static const bool no_one = getenv("ZL_W4_NO_ONE") != nullptr;
+    auto fits = [&](int nt, int warps, int subs, int stages, int rt) {
+        const int smem = v3_smem_fixed(nt, warps, subs, stages, rt) + v3_stage_bytes(mc, K);
+        if (G > 8 * warps * subs || smem > kV3Budget || mc > rt) return false;   // 8 = kMaxNg
+        // sub-major tile order (two sub-CTAs): one CTA per SM up to one per tile, every SM busy
+        const int sub_major = subs > 1 && v3_sub_major();
+        const int want = sub_major ? N / 32 : (N / 32 + subs - 1) / subs;
+        *plan = V3Plan{nt, warps, subs, stages, rt, nt == 1 && rt == nt * 8 && mc <= 4 && !no_one,
+                       want < sm_count ? want : sm_count, smem, sub_major};
+        return true;
+    };
+    if (tp_mode != 0) {   // fused tensor-parallel exchange: 4-stage variants
+        if (mc <= 8) return (tall && fits(1, 16, 1, 4, 8)) || fits(1, 8, 2, 4, 8);
+        if (mc <= 16) return (tall && fits(2, 16, 1, 4, 16)) || fits(2, 8, 2, 4, 16);
+        return false;
+    }
+    if (mc <= 2) {   // deepest ring that fits (reduction buffers shrunk to 2 token rows)
+        const int ms = v3_max_stages();
+        if (tall) {
+            if (ms >= 6 && fits(1, 16, 1, 6, 2)) return true;
+            if (ms >= 5 && fits(1, 16, 1, 5, 2)) return true;
+        } else {
+            if (ms >= 6 && fits(1, 8, 2, 6, 2)) return true;
+        }
+    }
+    if (mc <= 8) return (tall && fits(1, 16, 1, 4, 8)) || fits(1, 8, 2, 5, 8) || fits(1, 8, 2, 4, 8);
+    if (mc <= 16) return (tall && fits(2, 16, 1, 4, 16)) || fits(2, 8, 2, 4, 16);
+    return false;
 }
 
 // returns false when the staged activations do not fit shared memory (caller falls back to the fp16 kernels)
 bool launch_w4_v3(const W4Params& p, bool pdl, cudaStream_t stream, cudaError_t* err) {
-    const bool tall = v3_is_tall(p);
-    if (p.tp_mode != 0) {   // fused tensor-parallel exchange: 4-stage variants
-        if (p.mc <= 8) {
-            if (tall && v3_try<1, 16, 1, 4>(p, pdl, stream, err)) return true;
-            return v3_try<1, 8, 2, 4>(p, pdl, stream, err);
-        }
-        if (p.mc <= 16) {
-            if (tall && v3_try<2, 16, 1, 4>(p, pdl, stream, err)) return true;
-            return v3_try<2, 8, 2, 4>(p, pdl, stream, err);
-        }
-        return false;
+    V3Plan pl;
+    if (!w4_v3_plan(p.mc, p.N, p.K, p.tp_mode, v3_num_sms(), &pl)) return false;
+#define ZL_V3(NT, W, SB, ST, RT)                                                                               \
+    if (pl.nt == NT && pl.warps == W && pl.subs == SB && pl.stages == ST && pl.rt == RT) {                     \
+        *err = v3_run<NT, W, SB, ST, RT>(p, pl, pdl, stream);                                                  \
+        return true;                                                                                           \
     }
-    if (p.mc <= 2) {   // deepest ring that fits (reduction buffers shrunk to 2 token rows)
-        const int ms = v3_max_stages();
-        if (tall) {
-            if (ms >= 6 && v3_try<1, 16, 1, 6, 2>(p, pdl, stream, err)) return true;
-            if (ms >= 5 && v3_try<1, 16, 1, 5, 2>(p, pdl, stream, err)) return true;
-        } else {
-            if (ms >= 6 && v3_try<1, 8, 2, 6, 2>(p, pdl, stream, err)) return true;
-        }
-    }
-    if (p.mc <= 8) {
-        if (tall && v3_try<1, 16, 1, 4>(p, pdl, stream, err)) return true;
-        if (v3_try<1, 8, 2, 5>(p, pdl, stream, err)) return true;
-        return v3_try<1, 8, 2, 4>(p, pdl, stream, err);
-    }
-    if (p.mc <= 16) {
-        if (tall && v3_try<2, 16, 1, 4>(p, pdl, stream, err)) return true;
-        return v3_try<2, 8, 2, 4>(p, pdl, stream, err);
-    }
+    ZL_V3(1, 16, 1, 6, 2) ZL_V3(1, 16, 1, 5, 2) ZL_V3(1, 8, 2, 6, 2)
+    ZL_V3(1, 16, 1, 4, 8) ZL_V3(1, 8, 2, 5, 8) ZL_V3(1, 8, 2, 4, 8)
+    ZL_V3(2, 16, 1, 4, 16) ZL_V3(2, 8, 2, 4, 16)
+#undef ZL_V3
     return false;
 }
+
+bool w4_v3_l2_head(const void* packed, int mc, int N, int K, int tp_mode, int sm_count, int h, size_t whole_max,
+                   W4L2Head* out) {
+    *out = W4L2Head{};
+    V3Plan pl;
+    if (!packed || !w4_v3_plan(mc, N, K, tp_mode, sm_count, &pl)) return false;
+    out->base = static_cast<const uint8_t*>(packed);
+    out->n_tiles = N / 32;
+    out->G = K / kW4GroupK;
+    out->grid = pl.grid;
+    out->subs = pl.subs;
+    out->warps = pl.warps;
+    out->sub_major = pl.sub_major;
+    out->h = h;
+    const size_t blob = (size_t)out->n_tiles * out->G * kW4BlockBytes;
+    if (blob <= whole_max) {
+        out->whole_bytes = blob;
+    } else if (h <= 0) {
+        *out = W4L2Head{};
+        return false;
+    }
+    return true;
+}
+
+}  // namespace zl
+
+// host view of the v3 plan, for tests: out[0..8] = NT, warps per sub-CTA, sub-CTAs, ring stages, reduction rows, PACK,
+// grid, dynamic shared memory bytes, sub-major tile order.  Returns 0, or ZL_ERR_UNSUPPORTED when no v3 variant fits.
+extern "C" int zl_w4_v3_plan(int mc, int N, int K, int tp_mode, int sm_count, int* out) {
+    if (!out) return ZL_ERR_INVALID_ARG;
+    zl::V3Plan pl;
+    if (!zl::w4_v3_plan(mc, N, K, tp_mode, sm_count, &pl)) return ZL_ERR_UNSUPPORTED;
+    const int v[9] = {pl.nt, pl.warps, pl.subs, pl.stages, pl.rt, pl.pack, pl.grid, pl.smem, pl.sub_major};
+    for (int i = 0; i < 9; ++i) out[i] = v[i];
+    return 0;
+}
+
+// host view of the L2 head a predecessor prefetches for a v3 launch of (mc, N, K, tp_mode) on sm_count SMs at depth H
+// (the same v3_head_ranges the kernel runs): out[3 i ..] = successor warp, byte offset into the blob, bytes.  Returns the
+// number of ranges (<= max_ranges) or a negative error code.
+extern "C" int zl_w4_v3_l2_head(int mc, int N, int K, int tp_mode, int sm_count, int H, long long* out, int max_ranges) {
+    if (!out || H < 1) return ZL_ERR_INVALID_ARG;
+    zl::W4L2Head hd;
+    static const uint8_t kBase = 0;
+    if (!zl::w4_v3_l2_head(&kBase, mc, N, K, tp_mode, sm_count, H, 0, &hd)) return ZL_ERR_UNSUPPORTED;
+    int n = 0;
+    const int warps = hd.grid * hd.subs * hd.warps;
+    for (int sw = 0; sw < warps; ++sw)
+        zl::v3_head_ranges(hd, sw, [&](size_t off, size_t bytes) {
+            if (n < max_ranges) {
+                out[3 * n + 0] = sw;
+                out[3 * n + 1] = (long long)off;
+                out[3 * n + 2] = (long long)bytes;
+            }
+            ++n;
+        });
+    return n <= max_ranges ? n : ZL_ERR_INVALID_ARG;
+}
+
+namespace zl {
 
 bool w4_v3_fits(int mc, int N, int K) {
     const int G = K / kW4GroupK;

@@ -295,6 +295,45 @@ int zl_argmax(const float* logits, int32_t* out, int T, int V, void* workspace, 
 int zl_argmax_candidates(const float* logits, void* cand_out, int T, int V, int idx_offset, void* workspace,
                          size_t workspace_bytes, int pdl, zl_stream_t stream);
 int zl_argmax_merge(const void* cand_all, int32_t* out, int T, int ranks, int stride, int pdl, zl_stream_t stream);
+
+/* Next-token sampling (SearcherImplV1::random_sample, generator/batch_generator.cpp:1854-1883 = functions::softmax with
+ * temperature (softmax.cu) + beam_utility::random_sampler_gpu (generator/random_util.cu:81-198), with the penalties of
+ * beam_repetition_penalty (generator/beam_util.cu:198-281)).  Per task:
+ *   temperature >= 0, top_p in (0, 1], top_k >= 0 (0 or >= V: off), repetition_penalty > 0, presence_penalty, seed.
+ * A row's token depends only on its fp32 logits, its task's parameters and seed, its counter and its task's history:
+ *   1. penalties, on a copy of the logits, for every token set in the task's history bitmap (the distinct tokens
+ *      generated since the task's sampling was last set): presence_penalty != 0 ? l -= presence_penalty
+ *      : l = l < 0 ? l * repetition_penalty : l / repetition_penalty   (beam_util.cu:212-219);
+ *   2. temperature == 0 or top_k == 1: greedy, exactly zl_argmax's pick of the penalised row (ties -> lowest index);
+ *   3. otherwise x = l / temperature in descending order (ties by ascending index), w = exp(x - max x), Z = sum w,
+ *      C_j the inclusive cumulative sum in that order, P' = min(top_p * Z, C_{top_k-1}) (Z when top_k is off),
+ *      target = u * P'; the token is the first j with C_j >= target  (random_util.cu:89-106);
+ *   4. u = ((r >> 8) + 1) * 2^-24 with r = zl_sample_uniform(seed, counter);
+ *   5. -inf / NaN logits have probability 0; a row whose penalised max is not finite takes the greedy pick.
+ * Masses are summed as exact 2^-44 fixed-point integers (deterministic; a token below ~2^-45 of the row's maximum weight
+ * has probability 0).  After the pick the token's bit is set in the task's history.
+ * Whether to sample is the scheduler's decision: the reference samples only when top_p < 1 or top_k > 0
+ * (SearchTask::is_random, batch_generator.h:106); a scheduler maps is_random() == false to temperature = 0. */
+typedef struct zl_sample_params {
+    float temperature, top_p, repetition_penalty, presence_penalty;
+    int top_k;
+    uint64_t seed;
+} zl_sample_params_t;
+/* r: the first 32-bit output of Philox4x32-10 (curand_philox4x32_x.h round function and constants) with
+ * key = (seed low, seed high) and counter = (counter, 0, 0, 0).  The kernel draws the same r on the device. */
+unsigned zl_sample_uniform(uint64_t seed, unsigned counter);
+/* host check of n parameter sets (HOST pointer): ZL_ERR_INVALID_ARG for values outside the ranges above. */
+int zl_sample_check_params(const zl_sample_params_t* params_host, int n);
+/* 0 today: the sampler keeps everything in shared memory (ws may be NULL). */
+size_t zl_sample_workspace_bytes(int T, int V);
+/* logits (T, V) fp32; params indexed by task; row_task (T) maps rows to tasks (NULL: row i is task i); counter (T) the
+ * position of the input token whose logits each row holds (NULL: 0); history (tasks, history_words >= ceil(V/32)) u32
+ * bitmap or NULL (no penalties, nothing recorded; rows sharing a task must not pass a history); out (T) int32.
+ * V <= 262144 (ZL_ERR_UNSUPPORTED above).  One launch: one cluster of 8 CTAs per row.  Parameter values are not
+ * checked on the device: validate them with zl_sample_check_params. */
+int zl_sample(const float* logits, int T, int V, const zl_sample_params_t* params, const int32_t* row_task,
+              const int32_t* counter, uint32_t* history, int history_words, int32_t* out, void* ws, size_t ws_bytes,
+              int pdl, zl_stream_t stream);
 /* synthetic-checkpoint generators (bench / tests): counter-based hash RNG, reproducible per seed. */
 int zl_fill_random_u32(uint32_t* p, size_t n, uint64_t seed, zl_stream_t stream);
 int zl_fill_const_u32(uint32_t* p, size_t n, uint32_t value, zl_stream_t stream);
@@ -397,6 +436,13 @@ int zl_llama_sync(zl_llama_t* m);
  * overwrites the next-token / logits row 0 outputs, which zl_llama_step_device consumes before it returns. */
 int zl_llama_prefill(zl_llama_t* m, int task, const int32_t* tokens_host, int n, int pos0, int32_t* next_token_host,
                      float* logits_host);
+/* Per-task sampling (zl_sample's contract) for the picks of zl_llama_decode / step_device / prefill.  Copies *p (HOST
+ * pointer) to the device and clears the task's history; p == NULL returns the task to plain greedy.  Invalid values:
+ * ZL_ERR_INVALID_ARG; anything but plain greedy under tp_size > 1: ZL_ERR_UNSUPPORTED (vocabulary shards would need a
+ * global top-k / top-p threshold).  The decode step runs zl_sample instead of zl_argmax while a task in the batch
+ * samples or has penalties (counter = the input token's position; prefill: pos0 + n - 1), so a task draws the same
+ * tokens with host or device-resident stepping, with or without the graph.  The logits stay the raw lm_head output. */
+int zl_llama_set_sampling(zl_llama_t* m, int task, const zl_sample_params_t* p);
 zl_stream_t zl_llama_stream(zl_llama_t* m);
 /* bytes the step must read from HBM per rank (weights + lm_head + norms), kernel launches per step. */
 int zl_llama_stats(zl_llama_t* m, int B, double* weight_bytes, int* kernels_per_step);

@@ -56,6 +56,19 @@ class W4FusedArgs(ctypes.Structure):
     ]
 
 
+class SampleParams(ctypes.Structure):
+    """zl_sample_params_t"""
+    _fields_ = [
+        ("temperature", ctypes.c_float), ("top_p", ctypes.c_float), ("repetition_penalty", ctypes.c_float),
+        ("presence_penalty", ctypes.c_float), ("top_k", ctypes.c_int), ("seed", ctypes.c_uint64),
+    ]
+
+
+def sample_params(temperature=0.0, top_p=1.0, top_k=0, repetition_penalty=1.0, presence_penalty=0.0, seed=0):
+    return SampleParams(float(temperature), float(top_p), float(repetition_penalty), float(presence_penalty),
+                        int(top_k), int(seed) & 0xFFFFFFFFFFFFFFFF)
+
+
 _SCALARS = {
     "int": ctypes.c_int, "float": ctypes.c_float, "double": ctypes.c_double, "size_t": ctypes.c_size_t,
     "uint64_t": ctypes.c_uint64, "uint32_t": ctypes.c_uint32, "int32_t": ctypes.c_int32,
@@ -86,6 +99,7 @@ def parse_header(path=HEADER):
     src = re.sub(r"//[^\n]*", " ", src)
     src = re.sub(r"typedef struct zl_llama_config \{.*?\} zl_llama_config_t;", " ", src, flags=re.S)
     src = re.sub(r"typedef struct zl_w4_fused_args \{.*?\} zl_w4_fused_args_t;", " ", src, flags=re.S)
+    src = re.sub(r"typedef struct zl_sample_params \{.*?\} zl_sample_params_t;", " ", src, flags=re.S)
     protos = {}
     for m in re.finditer(r"([A-Za-z_][\w \*]*?)\b(zl_\w+)\s*\(([^;{}]*?)\)\s*;", src):
         ret, name, args = m.group(1).strip(), m.group(2), m.group(3).strip()

@@ -110,6 +110,12 @@ struct zl_llama {
     int32_t* d_tb = nullptr;      // token -> task map of the chunk being prefilled
     const int32_t* cur_tb = nullptr;   // token -> task map of the launch sequence being enqueued (d_iota at decode)
     int8_t* d_mask = nullptr;     // (chunk, max_seq) causal mask of the chunk
+    // sampling (zl_llama_set_sampling): per-task parameters and generated-token bitmaps on the device; samp_on[t] is set
+    // while task t samples or has penalties, and the step then runs zl_sample instead of zl_argmax
+    zl_sample_params_t* d_sparams = nullptr;   // (max_batch)
+    uint32_t* d_hist = nullptr;                // (max_batch, hwords)
+    int hwords = 0;
+    std::vector<char> samp_on;
 };
 
 namespace {
@@ -609,6 +615,18 @@ int alloc_runtime(zl_llama* m) {
     m->attn_ws_bytes = zl_decode_attention_workspace_bytes(T, 1, m->hq, d, c.max_seq);
     RCHECK(dmalloc(&m->attn_ws, m->attn_ws_bytes));
     RCHECK(dmalloc(&m->argmax_ws, zl_argmax_workspace_bytes(B)));
+    m->hwords = cdiv(m->vshard, 32);
+    RCHECK(dmalloc((void**)&m->d_hist, (size_t)B * m->hwords * 4));
+    ZL_CHECK_CUDA(cudaMemsetAsync(m->d_hist, 0, (size_t)B * m->hwords * 4, m->stream));
+    RCHECK(dmalloc((void**)&m->d_sparams, sizeof(zl_sample_params_t) * B));
+    {
+        const zl_sample_params_t greedy{0.f, 1.f, 1.f, 0.f, 0, 0};
+        std::vector<zl_sample_params_t> init(B, greedy);
+        ZL_CHECK_CUDA(cudaMemcpyAsync(m->d_sparams, init.data(), sizeof(zl_sample_params_t) * B, cudaMemcpyHostToDevice,
+                                      m->stream));
+        ZL_CHECK_CUDA(cudaStreamSynchronize(m->stream));   // `init` is pageable and goes out of scope
+    }
+    m->samp_on.assign(B, 0);
     ZL_CHECK_CUDA(cudaMallocHost((void**)&m->h_stage, sizeof(int32_t) * (4 * B + 4 + T)));
     ZL_CHECK_CUDA(cudaMallocHost((void**)&m->h_ring, sizeof(int32_t) * zl_llama::kStageSlots * 2 * B));
     for (int i = 0; i < zl_llama::kStageSlots; ++i)
@@ -871,7 +889,7 @@ int prefill_layers_dual(zl_llama* m, const PrefillChunk& pf) {
     return ZL_OK;
 }
 
-int enqueue_step(zl_llama* m, int n_tasks, int len_bucket, const PrefillChunk* pf = nullptr) {
+int enqueue_step(zl_llama* m, int n_tasks, int len_bucket, const PrefillChunk* pf = nullptr, bool sampler = false) {
     const auto& c = m->cfg;
     const int B = pf ? pf->n : n_tasks;   // rows (tokens) of every activation matrix in this launch sequence
     const int skip = debug_skip();
@@ -1025,7 +1043,14 @@ int enqueue_step(zl_llama* m, int n_tasks, int len_bucket, const PrefillChunk* p
     // vocab-parallel lm_head (embedding.cu:353-392): each rank owns vshard rows
     if (!(skip & 32))
         RCHECK(zl_dense_gemm_skinny(m->xn, D, m->lm_head, nullptr, m->logits, HB, m->vshard, D, dt, ZL_F32, P(64), st));
-    if (!tp) {
+    if (sampler) {
+        // one row per task at decode (row b = task b, counter = its input position); prefill: the task's last prompt
+        // position.  set_sampling keeps this off under tensor parallelism.
+        const int32_t* row_task = pf ? m->d_iota + pf->task : m->d_iota;
+        const int32_t* counter = pf ? m->d_pf_pos + (pf->n - 1) : m->d_pos;
+        RCHECK(zl_sample(m->logits, HB, m->vshard, m->d_sparams, row_task, counter, m->d_hist, m->hwords, m->d_next,
+                         nullptr, 0, P(128), st));
+    } else if (!tp) {
         RCHECK(zl_argmax(m->logits, m->d_next, HB, m->vshard, m->argmax_ws, zl_argmax_workspace_bytes(HB), P(128), st));
     } else {
         // instead of all-gathering (B, V) logits, exchange one {value, index} candidate per token
@@ -1045,15 +1070,23 @@ int len_bucket_of(const zl_llama* m, int max_len) {
     return b < m->cfg.max_seq ? b : (m->cfg.max_seq > 256 ? m->cfg.max_seq : 256);
 }
 
+bool sampler_on(const zl_llama* m, int first, int n) {
+    for (int t = first; t < first + n; ++t)
+        if (m->samp_on[t]) return true;
+    return false;
+}
+
 int run_step(zl_llama* m, int B) {
     const int bucket = len_bucket_of(m, m->cur_max_len);
-    if (!m->cfg.use_graph) return enqueue_step(m, B, bucket);
-    const long long key = ((long long)B << 32) | (unsigned)bucket;
+    const bool sampler = sampler_on(m, 0, B);
+    if (!m->cfg.use_graph) return enqueue_step(m, B, bucket, nullptr, sampler);
+    // parameter changes need no re-capture (they live on the device), only switching the sampler on or off does
+    const long long key = ((long long)B << 33) | ((long long)sampler << 32) | (unsigned)bucket;
     auto it = m->graphs.find(key);
     if (it == m->graphs.end()) {
         cudaGraph_t graph = nullptr;
         ZL_CHECK_CUDA(cudaStreamBeginCapture(m->stream, cudaStreamCaptureModeThreadLocal));
-        int rc = enqueue_step(m, B, bucket);
+        int rc = enqueue_step(m, B, bucket, nullptr, sampler);
         cudaError_t ce = cudaStreamEndCapture(m->stream, &graph);
         if (rc != ZL_OK) {
             if (graph) cudaGraphDestroy(graph);
@@ -1136,7 +1169,8 @@ extern "C" void zl_llama_destroy(zl_llama_t* m) {
     }
     for (void* p : {m->emb, m->lm_head_tied ? nullptr : m->lm_head, m->ln_f, m->h, m->xn, m->qkv, m->q, m->ao, m->act,
                     m->pend, m->gu, (void*)m->logits, (void*)m->cosb, (void*)m->sinb, (void*)m->d_tokens,
-                    m->h2, (void*)m->d_pos, (void*)m->d_lens, (void*)m->d_next, (void*)m->d_iota, m->attn_ws, m->argmax_ws, (void*)m->d_tb, (void*)m->d_mask, m->xq, (void*)m->xs})
+                    m->h2, (void*)m->d_pos, (void*)m->d_lens, (void*)m->d_next, (void*)m->d_iota, m->attn_ws, m->argmax_ws, (void*)m->d_tb, (void*)m->d_mask, m->xq, (void*)m->xs,
+                    (void*)m->d_hist, (void*)m->d_sparams})
         if (p) cudaFree(p);
     if (m->reduce_stream) {
         cudaStreamSynchronize(m->reduce_stream);
@@ -1446,7 +1480,7 @@ extern "C" int zl_llama_prefill(zl_llama_t* m, int task, const int32_t* tokens_h
         }
         ZL_CHECK_CUDA(cudaMemcpyAsync(m->d_pf_tokens, h_tok, cn * 4, cudaMemcpyHostToDevice, m->stream));
         PrefillChunk pc{task, pos0 + c0, cn, c0 + cn == n};
-        RCHECK(enqueue_step(m, 1, 0, &pc));
+        RCHECK(enqueue_step(m, 1, 0, &pc, sampler_on(m, task, 1)));
     }
     ZL_CHECK_CUDA(cudaMemcpyAsync(m->h_stage + 3 * m->cfg.max_batch, m->d_next, 4, cudaMemcpyDeviceToHost, m->stream));
     if (logits_host)
@@ -1454,6 +1488,24 @@ extern "C" int zl_llama_prefill(zl_llama_t* m, int task, const int32_t* tokens_h
     ZL_CHECK_CUDA(cudaStreamSynchronize(m->stream));
     *next_token_host = m->h_stage[3 * m->cfg.max_batch];
     if (pos0 + n > m->cur_max_len) m->cur_max_len = pos0 + n;
+    return ZL_OK;
+}
+
+extern "C" int zl_llama_set_sampling(zl_llama_t* m, int task, const zl_sample_params_t* p) {
+    if (p) RCHECK(zl_sample_check_params(p, 1));
+    ZL_CHECK_ARG(m && task >= 0 && task < m->cfg.max_batch);
+    const bool on = p && ((p->temperature > 0.f && p->top_k != 1) || p->repetition_penalty != 1.f ||
+                          p->presence_penalty != 0.f);
+    ZL_CHECK_SUPPORTED(!on || m->cfg.tp_size == 1);
+    if (!m->finalized) {
+        zl_set_last_error(__FILE__, __LINE__, "model not finalized");
+        return ZL_ERR_STATE;
+    }
+    const zl_sample_params_t q = p ? *p : zl_sample_params_t{0.f, 1.f, 1.f, 0.f, 0, 0};
+    // stream-ordered after every step already enqueued; the pageable source is staged before the call returns
+    ZL_CHECK_CUDA(cudaMemcpyAsync(m->d_sparams + task, &q, sizeof(q), cudaMemcpyHostToDevice, m->stream));
+    ZL_CHECK_CUDA(cudaMemsetAsync(m->d_hist + (size_t)task * m->hwords, 0, (size_t)m->hwords * 4, m->stream));
+    m->samp_on[task] = on ? 1 : 0;
     return ZL_OK;
 }
 

@@ -1,0 +1,455 @@
+// Next-token sampling on the GPU: repetition / presence penalties, temperature, top-k and top-p, in ONE launch for
+// every row of a batch, greedy and sampled rows alike.
+//
+// Stands in for SearcherImplV1::random_sample (reference src/generator/batch_generator.cpp:1854-1883), i.e.
+// functions::softmax with temperature + beam_utility::random_sampler_gpu (src/generator/random_util.cu:81-198: cub radix
+// sort of the vocabulary, inclusive scan, one-thread binary search, once per task) and for the penalty scatter
+// beam_repetition_penalty (src/generator/beam_util.cu:198-281).  No sort: the position where the descending cumulative
+// mass crosses a target is found by radix selection, once for the top-k mass C_{k-1} and once for the sampled token.
+//
+// One thread-block cluster of kCluster CTAs per row.  CTA r keeps its contiguous slice of the row, penalised and divided
+// by the temperature, in shared memory; every later pass runs over shared memory.  Per-CTA histograms are merged through
+// distributed shared memory in rank order, so every CTA of the cluster takes the same decisions.
+//
+// Masses are fixed point: w = round(exp(x - max x) * 2^44) as uint64, so sums are exact integers and do not depend on
+// the summation order (a launch is reproducible bit for bit, whatever the atomics' order).  A token whose weight is below
+// ~2^-45 of the maximum gets mass 0 and is never picked (probability < 3e-14 under the exact contract).
+#include "common.cuh"
+
+#include <cooperative_groups.h>
+
+namespace cg = cooperative_groups;
+
+namespace zl {
+
+constexpr int kSampleCluster = 8;
+constexpr int kSampleThreads = 1024;
+constexpr int kSampleMaxVocab = 262144;
+constexpr int kSampleMaxSlice = kSampleMaxVocab / kSampleCluster;
+constexpr float kMassScale = 17592186044416.0f;   // 2^44: V * 2^44 < 2^63 for V <= 2^18
+
+// Philox4x32-10 (Salmon et al., SC'11; the round function and constants of CUDA's curand_philox4x32_x.h), first output
+// word for key = (seed lo, seed hi), counter = (counter, 0, 0, 0).
+__host__ __device__ inline uint32_t philox_first(uint64_t seed, uint32_t counter) {
+    uint32_t c0 = counter, c1 = 0, c2 = 0, c3 = 0;
+    uint32_t k0 = (uint32_t)seed, k1 = (uint32_t)(seed >> 32);
+    for (int i = 0; i < 10; ++i) {
+        if (i) {
+            k0 += 0x9E3779B9u;
+            k1 += 0xBB67AE85u;
+        }
+        const uint64_t p0 = (uint64_t)0xD2511F53u * c0;
+        const uint64_t p1 = (uint64_t)0xCD9E8D57u * c2;
+        const uint32_t n0 = (uint32_t)(p1 >> 32) ^ c1 ^ k0;
+        const uint32_t n2 = (uint32_t)(p0 >> 32) ^ c3 ^ k1;
+        c1 = (uint32_t)p1;
+        c3 = (uint32_t)p0;
+        c0 = n0;
+        c2 = n2;
+    }
+    return c0;
+}
+
+// ascending key == descending x; -0 and +0 share one key (they compare equal, so they tie by index)
+__device__ __forceinline__ uint32_t desc_key(float x) {
+    const uint32_t u = __float_as_uint(x);
+    const uint32_t k = (u & 0x80000000u) ? ~u : (u | 0x80000000u);
+    return ~k;
+}
+// first radix digit: a monotone (non-increasing in x) bucket of width 1/4 below the row maximum.  Logit rows crowd into a
+// few float exponents, so the float's own top bits would send nearly every element to one shared-memory counter.
+__device__ __forceinline__ int bucket0(float x, float xmax) {
+    const float d = (xmax - x) * 4.0f;
+    return d < 255.0f ? (int)d : 255;
+}
+__device__ __forceinline__ unsigned long long mass_of(float x, float xmax) {
+    return __float2ull_rn(expf(x - xmax) * kMassScale);
+}
+
+struct SampleShared {
+    uint32_t cnt[2][256];   // this CTA's histogram of the current round (double-buffered across rounds)
+    unsigned long long mass[2][256];
+    uint32_t mcnt[256];     // cluster-merged histogram of the current round
+    unsigned long long mmass[256];
+    uint32_t cnt0[256];     // cluster-merged histogram of round 0 (shared by both selections)
+    unsigned long long mass0[256];
+    float wv[32], wx[32];
+    int wi[32];
+    float cta_best, cta_xmax;   // read by the other CTAs of the cluster
+    int cta_bi;
+    unsigned long long scan[32];
+    int sel_digit;
+    unsigned long long sel_cnt_before, sel_mass_before, sel_bin_cnt, sel_bin_mass, total_mass;
+    int tok;
+};
+
+// Warp 0: over 256 merged bins, find the first bin whose inclusive cumulative metric (mass or count) reaches `need`
+// (>= 1); write the digit, the count / mass of the bins before it and of the bin itself.
+__device__ void scan_select(SampleShared& s, const uint32_t* cnt, const unsigned long long* mass, bool by_mass,
+                            unsigned long long need) {
+    const int lane = threadIdx.x & 31;
+    unsigned long long tc = 0, tm = 0;
+#pragma unroll
+    for (int j = 0; j < 8; ++j) {
+        tc += cnt[lane * 8 + j];
+        tm += mass[lane * 8 + j];
+    }
+    unsigned long long ic = tc, im = tm;
+#pragma unroll
+    for (int o = 1; o < 32; o <<= 1) {
+        const unsigned long long a = __shfl_up_sync(0xffffffffu, ic, o);
+        const unsigned long long b = __shfl_up_sync(0xffffffffu, im, o);
+        if (lane >= o) {
+            ic += a;
+            im += b;
+        }
+    }
+    const unsigned long long total = __shfl_sync(0xffffffffu, by_mass ? im : ic, 31);
+    const unsigned long long total_m = __shfl_sync(0xffffffffu, im, 31);
+    if (need > total) need = total;   // exact integers make this a no-op; kept so a pick always exists
+    if (need < 1) need = 1;
+    const unsigned long long inc = by_mass ? im : ic, exc = inc - (by_mass ? tm : tc);
+    const unsigned hit = __ballot_sync(0xffffffffu, exc < need && inc >= need);
+    const int owner = hit ? __ffs(hit) - 1 : 0;
+    if (lane == 0) s.total_mass = total_m;
+    if (lane == owner) {
+        unsigned long long bc = ic - tc, bm = im - tm;
+        int d = lane * 8;
+        for (int j = 0; j < 8; ++j) {
+            const unsigned long long c = cnt[lane * 8 + j], m = mass[lane * 8 + j];
+            d = lane * 8 + j;
+            if ((by_mass ? bm + m : bc + c) >= need || j == 7 || !hit) {
+                s.sel_digit = d;
+                s.sel_cnt_before = bc;
+                s.sel_mass_before = bm;
+                s.sel_bin_cnt = c;
+                s.sel_bin_mass = m;
+                break;
+            }
+            bc += c;
+            bm += m;
+        }
+    }
+}
+
+struct SelResult {
+    int b0;
+    uint32_t key;   // full descending key of the selected tie group
+    unsigned long long cnt_before, mass_before, grp_cnt, grp_mass;
+};
+
+// Radix selection over the order (descending x, ascending index): the tie group of elements with equal x that contains
+// the `target`-th unit of the metric (count or mass) counted from the top.  Round 0 uses the merged bucket histogram,
+// rounds 1..4 the bytes of the descending key inside the selected bucket.  `rc` numbers the rounds for the histogram
+// double buffer.
+__device__ SelResult cluster_select(SampleShared& s, cg::cluster_group& cl, const float* xs, int n, float xmax,
+                                    bool by_mass, unsigned long long target, int& rc) {
+    SelResult r{};
+    if (threadIdx.x < 32) scan_select(s, s.cnt0, s.mass0, by_mass, target);
+    __syncthreads();
+    r.b0 = s.sel_digit;
+    r.cnt_before = s.sel_cnt_before;
+    r.mass_before = s.sel_mass_before;
+    r.grp_cnt = s.sel_bin_cnt;
+    r.grp_mass = s.sel_bin_mass;
+    uint32_t prefix = 0;
+    for (int round = 1; round <= 4; ++round, ++rc) {
+        const int buf = rc & 1;
+        if (threadIdx.x < 256) {
+            s.cnt[buf][threadIdx.x] = 0;
+            s.mass[buf][threadIdx.x] = 0;
+        }
+        __syncthreads();
+        const int shift = 32 - 8 * round;
+        for (int i = threadIdx.x; i < n; i += kSampleThreads) {
+            const float x = xs[i];
+            if (bucket0(x, xmax) != r.b0) continue;
+            const uint32_t k = desc_key(x);
+            if (round > 1 && (k >> (shift + 8)) != prefix) continue;
+            const int dg = (k >> shift) & 255;
+            atomicAdd(&s.cnt[buf][dg], 1u);
+            atomicAdd(&s.mass[buf][dg], mass_of(x, xmax));   // the count selection needs C_{k-1} too
+        }
+        cl.sync();
+        if (threadIdx.x < 256) {
+            uint32_t c = 0;
+            unsigned long long m = 0;
+            for (int q = 0; q < kSampleCluster; ++q) {
+                c += cl.map_shared_rank(&s.cnt[buf][0], q)[threadIdx.x];
+                m += cl.map_shared_rank(&s.mass[buf][0], q)[threadIdx.x];
+            }
+            s.mcnt[threadIdx.x] = c;
+            s.mmass[threadIdx.x] = m;
+        }
+        __syncthreads();
+        if (threadIdx.x < 32)
+            scan_select(s, s.mcnt, s.mmass, by_mass, target - (by_mass ? r.mass_before : r.cnt_before));
+        __syncthreads();
+        prefix = (prefix << 8) | (uint32_t)s.sel_digit;
+        r.cnt_before += s.sel_cnt_before;
+        r.mass_before += s.sel_mass_before;
+        r.grp_cnt = s.sel_bin_cnt;
+        r.grp_mass = s.sel_bin_mass;
+        __syncthreads();   // s.sel_* is rewritten by the next round's scan
+    }
+    r.key = prefix;
+    return r;
+}
+
+__global__ void __cluster_dims__(kSampleCluster, 1, 1) __launch_bounds__(kSampleThreads, 1)
+    k_sample(const float* __restrict__ logits, int T, int V, int S, const zl_sample_params_t* __restrict__ params,
+             const int32_t* __restrict__ row_task, const int32_t* __restrict__ counter, uint32_t* __restrict__ history,
+             int hwords, int32_t* __restrict__ out) {
+    extern __shared__ float xs[];
+    __shared__ SampleShared s;
+    cg::cluster_group cl = cg::this_cluster();
+    const int rank = (int)cl.block_rank();
+    const int row = blockIdx.z * gridDim.y + blockIdx.y, tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+    pdl_trigger();
+    if (row >= T) return;   // the whole cluster shares the row
+    pdl_wait();
+    const int task = row_task ? row_task[row] : row;
+    const zl_sample_params_t p = params[task];
+    const bool greedy = !(p.temperature > 0.f) || p.top_k == 1;
+    uint32_t* hist = history ? history + (size_t)task * hwords : nullptr;
+    const bool pen = hist && (p.presence_penalty != 0.f || p.repetition_penalty != 1.f);
+    const int lo = rank * S;
+    const int n = max(0, min(V, lo + S) - lo);
+    const float* src = logits + (size_t)row * V + lo;
+
+    // pass 1: penalties, the greedy pick of the penalised row (zl_argmax's rule: max, ties -> lowest index), max of x
+    float best = -INFINITY, xmax = -INFINITY;
+    int bi = 0x7fffffff;
+    for (int i = tid; i < n; i += kSampleThreads) {
+        float l = src[i];
+        const int g = lo + i;
+        if (pen && ((hist[g >> 5] >> (g & 31)) & 1u)) {   // beam_util.cu:212-219
+            if (p.presence_penalty != 0.f)
+                l = l - p.presence_penalty;
+            else
+                l = l < 0.f ? l * p.repetition_penalty : l / p.repetition_penalty;
+        }
+        if (l > best || (l == best && g < bi)) {
+            best = l;
+            bi = g;
+        }
+        if (!greedy) {
+            float x = l / p.temperature;
+            if (x != x) x = -INFINITY;   // NaN: probability 0
+            if (x == 0.f) x = 0.f;       // one key for -0 / +0
+            xs[i] = x;
+            xmax = fmaxf(xmax, x);
+        }
+    }
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) {
+        const float ov = __shfl_xor_sync(0xffffffffu, best, o);
+        const int oi = __shfl_xor_sync(0xffffffffu, bi, o);
+        if (ov > best || (ov == best && oi < bi)) {
+            best = ov;
+            bi = oi;
+        }
+        xmax = fmaxf(xmax, __shfl_xor_sync(0xffffffffu, xmax, o));
+    }
+    if (lane == 0) {
+        s.wv[warp] = best;
+        s.wi[warp] = bi;
+        s.wx[warp] = xmax;
+    }
+    __syncthreads();
+    if (tid == 0) {
+        for (int w = 1; w < kSampleThreads / 32; ++w) {
+            if (s.wv[w] > best || (s.wv[w] == best && s.wi[w] < bi)) {
+                best = s.wv[w];
+                bi = s.wi[w];
+            }
+            xmax = fmaxf(xmax, s.wx[w]);
+        }
+        s.cta_best = best;
+        s.cta_bi = bi;
+        s.cta_xmax = xmax;
+    }
+    cl.sync();
+    // every CTA merges the cluster's candidates in rank order (= index order: ties keep the lower index)
+    best = -INFINITY;
+    bi = 0x7fffffff;
+    xmax = -INFINITY;
+    for (int q = 0; q < kSampleCluster; ++q) {
+        SampleShared* o = cl.map_shared_rank(&s, q);
+        const float ov = o->cta_best;
+        const int oi = o->cta_bi;
+        if (ov > best || (ov == best && oi < bi)) {
+            best = ov;
+            bi = oi;
+        }
+        xmax = fmaxf(xmax, o->cta_xmax);
+    }
+    const int greedy_tok = (bi >= 0 && bi < V) ? bi : 0;
+
+    int tok = greedy_tok;
+    bool owner = rank == 0;   // the CTA that writes the result
+    // a row whose penalised maximum is not finite falls back to the greedy pick
+    if (!greedy && xmax > -INFINITY && xmax < INFINITY) {
+        // round 0: bucket histogram with masses, over the whole row
+        if (tid < 256) {
+            s.cnt[0][tid] = 0;
+            s.mass[0][tid] = 0;
+        }
+        __syncthreads();
+        for (int i = tid; i < n; i += kSampleThreads) {
+            const float x = xs[i];
+            const int b = bucket0(x, xmax);
+            atomicAdd(&s.cnt[0][b], 1u);
+            atomicAdd(&s.mass[0][b], mass_of(x, xmax));
+        }
+        cl.sync();
+        if (tid < 256) {
+            uint32_t c = 0;
+            unsigned long long m = 0;
+            for (int q = 0; q < kSampleCluster; ++q) {
+                c += cl.map_shared_rank(&s.cnt[0][0], q)[tid];
+                m += cl.map_shared_rank(&s.mass[0][0], q)[tid];
+            }
+            s.cnt0[tid] = c;
+            s.mass0[tid] = m;
+        }
+        __syncthreads();
+        int rc = 1;
+        if (tid < 32) scan_select(s, s.cnt0, s.mass0, true, 1);
+        __syncthreads();
+        const unsigned long long Z = s.total_mass;
+        __syncthreads();
+        // P' = min(top_p * Z, C_{k-1})   (random_util.cu:89-94)
+        unsigned long long P = Z;
+        if (p.top_p < 1.f) {
+            const double tp = (double)p.top_p * (double)Z;
+            P = tp >= 1.0 ? (unsigned long long)tp : 1ull;
+        }
+        if (p.top_k > 1 && p.top_k < V) {
+            const SelResult k = cluster_select(s, cl, xs, n, xmax, false, (unsigned long long)p.top_k, rc);
+            const unsigned long long pos = (unsigned long long)p.top_k - 1 - k.cnt_before;   // position in its tie group
+            const unsigned long long ck = k.mass_before + (k.grp_cnt ? (pos + 1) * (k.grp_mass / k.grp_cnt) : 0);
+            if (ck < P) P = ck;
+        }
+        if (P < 1) P = 1;
+        // target = u * P' with u = m / 2^24, m in [1, 2^24]; rounded up: C_j >= target <=> C_j >= ceil(m P' / 2^24)
+        const uint32_t r = philox_first(p.seed, counter ? (uint32_t)counter[row] : 0u);
+        const unsigned long long m = (unsigned long long)(r >> 8) + 1;
+        const unsigned long long target = m * (P >> 24) + ((m * (P & 0xFFFFFFull) + 0xFFFFFFull) >> 24);
+        const SelResult t = cluster_select(s, cl, xs, n, xmax, true, target, rc);
+        // inside the tie group every element carries the same mass: the pick is its p-th element in index order
+        unsigned long long pgrp = 0;
+        if (t.grp_cnt > 0 && t.grp_mass > 0) {
+            const unsigned long long wt = t.grp_mass / t.grp_cnt;
+            const unsigned long long need = target > t.mass_before ? target - t.mass_before : 1;
+            pgrp = (need + wt - 1) / wt - 1;
+            if (pgrp >= t.grp_cnt) pgrp = t.grp_cnt - 1;
+        }
+        // which CTA holds it: the last round's per-CTA counts of the group's bin, in rank order
+        const int lbuf = (rc - 1) & 1;
+        unsigned long long before = 0;
+        int q_own = kSampleCluster - 1;
+        for (int q = 0; q < kSampleCluster; ++q) {
+            const unsigned long long c = cl.map_shared_rank(&s.cnt[lbuf][0], q)[t.key & 255];
+            if (pgrp < before + c) {
+                q_own = q;
+                break;
+            }
+            before += c;
+        }
+        owner = rank == q_own;
+        tok = -1;
+        if (owner) {
+            const unsigned long long want = pgrp - before;
+            // each thread counts the group's elements in its contiguous chunk; block scan; the owning thread walks
+            const int per = (n + kSampleThreads - 1) / kSampleThreads;
+            const int a = tid * per, e = min(n, a + per);
+            uint32_t c = 0;
+            for (int i = a; i < e; ++i) c += (bucket0(xs[i], xmax) == t.b0 && desc_key(xs[i]) == t.key);
+            unsigned long long inc = c;
+#pragma unroll
+            for (int o = 1; o < 32; o <<= 1) {
+                const unsigned long long v = __shfl_up_sync(0xffffffffu, inc, o);
+                if (lane >= o) inc += v;
+            }
+            if (lane == 31) s.scan[warp] = inc;
+            if (tid == 0) s.tok = -1;
+            __syncthreads();
+            unsigned long long wbase = 0;
+            for (int w = 0; w < warp; ++w) wbase += s.scan[w];
+            const unsigned long long exc = wbase + inc - c;
+            if (c > 0 && want >= exc && want < exc + c) {
+                unsigned long long k = exc;
+                for (int i = a; i < e; ++i) {
+                    if (bucket0(xs[i], xmax) == t.b0 && desc_key(xs[i]) == t.key) {
+                        if (k == want) {
+                            s.tok = lo + i;
+                            break;
+                        }
+                        ++k;
+                    }
+                }
+            }
+            __syncthreads();
+            tok = s.tok >= 0 ? s.tok : greedy_tok;
+        }
+    }
+    if (owner && tid == 0) {
+        out[row] = tok;
+        if (hist) atomicOr(&hist[tok >> 5], 1u << (tok & 31));
+    }
+    cl.sync();   // no CTA leaves while another may still read its shared memory
+}
+
+}  // namespace zl
+
+using namespace zl;
+
+extern "C" unsigned zl_sample_uniform(uint64_t seed, unsigned counter) { return philox_first(seed, counter); }
+
+extern "C" size_t zl_sample_workspace_bytes(int T, int V) {
+    (void)T;
+    (void)V;
+    return 0;
+}
+
+extern "C" int zl_sample_check_params(const zl_sample_params_t* p, int n) {
+    ZL_CHECK_ARG(p && n > 0);
+    for (int i = 0; i < n; ++i) {
+        const zl_sample_params_t& q = p[i];
+        ZL_CHECK_ARG(q.temperature >= 0.f && q.temperature < INFINITY);
+        ZL_CHECK_ARG(q.top_p > 0.f && q.top_p <= 1.f);
+        ZL_CHECK_ARG(q.top_k >= 0);
+        ZL_CHECK_ARG(q.repetition_penalty > 0.f && q.repetition_penalty < INFINITY);
+        ZL_CHECK_ARG(q.presence_penalty > -INFINITY && q.presence_penalty < INFINITY);
+    }
+    return ZL_OK;
+}
+
+int prepare_sample() {
+    static bool done[64] = {};
+    int dev = 0;
+    cudaGetDevice(&dev);
+    if (dev >= 0 && dev < 64 && done[dev]) return ZL_OK;
+    ZL_CHECK_CUDA(cudaFuncSetAttribute(k_sample, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                       kSampleMaxSlice * (int)sizeof(float)));
+    if (dev >= 0 && dev < 64) done[dev] = true;
+    return ZL_OK;
+}
+
+extern "C" int zl_sample(const float* logits, int T, int V, const zl_sample_params_t* params, const int32_t* row_task,
+                         const int32_t* counter, uint32_t* history, int history_words, int32_t* out, void* ws,
+                         size_t ws_bytes, int pdl, zl_stream_t stream) {
+    (void)ws;
+    ZL_CHECK_ARG(logits && params && out && T > 0 && V > 0);
+    ZL_CHECK_SUPPORTED(V <= kSampleMaxVocab);
+    ZL_CHECK_ARG(!history || history_words >= cdiv(V, 32));
+    ZL_CHECK_ARG(ws_bytes >= zl_sample_workspace_bytes(T, V));
+    const int rc = prepare_sample();
+    if (rc != ZL_OK) return rc;
+    const int S = cdiv(V, kSampleCluster);
+    const int ty = T < 65535 ? T : 65535;   // rows: blockIdx.z * gridDim.y + blockIdx.y
+    ZL_CHECK_CUDA(launch(k_sample, dim3(kSampleCluster, ty, cdiv(T, ty)), dim3(kSampleThreads), (size_t)S * sizeof(float),
+                         stream, pdl != 0, logits, T, V, S, params, row_task, counter, history, history_words, out));
+    return ZL_OK;
+}

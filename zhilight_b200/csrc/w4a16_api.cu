@@ -14,6 +14,8 @@
 
 using namespace zl;
 
+int prepare_sample();   // sample.cu
+
 extern "C" int zl_prepare(void) {
     // opt-in shared memory sizes and the per-device split-k workspace of the wgmma kernel must be set up outside of
     // stream capture; idempotent per device
@@ -21,7 +23,7 @@ extern "C" int zl_prepare(void) {
     ZL_CHECK_CUDA(prepare_w4_v3());
     ZL_CHECK_CUDA(prepare_w4_tc());
     ZL_CHECK_CUDA(prepare_w8_tc());
-    return ZL_OK;
+    return prepare_sample();
 }
 
 // ZL_W4_NO_TC=1 (experiments): never route to the wgmma kernel

@@ -95,7 +95,8 @@ class LlamaDecoder:
         return (nxt, logits) if want_logits else nxt
 
     def prefill(self, task, tokens, pos0=0, want_logits=False):
-        """Chunked prefill of one task's prompt; returns the greedy next token [, logits of the last position]."""
+        """Chunked prefill of one task's prompt; returns the next token (greedy, or sampled per set_sampling)
+        [, logits of the last position]."""
         t = np.ascontiguousarray(tokens, dtype=np.int32)
         nxt = np.empty(1, dtype=np.int32)
         logits = np.empty((1, self.vocab_shard), dtype=np.float32) if want_logits else None
@@ -103,6 +104,13 @@ class LlamaDecoder:
             self.h, int(task), t.ctypes.data_as(ctypes.c_void_p), t.size, int(pos0),
             nxt.ctypes.data_as(ctypes.c_void_p), logits.ctypes.data_as(ctypes.c_void_p) if want_logits else None))
         return (int(nxt[0]), logits) if want_logits else int(nxt[0])
+
+    def set_sampling(self, task, temperature=0.0, top_p=1.0, top_k=0, repetition_penalty=1.0, presence_penalty=0.0,
+                     seed=0):
+        """Per-task sampling for the following steps (zl_llama_set_sampling); clears the task's penalty history.
+        The defaults are plain greedy."""
+        p = _lib.sample_params(temperature, top_p, top_k, repetition_penalty, presence_penalty, seed)
+        _lib.check(self.lib.zl_llama_set_sampling(self.h, int(task), ctypes.byref(p)))
 
     def set_state(self, tokens, positions):
         t = np.ascontiguousarray(tokens, dtype=np.int32)

@@ -392,3 +392,30 @@ def argmax(logits):
     ws = torch.empty(nb, dtype=torch.uint8, device=logits.device)
     _lib.call("zl_argmax", _p(logits), _p(out), t, v, _p(ws), nb, 0, _stream())
     return out
+
+
+def sample_params_array(params, n):
+    """Host zl_sample_params_t[n] from one parameter dict (every task) or a list of n dicts / SampleParams;
+    validated with zl_sample_check_params."""
+    if isinstance(params, (dict, _lib.SampleParams)):
+        params = [params] * n
+    if len(params) != n:
+        raise _lib.ZLError(-1, "need %d parameter sets, got %d" % (n, len(params)))
+    arr = (_lib.SampleParams * n)(*[q if isinstance(q, _lib.SampleParams) else _lib.sample_params(**q) for q in params])
+    _lib.call("zl_sample_check_params", ctypes.cast(arr, ctypes.c_void_p), n)
+    return arr
+
+
+def sample(logits, params, row_task=None, counter=None, history=None, pdl=False):
+    """Sampled (or greedy) next token per row of fp32 logits (T, V), zl_sample's contract.  params: one dict of
+    set_sampling's keywords for every row, or one per task (a list); row_task (T) int32 maps rows to tasks (default:
+    row i -> task i); counter (T) int32 (default 0); history (tasks, ceil(V/32)) int32 bitmap, updated in place, or None."""
+    t, v = logits.shape
+    n_tasks = len(params) if isinstance(params, (list, tuple)) else (history.shape[0] if history is not None else t)
+    arr = sample_params_array(params, n_tasks)
+    dparams = torch.frombuffer(bytearray(bytes(arr)), dtype=torch.uint8).to(logits.device)
+    out = torch.empty(t, dtype=torch.int32, device=logits.device)
+    hw = history.shape[1] if history is not None else 0
+    _lib.call("zl_sample", _p(logits), t, v, _p(dparams), _p(row_task), _p(counter), _p(history), hw, _p(out), None, 0,
+              int(pdl), _stream())
+    return out

@@ -125,6 +125,15 @@ int zl_w4a16_gemm(const void* x, int ldx, const void* packed, const void* bias, 
  *                       consumer), | 512 when the step has an ODD number of exchanges (the two slots must alternate across
  *                       step boundaries too); zl_comm_ll_begin_step(tp_comm) must be enqueued once per step before the
  *                       first such GEMM, on every rank.
+ *   k_perm != NULL (act-order / desc_act GPTQ): y = W . x[:, k_perm], K int32 entries.  W is packed from the
+ *                       sequentialised k-major tensors (zl_gptq_shuffle with q_perm = k_perm, the reference's
+ *                       make_sequential, q_gemm.cu:794-829) and the activations are gathered while the integer kernel
+ *                       stages them, where the reference runs permute_input first (gptq/utils.cu:322-398, called at
+ *                       q_gemm_k_major.cu:1094, 1105).  ln_weight keeps the caller's (unpermuted) order: the prologue
+ *                       uses x[k_perm[i]] * ln_weight[k_perm[i]]; the RMS is over the whole row, so the permutation does
+ *                       not change it.  Only the exact-integer route (zl_w4_int_layout_route == 3) takes k_perm: the
+ *                       wgmma and fp16 routes, and tp_mode != 0, return ZL_ERR_UNSUPPORTED (permute x with
+ *                       zl_gather_cols_16 first).
  * bias is indexed by PACKED row. */
 typedef struct zl_comm zl_comm_t;
 typedef struct zl_w4_fused_args {
@@ -137,7 +146,10 @@ typedef struct zl_w4_fused_args {
     const void* prefetch_ptr; size_t prefetch_bytes; /* next kernel's weights: pulled into L2 as this one drains (may be NULL) */
     int variant; /* layout of `packed`: 0 ZLW4, 1 ZLW4I (integer kernel; needs the staged activations to fit smem) */
     zl_comm_t* tp_comm; int tp_mode; void* tp_h_out; int tp_index;
+    const int32_t* k_perm; /* act-order activation permutation (K), or NULL */
 } zl_w4_fused_args_t;
+/* sizeof(zl_w4_fused_args_t) and offsetof(zl_w4_fused_args_t, k_perm), so that bindings can check their mirror. */
+int zl_w4_fused_args_layout(size_t* size, size_t* k_perm_offset);
 int zl_w4a16_gemm_fused(const zl_w4_fused_args_t* args, zl_stream_t stream);
 /* 1 if the exact-integer kernel (variant 1, M <= 16) can run this shape: its staged activations must fit shared memory. */
 int zl_w4_int_kernel_fits(int M, int N, int K);
@@ -169,6 +181,10 @@ int zl_w4_set_trace(void* buf);
 int zl_qkv_rope_row_map(int32_t* row_map, int n_heads_total, int dim_head, zl_stream_t stream);
 /* dst[i] = src[map[i]] for 16-bit elements (bias permutation to packed-row order). */
 int zl_gather_rows_16(const void* src, const int32_t* map, void* dst, int n, zl_stream_t stream);
+/* y[m, i] = x[m, perm[i]] for 16-bit x (M, K) with row stride ldx and y (M, K) dense: the act-order activation permute
+ * (nn::gptq::permute_input, gptq/utils.cu:322-398) for the GEMM routes that read x through TMA and cannot gather.
+ * K % 8 == 0, ldx % 8 == 0, x and y 16-byte aligned.  pdl != 0 -> programmatic dependent launch. */
+int zl_gather_cols_16(const void* x, int ldx, const int32_t* perm, void* y, int M, int K, int pdl, zl_stream_t stream);
 
 /* ---- W8A8 Linear: SmoothQuant INT8 (Int8Linear, src/nn/linear/linear.cpp:432-636) and per-tensor FP8 e4m3
  * (Fp8Linear, linear.cpp:1612-1695) ---------------------------------------------------------------------- */

@@ -53,6 +53,7 @@ class W4FusedArgs(ctypes.Structure):
         ("prefetch_ptr", ctypes.c_void_p), ("prefetch_bytes", ctypes.c_size_t),
         ("variant", ctypes.c_int),
         ("tp_comm", ctypes.c_void_p), ("tp_mode", ctypes.c_int), ("tp_h_out", ctypes.c_void_p), ("tp_index", ctypes.c_int),
+        ("k_perm", ctypes.c_void_p),
     ]
 
 

@@ -368,3 +368,40 @@ extern "C" int zl_w4_unpack(const void* packed, uint32_t* qweight_km, uint8_t* q
                             int N, int K, int group_size, zl_stream_t stream) {
     return zl_w4_unpack_v(packed, qweight_km, qzeros_km, scales_km, N, K, group_size, kW4VariantHalf, stream);
 }
+
+// ---- act-order activation permute: y[m, i] = x[m, perm[i]] (nn::gptq::permute_input, gptq/utils.cu:322-398) -------
+// For the GEMM routes whose activation tiles arrive by TMA and so cannot gather (the integer kernel gathers while it
+// stages).  8 output columns per thread: two 16-byte index loads, eight 2-byte gathers, one 16-byte store.
+namespace zl {
+__global__ void k_gather_cols_16(const uint16_t* __restrict__ x, int ldx, const int32_t* __restrict__ perm,
+                                 uint16_t* __restrict__ y, int K) {
+    pdl_trigger();
+    const int c8 = blockIdx.x * blockDim.x + threadIdx.x;
+    const bool live = c8 * 8 < K;
+    int4 a = make_int4(0, 0, 0, 0), b = a;
+    if (live) {   // the permutation is a constant: load it before waiting on the producer of x
+        a = __ldg(reinterpret_cast<const int4*>(perm) + 2 * c8);
+        b = __ldg(reinterpret_cast<const int4*>(perm) + 2 * c8 + 1);
+    }
+    pdl_wait();
+    if (!live) return;
+    const uint16_t* xr = x + (size_t)blockIdx.y * ldx;
+    uint4 o;
+    o.x = (uint32_t)xr[a.x] | ((uint32_t)xr[a.y] << 16);
+    o.y = (uint32_t)xr[a.z] | ((uint32_t)xr[a.w] << 16);
+    o.z = (uint32_t)xr[b.x] | ((uint32_t)xr[b.y] << 16);
+    o.w = (uint32_t)xr[b.z] | ((uint32_t)xr[b.w] << 16);
+    *reinterpret_cast<uint4*>(y + (size_t)blockIdx.y * K + c8 * 8) = o;
+}
+}  // namespace zl
+
+extern "C" int zl_gather_cols_16(const void* x, int ldx, const int32_t* perm, void* y, int M, int K, int pdl,
+                                 zl_stream_t stream) {
+    ZL_CHECK_ARG(x && perm && y && M > 0 && M <= 65535 && K > 0 && K % 8 == 0 && ldx >= K && ldx % 8 == 0);
+    ZL_CHECK_ARG((reinterpret_cast<uintptr_t>(x) & 15) == 0 && (reinterpret_cast<uintptr_t>(y) & 15) == 0 &&
+                 (reinterpret_cast<uintptr_t>(perm) & 15) == 0);
+    const dim3 grid(zl::cdiv(K / 8, 128), M);
+    ZL_CHECK_CUDA(zl::launch(zl::k_gather_cols_16, grid, dim3(128), 0, (cudaStream_t)stream, pdl != 0,
+                             (const uint16_t*)x, ldx, perm, (uint16_t*)y, K));
+    return ZL_OK;
+}

@@ -32,6 +32,7 @@ struct W4Lin {
     void* packed_i = nullptr;   // ZLW4I (exact-integer IMMA kernel, small M)
     void* bias = nullptr;
     int N = 0, K = 0;
+    int32_t* k_perm = nullptr;  // act-order: the GEMM reads x[:, k_perm] (K int32, device); nullptr: sequential g_idx
 };
 struct DenseLin {
     void* w = nullptr;
@@ -110,6 +111,7 @@ struct zl_llama {
     int32_t* d_tb = nullptr;      // token -> task map of the chunk being prefilled
     const int32_t* cur_tb = nullptr;   // token -> task map of the launch sequence being enqueued (d_iota at decode)
     int8_t* d_mask = nullptr;     // (chunk, max_seq) causal mask of the chunk
+    void* xperm = nullptr;        // act-order: activations permuted for the GEMM routes that cannot gather (tok_cap x max K)
     // sampling (zl_llama_set_sampling): per-task parameters and generated-token bitmaps on the device; samp_on[t] is set
     // while task t samples or has penalties, and the step then runs zl_sample instead of zl_argmax
     zl_sample_params_t* d_sparams = nullptr;   // (max_batch)
@@ -245,43 +247,73 @@ int fail_state(int line, const std::string& msg, int code = ZL_ERR_STATE) {
     return code;
 }
 
-// g_idx of a desc_act / act-order checkpoint is not k / group_size; the reference then gathers rows by argsort(g_idx)
-// and permutes the activations at run time (linear.cpp:1092-1094, 1145-1146, 1168-1210).  The fused kernels here have no
-// run-time activation permute, so such a checkpoint is rejected at load instead of producing garbage.
-int check_g_idx_sequential(zl_llama* m, const std::string& prefix, int K) {
+// g_idx of a desc_act / act-order checkpoint is not k / group_size.  Like the reference (linear.cpp:1092-1094,
+// 1145-1146), the load sorts it into a permutation -- argsort_cpu, a stable bucket sort of k by group
+// (linear.cpp:1010-1028) -- gathers the weight rows with it (zl_gptq_shuffle with q_perm, make_sequential) and the GEMMs
+// read x[:, perm] at run time.  perm is left empty when g_idx is missing or sequential: such Linears load exactly as before.
+int g_idx_perm(zl_llama* m, const std::string& prefix, int K, std::vector<int32_t>* perm) {
+    perm->clear();
     const Staged* gi = find(m, prefix + ".g_idx");
     if (!gi) return ZL_OK;
     if ((size_t)gi->rows * gi->cols != (size_t)K || gi->elem != 4)
         return fail_state(__LINE__, "ill-shaped g_idx for " + prefix + " (expected K int32)");
+    const int g = m->cfg.group_size, G = K / g;
     std::vector<int32_t> host(K);
     ZL_CHECK_CUDA(cudaMemcpyAsync(host.data(), gi->ptr, (size_t)K * 4, cudaMemcpyDeviceToHost, m->stream));
     ZL_CHECK_CUDA(cudaStreamSynchronize(m->stream));
-    for (int k = 0; k < K; ++k)
-        if (host[k] != k / m->cfg.group_size)
-            return fail_state(__LINE__, "act-order (desc_act) GPTQ checkpoint: " + prefix +
-                                            ".g_idx is not sequential; not supported by the fused W4 kernels",
-                              ZL_ERR_UNSUPPORTED);
+    bool sequential = true;
+    for (int k = 0; k < K && sequential; ++k) sequential = host[k] == k / g;
+    if (sequential) return ZL_OK;
+    if (m->cfg.tp_size > 1) {
+        return fail_state(__LINE__, "act-order (desc_act) GPTQ checkpoint (" + prefix + ".g_idx) with tp_size > 1: a rank's "
+                                        "o_proj input shard does not hold the columns its permuted K shard needs",
+                          ZL_ERR_UNSUPPORTED);
+    }
+    // K entries, none past the last group and none in a full group: every group has exactly g members
+    std::vector<int> count(G, 0);
+    perm->assign(K, 0);
+    for (int k = 0; k < K; ++k) {
+        const int grp = host[k];
+        if (grp < 0 || grp >= G || count[grp] >= g) {
+            perm->clear();
+            return fail_state(__LINE__, "malformed g_idx for " + prefix + ": every group of " + std::to_string(g) +
+                                            " columns must appear exactly " + std::to_string(g) + " times",
+                              ZL_ERR_INVALID_ARG);
+        }
+        (*perm)[grp * g + count[grp]++] = k;
+    }
     return ZL_OK;
 }
 
 // HF GPTQ/AWQ tensors of one Linear -> reference k-major tensors written at row offset n_off of the fused
-// k-major buffers (linear.cpp:1139-1160 preprocess_weight + 1085-1099 transpose_weight).
-int to_k_major(zl_llama* m, const std::string& prefix, int K, int N, uint32_t* qw_km, uint8_t* qz_km, __half* sc_km,
-               int n_off, int n_total) {
+// k-major buffers (linear.cpp:1139-1160 preprocess_weight + 1085-1099 transpose_weight).  q_perm (device, K) or nullptr:
+// the act-order permutation the weight rows are gathered with.
+// presence, shape and element size of one Linear's GPTQ/AWQ tensors
+int check_quant_tensors(zl_llama* m, const std::string& prefix, int K, int N) {
     const Staged* qw = find(m, prefix + ".qweight");
     const Staged* qz = find(m, prefix + ".qzeros");
     const Staged* sc = find(m, prefix + ".scales");
     if (!qw || !qz || !sc) return fail_state(__LINE__, "missing GPTQ tensors for " + prefix);
     const int G = K / m->cfg.group_size;
     const bool awq = m->cfg.quant_type == 6;
-    // every shape / element size is validated BEFORE the first kernel touches the tensors (in-place transforms below)
     const bool qw_ok = awq ? (qw->rows == K && qw->cols == N / 8) : (qw->rows == K / 8 && qw->cols == N);
     if (!qw_ok || qw->elem != 4) return fail_state(__LINE__, "ill-shaped qweight for " + prefix, ZL_ERR_INVALID_ARG);
     if (qz->rows != G || qz->cols != N / 8 || qz->elem != 4)
         return fail_state(__LINE__, "ill-shaped qzeros for " + prefix + " (expected (K/g, N/8) int32)", ZL_ERR_INVALID_ARG);
     if (sc->rows != G || sc->cols != N || sc->elem != 2)
         return fail_state(__LINE__, "ill-shaped scales for " + prefix + " (expected (K/g, N) fp16)", ZL_ERR_INVALID_ARG);
-    RCHECK(check_g_idx_sequential(m, prefix, K));
+    return ZL_OK;
+}
+
+int to_k_major(zl_llama* m, const std::string& prefix, int K, int N, uint32_t* qw_km, uint8_t* qz_km, __half* sc_km,
+               int n_off, int n_total, const int32_t* q_perm = nullptr) {
+    // every shape / element size is validated BEFORE the first kernel touches the tensors (in-place transforms below)
+    RCHECK(check_quant_tensors(m, prefix, K, N));
+    const Staged* qw = find(m, prefix + ".qweight");
+    const Staged* qz = find(m, prefix + ".qzeros");
+    const Staged* sc = find(m, prefix + ".scales");
+    const int G = K / m->cfg.group_size;
+    const bool awq = m->cfg.quant_type == 6;
     cudaStream_t st = m->stream;
     DevTmp tmp;
     uint32_t* w_kn = nullptr;   // (K/8, N)
@@ -291,7 +323,9 @@ int to_k_major(zl_llama* m, const std::string& prefix, int K, int N, uint32_t* q
         RCHECK(zl_awq_un_shuffle((uint32_t*)qz->ptr, G, N / 8, st));
     } else {
         w_kn = (uint32_t*)qw->ptr;
-        RCHECK(zl_gptq_shuffle(w_kn, nullptr, nullptr, K, N, st));
+        uint32_t* scratch = nullptr;
+        if (q_perm) RCHECK(tmp.alloc((void**)&scratch, (size_t)(K / 8) * N * 4));
+        RCHECK(zl_gptq_shuffle(w_kn, q_perm, scratch, K, N, st));
         RCHECK(zl_gptq_increase_zero((uint32_t*)qz->ptr, (size_t)G * (N / 8), st));
     }
     uint8_t* z8 = nullptr;   // (G, N)
@@ -306,8 +340,10 @@ int to_k_major(zl_llama* m, const std::string& prefix, int K, int N, uint32_t* q
     return ZL_OK;
 }
 
+// out_rows (swiglu only, act-order w_out): w_out's permutation, folded into the gate / up row order.
+// keep_perm = false: the weight rows are sequentialised but the GEMM runs without k_perm (its producer wrote x permuted).
 int build_w4(zl_llama* m, const std::vector<std::string>& prefixes, const std::vector<int>& ns, int K, bool swiglu,
-             W4Lin* out, bool qkv_rope = false) {
+             W4Lin* out, bool qkv_rope = false, const std::vector<int32_t>* out_rows = nullptr, bool keep_perm = true) {
     int N = 0;
     for (int n : ns) N += n;
     const int G = K / m->cfg.group_size;
@@ -315,18 +351,54 @@ int build_w4(zl_llama* m, const std::vector<std::string>& prefixes, const std::v
     uint8_t* qz_km = nullptr;
     __half* sc_km = nullptr;
     DevTmp tmp;   // released on every exit path
+    // act-order: Linears fused along N share their input, so they must share its permutation.  Real checkpoints give
+    // q / k / v (and gate / up) the same g_idx: their GPTQ Hessian is that of the same input.
+    std::vector<int32_t> perm, other;
+    for (size_t i = 0; i < prefixes.size(); ++i) {
+        RCHECK(check_quant_tensors(m, prefixes[i], K, ns[i]));   // the errors of a Linear keep their order
+        RCHECK(g_idx_perm(m, prefixes[i], K, i ? &other : &perm));
+        if (i && other != perm)
+            return fail_state(__LINE__, "act-order g_idx of " + prefixes[i] + " differs from " + prefixes[0] +
+                                            ": Linears fused on one input need one permutation",
+                              ZL_ERR_UNSUPPORTED);
+    }
+    if (!perm.empty() && m->cfg.quant_type == 6)
+        return fail_state(__LINE__, "non-sequential g_idx on an AWQ checkpoint: " + prefixes[0], ZL_ERR_UNSUPPORTED);
+    int32_t* d_perm = nullptr;
+    if (!perm.empty()) {
+        if (keep_perm) {
+            RCHECK(dmalloc((void**)&out->k_perm, (size_t)K * 4));
+            d_perm = out->k_perm;
+        } else {
+            RCHECK(tmp.alloc((void**)&d_perm, (size_t)K * 4));
+        }
+        ZL_CHECK_CUDA(cudaMemcpyAsync(d_perm, perm.data(), (size_t)K * 4, cudaMemcpyHostToDevice, m->stream));
+    }
     RCHECK(tmp.alloc((void**)&qw_km, (size_t)N * (K / 8) * 4));
     RCHECK(tmp.alloc((void**)&qz_km, (size_t)N * G));
     RCHECK(tmp.alloc((void**)&sc_km, (size_t)N * G * 2));
     int off = 0;
     bool any_bias = false;
     for (size_t i = 0; i < prefixes.size(); ++i) {
-        RCHECK(to_k_major(m, prefixes[i], K, ns[i], qw_km, qz_km, sc_km, off, N));
+        RCHECK(to_k_major(m, prefixes[i], K, ns[i], qw_km, qz_km, sc_km, off, N, d_perm));
         if (find(m, prefixes[i] + ".bias")) any_bias = true;
         off += ns[i];
     }
     int32_t* row_map = nullptr;
-    if (swiglu) {
+    if (swiglu && out_rows && !out_rows->empty()) {
+        // PERMUTE_FF_UP_OUT (linear.cpp:1168-1210): gate row j and up row j of the pack (still interleaved 8 + 8 per
+        // 16-row tile for the SwiGLU epilogue) come from source row out_rows[j], so the SwiGLU output is already in
+        // w_out's sequentialised k order and the down GEMM needs no permute
+        const int F = N / 2;
+        std::vector<int32_t> h(N);
+        for (int p = 0; p < N; ++p) {
+            const int r = p & 15;
+            h[p] = (r < 8 ? 0 : F) + (*out_rows)[(p >> 4) * 8 + (r & 7)];
+        }
+        RCHECK(tmp.alloc((void**)&row_map, (size_t)N * 4));
+        ZL_CHECK_CUDA(cudaMemcpyAsync(row_map, h.data(), (size_t)N * 4, cudaMemcpyHostToDevice, m->stream));
+        ZL_CHECK_CUDA(cudaStreamSynchronize(m->stream));   // h is pageable and goes out of scope
+    } else if (swiglu) {
         RCHECK(tmp.alloc((void**)&row_map, (size_t)N * 4));
         k_swiglu_row_map<<<cdiv(N, 256), 256, 0, m->stream>>>(row_map, N / 2);
         ZL_CHECK_LAUNCH();
@@ -524,10 +596,14 @@ int finalize_layer(zl_llama* m, int l) {
     const std::vector<std::string> gu = {p + "ff.w_in", p + "ff.w_gated"};
     const std::vector<int> gu_n = {m->ff, m->ff};
     if (c.quant_type == 5 || c.quant_type == 6) {
+        // act-order w_out: its permutation orders the gate / up rows, so down runs without one.  A bad w_out g_idx is
+        // reported by its own build_w4 below, after the errors of the Linears built before it.
+        std::vector<int32_t> down_perm;
+        if (g_idx_perm(m, p + "ff.w_out", m->ff, &down_perm) != ZL_OK) down_perm.clear();
         RCHECK(build_w4(m, qkv, qkv_n, D, false, &L.q_qkv, c.fuse >= 2));
         RCHECK(build_w4(m, {p + "attn.attn_out"}, {D}, m->hq * d, false, &L.q_o));
-        RCHECK(build_w4(m, gu, gu_n, D, true, &L.q_gu));
-        RCHECK(build_w4(m, {p + "ff.w_out"}, {D}, m->ff, false, &L.q_down));
+        RCHECK(build_w4(m, gu, gu_n, D, true, &L.q_gu, false, &down_perm));
+        RCHECK(build_w4(m, {p + "ff.w_out"}, {D}, m->ff, false, &L.q_down, false, nullptr, false));
     } else if (c.quant_type == 7) {
         RCHECK(build_fp8(m, qkv, qkv_n, D, &L.d_qkv));
         RCHECK(build_fp8(m, {p + "attn.attn_out"}, {D}, m->hq * d, &L.d_o));
@@ -588,6 +664,9 @@ int alloc_runtime(zl_llama* m) {
     RCHECK(dmalloc(&m->ao, (size_t)T * m->hq * d * 2));
     RCHECK(dmalloc(&m->gu, (size_t)T * 2 * m->ff * 2));
     RCHECK(dmalloc(&m->act, (size_t)T * m->ff * 2));
+    bool act_order = false;
+    for (const auto& L : m->layers) act_order |= L.q_qkv.k_perm || L.q_o.k_perm || L.q_gu.k_perm;
+    if (act_order) RCHECK(dmalloc(&m->xperm, (size_t)T * (D > m->hq * d ? D : m->hq * d) * 2));
     RCHECK(dmalloc((void**)&m->logits, (size_t)B * c.vocab_size * 4));
     RCHECK(dmalloc(&m->cand, (size_t)((B * 8 + 15) / 16) * 16));
     RCHECK(dmalloc(&m->cand_all, (size_t)((B * 8 + 15) / 16) * 16 * c.tp_size));
@@ -710,14 +789,22 @@ int w4_gemm(zl_llama* m, const void* x, int ldx, const W4Lin& w, const void* res
     const bool use_int = route != 0;
     a.packed = use_int ? w.packed_i : w.packed;
     a.variant = use_int ? 1 : 0;
-    if (route == 4 && ln_w) {
+    if ((route == 4 || (w.k_perm && route != 3)) && ln_w) {
         // the wgmma kernel reads x through the TMA engine: the RMSNorm runs as its own kernel (reference order,
-        // block.cpp:125,131) into the matching rows of xn
+        // block.cpp:125,131) into the matching rows of xn.  So does an act-order GEMM that is not gathered while staged.
         const size_t off = (const char*)x - (const char*)m->h;
         void* xn = (char*)m->xn + off;
         RCHECK(zl_rmsnorm(x, ln_w, xn, B, w.K, c.eps, 1.f, c.dtype, force_no_pdl ? 0 : c.use_pdl, m->stream));
         a.x = xn;
         ln_w = nullptr;
+    }
+    if (w.k_perm && route == 3) {
+        a.k_perm = w.k_perm;   // gathered while the integer kernel stages x
+    } else if (w.k_perm) {
+        // the other routes read x in tiles: permute it first (permute_input, gptq/utils.cu:322-398)
+        RCHECK(zl_gather_cols_16(a.x, a.ldx, w.k_perm, m->xperm, B, w.K, force_no_pdl ? 0 : c.use_pdl, m->stream));
+        a.x = m->xperm;
+        a.ldx = w.K;
     }
     W4L2Head l2;
     if (layer >= 0 && route == 3 && (l2_head_depth() > 0 || l2_whole_max() > 0)) {
@@ -1163,14 +1250,15 @@ extern "C" void zl_llama_destroy(zl_llama_t* m) {
     for (auto& s : m->staged) cudaFree(s.second.ptr);
     for (auto& L : m->layers) {
         for (void* p : {L.ln_attn, L.ln_ff, L.q_qkv.packed, L.q_qkv.bias, L.q_o.packed, L.q_o.bias, L.q_gu.packed,
-                        L.q_down.packed, L.q_down.bias, L.q_qkv.packed_i, L.q_o.packed_i, L.q_gu.packed_i, L.q_down.packed_i, L.d_qkv.w, L.d_qkv.bias, L.d_o.w, L.d_o.bias, L.d_gu.w,
+                        L.q_down.packed, L.q_down.bias, (void*)L.q_qkv.k_perm, (void*)L.q_o.k_perm, (void*)L.q_gu.k_perm,
+                        (void*)L.q_down.k_perm, L.q_qkv.packed_i, L.q_o.packed_i, L.q_gu.packed_i, L.q_down.packed_i, L.d_qkv.w, L.d_qkv.bias, L.d_o.w, L.d_o.bias, L.d_gu.w,
                         L.d_gu.bias, L.d_down.w, L.d_down.bias, L.d_qkv.w8, L.d_qkv.w_scale, L.d_o.w8, L.d_o.w_scale, L.d_gu.w8, L.d_gu.w_scale, L.d_down.w8, L.d_down.w_scale, L.kbuf, L.vbuf, (void*)L.k_addrs, (void*)L.v_addrs})
             if (p) cudaFree(p);
     }
     for (void* p : {m->emb, m->lm_head_tied ? nullptr : m->lm_head, m->ln_f, m->h, m->xn, m->qkv, m->q, m->ao, m->act,
                     m->pend, m->gu, (void*)m->logits, (void*)m->cosb, (void*)m->sinb, (void*)m->d_tokens,
                     m->h2, (void*)m->d_pos, (void*)m->d_lens, (void*)m->d_next, (void*)m->d_iota, m->attn_ws, m->argmax_ws, (void*)m->d_tb, (void*)m->d_mask, m->xq, (void*)m->xs,
-                    (void*)m->d_hist, (void*)m->d_sparams})
+                    (void*)m->d_hist, (void*)m->d_sparams, m->xperm})
         if (p) cudaFree(p);
     if (m->reduce_stream) {
         cudaStreamSynchronize(m->reduce_stream);

@@ -51,6 +51,8 @@ struct W4Params {
     int tp_mode = 0;
     int tp_index = 0;              // exchange index within the step (< 512): parity of the slot + part of the word tag
     __half* tp_h_out = nullptr;
+    // act-order: the staging loop reads x[k_perm[i]] and ln_w[k_perm[i]] (integer kernel only; zl_w4_fused_args_t.k_perm)
+    const int32_t* k_perm = nullptr;
 };
 
 // zl_w4a16_gemm_fused with the L2 head of the successor GEMM as a descriptor (l2 == nullptr: the public whole-range

@@ -93,6 +93,13 @@ extern "C" int zl_w4a16_gemm_fused(const zl_w4_fused_args_t* a, zl_stream_t stre
     return zl::w4a16_gemm_fused_l2(a, nullptr, stream);
 }
 
+extern "C" int zl_w4_fused_args_layout(size_t* size, size_t* k_perm_offset) {
+    ZL_CHECK_ARG(size && k_perm_offset);
+    *size = sizeof(zl_w4_fused_args_t);
+    *k_perm_offset = offsetof(zl_w4_fused_args_t, k_perm);
+    return ZL_OK;
+}
+
 int zl::w4a16_gemm_fused_l2(const zl_w4_fused_args_t* a, const W4L2Head* l2, zl_stream_t stream) {
     {
         static bool prepared[64] = {};
@@ -115,6 +122,8 @@ int zl::w4a16_gemm_fused_l2(const zl_w4_fused_args_t* a, const W4L2Head* l2, zl_
     ZL_CHECK_ARG(a->epilogue == ZL_EPI_QKV_ROPE || a->y != nullptr || a->tp_mode == 2);
     ZL_CHECK_ARG(a->ln_weight == nullptr || (reinterpret_cast<uintptr_t>(a->ln_weight) & 15) == 0);
     ZL_CHECK_ARG((reinterpret_cast<uintptr_t>(a->prefetch_ptr) & 15) == 0);
+    ZL_CHECK_ARG((reinterpret_cast<uintptr_t>(a->k_perm) & 15) == 0);
+    ZL_CHECK_SUPPORTED(!(a->k_perm && a->tp_mode != 0) && "k_perm (act-order) is not combined with tp_mode");
     if (a->epilogue == ZL_EPI_QKV_ROPE) {
         ZL_CHECK_ARG(a->cos && a->sin && a->q_out && a->token_batch && a->placement && a->k_addrs && a->v_addrs);
         ZL_CHECK_ARG(a->num_heads > 0 && a->num_kv_heads > 0 && a->dim_head > 0);
@@ -145,6 +154,8 @@ int zl::w4a16_gemm_fused_l2(const zl_w4_fused_args_t* a, const W4L2Head* l2, zl_
     const int route = a->variant == kW4VariantInt ? int_layout_route(a->M, a->N, a->K) : 2;
     ZL_CHECK_SUPPORTED(route != 0 && "ZLW4I layout: M > 16 (or staged activations too large) and N % 128 != 0: use variant 0");
     ZL_CHECK_SUPPORTED(!(route == 4 && a->ln_weight) && "the wgmma kernel has no fused RMSNorm prologue: run zl_rmsnorm first");
+    ZL_CHECK_SUPPORTED(!(route != 3 && a->k_perm) &&
+                       "only the exact-integer kernel gathers k_perm: permute x with zl_gather_cols_16 first");
     const int step = route == 4 ? 256 : 32;
     for (int m0 = 0; m0 < a->M; m0 += step) {
         W4Params p;
@@ -184,6 +195,7 @@ int zl::w4a16_gemm_fused_l2(const zl_w4_fused_args_t* a, const W4L2Head* l2, zl_
         p.tp_mode = a->tp_mode;
         p.tp_index = a->tp_index;
         p.tp_h_out = static_cast<__half*>(a->tp_h_out);
+        p.k_perm = a->k_perm;
         if (l2) {
             p.l2 = *l2;
         } else if (a->prefetch_ptr && a->prefetch_bytes) {

@@ -176,15 +176,54 @@ __device__ __forceinline__ void pack_blocks(const W4Params& p, const uint8_t* ri
     }
 }
 
+// act-order: the 4 source columns of lane's k in group gi, one 16-byte load (an L1 hit after the first token)
+__device__ __forceinline__ int4 v3_k_src(const int32_t* k_perm, int gi, int lane) {
+    return __ldg(reinterpret_cast<const int4*>(k_perm + gi * kW4GroupK + lane * 4));
+}
+
+// act-order: out[gl] = the 4 fp16 src[k_perm[k]] of lane's k in group warp + gl * WT.  The row is first copied coalesced
+// into shared memory -- elements k < K/2 into row_hi, the rest into row_lo (K bytes each: a token's own, not yet written
+// staging rows) -- and the scattered reads go there.  Read straight from global memory, every CTA sent 16x the L2 requests
+// of the contiguous loads, all to the same few lines, and batch-1 decode ran at half speed.  Called by every thread.
+template <int WT, int NG>
+__device__ __forceinline__ void v3_gather_row(const __half* src, int K, const int32_t* k_perm, uint8_t* row_hi,
+                                              uint8_t* row_lo, int warp, int lane, uint2 (&out)[NG]) {
+    const int half = K / 2, G = K / kW4GroupK;
+    for (int e = threadIdx.x * 4; e < K; e += WT * 32 * 4)   // K / 2 is a multiple of 64: 4 elements never straddle it
+        *reinterpret_cast<uint2*>(e < half ? row_hi + e * 2 : row_lo + (e - half) * 2) = ld_cg_u2(src + e);
+    __syncthreads();
+    auto at = [&](int i) -> uint32_t {
+        return *reinterpret_cast<const uint16_t*>(i < half ? row_hi + i * 2 : row_lo + (i - half) * 2);
+    };
+#pragma unroll
+    for (int gl = 0; gl < NG; ++gl) {
+        const int gi = warp + gl * WT;
+        if (gi < G) {
+            const int4 ix = v3_k_src(k_perm, gi, lane);
+            out[gl] = make_uint2(at(ix.x) | (at(ix.y) << 16), at(ix.z) | (at(ix.w) << 16));
+        }
+    }
+    __syncthreads();   // every lane holds its values before the rows are overwritten
+}
+
 // PACK (mc <= 4): the MMA N dimension (8 columns) is mostly padding at tiny batch, so the two 8-bit digits of the
 // 16-bit activation mantissas share ONE IMMA: column 2i carries token i's high digit, column 2i+1 its low digit, both
 // signed (m = 256*hi' + lo', lo' = int8(m & 0xff), hi' = (m + 128) >> 8, |m| <= 2^14).  Half the IMMAs, half the B
 // loads, and the per-group int->float epilogue only touches real tokens.
-template <int NT, bool NORM, int WARPS, int SUBS, int STAGES, int RT = NT * 8, bool PACK = false, int TPX = 0>
+//
+// GATHER (act-order, p.k_perm != nullptr): the staging loop reads x[k_perm[k]] instead of x[k], and the RMSNorm weights
+// ln_w[k_perm[k]], so W may be the sequentialised weight of a desc_act checkpoint.  The reference permutes x in a kernel
+// of its own first (permute_input, gptq/utils.cu:322-398); here the activations are read once either way, so the gather
+// costs no launch and no extra pass over x: each token's row is read coalesced into shared memory and permuted from
+// there (v3_gather_row).  The RMSNorm weights are gathered the same way before pdl_wait (they and k_perm are constants).
+template <int NT, bool NORM, int WARPS, int SUBS, int STAGES, int RT = NT * 8, bool PACK = false, int TPX = 0,
+          bool GATHER = false>
 __global__ void __launch_bounds__(WARPS * SUBS * 32, 1) k_w4a16_v3(const W4Params p) {
     using S = V3Smem<NT, WARPS, SUBS, STAGES, RT>;
     // the tensor-parallel exchange code is compiled only into the TPX instantiations: carried as a run-time branch it cost
-    // every launch 10-20 registers (to the 128-register cap of the 512-thread CTA) and ~5 % of a single-GPU decode step
+    // every launch 10-20 registers (to the 128-register cap of the 512-thread CTA) and ~5 % of a single-GPU decode step.
+    // The act-order gather is a template flag for the same reason.
+    static_assert(!(GATHER && TPX), "act-order gather and tensor-parallel exchange are not combined");
     constexpr int tp_mode = TPX;   // 0 none, 1 reduce-in while staging, 2 push from the epilogue (== p.tp_mode, checked by the launcher)
     constexpr int WT = WARPS * SUBS;
     extern __shared__ __align__(128) uint8_t smem[];
@@ -270,7 +309,9 @@ __global__ void __launch_bounds__(WARPS * SUBS * 32, 1) k_w4a16_v3(const W4Param
     // staging assignment: group gi -> warp gi % WT.  RMSNorm weights are constants: fetch them before the wait.
     constexpr int kMaxNg = 8;   // groups per warp kept in registers during staging (K <= 8*WT*128)
     uint2 lnw[kMaxNg];
-    if (NORM) {
+    if constexpr (GATHER) {
+        if (NORM) v3_gather_row<WT>(p.ln_w, p.K, p.k_perm, xs_hi, xs_lo, warp, lane, lnw);   // staging rows of token 0
+    } else if (NORM) {
 #pragma unroll
         for (int gl = 0; gl < kMaxNg; ++gl) {
             const int gi = warp + gl * WT;
@@ -309,10 +350,15 @@ __global__ void __launch_bounds__(WARPS * SUBS * 32, 1) k_w4a16_v3(const W4Param
     // ---- stage the activations as block-floating-point integers, once per CTA ----
     for (int tok = 0; tok < p.mc; ++tok) {
         uint2 raw[kMaxNg];
+        if constexpr (GATHER) {
+            v3_gather_row<WT>(p.x + (size_t)tok * p.ldx, p.K, p.k_perm, xs_hi + tok * row_b, xs_lo + tok * row_b, warp, lane,
+                              raw);
+        } else {
 #pragma unroll
-        for (int gl = 0; gl < kMaxNg; ++gl) {
-            const int gi = warp + gl * WT;
-            if (gi < G) raw[gl] = ld_cg_u2(p.x + (size_t)tok * p.ldx + gi * kW4GroupK + lane * 4);
+            for (int gl = 0; gl < kMaxNg; ++gl) {
+                const int gi = warp + gl * WT;
+                if (gi < G) raw[gl] = ld_cg_u2(p.x + (size_t)tok * p.ldx + gi * kW4GroupK + lane * 4);
+            }
         }
         if (tp_mode == 1) {
             // x := T(T(sum_r partial_r) + x): fp32 sum in rank order (identical on every rank and CTA), the reference's
@@ -727,6 +773,9 @@ static cudaError_t launch_v3_t(const W4Params& params, const V3Plan& pl, bool pd
             return cudaErrorNotSupported;
         }
     }
+    if (p.k_perm)   // act-order (the front end rejects k_perm with tp_mode)
+        return launch(k_w4a16_v3<NT, NORM, WARPS, SUBS, STAGES, RT, PACK, 0, true>, grid, block, (size_t)pl.smem, stream, pdl,
+                      p);
     return launch(k_w4a16_v3<NT, NORM, WARPS, SUBS, STAGES, RT, PACK>, grid, block, (size_t)pl.smem, stream, pdl, p);
 }
 
@@ -893,22 +942,29 @@ bool w4_v3_fits(int mc, int N, int K) {
     return false;
 }
 
+// opt-in shared memory of one single-GPU variant, with and without the act-order gather
+template <int NT, bool NORM, int W, int SB, int ST, int RT = NT * 8, bool PK = false>
+static cudaError_t v3_set_smem() {
+    cudaError_t e = cudaFuncSetAttribute(k_w4a16_v3<NT, NORM, W, SB, ST, RT, PK>,
+                                         cudaFuncAttributeMaxDynamicSharedMemorySize, kV3Budget);
+    if (e != cudaSuccess) return e;
+    return cudaFuncSetAttribute(k_w4a16_v3<NT, NORM, W, SB, ST, RT, PK, 0, true>,
+                                cudaFuncAttributeMaxDynamicSharedMemorySize, kV3Budget);
+}
+
 cudaError_t prepare_w4_v3() {
     cudaError_t e;
 #define ZL_SET(NT, NORM, W, SB, ST)                                                                            \
-    e = cudaFuncSetAttribute(k_w4a16_v3<NT, NORM, W, SB, ST>, cudaFuncAttributeMaxDynamicSharedMemorySize,      \
-                             kV3Budget);                                                                        \
+    e = v3_set_smem<NT, NORM, W, SB, ST>();                                                                    \
     if (e != cudaSuccess) return e;
 #define ZL_SET1(NORM, W, SB, ST)                                                                               \
-    e = cudaFuncSetAttribute(k_w4a16_v3<1, NORM, W, SB, ST, 8, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, \
-                             kV3Budget);                                                                        \
+    e = v3_set_smem<1, NORM, W, SB, ST, 8, true>();                                                            \
     if (e != cudaSuccess) return e;
     ZL_SET1(false, 8, 2, 5) ZL_SET1(true, 8, 2, 5) ZL_SET1(false, 8, 2, 4) ZL_SET1(true, 8, 2, 4)
     ZL_SET1(false, 16, 1, 4) ZL_SET1(true, 16, 1, 4)
 #undef ZL_SET1
 #define ZL_SET2(NORM, W, SB, ST)                                                                               \
-    e = cudaFuncSetAttribute(k_w4a16_v3<1, NORM, W, SB, ST, 2>, cudaFuncAttributeMaxDynamicSharedMemorySize,    \
-                             kV3Budget);                                                                        \
+    e = v3_set_smem<1, NORM, W, SB, ST, 2>();                                                                  \
     if (e != cudaSuccess) return e;
     ZL_SET2(false, 16, 1, 6) ZL_SET2(true, 16, 1, 6) ZL_SET2(false, 16, 1, 5) ZL_SET2(true, 16, 1, 5)
     ZL_SET2(false, 8, 2, 6) ZL_SET2(true, 8, 2, 6)

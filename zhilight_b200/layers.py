@@ -58,10 +58,15 @@ class Linear:
         else:
             is_awq = q == QUANT_AWQ
             g_idx = sd.get("g_idx")
+            self._k_perm = None
             if g_idx is not None and not torch.equal(g_idx.cpu().int(),
                                                      (torch.arange(k) // self.group_size).int()):
-                raise _lib.ZLError(-3, "act-order (desc_act) checkpoints are not supported on the H100 path")
-            qw, qz, sc = ops.gptq_to_k_major(sd["qweight"].int(), sd["qzeros"].int(), sd["scales"].half(), is_awq)
+                if q != QUANT_GPTQ:   # Marlin refuses act-order like the reference (linear.cpp:1418); AWQ has no g_idx
+                    raise _lib.ZLError(-3, "act-order (desc_act) checkpoints are only supported with QuantType 5")
+                qw, qz, sc, self._k_perm = ops.gptq_to_k_major_act_order(
+                    sd["qweight"].int(), sd["qzeros"].int(), sd["scales"].half(), g_idx, self.group_size)
+            else:
+                qw, qz, sc = ops.gptq_to_k_major(sd["qweight"].int(), sd["qzeros"].int(), sd["scales"].half(), is_awq)
             self._p = {"qweight": qw, "qzeros": qz, "scales": sc}
             variant = 1 if _lib.load().zl_w4_int_kernel_fits(32, n, k) else 0
             self._packed = ops.w4_pack(qw, qz, sc, self.group_size, self.sym, None, variant)
@@ -90,7 +95,11 @@ class Linear:
         elif q == QUANT_FP8:
             y = ops.fp8_linear(x2, self._p["weight"], self._p["weight_scale"], self.bias)
         else:
-            y = ops.w4a16_gemm_fused(x2, self._packed, n, k, self.group_size, bias=self.bias, variant=self._variant)
+            kp = self._k_perm
+            if kp is not None and not (self._variant == 1 and _lib.load().zl_w4_int_layout_route(x2.shape[0], n, k) == 3):
+                x2, kp = ops.gather_cols(x2, kp), None   # only the integer kernel gathers while it stages x
+            y = ops.w4a16_gemm_fused(x2, self._packed, n, k, self.group_size, bias=self.bias, variant=self._variant,
+                                     k_perm=kp)
         if self.activation:
             y = ops.activation(y, self.activation)
         return y.reshape(*x.shape[:-1], n)

@@ -95,6 +95,48 @@ def gptq_to_k_major(qweight, qzeros, scales, is_awq=False):
     return transpose_2d(qw), transpose_2d(z8), transpose_2d(scales.contiguous())
 
 
+def act_order_perm(g_idx, group_size=128):
+    """The act-order permutation of a desc_act checkpoint's g_idx (host int32 tensor, K), or None when g_idx is
+    sequential.  Same order as the reference's argsort_cpu (linear.cpp:1010-1028): a stable bucket sort of k by group."""
+    gi = torch.as_tensor(g_idx).cpu().to(torch.int64).reshape(-1)
+    k = gi.numel()
+    if torch.equal(gi, torch.arange(k) // group_size):
+        return None
+    if k % group_size or gi.min() < 0 or gi.max() >= k // group_size or \
+            not bool((torch.bincount(gi, minlength=k // group_size) == group_size).all()):
+        raise _lib.ZLError(-1, "malformed g_idx: every group of %d columns must appear exactly %d times"
+                           % (group_size, group_size))
+    return torch.sort(gi, stable=True).indices.to(torch.int32)
+
+
+def gptq_to_k_major_act_order(qweight, qzeros, scales, g_idx, group_size=128):
+    """gptq_to_k_major for a GPTQ checkpoint that may be act-order: returns (qweight_km, qzeros_km, scales_km, k_perm),
+    the k-major tensors sequentialised with k_perm (make_sequential, q_gemm.cu:794-829) and k_perm itself (K int32 on the
+    weights' device), or k_perm = None for a sequential g_idx.  A GEMM on these weights takes x[:, k_perm]."""
+    perm = act_order_perm(g_idx, group_size) if g_idx is not None else None
+    if perm is None:
+        return gptq_to_k_major(qweight, qzeros, scales) + (None,)
+    perm = perm.to(qweight.device)
+    qw = gptq_shuffle(qweight.clone(), perm)
+    z8 = q4_to_q8(gptq_increase_zero(qzeros.clone()))
+    return transpose_2d(qw), transpose_2d(z8), transpose_2d(scales.contiguous()), perm
+
+
+def gather_cols(x, perm, pdl=False):
+    """zl_gather_cols_16: y[m, i] = x[m, perm[i]] for a 16-bit x (M, K) with unit column stride; perm (K) int32."""
+    if x.element_size() != 2 or not x.is_floating_point():
+        raise _lib.ZLError(-2, "gather_cols needs a 16-bit float x, got %s" % x.dtype)
+    if x.dim() != 2 or x.stride(1) != 1:
+        raise _lib.ZLError(-1, "gather_cols needs a 2-D x with unit column stride")
+    if perm.dtype != torch.int32 or perm.numel() != x.shape[1]:
+        raise _lib.ZLError(-1, "gather_cols needs perm as K int32 entries")
+    m, k = x.shape
+    y = torch.empty((m, k), dtype=x.dtype, device=x.device)
+    _lib.call("zl_gather_cols_16", ctypes.c_void_p(x.data_ptr()), x.stride(0), _p(perm), _p(y), m, k, int(pdl),
+              _stream())
+    return y
+
+
 def gptq_dequant_k_major(qweight_km, qzeros_km, scales_km):
     n, k8 = qweight_km.shape
     g = scales_km.shape[1]
@@ -163,9 +205,10 @@ def gather_rows_16(src, row_map):
 
 
 def w4a16_gemm_fused(x, packed, n, k, group_size=128, bias=None, residual=None, epilogue=EPI_NONE, pdl=False, out=None,
-                     ln_weight=None, eps=1e-5, rope=None, variant=0):
+                     ln_weight=None, eps=1e-5, rope=None, variant=0, k_perm=None):
     """zl_w4a16_gemm_fused.  rope = dict(cos, sin, token_batch, placement, k_bufs, v_bufs, num_heads, num_kv_heads,
-    dim_head) for EPI_QKV_ROPE (returns q); bias must be in packed-row order."""
+    dim_head) for EPI_QKV_ROPE (returns q); bias must be in packed-row order.  k_perm (K int32, act-order): y = W . x[:, k_perm]
+    with W packed from the sequentialised weights (exact-integer route only; elsewhere gather_cols first)."""
     if x.dtype != torch.float16:
         raise _lib.ZLError(-2, "A must be half")
     m = x.shape[0]
@@ -174,6 +217,7 @@ def w4a16_gemm_fused(x, packed, n, k, group_size=128, bias=None, residual=None, 
     a.M, a.N, a.K, a.group_size, a.epilogue, a.pdl = m, n, k, group_size, epilogue, int(pdl)
     a.ln_weight, a.eps = _dp(ln_weight), eps
     a.variant = int(variant)
+    a.k_perm = _dp(k_perm)
     keep = []
     if epilogue == EPI_QKV_ROPE:
         r = rope

@@ -8,7 +8,6 @@ for l in sys.stdin:
 "; }
 run "default" ""
 ZL_DENSE_NO_PDL=1 run "dense no pdl" ""
-ZL_DEBUG_SKIP=32 run "skip lm_head" ""
 run "no-graph" "--no-graph"
 run "no-pdl (whole step)" "--no-pdl"
 timeout 120 python tools/microbench.py 2>/dev/null | grep -i "dense\|lm_head" | head -5

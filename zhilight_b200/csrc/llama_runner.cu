@@ -14,6 +14,7 @@
 #include <cstdlib>
 #include <cstring>
 #include <map>
+#include <memory>
 #include <utility>
 #include <string>
 #include <vector>
@@ -22,37 +23,49 @@ extern unsigned long long* g_w4_trace;   // debug timeline buffer (zl_w4_set_tra
 
 namespace {
 
+// owning handles: device memory (cudaMalloc) and pinned host memory (cudaMallocHost)
+struct CudaFree {
+    void operator()(void* p) const { cudaFree(p); }
+};
+struct CudaFreeHost {
+    void operator()(void* p) const { cudaFreeHost(p); }
+};
+template <typename T = void>
+using dev_ptr = std::unique_ptr<T, CudaFree>;
+template <typename T>
+using host_ptr = std::unique_ptr<T, CudaFreeHost>;
+
 struct Staged {
-    void* ptr = nullptr;
+    dev_ptr<> ptr;
     int rows = 0, cols = 0, elem = 0;
 };
 
 struct W4Lin {
-    void* packed = nullptr;     // ZLW4  (fp16 HMMA kernels) -- only kept when some batch size needs it
-    void* packed_i = nullptr;   // ZLW4I (exact-integer IMMA kernel, small M)
-    void* bias = nullptr;
+    dev_ptr<> packed;     // ZLW4  (fp16 HMMA kernels) -- only kept when some batch size needs it
+    dev_ptr<> packed_i;   // ZLW4I (exact-integer IMMA kernel, small M)
+    dev_ptr<> bias;
     int N = 0, K = 0;
-    int32_t* k_perm = nullptr;  // act-order: the GEMM reads x[:, k_perm] (K int32, device); nullptr: sequential g_idx
+    dev_ptr<int32_t> k_perm;   // act-order: the GEMM reads x[:, k_perm] (K int32); empty: sequential g_idx
 };
 struct DenseLin {
-    void* w = nullptr;
-    void* bias = nullptr;
+    dev_ptr<> w;
+    dev_ptr<> bias;
     int N = 0, K = 0;
     // W8A8 (quant_type 2 / 7): 8-bit weights (N, K) + per-row scales; w is released
-    void* w8 = nullptr;
-    void* w_scale = nullptr;   // int8: (N) in the activation dtype (linear.cpp:541); fp8: (N) f32 rows
-    int w8_kind = -1;          // ZL_W8_INT8 or ZL_W8_FP8_ROWS
+    dev_ptr<> w8;
+    dev_ptr<> w_scale;   // int8: (N) in the activation dtype (linear.cpp:541); fp8: (N) f32 rows
+    int w8_kind = -1;    // ZL_W8_INT8 or ZL_W8_FP8_ROWS
 };
 
 struct Layer {
-    void* ln_attn = nullptr;
-    void* ln_ff = nullptr;
+    dev_ptr<> ln_attn;
+    dev_ptr<> ln_ff;
     W4Lin q_qkv, q_o, q_gu, q_down;
     DenseLin d_qkv, d_o, d_gu, d_down;
-    void* kbuf = nullptr;   // (max_batch, max_seq, Hkv, d)
-    void* vbuf = nullptr;
-    void** k_addrs = nullptr;   // device (max_batch)
-    void** v_addrs = nullptr;
+    dev_ptr<> kbuf;   // (max_batch, max_seq, Hkv, d)
+    dev_ptr<> vbuf;
+    dev_ptr<void*> k_addrs;   // (max_batch)
+    dev_ptr<void*> v_addrs;
 };
 
 }  // namespace
@@ -62,40 +75,39 @@ struct zl_llama {
     cudaStream_t stream = nullptr;
     std::map<std::string, Staged> staged;
     std::vector<Layer> layers;
-    void* emb = nullptr;
-    void* lm_head = nullptr;
-    void* ln_f = nullptr;
-    bool lm_head_tied = false;
+    dev_ptr<> emb;
+    dev_ptr<> lm_head_shard;        // untied lm_head (this rank's vocabulary rows)
+    const void* lm_head = nullptr;  // lm_head_shard, or emb when tied
+    dev_ptr<> ln_f;
     bool finalized = false;
     // local (per-rank) sizes
     int hq = 0, hkv = 0, ff = 0;
     // activations
-    void* h2 = nullptr;   // second residual-stream buffer: the fused TP exchange ping-pongs between h and h2
-    void *h = nullptr, *xn = nullptr, *qkv = nullptr, *q = nullptr, *ao = nullptr, *act = nullptr,
-         *pend = nullptr, *gu = nullptr;
-    float* logits = nullptr;
-    float *cosb = nullptr, *sinb = nullptr;
-    int32_t *d_tokens = nullptr, *d_pos = nullptr, *d_lens = nullptr, *d_next = nullptr, *d_iota = nullptr;
-    void* attn_ws = nullptr;
+    dev_ptr<> h2;   // second residual-stream buffer: the fused TP exchange ping-pongs between h and h2
+    dev_ptr<> h, xn, qkv, q, ao, act, pend, gu;
+    dev_ptr<float> logits;
+    dev_ptr<float> cosb, sinb;
+    dev_ptr<int32_t> d_tokens, d_pos, d_lens, d_next, d_iota;
+    dev_ptr<> attn_ws;
     size_t attn_ws_bytes = 0;
-    void* argmax_ws = nullptr;
-    int32_t* h_stage = nullptr;   // pinned: tokens | pos | lens | next
+    dev_ptr<> argmax_ws;
+    host_ptr<int32_t> h_stage;   // tokens | pos | lens | next
     // zl_llama_set_state staging: pinned H2D copies read the host buffer when they EXECUTE, so a set_state -> step_device
     // loop that runs ahead of the GPU must not rewrite a slot whose copy is still queued: ring of slots, one event each
     static constexpr int kStageSlots = 8;
-    int32_t* h_ring = nullptr;    // pinned [kStageSlots][2 * max_batch]
+    host_ptr<int32_t> h_ring;    // [kStageSlots][2 * max_batch]
     cudaEvent_t ring_ev[kStageSlots] = {};
     bool ring_used[kStageSlots] = {};
     int ring_next = 0;
     // prefill keeps its own (token, position) arrays: the decode-state arrays d_tokens / d_pos of tasks 0..B-1 survive a
     // prefill that happens between two zl_llama_step_device calls (continuous batching)
-    int32_t *d_pf_tokens = nullptr, *d_pf_pos = nullptr;
+    dev_ptr<int32_t> d_pf_tokens, d_pf_pos;
     const int32_t* cur_pos = nullptr;      // positions of the launch sequence being enqueued (d_pos or d_pf_pos)
     const int32_t* cur_tokens = nullptr;
     zl_comm_t* comm = nullptr;            // TP exchange (set by zl_llama_set_comm when tp_size > 1)
     int vshard = 0;                       // vocabulary rows of lm_head held by this rank
-    void* cand = nullptr;                 // [B] {float value, int index} local argmax candidates
-    void* cand_all = nullptr;             // [tp][B] gathered candidates
+    dev_ptr<> cand;                       // [B] {float value, int index} local argmax candidates
+    dev_ptr<> cand_all;                   // [tp][B] gathered candidates
     std::map<long long, cudaGraphExec_t> graphs;   // key = B * 2^32 + attention length bucket
     int cur_max_len = 0;                            // host-side upper bound of buf_lens (positions + 1)
     double weight_bytes = 0;
@@ -106,16 +118,16 @@ struct zl_llama {
     cudaStream_t reduce_stream = nullptr;
     cudaEvent_t ev_o[2] = {nullptr, nullptr}, ev_r1[2] = {nullptr, nullptr}, ev_dn[2] = {nullptr, nullptr},
                 ev_r2[2] = {nullptr, nullptr};
-    void* xq = nullptr;           // W8A8: quantised activations of the Linear being run (tok_cap x max K bytes)
-    float* xs = nullptr;          //       their scales (tok_cap)
-    int32_t* d_tb = nullptr;      // token -> task map of the chunk being prefilled
+    dev_ptr<> xq;              // W8A8: quantised activations of the Linear being run (tok_cap x max K bytes)
+    dev_ptr<float> xs;         //       their scales (tok_cap)
+    dev_ptr<int32_t> d_tb;     // token -> task map of the chunk being prefilled
     const int32_t* cur_tb = nullptr;   // token -> task map of the launch sequence being enqueued (d_iota at decode)
-    int8_t* d_mask = nullptr;     // (chunk, max_seq) causal mask of the chunk
-    void* xperm = nullptr;        // act-order: activations permuted for the GEMM routes that cannot gather (tok_cap x max K)
+    dev_ptr<int8_t> d_mask;    // (chunk, max_seq) causal mask of the chunk
+    dev_ptr<> xperm;           // act-order: activations permuted for the GEMM routes that cannot gather (tok_cap x max K)
     // sampling (zl_llama_set_sampling): per-task parameters and generated-token bitmaps on the device; samp_on[t] is set
     // while task t samples or has penalties, and the step then runs zl_sample instead of zl_argmax
-    zl_sample_params_t* d_sparams = nullptr;   // (max_batch)
-    uint32_t* d_hist = nullptr;                // (max_batch, hwords)
+    dev_ptr<zl_sample_params_t> d_sparams;   // (max_batch)
+    dev_ptr<uint32_t> d_hist;                // (max_batch, hwords)
     int hwords = 0;
     std::vector<char> samp_on;
 };
@@ -130,10 +142,11 @@ using namespace zl;
         if (_rc != ZL_OK) return _rc; \
     } while (0)
 
-
-
-int dmalloc(void** p, size_t bytes) {
-    ZL_CHECK_CUDA(cudaMalloc(p, bytes ? bytes : 16));
+template <typename T>
+int dmalloc(dev_ptr<T>* p, size_t bytes) {
+    void* raw = nullptr;
+    ZL_CHECK_CUDA(cudaMalloc(&raw, bytes ? bytes : 16));
+    p->reset(static_cast<T*>(raw));
     return ZL_OK;
 }
 
@@ -220,27 +233,7 @@ const Staged* find(const zl_llama* m, const std::string& name) {
     return it == m->staged.end() ? nullptr : &it->second;
 }
 
-void drop(zl_llama* m, const std::string& name) {
-    auto it = m->staged.find(name);
-    if (it != m->staged.end()) {
-        cudaFree(it->second.ptr);
-        m->staged.erase(it);
-    }
-}
-
-// frees device temporaries on every exit path of a load helper
-struct DevTmp {
-    std::vector<void*> ptrs;
-    ~DevTmp() {
-        for (void* p : ptrs)
-            if (p) cudaFree(p);
-    }
-    int alloc(void** p, size_t bytes) {
-        int rc = dmalloc(p, bytes);
-        if (rc == ZL_OK) ptrs.push_back(*p);
-        return rc;
-    }
-};
+void drop(zl_llama* m, const std::string& name) { m->staged.erase(name); }
 
 int fail_state(int line, const std::string& msg, int code = ZL_ERR_STATE) {
     zl_set_last_error(__FILE__, line, msg.c_str());
@@ -259,7 +252,7 @@ int g_idx_perm(zl_llama* m, const std::string& prefix, int K, std::vector<int32_
         return fail_state(__LINE__, "ill-shaped g_idx for " + prefix + " (expected K int32)");
     const int g = m->cfg.group_size, G = K / g;
     std::vector<int32_t> host(K);
-    ZL_CHECK_CUDA(cudaMemcpyAsync(host.data(), gi->ptr, (size_t)K * 4, cudaMemcpyDeviceToHost, m->stream));
+    ZL_CHECK_CUDA(cudaMemcpyAsync(host.data(), gi->ptr.get(), (size_t)K * 4, cudaMemcpyDeviceToHost, m->stream));
     ZL_CHECK_CUDA(cudaStreamSynchronize(m->stream));
     bool sequential = true;
     for (int k = 0; k < K && sequential; ++k) sequential = host[k] == k / g;
@@ -285,9 +278,6 @@ int g_idx_perm(zl_llama* m, const std::string& prefix, int K, std::vector<int32_
     return ZL_OK;
 }
 
-// HF GPTQ/AWQ tensors of one Linear -> reference k-major tensors written at row offset n_off of the fused
-// k-major buffers (linear.cpp:1139-1160 preprocess_weight + 1085-1099 transpose_weight).  q_perm (device, K) or nullptr:
-// the act-order permutation the weight rows are gathered with.
 // presence, shape and element size of one Linear's GPTQ/AWQ tensors
 int check_quant_tensors(zl_llama* m, const std::string& prefix, int K, int N) {
     const Staged* qw = find(m, prefix + ".qweight");
@@ -305,8 +295,11 @@ int check_quant_tensors(zl_llama* m, const std::string& prefix, int K, int N) {
     return ZL_OK;
 }
 
+// HF GPTQ/AWQ tensors of one Linear -> reference k-major tensors written at row offset n_off of the fused
+// k-major buffers (linear.cpp:1139-1160 preprocess_weight + 1085-1099 transpose_weight).  q_perm (device, K) or nullptr:
+// the act-order permutation the weight rows are gathered with.
 int to_k_major(zl_llama* m, const std::string& prefix, int K, int N, uint32_t* qw_km, uint8_t* qz_km, __half* sc_km,
-               int n_off, int n_total, const int32_t* q_perm = nullptr) {
+               int n_off, const int32_t* q_perm = nullptr) {
     // every shape / element size is validated BEFORE the first kernel touches the tensors (in-place transforms below)
     RCHECK(check_quant_tensors(m, prefix, K, N));
     const Staged* qw = find(m, prefix + ".qweight");
@@ -315,28 +308,63 @@ int to_k_major(zl_llama* m, const std::string& prefix, int K, int N, uint32_t* q
     const int G = K / m->cfg.group_size;
     const bool awq = m->cfg.quant_type == 6;
     cudaStream_t st = m->stream;
-    DevTmp tmp;
+    uint32_t* qz_p = static_cast<uint32_t*>(qz->ptr.get());
+    dev_ptr<uint32_t> tmp;   // AWQ: the un-shuffled weight; act-order GPTQ: the gather's scratch
     uint32_t* w_kn = nullptr;   // (K/8, N)
     if (awq) {
-        RCHECK(tmp.alloc((void**)&w_kn, (size_t)(K / 8) * N * 4));
-        RCHECK(zl_awq_shuffle((const uint32_t*)qw->ptr, w_kn, K, N, 1, st));
-        RCHECK(zl_awq_un_shuffle((uint32_t*)qz->ptr, G, N / 8, st));
+        RCHECK(dmalloc(&tmp, (size_t)(K / 8) * N * 4));
+        w_kn = tmp.get();
+        RCHECK(zl_awq_shuffle(static_cast<const uint32_t*>(qw->ptr.get()), w_kn, K, N, 1, st));
+        RCHECK(zl_awq_un_shuffle(qz_p, G, N / 8, st));
     } else {
-        w_kn = (uint32_t*)qw->ptr;
-        uint32_t* scratch = nullptr;
-        if (q_perm) RCHECK(tmp.alloc((void**)&scratch, (size_t)(K / 8) * N * 4));
-        RCHECK(zl_gptq_shuffle(w_kn, q_perm, scratch, K, N, st));
-        RCHECK(zl_gptq_increase_zero((uint32_t*)qz->ptr, (size_t)G * (N / 8), st));
+        w_kn = static_cast<uint32_t*>(qw->ptr.get());
+        if (q_perm) RCHECK(dmalloc(&tmp, (size_t)(K / 8) * N * 4));
+        RCHECK(zl_gptq_shuffle(w_kn, q_perm, tmp.get(), K, N, st));
+        RCHECK(zl_gptq_increase_zero(qz_p, (size_t)G * (N / 8), st));
     }
-    uint8_t* z8 = nullptr;   // (G, N)
-    RCHECK(tmp.alloc((void**)&z8, (size_t)G * N));
-    RCHECK(zl_q4_to_q8((const uint32_t*)qz->ptr, z8, (size_t)G * (N / 8), st));
+    dev_ptr<uint8_t> z8;   // (G, N)
+    RCHECK(dmalloc(&z8, (size_t)G * N));
+    RCHECK(zl_q4_to_q8(qz_p, z8.get(), (size_t)G * (N / 8), st));
     // transposes straight into the fused buffers (row offset n_off)
     RCHECK(zl_transpose_2d(w_kn, qw_km + (size_t)n_off * (K / 8), K / 8, N, 4, st));
-    RCHECK(zl_transpose_2d(z8, qz_km + (size_t)n_off * G, G, N, 1, st));
-    RCHECK(zl_transpose_2d(sc->ptr, sc_km + (size_t)n_off * G, G, N, 2, st));
+    RCHECK(zl_transpose_2d(z8.get(), qz_km + (size_t)n_off * G, G, N, 1, st));
+    RCHECK(zl_transpose_2d(sc->ptr.get(), sc_km + (size_t)n_off * G, G, N, 2, st));
     ZL_CHECK_CUDA(cudaStreamSynchronize(st));
-    (void)n_total;
+    return ZL_OK;
+}
+
+// ZL_W4_FORCE_HALF (A/B baseline): every W4 GEMM takes the fp16 mma.sync route.  Read once per process.
+bool force_half() {
+    static const bool v = getenv("ZL_W4_FORCE_HALF") != nullptr;
+    return v;
+}
+
+// The kernel that serves a W4 Linear at B rows: 3 exact-integer, 4 wgmma, 0 fp16 mma.sync.
+int route_of(const W4Lin& w, int B) { return w.packed_i && !force_half() ? zl_w4_int_layout_route(B, w.N, w.K) : 0; }
+
+// The (N) fp16 bias of Linears fused along N: zeros, with each present `prefix.bias` at its row offset.  *out stays
+// empty when none has one.  Every staged bias is checked before the first copy.
+int build_bias(zl_llama* m, const std::vector<std::string>& prefixes, const std::vector<int>& ns, dev_ptr<>* out) {
+    int N = 0;
+    bool any = false;
+    for (size_t i = 0; i < prefixes.size(); ++i) {
+        const Staged* b = find(m, prefixes[i] + ".bias");
+        if (b && ((size_t)b->rows * b->cols != (size_t)ns[i] || b->elem != 2))
+            return fail_state(__LINE__, "ill-shaped bias " + prefixes[i] + ".bias (expected " + std::to_string(ns[i]) +
+                                            " fp16)", ZL_ERR_INVALID_ARG);
+        any |= b != nullptr;
+        N += ns[i];
+    }
+    if (!any) return ZL_OK;
+    RCHECK(dmalloc(out, (size_t)N * 2));
+    ZL_CHECK_CUDA(cudaMemsetAsync(out->get(), 0, (size_t)N * 2, m->stream));
+    int off = 0;
+    for (size_t i = 0; i < prefixes.size(); ++i) {
+        if (const Staged* b = find(m, prefixes[i] + ".bias"))
+            ZL_CHECK_CUDA(cudaMemcpyAsync((char*)out->get() + (size_t)off * 2, b->ptr.get(), (size_t)ns[i] * 2,
+                                          cudaMemcpyDeviceToDevice, m->stream));
+        off += ns[i];
+    }
     return ZL_OK;
 }
 
@@ -347,10 +375,6 @@ int build_w4(zl_llama* m, const std::vector<std::string>& prefixes, const std::v
     int N = 0;
     for (int n : ns) N += n;
     const int G = K / m->cfg.group_size;
-    uint32_t* qw_km = nullptr;
-    uint8_t* qz_km = nullptr;
-    __half* sc_km = nullptr;
-    DevTmp tmp;   // released on every exit path
     // act-order: Linears fused along N share their input, so they must share its permutation.  Real checkpoints give
     // q / k / v (and gate / up) the same g_idx: their GPTQ Hessian is that of the same input.
     std::vector<int32_t> perm, other;
@@ -364,27 +388,24 @@ int build_w4(zl_llama* m, const std::vector<std::string>& prefixes, const std::v
     }
     if (!perm.empty() && m->cfg.quant_type == 6)
         return fail_state(__LINE__, "non-sequential g_idx on an AWQ checkpoint: " + prefixes[0], ZL_ERR_UNSUPPORTED);
-    int32_t* d_perm = nullptr;
+    dev_ptr<int32_t> perm_tmp;   // keep_perm = false: the permutation only serves the weight gather
+    dev_ptr<int32_t>& d_perm = keep_perm ? out->k_perm : perm_tmp;
     if (!perm.empty()) {
-        if (keep_perm) {
-            RCHECK(dmalloc((void**)&out->k_perm, (size_t)K * 4));
-            d_perm = out->k_perm;
-        } else {
-            RCHECK(tmp.alloc((void**)&d_perm, (size_t)K * 4));
-        }
-        ZL_CHECK_CUDA(cudaMemcpyAsync(d_perm, perm.data(), (size_t)K * 4, cudaMemcpyHostToDevice, m->stream));
+        RCHECK(dmalloc(&d_perm, (size_t)K * 4));
+        ZL_CHECK_CUDA(cudaMemcpyAsync(d_perm.get(), perm.data(), (size_t)K * 4, cudaMemcpyHostToDevice, m->stream));
     }
-    RCHECK(tmp.alloc((void**)&qw_km, (size_t)N * (K / 8) * 4));
-    RCHECK(tmp.alloc((void**)&qz_km, (size_t)N * G));
-    RCHECK(tmp.alloc((void**)&sc_km, (size_t)N * G * 2));
+    dev_ptr<uint32_t> qw_km;
+    dev_ptr<uint8_t> qz_km;
+    dev_ptr<__half> sc_km;
+    RCHECK(dmalloc(&qw_km, (size_t)N * (K / 8) * 4));
+    RCHECK(dmalloc(&qz_km, (size_t)N * G));
+    RCHECK(dmalloc(&sc_km, (size_t)N * G * 2));
     int off = 0;
-    bool any_bias = false;
     for (size_t i = 0; i < prefixes.size(); ++i) {
-        RCHECK(to_k_major(m, prefixes[i], K, ns[i], qw_km, qz_km, sc_km, off, N, d_perm));
-        if (find(m, prefixes[i] + ".bias")) any_bias = true;
+        RCHECK(to_k_major(m, prefixes[i], K, ns[i], qw_km.get(), qz_km.get(), sc_km.get(), off, d_perm.get()));
         off += ns[i];
     }
-    int32_t* row_map = nullptr;
+    dev_ptr<int32_t> row_map;
     if (swiglu && out_rows && !out_rows->empty()) {
         // PERMUTE_FF_UP_OUT (linear.cpp:1168-1210): gate row j and up row j of the pack (still interleaved 8 + 8 per
         // 16-row tile for the SwiGLU epilogue) come from source row out_rows[j], so the SwiGLU output is already in
@@ -395,54 +416,41 @@ int build_w4(zl_llama* m, const std::vector<std::string>& prefixes, const std::v
             const int r = p & 15;
             h[p] = (r < 8 ? 0 : F) + (*out_rows)[(p >> 4) * 8 + (r & 7)];
         }
-        RCHECK(tmp.alloc((void**)&row_map, (size_t)N * 4));
-        ZL_CHECK_CUDA(cudaMemcpyAsync(row_map, h.data(), (size_t)N * 4, cudaMemcpyHostToDevice, m->stream));
+        RCHECK(dmalloc(&row_map, (size_t)N * 4));
+        ZL_CHECK_CUDA(cudaMemcpyAsync(row_map.get(), h.data(), (size_t)N * 4, cudaMemcpyHostToDevice, m->stream));
         ZL_CHECK_CUDA(cudaStreamSynchronize(m->stream));   // h is pageable and goes out of scope
     } else if (swiglu) {
-        RCHECK(tmp.alloc((void**)&row_map, (size_t)N * 4));
-        k_swiglu_row_map<<<cdiv(N, 256), 256, 0, m->stream>>>(row_map, N / 2);
+        RCHECK(dmalloc(&row_map, (size_t)N * 4));
+        k_swiglu_row_map<<<cdiv(N, 256), 256, 0, m->stream>>>(row_map.get(), N / 2);
         ZL_CHECK_LAUNCH();
     } else if (qkv_rope) {
-        RCHECK(tmp.alloc((void**)&row_map, (size_t)N * 4));
-        RCHECK(zl_qkv_rope_row_map(row_map, N / m->cfg.dim_head, m->cfg.dim_head, m->stream));
+        RCHECK(dmalloc(&row_map, (size_t)N * 4));
+        RCHECK(zl_qkv_rope_row_map(row_map.get(), N / m->cfg.dim_head, m->cfg.dim_head, m->stream));
     }
     const size_t pbytes = zl_w4_packed_bytes(N, K, m->cfg.group_size);
     ZL_CHECK_SUPPORTED(pbytes > 0);
     // the ZLW4I layout serves the exact-integer kernel (M <= 16 when its staged activations fit) and the wgmma kernel
     // (any M, N % 128 == 0); the fp16 mma.sync layout is only materialised when some launch size has neither
     const int m_max = m->cfg.prefill_chunk > m->cfg.max_batch ? m->cfg.prefill_chunk : m->cfg.max_batch;
-    bool need_half = getenv("ZL_W4_FORCE_HALF") != nullptr;
+    bool need_half = force_half();
     for (int mm = 1; mm <= (m_max < 17 ? m_max : 17); ++mm)
         if (!zl_w4_int_layout_route(mm, N, K)) need_half = true;
     RCHECK(dmalloc(&out->packed_i, pbytes));
-    RCHECK(zl_w4_pack_v(qw_km, qz_km, sc_km, row_map, out->packed_i, N, K, m->cfg.group_size, m->cfg.sym, 1,
-                        m->stream));
+    RCHECK(zl_w4_pack_v(qw_km.get(), qz_km.get(), sc_km.get(), row_map.get(), out->packed_i.get(), N, K,
+                        m->cfg.group_size, m->cfg.sym, 1, m->stream));
     if (need_half) {
         RCHECK(dmalloc(&out->packed, pbytes));
-        RCHECK(zl_w4_pack_v(qw_km, qz_km, sc_km, row_map, out->packed, N, K, m->cfg.group_size, m->cfg.sym, 0,
-                            m->stream));
+        RCHECK(zl_w4_pack_v(qw_km.get(), qz_km.get(), sc_km.get(), row_map.get(), out->packed.get(), N, K,
+                            m->cfg.group_size, m->cfg.sym, 0, m->stream));
     }
-    if (any_bias && !swiglu) {
-        RCHECK(dmalloc(&out->bias, (size_t)N * 2));
-        ZL_CHECK_CUDA(cudaMemsetAsync(out->bias, 0, (size_t)N * 2, m->stream));
-        off = 0;
-        for (size_t i = 0; i < prefixes.size(); ++i) {
-            const Staged* b = find(m, prefixes[i] + ".bias");
-            if (b) {
-                if ((size_t)b->rows * b->cols != (size_t)ns[i] || b->elem != 2)
-                    return fail_state(__LINE__, "ill-shaped bias for " + prefixes[i], ZL_ERR_INVALID_ARG);
-                ZL_CHECK_CUDA(cudaMemcpyAsync((char*)out->bias + (size_t)off * 2, b->ptr, (size_t)ns[i] * 2,
-                                              cudaMemcpyDeviceToDevice, m->stream));
-            }
-            off += ns[i];
-        }
-        if (row_map) {   // the fused epilogues index bias by packed row
-            void* pb = nullptr;
+    if (!swiglu) {
+        RCHECK(build_bias(m, prefixes, ns, &out->bias));
+        if (out->bias && row_map) {   // the fused epilogues index bias by packed row
+            dev_ptr<> pb;
             RCHECK(dmalloc(&pb, (size_t)N * 2));
-            RCHECK(zl_gather_rows_16(out->bias, row_map, pb, N, m->stream));
+            RCHECK(zl_gather_rows_16(out->bias.get(), row_map.get(), pb.get(), N, m->stream));
             ZL_CHECK_CUDA(cudaStreamSynchronize(m->stream));
-            cudaFree(out->bias);
-            out->bias = pb;
+            out->bias = std::move(pb);
         }
     }
     ZL_CHECK_CUDA(cudaStreamSynchronize(m->stream));
@@ -465,30 +473,17 @@ int build_dense(zl_llama* m, const std::vector<std::string>& prefixes, const std
     for (int n : ns) N += n;
     RCHECK(dmalloc(&out->w, (size_t)N * K * 2));
     int off = 0;
-    bool any_bias = false;
     for (size_t i = 0; i < prefixes.size(); ++i) {
         const Staged* w = find(m, prefixes[i] + ".weight");
         if (!w || w->rows != ns[i] || w->cols != K || w->elem != 2) {
             zl_set_last_error(__FILE__, __LINE__, ("missing/ill-shaped dense weight " + prefixes[i]).c_str());
             return ZL_ERR_STATE;
         }
-        ZL_CHECK_CUDA(cudaMemcpyAsync((char*)out->w + (size_t)off * K * 2, w->ptr, (size_t)ns[i] * K * 2,
+        ZL_CHECK_CUDA(cudaMemcpyAsync((char*)out->w.get() + (size_t)off * K * 2, w->ptr.get(), (size_t)ns[i] * K * 2,
                                       cudaMemcpyDeviceToDevice, m->stream));
-        if (find(m, prefixes[i] + ".bias")) any_bias = true;
         off += ns[i];
     }
-    if (any_bias) {
-        RCHECK(dmalloc(&out->bias, (size_t)N * 2));
-        ZL_CHECK_CUDA(cudaMemsetAsync(out->bias, 0, (size_t)N * 2, m->stream));
-        off = 0;
-        for (size_t i = 0; i < prefixes.size(); ++i) {
-            const Staged* b = find(m, prefixes[i] + ".bias");
-            if (b)
-                ZL_CHECK_CUDA(cudaMemcpyAsync((char*)out->bias + (size_t)off * 2, b->ptr, (size_t)ns[i] * 2,
-                                              cudaMemcpyDeviceToDevice, m->stream));
-            off += ns[i];
-        }
-    }
+    RCHECK(build_bias(m, prefixes, ns, &out->bias));
     ZL_CHECK_CUDA(cudaStreamSynchronize(m->stream));
     for (auto& p : prefixes) {
         drop(m, p + ".weight");
@@ -504,20 +499,19 @@ int build_dense(zl_llama* m, const std::vector<std::string>& prefixes, const std
 // as the activations; the scale is kept in the activation dtype (functions::typecast, linear.cpp:541).
 int dense_to_int8(zl_llama* m, DenseLin* d) {
     const auto& c = m->cfg;
-    float* sf = nullptr;
+    dev_ptr<float> sf;
     RCHECK(dmalloc(&d->w8, (size_t)d->N * d->K));
-    RCHECK(dmalloc((void**)&sf, (size_t)d->N * 4));
+    RCHECK(dmalloc(&sf, (size_t)d->N * 4));
     RCHECK(dmalloc(&d->w_scale, (size_t)d->N * 2));
-    RCHECK(zl_int8_quant_per_token(d->w, d->K, d->w8, sf, d->N, d->K, c.dtype, 0, m->stream));
+    RCHECK(zl_int8_quant_per_token(d->w.get(), d->K, d->w8.get(), sf.get(), d->N, d->K, c.dtype, 0, m->stream));
     if (c.dtype == ZL_F16)
-        k_f32_to_t<__half><<<cdiv(d->N, 256), 256, 0, m->stream>>>(sf, static_cast<__half*>(d->w_scale), d->N);
+        k_f32_to_t<__half><<<cdiv(d->N, 256), 256, 0, m->stream>>>(sf.get(), static_cast<__half*>(d->w_scale.get()), d->N);
     else
-        k_f32_to_t<__nv_bfloat16><<<cdiv(d->N, 256), 256, 0, m->stream>>>(sf, static_cast<__nv_bfloat16*>(d->w_scale), d->N);
+        k_f32_to_t<__nv_bfloat16><<<cdiv(d->N, 256), 256, 0, m->stream>>>(
+            sf.get(), static_cast<__nv_bfloat16*>(d->w_scale.get()), d->N);
     ZL_CHECK_LAUNCH();
     ZL_CHECK_CUDA(cudaStreamSynchronize(m->stream));
-    cudaFree(sf);
-    cudaFree(d->w);
-    d->w = nullptr;
+    d->w.reset();
     d->w8_kind = ZL_W8_INT8;
     m->weight_bytes += (double)d->N * d->K + (double)d->N * 2 - (double)d->N * d->K * 2;
     return ZL_OK;
@@ -531,7 +525,6 @@ int build_fp8(zl_llama* m, const std::vector<std::string>& prefixes, const std::
     RCHECK(dmalloc(&out->w8, (size_t)N * K));
     RCHECK(dmalloc(&out->w_scale, (size_t)N * 4));
     int off = 0;
-    bool any_bias = false;
     for (size_t i = 0; i < prefixes.size(); ++i) {
         const Staged* w = find(m, prefixes[i] + ".weight");
         const Staged* ws = find(m, prefixes[i] + ".weight_scale");
@@ -539,26 +532,14 @@ int build_fp8(zl_llama* m, const std::vector<std::string>& prefixes, const std::
             zl_set_last_error(__FILE__, __LINE__, ("missing/ill-shaped fp8 weight or weight_scale " + prefixes[i]).c_str());
             return ZL_ERR_STATE;
         }
-        ZL_CHECK_CUDA(cudaMemcpyAsync((char*)out->w8 + (size_t)off * K, w->ptr, (size_t)ns[i] * K, cudaMemcpyDeviceToDevice,
-                                      m->stream));
-        k_fill_from_scalar<<<cdiv(ns[i], 256), 256, 0, m->stream>>>(static_cast<float*>(out->w_scale) + off, ns[i],
-                                                                     static_cast<const float*>(ws->ptr));
+        ZL_CHECK_CUDA(cudaMemcpyAsync((char*)out->w8.get() + (size_t)off * K, w->ptr.get(), (size_t)ns[i] * K,
+                                      cudaMemcpyDeviceToDevice, m->stream));
+        k_fill_from_scalar<<<cdiv(ns[i], 256), 256, 0, m->stream>>>(static_cast<float*>(out->w_scale.get()) + off, ns[i],
+                                                                     static_cast<const float*>(ws->ptr.get()));
         ZL_CHECK_LAUNCH();
-        if (find(m, prefixes[i] + ".bias")) any_bias = true;
         off += ns[i];
     }
-    if (any_bias) {
-        RCHECK(dmalloc(&out->bias, (size_t)N * 2));
-        ZL_CHECK_CUDA(cudaMemsetAsync(out->bias, 0, (size_t)N * 2, m->stream));
-        off = 0;
-        for (size_t i = 0; i < prefixes.size(); ++i) {
-            const Staged* b = find(m, prefixes[i] + ".bias");
-            if (b)
-                ZL_CHECK_CUDA(cudaMemcpyAsync((char*)out->bias + (size_t)off * 2, b->ptr, (size_t)ns[i] * 2,
-                                              cudaMemcpyDeviceToDevice, m->stream));
-            off += ns[i];
-        }
-    }
+    RCHECK(build_bias(m, prefixes, ns, &out->bias));
     ZL_CHECK_CUDA(cudaStreamSynchronize(m->stream));
     for (auto& p : prefixes) {
         drop(m, p + ".weight");
@@ -572,13 +553,13 @@ int build_fp8(zl_llama* m, const std::vector<std::string>& prefixes, const std::
     return ZL_OK;
 }
 
-int take_vector(zl_llama* m, const std::string& name, int n, void** out) {
+int take_vector(zl_llama* m, const std::string& name, int n, dev_ptr<>* out) {
     auto it = m->staged.find(name);
     if (it == m->staged.end() || (size_t)it->second.rows * it->second.cols != (size_t)n || it->second.elem != 2) {
         zl_set_last_error(__FILE__, __LINE__, ("missing/ill-shaped tensor " + name).c_str());
         return ZL_ERR_STATE;
     }
-    *out = it->second.ptr;
+    *out = std::move(it->second.ptr);
     m->staged.erase(it);
     m->weight_bytes += (double)n * 2;
     return ZL_OK;
@@ -626,11 +607,11 @@ int finalize_globals(zl_llama* m) {
     m->weight_bytes -= (double)c.vocab_size * c.dim_model * 2;   // the embedding table is gathered, not streamed
     RCHECK(take_vector(m, "output_layernorm.weight", c.dim_model, &m->ln_f));
     if (find(m, "lm_head.weight")) {
-        RCHECK(take_vector(m, "lm_head.weight", m->vshard * c.dim_model, &m->lm_head));   // vocab-parallel shard
+        RCHECK(take_vector(m, "lm_head.weight", m->vshard * c.dim_model, &m->lm_head_shard));   // vocab-parallel shard
+        m->lm_head = m->lm_head_shard.get();
     } else {
         ZL_CHECK_SUPPORTED(c.tp_size == 1);   // tied lm_head is only wired for a single rank
-        m->lm_head = m->emb;   // tied (Llama-3.2-1B)
-        m->lm_head_tied = true;
+        m->lm_head = m->emb.get();   // tied (Llama-3.2-1B)
         m->weight_bytes += (double)c.vocab_size * c.dim_model * 2;
     }
     return ZL_OK;
@@ -645,12 +626,12 @@ int alloc_runtime(zl_llama* m) {
         RCHECK(dmalloc(&L.vbuf, kv_task * B));
         // never-written rows must be finite: masked keys still multiply their V rows by an exact 0, and with the
         // dual-stream prefill one half's attention sees the other half's rows before they are appended
-        ZL_CHECK_CUDA(cudaMemsetAsync(L.kbuf, 0, kv_task * B, m->stream));
-        ZL_CHECK_CUDA(cudaMemsetAsync(L.vbuf, 0, kv_task * B, m->stream));
-        RCHECK(dmalloc((void**)&L.k_addrs, sizeof(void*) * B));
-        RCHECK(dmalloc((void**)&L.v_addrs, sizeof(void*) * B));
-        k_ptr_table<<<cdiv(B, 256), 256, 0, m->stream>>>(L.k_addrs, (char*)L.kbuf, kv_task, B);
-        k_ptr_table<<<cdiv(B, 256), 256, 0, m->stream>>>(L.v_addrs, (char*)L.vbuf, kv_task, B);
+        ZL_CHECK_CUDA(cudaMemsetAsync(L.kbuf.get(), 0, kv_task * B, m->stream));
+        ZL_CHECK_CUDA(cudaMemsetAsync(L.vbuf.get(), 0, kv_task * B, m->stream));
+        RCHECK(dmalloc(&L.k_addrs, sizeof(void*) * B));
+        RCHECK(dmalloc(&L.v_addrs, sizeof(void*) * B));
+        k_ptr_table<<<cdiv(B, 256), 256, 0, m->stream>>>(L.k_addrs.get(), (char*)L.kbuf.get(), kv_task, B);
+        k_ptr_table<<<cdiv(B, 256), 256, 0, m->stream>>>(L.v_addrs.get(), (char*)L.vbuf.get(), kv_task, B);
         ZL_CHECK_LAUNCH();
     }
     const int T = c.prefill_chunk > B ? c.prefill_chunk : B;   // tokens per launch: decode batch or prefill chunk
@@ -667,47 +648,50 @@ int alloc_runtime(zl_llama* m) {
     bool act_order = false;
     for (const auto& L : m->layers) act_order |= L.q_qkv.k_perm || L.q_o.k_perm || L.q_gu.k_perm;
     if (act_order) RCHECK(dmalloc(&m->xperm, (size_t)T * (D > m->hq * d ? D : m->hq * d) * 2));
-    RCHECK(dmalloc((void**)&m->logits, (size_t)B * c.vocab_size * 4));
+    RCHECK(dmalloc(&m->logits, (size_t)B * c.vocab_size * 4));
     RCHECK(dmalloc(&m->cand, (size_t)((B * 8 + 15) / 16) * 16));
     RCHECK(dmalloc(&m->cand_all, (size_t)((B * 8 + 15) / 16) * 16 * c.tp_size));
-    RCHECK(dmalloc((void**)&m->cosb, (size_t)T * d * 4));
-    RCHECK(dmalloc((void**)&m->sinb, (size_t)T * d * 4));
-    RCHECK(dmalloc((void**)&m->d_tokens, B * 4));
-    RCHECK(dmalloc((void**)&m->d_pos, B * 4));
-    RCHECK(dmalloc((void**)&m->d_lens, B * 4));
+    RCHECK(dmalloc(&m->cosb, (size_t)T * d * 4));
+    RCHECK(dmalloc(&m->sinb, (size_t)T * d * 4));
+    RCHECK(dmalloc(&m->d_tokens, B * 4));
+    RCHECK(dmalloc(&m->d_pos, B * 4));
+    RCHECK(dmalloc(&m->d_lens, B * 4));
     if (c.quant_type == 2 || c.quant_type == 7) {
         int kmax = D > m->ff ? D : m->ff;
         kmax = kmax > m->hq * d ? kmax : m->hq * d;
         RCHECK(dmalloc(&m->xq, (size_t)T * kmax));
-        RCHECK(dmalloc((void**)&m->xs, (size_t)T * 4));
+        RCHECK(dmalloc(&m->xs, (size_t)T * 4));
     }
     if (c.prefill_chunk > 0) {
-        RCHECK(dmalloc((void**)&m->d_tb, T * 4));
-        RCHECK(dmalloc((void**)&m->d_pf_tokens, T * 4));
-        RCHECK(dmalloc((void**)&m->d_pf_pos, T * 4));
-        RCHECK(dmalloc((void**)&m->d_mask, (size_t)c.prefill_chunk * c.max_seq));
+        RCHECK(dmalloc(&m->d_tb, T * 4));
+        RCHECK(dmalloc(&m->d_pf_tokens, T * 4));
+        RCHECK(dmalloc(&m->d_pf_pos, T * 4));
+        RCHECK(dmalloc(&m->d_mask, (size_t)c.prefill_chunk * c.max_seq));
     }
-    RCHECK(dmalloc((void**)&m->d_next, B * 4));
-    RCHECK(dmalloc((void**)&m->d_iota, B * 4));
-    k_iota<<<cdiv(B, 256), 256, 0, m->stream>>>(m->d_iota, B);
+    RCHECK(dmalloc(&m->d_next, B * 4));
+    RCHECK(dmalloc(&m->d_iota, B * 4));
+    k_iota<<<cdiv(B, 256), 256, 0, m->stream>>>(m->d_iota.get(), B);
     ZL_CHECK_LAUNCH();
     m->attn_ws_bytes = zl_decode_attention_workspace_bytes(T, 1, m->hq, d, c.max_seq);
     RCHECK(dmalloc(&m->attn_ws, m->attn_ws_bytes));
     RCHECK(dmalloc(&m->argmax_ws, zl_argmax_workspace_bytes(B)));
     m->hwords = cdiv(m->vshard, 32);
-    RCHECK(dmalloc((void**)&m->d_hist, (size_t)B * m->hwords * 4));
-    ZL_CHECK_CUDA(cudaMemsetAsync(m->d_hist, 0, (size_t)B * m->hwords * 4, m->stream));
-    RCHECK(dmalloc((void**)&m->d_sparams, sizeof(zl_sample_params_t) * B));
+    RCHECK(dmalloc(&m->d_hist, (size_t)B * m->hwords * 4));
+    ZL_CHECK_CUDA(cudaMemsetAsync(m->d_hist.get(), 0, (size_t)B * m->hwords * 4, m->stream));
+    RCHECK(dmalloc(&m->d_sparams, sizeof(zl_sample_params_t) * B));
     {
         const zl_sample_params_t greedy{0.f, 1.f, 1.f, 0.f, 0, 0};
         std::vector<zl_sample_params_t> init(B, greedy);
-        ZL_CHECK_CUDA(cudaMemcpyAsync(m->d_sparams, init.data(), sizeof(zl_sample_params_t) * B, cudaMemcpyHostToDevice,
+        ZL_CHECK_CUDA(cudaMemcpyAsync(m->d_sparams.get(), init.data(), sizeof(zl_sample_params_t) * B, cudaMemcpyHostToDevice,
                                       m->stream));
         ZL_CHECK_CUDA(cudaStreamSynchronize(m->stream));   // `init` is pageable and goes out of scope
     }
     m->samp_on.assign(B, 0);
-    ZL_CHECK_CUDA(cudaMallocHost((void**)&m->h_stage, sizeof(int32_t) * (4 * B + 4 + T)));
-    ZL_CHECK_CUDA(cudaMallocHost((void**)&m->h_ring, sizeof(int32_t) * zl_llama::kStageSlots * 2 * B));
+    int32_t *stage = nullptr, *ring = nullptr;
+    ZL_CHECK_CUDA(cudaMallocHost((void**)&stage, sizeof(int32_t) * (4 * B + 4 + T)));
+    m->h_stage.reset(stage);
+    ZL_CHECK_CUDA(cudaMallocHost((void**)&ring, sizeof(int32_t) * zl_llama::kStageSlots * 2 * B));
+    m->h_ring.reset(ring);
     for (int i = 0; i < zl_llama::kStageSlots; ++i)
         ZL_CHECK_CUDA(cudaEventCreateWithFlags(&m->ring_ev[i], cudaEventDisableTiming));
     ZL_CHECK_CUDA(cudaStreamSynchronize(m->stream));
@@ -740,145 +724,223 @@ static size_t l2_whole_max() {
     return (size_t)v << 20;
 }
 
-static bool w4_routes_v3(const W4Lin& w, int B) {
-    return w.packed_i && !getenv("ZL_W4_FORCE_HALF") && zl_w4_int_layout_route(B, w.N, w.K) == 3;
-}
-
-// the successor of GEMM `slot` (0 qkv, 2 o, 3 gate_up, 4 down) of layer l in the decode chain -- qkv -> o -> gate_up -> down
-// -> next layer's qkv -- and its tensor-parallel mode given this GEMM's (the fused exchange alternates push / reduce-in; the
-// last layer's down keeps the stand-alone all-reduce).  The lm_head boundary is left out.
-static const W4Lin* w4_successor(zl_llama* m, int l, int slot, int tp_mode, int* succ_tp) {
-    Layer& L = m->layers[l];
-    const bool last = l + 1 >= m->cfg.num_layers;
-    *succ_tp = 0;
-    switch (slot) {
-        case 0: *succ_tp = tp_mode ? 2 : 0; return &L.q_o;
-        case 2: *succ_tp = tp_mode ? 1 : 0; return &L.q_gu;
-        case 3: *succ_tp = tp_mode && !last ? 2 : 0; return &L.q_down;
-        case 4: *succ_tp = tp_mode ? 1 : 0; return last ? nullptr : &m->layers[l + 1].q_qkv;
-        default: return nullptr;
-    }
-}
-
-// ZL_NO_PDL_MASK (experiments): launch these kernels with a full dependency instead of a programmatic one.
-// 1 qkv GEMM, 2 attention, 4 o GEMM, 8 gate_up GEMM, 16 down GEMM, 32 final norm, 64 lm_head, 128 argmax.
+// The launches of the decode chain, in order.  ZL_NO_PDL_MASK (experiments): bit 1 << stage launches that stage with a full
+// dependency instead of a programmatic one (1 qkv GEMM, 2 attention, 4 o GEMM, 8 gate_up GEMM, 16 down GEMM, 32 final
+// norm, 64 lm_head, 128 argmax / sampler).
 // Single GPU, default 66 = lm_head + attention (a PDL-launched lm_head measured much slower, tools/gpu_tail.sh): on an
 // H100 80GB HBM3 at 400 W, Llama-3.1-8B batch-1 decode measured 425.8 tok/s (425.6-426.2 over 5 runs) against 413.2
 // (412.5-415.2) with the o GEMM also fully dependent (70), 420 with attention PDL-launched too (64), and 400-405 with
 // lm_head PDL-launched (2, 0)
 // (profiles/l2_head_ab.txt): an o GEMM launched early stages its ring fill while attention runs.
 // Tensor parallel (exchange inside the GEMMs): 68, a PDL-launched attention kernel measured faster there.
-static int no_pdl_mask(bool tensor_parallel = false) {
-    static int v = -2;
-    if (v == -2) {
+enum Stage { kQkv, kAttn, kO, kGateUp, kDown, kFinalNorm, kLmHead, kPick };
+
+static int stage_pdl(const zl_llama* m, Stage s) {
+    static int mask = -2;
+    if (mask == -2) {
         const char* e = getenv("ZL_NO_PDL_MASK");
-        v = e ? atoi(e) : -1;
+        mask = e ? atoi(e) : -1;
     }
-    if (v >= 0) return v;
-    return tensor_parallel ? 68 : 66;
+    const int npm = mask >= 0 ? mask : m->cfg.tp_size > 1 ? 68 : 66;
+    return (npm >> s & 1) ? 0 : m->cfg.use_pdl;
 }
 
-int w4_gemm(zl_llama* m, const void* x, int ldx, const W4Lin& w, const void* residual, void* y, int B, int epi,
-            const void* ln_w, const Layer* rope_layer, int layer = -1, int slot = -1, int row0 = 0, int force_no_pdl = 0,
-            int tp_mode = 0, void* tp_h_out = nullptr, int tp_index = 0) {
+// the successor of W4 GEMM stage s of layer l in the decode chain -- qkv -> o -> gate_up -> down -> next layer's qkv -- and
+// its tensor-parallel mode given this GEMM's (the fused exchange alternates push / reduce-in; the last layer's down keeps
+// the stand-alone all-reduce).  The lm_head boundary is left out.
+static const W4Lin* w4_successor(zl_llama* m, int l, Stage s, int tp_mode, int* succ_tp) {
+    Layer& L = m->layers[l];
+    const bool last = l + 1 >= m->cfg.num_layers;
+    *succ_tp = 0;
+    switch (s) {
+        case kQkv: *succ_tp = tp_mode ? 2 : 0; return &L.q_o;
+        case kO: *succ_tp = tp_mode ? 1 : 0; return &L.q_gu;
+        case kGateUp: *succ_tp = tp_mode && !last ? 2 : 0; return &L.q_down;
+        case kDown: *succ_tp = tp_mode ? 1 : 0; return last ? nullptr : &m->layers[l + 1].q_qkv;
+        default: return nullptr;
+    }
+}
+
+// row `row` of an fp16 activation matrix of `width` columns
+void* rows(const void* base, int row, int width) { return (char*)base + (size_t)row * width * 2; }
+
+// One launch sequence of the layer GEMMs -- a decode step, one half of a dual-stream prefill chunk, or
+// zl_llama_bench_gemms -- and the residual stream it updates.
+struct Chain {
+    enum Sink {
+        kAddResidual,   // o / down add their output to the residual stream in the epilogue
+        kPartial,       // o / down write partial sums to pend; the caller reduces them (dual-stream prefill)
+        kAllReduce,     // tensor parallel: o / down partial sums -> one-shot all-reduce fused with the residual add
+    };
+    int row0 = 0, n = 0;       // rows of the activation matrices this sequence covers
+    Sink sink = kAddResidual;
+    bool no_pdl = false;       // full dependencies and no L2 head: the next launch is not the chain successor (dual stream)
+    bool gemm_only = false;    // launch only what the GEMMs of this fuse level comprise: no stand-alone RMSNorm (fuse 0)
+                               // or RoPE / KV append (fuse < 2)
+    void* h = nullptr;         // current residual stream
+    // Fused tensor-parallel exchange (decode-sized W4 steps): the row-parallel GEMMs (o, down but the last layer's) push
+    // their fp16 partial tiles into every rank's inbox from the epilogue; the next GEMM (gate_up, next layer's qkv)
+    // reduces them in rank order while it stages its activations and writes the new residual stream to ho, the other of
+    // h / h2.  Producer and consumer of one exchange use the same index; the word tags in comm_dev.cuh depend on it.
+    bool fused = false;
+    void* ho = nullptr;
+    bool pending = false;      // partial sums of the previous row-parallel GEMM are in flight to the inboxes
+    int xi = 0;                // index of the next exchange of the step
+    int xodd = 0;              // 2 L - 1 exchanges per step: odd -> bit 9 of tp_index
+
+    void push(zl_w4_fused_args_t* a) {
+        a->tp_mode = 2;
+        a->tp_index = (xi++) | xodd;
+        pending = true;
+    }
+    // call after a->x is taken from h
+    void reduce_in(zl_w4_fused_args_t* a) {
+        if (!pending) return;
+        a->tp_mode = 1;
+        a->tp_h_out = ho;
+        a->tp_index = (xi - 1) | xodd;
+        std::swap(h, ho);
+        pending = false;
+    }
+};
+
+// One W4 GEMM of stage s of layer l.  The caller sets a's activation, output, epilogue, RoPE and exchange fields; this adds
+// the weights, the RMSNorm ln_w (fused into the GEMM or as its own kernel), the act-order gather, the PDL flag and the L2
+// head of the successor.
+int w4_gemm(zl_llama* m, int l, Stage s, const Chain& ch, const W4Lin& w, const void* ln_w, zl_w4_fused_args_t a) {
     const auto& c = m->cfg;
-    zl_w4_fused_args_t a = {};
-    a.x = x;
-    a.ldx = ldx;
-    const int route = (w.packed_i && !getenv("ZL_W4_FORCE_HALF")) ? zl_w4_int_layout_route(B, w.N, w.K) : 0;
-    const bool use_int = route != 0;
-    a.packed = use_int ? w.packed_i : w.packed;
-    a.variant = use_int ? 1 : 0;
-    if ((route == 4 || (w.k_perm && route != 3)) && ln_w) {
-        // the wgmma kernel reads x through the TMA engine: the RMSNorm runs as its own kernel (reference order,
-        // block.cpp:125,131) into the matching rows of xn.  So does an act-order GEMM that is not gathered while staged.
-        const size_t off = (const char*)x - (const char*)m->h;
-        void* xn = (char*)m->xn + off;
-        RCHECK(zl_rmsnorm(x, ln_w, xn, B, w.K, c.eps, 1.f, c.dtype, force_no_pdl ? 0 : c.use_pdl, m->stream));
-        a.x = xn;
-        ln_w = nullptr;
-    }
-    if (w.k_perm && route == 3) {
-        a.k_perm = w.k_perm;   // gathered while the integer kernel stages x
-    } else if (w.k_perm) {
-        // the other routes read x in tiles: permute it first (permute_input, gptq/utils.cu:322-398)
-        RCHECK(zl_gather_cols_16(a.x, a.ldx, w.k_perm, m->xperm, B, w.K, force_no_pdl ? 0 : c.use_pdl, m->stream));
-        a.x = m->xperm;
-        a.ldx = w.K;
-    }
-    W4L2Head l2;
-    if (layer >= 0 && route == 3 && (l2_head_depth() > 0 || l2_whole_max() > 0)) {
-        int succ_tp = 0;
-        const W4Lin* nx = w4_successor(m, layer, slot, tp_mode, &succ_tp);
-        if (nx && w4_routes_v3(*nx, B))
-            w4_v3_l2_head(nx->packed_i, B, nx->N, nx->K, succ_tp, device_sm_count(), l2_head_depth(), l2_whole_max(), &l2);
-    }
+    const int route = route_of(w, ch.n);
+    a.packed = route ? w.packed_i.get() : w.packed.get();
+    a.variant = route ? 1 : 0;
     if (!a.packed) {
         zl_set_last_error(__FILE__, __LINE__, "no packed weight variant for this batch size");
         return ZL_ERR_STATE;
     }
-    a.bias = w.bias;
-    a.residual = residual;
-    a.y = y;
-    a.M = B;
+    const int pdl = ch.no_pdl ? 0 : c.use_pdl;
+    if (ln_w && (c.fuse == 0 || route == 4 || (w.k_perm && route != 3))) {
+        // the RMSNorm runs as its own kernel (reference order, block.cpp:125,131) into the matching rows of xn: at fuse 0,
+        // for the wgmma kernel, which reads x through the TMA engine, and for an act-order GEMM not gathered while staged
+        void* xn = rows(m->xn.get(), ch.row0, w.K);
+        if (c.fuse > 0 || !ch.gemm_only)
+            RCHECK(zl_rmsnorm(a.x, ln_w, xn, ch.n, w.K, c.eps, 1.f, c.dtype, pdl, m->stream));
+        a.x = xn;
+        ln_w = nullptr;
+    }
+    if (w.k_perm && route == 3) {
+        a.k_perm = w.k_perm.get();   // gathered while the integer kernel stages x
+    } else if (w.k_perm) {
+        // the other routes read x in tiles: permute it first (permute_input, gptq/utils.cu:322-398)
+        RCHECK(zl_gather_cols_16(a.x, a.ldx, w.k_perm.get(), m->xperm.get(), ch.n, w.K, pdl, m->stream));
+        a.x = m->xperm.get();
+        a.ldx = w.K;
+    }
+    W4L2Head l2;
+    if (!ch.no_pdl && route == 3 && (l2_head_depth() > 0 || l2_whole_max() > 0)) {
+        int succ_tp = 0;
+        const W4Lin* nx = w4_successor(m, l, s, a.tp_mode, &succ_tp);
+        if (nx && route_of(*nx, ch.n) == 3)
+            w4_v3_l2_head(nx->packed_i.get(), ch.n, nx->N, nx->K, succ_tp, device_sm_count(), l2_head_depth(),
+                          l2_whole_max(), &l2);
+    }
+    a.bias = w.bias.get();
+    a.M = ch.n;
     a.N = w.N;
     a.K = w.K;
     a.group_size = c.group_size;
-    a.epilogue = epi;
-    {
-        const int bit = slot == 0 ? 1 : slot == 2 ? 4 : slot == 3 ? 8 : slot == 4 ? 16 : 0;
-        a.pdl = (no_pdl_mask(c.tp_size > 1) & bit) ? 0 : c.use_pdl;
-    }
+    a.pdl = ch.no_pdl ? 0 : stage_pdl(m, s);
     a.ln_weight = ln_w;
     a.eps = c.eps;
-    if (rope_layer) {
-        // row0: first token row of this call inside the step's activation matrices (dual-stream prefill halves)
-        a.cos = m->cosb + (size_t)row0 * c.dim_head;
-        a.sin = m->sinb + (size_t)row0 * c.dim_head;
-        a.q_out = (char*)m->q + (size_t)row0 * m->hq * c.dim_head * 2;
-        a.token_batch = m->cur_tb + row0;
-        a.placement = m->cur_pos + row0;
-        a.k_addrs = rope_layer->k_addrs;
-        a.v_addrs = rope_layer->v_addrs;
-        a.num_heads = m->hq;
-        a.num_kv_heads = m->hkv;
-        a.dim_head = c.dim_head;
-    }
-    if (force_no_pdl) a.pdl = 0;
-    if (tp_mode) {
-        a.tp_comm = m->comm;
-        a.tp_mode = tp_mode;
-        a.tp_h_out = tp_h_out;
-        a.tp_index = tp_index;
-    }
+    if (a.tp_mode) a.tp_comm = m->comm;
     return w4a16_gemm_fused_l2(&a, &l2, m->stream);
 }
 
-static int num_sms() { return device_sm_count(); }
-
-// ZL_DEBUG_SKIP (bit mask, timing experiments only -- results are wrong when set):
-// 1 attention, 2 qkv GEMM, 4 o GEMM, 8 gate/up GEMM, 16 down GEMM, 32 lm_head, 64 rope/append kernel
-static int debug_skip() {
-    static int v = -1;
-    if (v < 0) {
-        const char* e = getenv("ZL_DEBUG_SKIP");
-        v = e ? atoi(e) : 0;
+// qkv: RMSNorm + GEMM; at fuse >= 2 the epilogue splits q / k / v, applies RoPE and appends K / V, otherwise
+// zl_qkv_rope_append does
+int qkv_gemm(zl_llama* m, int l, Chain& ch) {
+    const auto& c = m->cfg;
+    const Layer& L = m->layers[l];
+    const int d = c.dim_head, hqkv = (m->hq + 2 * m->hkv) * d;
+    zl_w4_fused_args_t a = {};
+    a.x = rows(ch.h, ch.row0, c.dim_model);
+    a.ldx = c.dim_model;
+    const float* cos = m->cosb.get() + (size_t)ch.row0 * d;
+    const float* sin = m->sinb.get() + (size_t)ch.row0 * d;
+    void* q = rows(m->q.get(), ch.row0, m->hq * d);
+    const int32_t* tb = m->cur_tb + ch.row0;
+    const int32_t* pos = m->cur_pos + ch.row0;
+    if (c.fuse >= 2) {
+        a.epilogue = ZL_EPI_QKV_ROPE;
+        a.cos = cos;
+        a.sin = sin;
+        a.q_out = q;
+        a.token_batch = tb;
+        a.placement = pos;
+        a.k_addrs = L.k_addrs.get();
+        a.v_addrs = L.v_addrs.get();
+        a.num_heads = m->hq;
+        a.num_kv_heads = m->hkv;
+        a.dim_head = d;
+    } else {
+        a.y = rows(m->qkv.get(), ch.row0, hqkv);
     }
-    return v;
+    ch.reduce_in(&a);
+    RCHECK(w4_gemm(m, l, kQkv, ch, L.q_qkv, L.ln_attn.get(), a));
+    if (c.fuse >= 2 || ch.gemm_only) return ZL_OK;
+    return zl_qkv_rope_append(cos, sin, a.y, q, tb, pos, L.k_addrs.get(), L.v_addrs.get(), ch.n, m->hq, m->hkv, d, 1, 1,
+                              m->d_lens.get(), c.dtype, ch.no_pdl ? 0 : c.use_pdl, m->stream);
 }
+
+// gate_up: RMSNorm + GEMM + SwiGLU epilogue into act
+int gate_up_gemm(zl_llama* m, int l, Chain& ch) {
+    const auto& c = m->cfg;
+    zl_w4_fused_args_t a = {};
+    a.x = rows(ch.h, ch.row0, c.dim_model);
+    a.ldx = c.dim_model;
+    a.y = rows(m->act.get(), ch.row0, m->ff);
+    a.epilogue = ZL_EPI_SWIGLU;
+    ch.reduce_in(&a);
+    return w4_gemm(m, l, kGateUp, ch, m->layers[l].q_gu, m->layers[l].ln_ff.get(), a);
+}
+
+// o (input ao) and down (input act): row-parallel under tensor parallelism, their output goes to ch.sink
+int row_parallel_gemm(zl_llama* m, int l, Stage s, Chain& ch) {
+    const auto& c = m->cfg;
+    const W4Lin& w = s == kO ? m->layers[l].q_o : m->layers[l].q_down;
+    zl_w4_fused_args_t a = {};
+    a.x = rows(s == kO ? m->ao.get() : m->act.get(), ch.row0, w.K);
+    a.ldx = w.K;
+    // the last layer's down keeps the stand-alone all-reduce: the final norm is not a GEMM
+    const bool push = ch.fused && (s == kO || l + 1 < c.num_layers);
+    if (push) {
+        ch.push(&a);
+    } else if (ch.sink == Chain::kAddResidual) {
+        a.residual = a.y = rows(ch.h, ch.row0, c.dim_model);
+        a.epilogue = ZL_EPI_RESIDUAL;
+    } else {
+        a.y = rows(m->pend.get(), ch.row0, c.dim_model);
+    }
+    RCHECK(w4_gemm(m, l, s, ch, w, nullptr, a));
+    if (push || ch.sink != Chain::kAllReduce) return ZL_OK;
+    return zl_allreduce_one_shot(m->comm, a.y, ch.h, ch.h, (size_t)ch.n * c.dim_model, c.dtype, c.tp_int8,
+                                 ch.no_pdl ? 0 : c.use_pdl, m->stream);
+}
+int o_gemm(zl_llama* m, int l, Chain& ch) { return row_parallel_gemm(m, l, kO, ch); }
+int down_gemm(zl_llama* m, int l, Chain& ch) { return row_parallel_gemm(m, l, kDown, ch); }
 
 // One non-W4 Linear of the decode chain: dense (NormalLinear), or W8A8 = activation quant + fused 8-bit GEMM
 // (Int8Linear::forward / Fp8Linear::forward in two launches instead of three).
 int dense_or_w8(zl_llama* m, const void* x, const DenseLin& L, void* y, int B, int pdl) {
     const auto& c = m->cfg;
     cudaStream_t st = m->stream;
-    if (!L.w8) return zl_dense_gemm_skinny(x, L.K, L.w, L.bias, y, B, L.N, L.K, c.dtype, c.dtype, pdl, st);
+    if (!L.w8) return zl_dense_gemm_skinny(x, L.K, L.w.get(), L.bias.get(), y, B, L.N, L.K, c.dtype, c.dtype, pdl, st);
     if (L.w8_kind == ZL_W8_INT8) {
-        RCHECK(zl_int8_quant_per_token(x, L.K, m->xq, m->xs, B, L.K, c.dtype, pdl, st));
-        return zl_w8a8_gemm(m->xq, m->xs, L.w8, L.w_scale, c.dtype, L.bias, y, B, L.N, L.K, ZL_W8_INT8, c.dtype, pdl, st);
+        RCHECK(zl_int8_quant_per_token(x, L.K, m->xq.get(), m->xs.get(), B, L.K, c.dtype, pdl, st));
+        return zl_w8a8_gemm(m->xq.get(), m->xs.get(), L.w8.get(), L.w_scale.get(), c.dtype, L.bias.get(), y, B, L.N, L.K,
+                            ZL_W8_INT8, c.dtype, pdl, st);
     }
-    RCHECK(zl_fp8_quant_per_tensor(x, m->xq, m->xs, (size_t)B * L.K, c.dtype, pdl, st));
-    return zl_w8a8_gemm(m->xq, m->xs, L.w8, L.w_scale, ZL_F32, L.bias, y, B, L.N, L.K, ZL_W8_FP8_ROWS, c.dtype, pdl, st);
+    RCHECK(zl_fp8_quant_per_tensor(x, m->xq.get(), m->xs.get(), (size_t)B * L.K, c.dtype, pdl, st));
+    return zl_w8a8_gemm(m->xq.get(), m->xs.get(), L.w8.get(), L.w_scale.get(), ZL_F32, L.bias.get(), y, B, L.N, L.K,
+                        ZL_W8_FP8_ROWS, c.dtype, pdl, st);
 }
 
 // pf != nullptr: one chunk of a prompt (tokens of ONE task at consecutive positions) instead of one token per task
@@ -923,52 +985,46 @@ int prefill_layers_dual(zl_llama* m, const PrefillChunk& pf) {
     cudaStream_t cs = m->stream, rs = m->reduce_stream;
     const float scale = 1.0f / sqrtf((float)d);
     const int n0 = (pf.n / 2 + 7) / 8 * 8 < pf.n ? (pf.n / 2 + 7) / 8 * 8 : pf.n / 2;   // rows of half 0
-    const int r0[2] = {0, n0}, nh[2] = {n0, pf.n - n0};
     const int len_buf = pf.pos0 + pf.n;
-    auto rows = [&](void* base, int row, size_t row_bytes) { return (char*)base + (size_t)row * row_bytes; };
-    auto reduce = [&](int h) -> int {   // h rows: h += sum over ranks of pend
-        void* hp = rows(m->h, r0[h], (size_t)D * 2);
-        void* pp = rows(m->pend, r0[h], (size_t)D * 2);
-        if (tp) return zl_allreduce_one_shot(m->comm, pp, hp, hp, (size_t)nh[h] * D, dt, c.tp_int8, 0, rs);
-        return zl_element_add_scale(hp, pp, hp, (size_t)nh[h] * D, 1.0f, dt, rs);
+    Chain half[2];
+    for (int h = 0; h < 2; ++h) {
+        half[h].row0 = h ? n0 : 0;
+        half[h].n = h ? pf.n - n0 : n0;
+        half[h].sink = Chain::kPartial;
+        half[h].no_pdl = true;
+        half[h].h = m->h.get();
+    }
+    auto reduce = [&](const Chain& ch) -> int {   // h rows: h += sum over ranks of pend
+        void* hp = rows(m->h.get(), ch.row0, D);
+        void* pp = rows(m->pend.get(), ch.row0, D);
+        if (tp) return zl_allreduce_one_shot(m->comm, pp, hp, hp, (size_t)ch.n * D, dt, c.tp_int8, 0, rs);
+        return zl_element_add_scale(hp, pp, hp, (size_t)ch.n * D, 1.0f, dt, rs);
     };
     for (int l = 0; l < c.num_layers; ++l) {
         Layer& L = m->layers[l];
         for (int h = 0; h < 2; ++h) {   // S1
             if (l > 0) ZL_CHECK_CUDA(cudaStreamWaitEvent(cs, m->ev_r2[h], 0));
-            void* hp = rows(m->h, r0[h], (size_t)D * 2);
-            if (c.fuse >= 2) {
-                RCHECK(w4_gemm(m, hp, D, L.q_qkv, nullptr, nullptr, nh[h], ZL_EPI_QKV_ROPE, L.ln_attn, &L, -1, -1, r0[h], 1));
-            } else {
-                void* qp = rows(m->qkv, r0[h], (size_t)(m->hq + 2 * m->hkv) * d * 2);
-                RCHECK(w4_gemm(m, hp, D, L.q_qkv, nullptr, qp, nh[h], ZL_EPI_NONE, L.ln_attn, nullptr, -1, -1, 0, 1));
-                RCHECK(zl_qkv_rope_append(m->cosb + (size_t)r0[h] * d, m->sinb + (size_t)r0[h] * d, qp,
-                                          rows(m->q, r0[h], (size_t)m->hq * d * 2), m->cur_tb + r0[h], m->cur_pos + r0[h],
-                                          L.k_addrs, L.v_addrs, nh[h], m->hq, m->hkv, d, 1, 1, m->d_lens, dt, 0, cs));
-            }
+            const int r0 = half[h].row0;
+            RCHECK(qkv_gemm(m, l, half[h]));
             // causal rows r0.. of the chunk's mask; keys of BOTH halves are visible as far as the mask allows, so half 1
             // needs half 0's K/V rows, which the same stream appended just before
-            RCHECK(zl_decode_attention(rows(m->q, r0[h], (size_t)m->hq * d * 2), m->d_lens + pf.task, L.k_addrs + pf.task,
-                                       L.v_addrs + pf.task, m->d_mask + (size_t)r0[h] * len_buf, scale, len_buf,
-                                       rows(m->ao, r0[h], (size_t)m->hq * d * 2), 1, nh[h], m->hq, m->hkv, d, 1, m->attn_ws,
-                                       m->attn_ws_bytes, dt, 0, cs));
-            RCHECK(w4_gemm(m, rows(m->ao, r0[h], (size_t)m->hq * d * 2), m->hq * d, L.q_o, nullptr,
-                           rows(m->pend, r0[h], (size_t)D * 2), nh[h], ZL_EPI_NONE, nullptr, nullptr, -1, -1, 0, 1));
+            RCHECK(zl_decode_attention(rows(m->q.get(), r0, m->hq * d), m->d_lens.get() + pf.task,
+                                       L.k_addrs.get() + pf.task, L.v_addrs.get() + pf.task,
+                                       m->d_mask.get() + (size_t)r0 * len_buf, scale, len_buf, rows(m->ao.get(), r0, m->hq * d),
+                                       1, half[h].n, m->hq, m->hkv, d, 1, m->attn_ws.get(), m->attn_ws_bytes, dt, 0, cs));
+            RCHECK(o_gemm(m, l, half[h]));
             ZL_CHECK_CUDA(cudaEventRecord(m->ev_o[h], cs));
             ZL_CHECK_CUDA(cudaStreamWaitEvent(rs, m->ev_o[h], 0));   // R1
-            RCHECK(reduce(h));
+            RCHECK(reduce(half[h]));
             ZL_CHECK_CUDA(cudaEventRecord(m->ev_r1[h], rs));
         }
         for (int h = 0; h < 2; ++h) {   // S3
             ZL_CHECK_CUDA(cudaStreamWaitEvent(cs, m->ev_r1[h], 0));
-            void* hp = rows(m->h, r0[h], (size_t)D * 2);
-            void* ap = rows(m->act, r0[h], (size_t)m->ff * 2);
-            RCHECK(w4_gemm(m, hp, D, L.q_gu, nullptr, ap, nh[h], ZL_EPI_SWIGLU, L.ln_ff, nullptr, -1, -1, 0, 1));
-            RCHECK(w4_gemm(m, ap, m->ff, L.q_down, nullptr, rows(m->pend, r0[h], (size_t)D * 2), nh[h], ZL_EPI_NONE, nullptr,
-                           nullptr, -1, -1, 0, 1));
+            RCHECK(gate_up_gemm(m, l, half[h]));
+            RCHECK(down_gemm(m, l, half[h]));
             ZL_CHECK_CUDA(cudaEventRecord(m->ev_dn[h], cs));
             ZL_CHECK_CUDA(cudaStreamWaitEvent(rs, m->ev_dn[h], 0));   // R2
-            RCHECK(reduce(h));
+            RCHECK(reduce(half[h]));
             ZL_CHECK_CUDA(cudaEventRecord(m->ev_r2[h], rs));
         }
     }
@@ -979,10 +1035,7 @@ int prefill_layers_dual(zl_llama* m, const PrefillChunk& pf) {
 int enqueue_step(zl_llama* m, int n_tasks, int len_bucket, const PrefillChunk* pf = nullptr, bool sampler = false) {
     const auto& c = m->cfg;
     const int B = pf ? pf->n : n_tasks;   // rows (tokens) of every activation matrix in this launch sequence
-    const int skip = debug_skip();
     const int D = c.dim_model, d = c.dim_head, dt = c.dtype, pdl = c.use_pdl;
-    const int npm = no_pdl_mask(c.tp_size > 1);
-    auto P = [&](int bit) { return (npm & bit) ? 0 : pdl; };
     cudaStream_t st = m->stream;
     const bool w4 = c.quant_type == 5 || c.quant_type == 6;
     const bool tp = c.tp_size > 1;
@@ -993,159 +1046,117 @@ int enqueue_step(zl_llama* m, int n_tasks, int len_bucket, const PrefillChunk* p
     const float scale = 1.0f / sqrtf((float)d);   // attention.cpp:89
 
     if (pf) {
-        k_prefill_setup<<<8, 256, 0, st>>>(m->d_pf_pos, m->d_tb, m->d_lens, m->d_mask, pf->task, pf->pos0, pf->n);
+        k_prefill_setup<<<8, 256, 0, st>>>(m->d_pf_pos.get(), m->d_tb.get(), m->d_lens.get(), m->d_mask.get(), pf->task,
+                                           pf->pos0, pf->n);
         ZL_CHECK_LAUNCH();
     } else {
-        ZL_CHECK_CUDA(launch(k_lens_from_pos, dim3(cdiv(B, 64)), dim3(64), 0, st, false, (const int32_t*)m->d_pos,
-                             m->d_lens, B, g_w4_trace));
+        ZL_CHECK_CUDA(launch(k_lens_from_pos, dim3(cdiv(B, 64)), dim3(64), 0, st, false, (const int32_t*)m->d_pos.get(),
+                             m->d_lens.get(), B, g_w4_trace));
     }
-    m->cur_tb = pf ? m->d_tb : m->d_iota;
-    m->cur_pos = pf ? m->d_pf_pos : m->d_pos;
-    m->cur_tokens = pf ? m->d_pf_tokens : m->d_tokens;
-    RCHECK(zl_rope_cos_sin(m->cur_pos, m->cosb, m->sinb, B, d, c.rope_theta, c.rope_llama3_factor,
+    m->cur_tb = pf ? m->d_tb.get() : m->d_iota.get();
+    m->cur_pos = pf ? m->d_pf_pos.get() : m->d_pos.get();
+    m->cur_tokens = pf ? m->d_pf_tokens.get() : m->d_tokens.get();
+    RCHECK(zl_rope_cos_sin(m->cur_pos, m->cosb.get(), m->sinb.get(), B, d, c.rope_theta, c.rope_llama3_factor,
                            c.rope_low_freq_factor, c.rope_high_freq_factor, c.rope_orig_ctx, 1, st));
-    RCHECK(zl_embedding(m->cur_tokens, m->emb, m->h, B, D, c.vocab_size, dt, 0, st));
+    RCHECK(zl_embedding(m->cur_tokens, m->emb.get(), m->h.get(), B, D, c.vocab_size, dt, 0, st));
     const bool dual = pf && prefill_dual_enabled(m, pf->n);
     if (dual) RCHECK(prefill_layers_dual(m, *pf));
-    // Tensor parallel, decode-sized launches of a W4 model: the exchange rides inside the GEMMs.  The row-parallel GEMMs
-    // (o_proj, w_out) push their fp16 partial tiles into every rank's inbox from the epilogue; the next GEMM (gate_up, next
-    // layer's qkv) reduces them in rank order while it stages its activations and writes the new residual stream to the
-    // other of the two buffers h / h2.  Only the last layer's w_out keeps the stand-alone one-shot kernel (the final norm
-    // is not a GEMM).  ZL_TP_UNFUSED=1 keeps the separate exchange kernels everywhere (A/B).
-    bool tp_fused = tp && w4 && !pf && c.fuse >= 1 && !c.tp_int8 && dt == ZL_F16 && !getenv("ZL_TP_UNFUSED") && !skip &&
-                    (size_t)B * D * 2 <= zl_comm_slot_bytes(m->comm) && 2 * c.num_layers <= 512;
-    if (tp_fused) {
+    Chain ch;
+    ch.n = B;
+    ch.sink = tp ? Chain::kAllReduce : Chain::kAddResidual;
+    ch.h = m->h.get();
+    ch.ho = m->h2.get();
+    // Tensor parallel, decode-sized launches of a W4 model: the exchange rides inside the GEMMs (Chain).  ZL_TP_UNFUSED=1
+    // keeps the separate exchange kernels everywhere (A/B).
+    ch.fused = tp && w4 && !pf && c.fuse >= 1 && !c.tp_int8 && dt == ZL_F16 && !getenv("ZL_TP_UNFUSED") &&
+               (size_t)B * D * 2 <= zl_comm_slot_bytes(m->comm) && 2 * c.num_layers <= 512;
+    if (ch.fused) {
         const Layer& L0 = m->layers[0];
         for (const W4Lin* w : {&L0.q_qkv, &L0.q_o, &L0.q_gu, &L0.q_down})
-            if (!w->packed_i || zl_w4_int_layout_route(B, w->N, w->K) != 3) tp_fused = false;
+            if (route_of(*w, B) != 3) ch.fused = false;
     }
-    if (tp_fused) RCHECK(zl_comm_ll_begin_step(m->comm, st));   // the word tags of this step's exchanges
-    void* hc = m->h;    // current residual stream
-    void* ho = m->h2;   // where the next fused reduce-in writes it
-    bool pending = false;   // partial sums of the previous row-parallel GEMM are in flight to the inboxes
-    int xi = 0;             // index of the next exchange of the step (producer and consumer use the same one)
-    const int xodd = ((2 * c.num_layers - 1) & 1) << 9;   // 2 L - 1 exchanges per step: odd -> bit 9 of tp_index
+    if (ch.fused) RCHECK(zl_comm_ll_begin_step(m->comm, st));   // the word tags of this step's exchanges
+    ch.xodd = ((2 * c.num_layers - 1) & 1) << 9;
     for (int l = 0; l < (dual ? 0 : c.num_layers); ++l) {
         Layer& L = m->layers[l];
         if (w4) {
-            const void* xin = m->xn;
-            const void* lnw = nullptr;
-            if (c.fuse >= 1) {
-                xin = hc;
-                lnw = L.ln_attn;
-            } else {
-                RCHECK(zl_rmsnorm(hc, L.ln_attn, m->xn, B, D, c.eps, 1.f, dt, pdl, st));
-            }
-            const int tpm = pending ? 1 : 0;
-            if (skip & 2) {
-            } else if (c.fuse >= 2) {
-                RCHECK(w4_gemm(m, xin, D, L.q_qkv, nullptr, nullptr, B, ZL_EPI_QKV_ROPE, lnw, &L, l, 0, 0, 0, tpm, ho, (xi - 1) | xodd));
-            } else {
-                RCHECK(w4_gemm(m, xin, D, L.q_qkv, nullptr, m->qkv, B, ZL_EPI_NONE, lnw, nullptr, l, 0, 0, 0, tpm, ho, (xi - 1) | xodd));
-            }
-            if (pending) {
-                std::swap(hc, ho);
-                pending = false;
-            }
+            RCHECK(qkv_gemm(m, l, ch));
         } else {
             // residual of the previous layer's FFN is folded into this norm (block.cpp:139-141 + 131)
-            RCHECK(zl_add_rmsnorm(m->h, l == 0 ? nullptr : m->pend, L.ln_attn, m->h, m->xn, B, D, c.eps, 1.f, 0, dt,
-                                  pdl, st));
-            RCHECK(dense_or_w8(m, m->xn, L.d_qkv, m->qkv, B, pdl));
+            RCHECK(zl_add_rmsnorm(m->h.get(), l == 0 ? nullptr : m->pend.get(), L.ln_attn.get(), m->h.get(), m->xn.get(),
+                                  B, D, c.eps, 1.f, 0, dt, pdl, st));
+            RCHECK(dense_or_w8(m, m->xn.get(), L.d_qkv, m->qkv.get(), B, pdl));
+            RCHECK(zl_qkv_rope_append(m->cosb.get(), m->sinb.get(), m->qkv.get(), m->q.get(), m->cur_tb, m->cur_pos,
+                                      L.k_addrs.get(), L.v_addrs.get(), B, m->hq, m->hkv, d, 1, 1, m->d_lens.get(), dt,
+                                      pdl, st));
         }
-        if (!(w4 && c.fuse >= 2) && !(skip & 64))
-            RCHECK(zl_qkv_rope_append(m->cosb, m->sinb, m->qkv, m->q, m->cur_tb, m->cur_pos, L.k_addrs, L.v_addrs, B,
-                                      m->hq, m->hkv, d, 1, 1, m->d_lens, dt, pdl, st));
         if (pf) {
             // one task, len_q = chunk, causal int8 mask (Attention::dynamic_batch_forward with len_q > 1, attention.cpp:846-964)
-            RCHECK(zl_decode_attention(m->q, m->d_lens + pf->task, L.k_addrs + pf->task, L.v_addrs + pf->task, m->d_mask,
-                                       scale, pf->pos0 + pf->n, m->ao, 1, pf->n, m->hq, m->hkv, d, 1, m->attn_ws,
-                                       m->attn_ws_bytes, dt, pdl, st));
-        } else if (!(skip & 1))
-            RCHECK(zl_decode_attention(m->q, m->d_lens, L.k_addrs, L.v_addrs, nullptr, scale, len_bucket, m->ao, B, 1,
-                                       m->hq, m->hkv, d, 1, m->attn_ws, m->attn_ws_bytes, dt, P(2), st));
-        if (w4) {
-            if (skip & 4) {
-            } else if (tp_fused) {
-                RCHECK(w4_gemm(m, m->ao, m->hq * d, L.q_o, nullptr, nullptr, B, ZL_EPI_NONE, nullptr, nullptr, l, 2, 0, 0, 2, nullptr, (xi++) | xodd));
-                pending = true;
-            } else if (tp) {
-                // row-parallel: partial sums -> one-shot NVLink all-reduce fused with the residual add
-                RCHECK(w4_gemm(m, m->ao, m->hq * d, L.q_o, nullptr, m->pend, B, ZL_EPI_NONE, nullptr, nullptr, l, 2));
-                RCHECK(zl_allreduce_one_shot(m->comm, m->pend, hc, hc, (size_t)B * D, dt, c.tp_int8, pdl, st));
-            } else {
-                RCHECK(w4_gemm(m, m->ao, m->hq * d, L.q_o, hc, hc, B, ZL_EPI_RESIDUAL, nullptr, nullptr, l, 2));
-            }
-            const void* xin = m->xn;
-            const void* lnw = nullptr;
-            if (c.fuse >= 1) {
-                xin = hc;
-                lnw = L.ln_ff;
-            } else {
-                RCHECK(zl_rmsnorm(hc, L.ln_ff, m->xn, B, D, c.eps, 1.f, dt, pdl, st));
-            }
-            if (!(skip & 8))
-                RCHECK(w4_gemm(m, xin, D, L.q_gu, nullptr, m->act, B, ZL_EPI_SWIGLU, lnw, nullptr, l, 3, 0, 0, pending ? 1 : 0, ho, (xi - 1) | xodd));
-            if (pending) {
-                std::swap(hc, ho);
-                pending = false;
-            }
-            if (skip & 16) {
-            } else if (tp_fused && l + 1 < c.num_layers) {
-                RCHECK(w4_gemm(m, m->act, m->ff, L.q_down, nullptr, nullptr, B, ZL_EPI_NONE, nullptr, nullptr, l, 4, 0, 0, 2, nullptr, (xi++) | xodd));
-                pending = true;
-            } else if (tp) {
-                RCHECK(w4_gemm(m, m->act, m->ff, L.q_down, nullptr, m->pend, B, ZL_EPI_NONE, nullptr, nullptr, l, 4));
-                RCHECK(zl_allreduce_one_shot(m->comm, m->pend, hc, hc, (size_t)B * D, dt, c.tp_int8, pdl, st));
-            } else {
-                RCHECK(w4_gemm(m, m->act, m->ff, L.q_down, hc, hc, B, ZL_EPI_RESIDUAL, nullptr, nullptr, l, 4));
-            }
+            RCHECK(zl_decode_attention(m->q.get(), m->d_lens.get() + pf->task, L.k_addrs.get() + pf->task,
+                                       L.v_addrs.get() + pf->task, m->d_mask.get(), scale, pf->pos0 + pf->n, m->ao.get(),
+                                       1, pf->n, m->hq, m->hkv, d, 1, m->attn_ws.get(), m->attn_ws_bytes, dt, pdl, st));
         } else {
-            RCHECK(dense_or_w8(m, m->ao, L.d_o, m->pend, B, pdl));
-            if (tp) RCHECK(zl_allreduce_one_shot(m->comm, m->pend, nullptr, m->pend, (size_t)B * D, dt, c.tp_int8, pdl, st));
-            RCHECK(zl_add_rmsnorm(m->h, m->pend, L.ln_ff, m->h, m->xn, B, D, c.eps, 1.f, 0, dt, pdl, st));
-            RCHECK(dense_or_w8(m, m->xn, L.d_gu, m->gu, B, pdl));
-            RCHECK(zl_gate_mul(m->gu, 2 * m->ff, (char*)m->gu + (size_t)m->ff * 2, 2 * m->ff, m->act, m->ff, B,
-                               m->ff, 0, dt, st));
-            RCHECK(dense_or_w8(m, m->act, L.d_down, m->pend, B, pdl));
-            if (tp) RCHECK(zl_allreduce_one_shot(m->comm, m->pend, nullptr, m->pend, (size_t)B * D, dt, c.tp_int8, pdl, st));
+            RCHECK(zl_decode_attention(m->q.get(), m->d_lens.get(), L.k_addrs.get(), L.v_addrs.get(), nullptr, scale,
+                                       len_bucket, m->ao.get(), B, 1, m->hq, m->hkv, d, 1, m->attn_ws.get(),
+                                       m->attn_ws_bytes, dt, stage_pdl(m, kAttn), st));
+        }
+        if (w4) {
+            RCHECK(o_gemm(m, l, ch));
+            RCHECK(gate_up_gemm(m, l, ch));
+            RCHECK(down_gemm(m, l, ch));
+        } else {
+            RCHECK(dense_or_w8(m, m->ao.get(), L.d_o, m->pend.get(), B, pdl));
+            if (tp)
+                RCHECK(zl_allreduce_one_shot(m->comm, m->pend.get(), nullptr, m->pend.get(), (size_t)B * D, dt, c.tp_int8,
+                                             pdl, st));
+            RCHECK(zl_add_rmsnorm(m->h.get(), m->pend.get(), L.ln_ff.get(), m->h.get(), m->xn.get(), B, D, c.eps, 1.f, 0,
+                                  dt, pdl, st));
+            RCHECK(dense_or_w8(m, m->xn.get(), L.d_gu, m->gu.get(), B, pdl));
+            RCHECK(zl_gate_mul(m->gu.get(), 2 * m->ff, (char*)m->gu.get() + (size_t)m->ff * 2, 2 * m->ff, m->act.get(),
+                               m->ff, B, m->ff, 0, dt, st));
+            RCHECK(dense_or_w8(m, m->act.get(), L.d_down, m->pend.get(), B, pdl));
+            if (tp)
+                RCHECK(zl_allreduce_one_shot(m->comm, m->pend.get(), nullptr, m->pend.get(), (size_t)B * D, dt, c.tp_int8,
+                                             pdl, st));
         }
     }
     if (pf) {
         if (!pf->last) return ZL_OK;
         // only the last prompt position feeds the head: move it to row 0 semantics by pointing at its row
-        const size_t off = (size_t)(pf->n - 1) * D * 2;
+        void* hl = rows(m->h.get(), pf->n - 1, D);
         if (w4) {
-            RCHECK(zl_rmsnorm((char*)m->h + off, m->ln_f, m->xn, 1, D, c.eps, 1.f, dt, pdl, st));
+            RCHECK(zl_rmsnorm(hl, m->ln_f.get(), m->xn.get(), 1, D, c.eps, 1.f, dt, pdl, st));
         } else {
-            RCHECK(zl_add_rmsnorm((char*)m->h + off, (char*)m->pend + off, m->ln_f, (char*)m->h + off, m->xn, 1, D, c.eps,
-                                  1.f, 0, dt, pdl, st));
+            RCHECK(zl_add_rmsnorm(hl, rows(m->pend.get(), pf->n - 1, D), m->ln_f.get(), hl, m->xn.get(), 1, D, c.eps, 1.f,
+                                  0, dt, pdl, st));
         }
     } else if (w4) {
-        RCHECK(zl_rmsnorm(hc, m->ln_f, m->xn, B, D, c.eps, 1.f, dt, P(32), st));
+        RCHECK(zl_rmsnorm(ch.h, m->ln_f.get(), m->xn.get(), B, D, c.eps, 1.f, dt, stage_pdl(m, kFinalNorm), st));
     } else {
-        RCHECK(zl_add_rmsnorm(m->h, m->pend, m->ln_f, m->h, m->xn, B, D, c.eps, 1.f, 0, dt, P(32), st));
+        RCHECK(zl_add_rmsnorm(m->h.get(), m->pend.get(), m->ln_f.get(), m->h.get(), m->xn.get(), B, D, c.eps, 1.f, 0, dt,
+                              stage_pdl(m, kFinalNorm), st));
     }
     const int HB = pf ? 1 : B;   // rows that reach lm_head
     // vocab-parallel lm_head (embedding.cu:353-392): each rank owns vshard rows
-    if (!(skip & 32))
-        RCHECK(zl_dense_gemm_skinny(m->xn, D, m->lm_head, nullptr, m->logits, HB, m->vshard, D, dt, ZL_F32, P(64), st));
+    RCHECK(zl_dense_gemm_skinny(m->xn.get(), D, m->lm_head, nullptr, m->logits.get(), HB, m->vshard, D, dt, ZL_F32,
+                                stage_pdl(m, kLmHead), st));
     if (sampler) {
         // one row per task at decode (row b = task b, counter = its input position); prefill: the task's last prompt
         // position.  set_sampling keeps this off under tensor parallelism.
-        const int32_t* row_task = pf ? m->d_iota + pf->task : m->d_iota;
-        const int32_t* counter = pf ? m->d_pf_pos + (pf->n - 1) : m->d_pos;
-        RCHECK(zl_sample(m->logits, HB, m->vshard, m->d_sparams, row_task, counter, m->d_hist, m->hwords, m->d_next,
-                         nullptr, 0, P(128), st));
+        const int32_t* row_task = pf ? m->d_iota.get() + pf->task : m->d_iota.get();
+        const int32_t* counter = pf ? m->d_pf_pos.get() + (pf->n - 1) : m->d_pos.get();
+        RCHECK(zl_sample(m->logits.get(), HB, m->vshard, m->d_sparams.get(), row_task, counter, m->d_hist.get(), m->hwords,
+                         m->d_next.get(), nullptr, 0, stage_pdl(m, kPick), st));
     } else if (!tp) {
-        RCHECK(zl_argmax(m->logits, m->d_next, HB, m->vshard, m->argmax_ws, zl_argmax_workspace_bytes(HB), P(128), st));
+        RCHECK(zl_argmax(m->logits.get(), m->d_next.get(), HB, m->vshard, m->argmax_ws.get(), zl_argmax_workspace_bytes(HB),
+                         stage_pdl(m, kPick), st));
     } else {
         // instead of all-gathering (B, V) logits, exchange one {value, index} candidate per token
         const int stride = ((HB * 8 + 15) / 16) * 2;   // int2 records per rank slot (16-byte multiple)
-        RCHECK(zl_argmax_candidates(m->logits, m->cand, HB, m->vshard, c.tp_rank * m->vshard, m->argmax_ws,
-                                    zl_argmax_workspace_bytes(HB), pdl, st));
-        RCHECK(zl_allgather_small(m->comm, m->cand, m->cand_all, (size_t)stride * 8, pdl, st));
-        RCHECK(zl_argmax_merge(m->cand_all, m->d_next, HB, c.tp_size, stride, pdl, st));
+        RCHECK(zl_argmax_candidates(m->logits.get(), m->cand.get(), HB, m->vshard, c.tp_rank * m->vshard,
+                                    m->argmax_ws.get(), zl_argmax_workspace_bytes(HB), pdl, st));
+        RCHECK(zl_allgather_small(m->comm, m->cand.get(), m->cand_all.get(), (size_t)stride * 8, pdl, st));
+        RCHECK(zl_argmax_merge(m->cand_all.get(), m->d_next.get(), HB, c.tp_size, stride, pdl, st));
     }
     return ZL_OK;
 }
@@ -1246,35 +1257,16 @@ extern "C" int zl_llama_set_comm(zl_llama_t* m, zl_comm_t* comm) {
 extern "C" void zl_llama_destroy(zl_llama_t* m) {
     if (!m) return;
     cudaStreamSynchronize(m->stream);
+    if (m->reduce_stream) cudaStreamSynchronize(m->reduce_stream);
     for (auto& g : m->graphs) cudaGraphExecDestroy(g.second);
-    for (auto& s : m->staged) cudaFree(s.second.ptr);
-    for (auto& L : m->layers) {
-        for (void* p : {L.ln_attn, L.ln_ff, L.q_qkv.packed, L.q_qkv.bias, L.q_o.packed, L.q_o.bias, L.q_gu.packed,
-                        L.q_down.packed, L.q_down.bias, (void*)L.q_qkv.k_perm, (void*)L.q_o.k_perm, (void*)L.q_gu.k_perm,
-                        (void*)L.q_down.k_perm, L.q_qkv.packed_i, L.q_o.packed_i, L.q_gu.packed_i, L.q_down.packed_i, L.d_qkv.w, L.d_qkv.bias, L.d_o.w, L.d_o.bias, L.d_gu.w,
-                        L.d_gu.bias, L.d_down.w, L.d_down.bias, L.d_qkv.w8, L.d_qkv.w_scale, L.d_o.w8, L.d_o.w_scale, L.d_gu.w8, L.d_gu.w_scale, L.d_down.w8, L.d_down.w_scale, L.kbuf, L.vbuf, (void*)L.k_addrs, (void*)L.v_addrs})
-            if (p) cudaFree(p);
-    }
-    for (void* p : {m->emb, m->lm_head_tied ? nullptr : m->lm_head, m->ln_f, m->h, m->xn, m->qkv, m->q, m->ao, m->act,
-                    m->pend, m->gu, (void*)m->logits, (void*)m->cosb, (void*)m->sinb, (void*)m->d_tokens,
-                    m->h2, (void*)m->d_pos, (void*)m->d_lens, (void*)m->d_next, (void*)m->d_iota, m->attn_ws, m->argmax_ws, (void*)m->d_tb, (void*)m->d_mask, m->xq, (void*)m->xs,
-                    (void*)m->d_hist, (void*)m->d_sparams, m->xperm})
-        if (p) cudaFree(p);
-    if (m->reduce_stream) {
-        cudaStreamSynchronize(m->reduce_stream);
-        for (int h = 0; h < 2; ++h)
-            for (cudaEvent_t e : {m->ev_o[h], m->ev_r1[h], m->ev_dn[h], m->ev_r2[h]})
-                if (e) cudaEventDestroy(e);
-        cudaStreamDestroy(m->reduce_stream);
-    }
-    if (m->h_stage) cudaFreeHost(m->h_stage);
-    if (m->h_ring) cudaFreeHost(m->h_ring);
+    for (int h = 0; h < 2; ++h)
+        for (cudaEvent_t e : {m->ev_o[h], m->ev_r1[h], m->ev_dn[h], m->ev_r2[h]})
+            if (e) cudaEventDestroy(e);
     for (cudaEvent_t e : m->ring_ev)
         if (e) cudaEventDestroy(e);
-    for (void* p : {(void*)m->d_pf_tokens, (void*)m->d_pf_pos})
-        if (p) cudaFree(p);
+    if (m->reduce_stream) cudaStreamDestroy(m->reduce_stream);
     cudaStreamDestroy(m->stream);
-    delete m;
+    delete m;   // the members free their device and pinned buffers
 }
 
 extern "C" int zl_llama_load_tensor(zl_llama_t* m, const char* name, const void* data_host, int rows, int cols,
@@ -1290,10 +1282,9 @@ extern "C" int zl_llama_load_tensor(zl_llama_t* m, const char* name, const void*
     s.elem = elem_bytes;
     const size_t bytes = (size_t)rows * cols * elem_bytes;
     RCHECK(dmalloc(&s.ptr, bytes));
-    ZL_CHECK_CUDA(cudaMemcpyAsync(s.ptr, data_host, bytes, cudaMemcpyHostToDevice, m->stream));
+    ZL_CHECK_CUDA(cudaMemcpyAsync(s.ptr.get(), data_host, bytes, cudaMemcpyHostToDevice, m->stream));
     ZL_CHECK_CUDA(cudaStreamSynchronize(m->stream));
-    drop(m, name);
-    m->staged[name] = s;
+    m->staged[name] = std::move(s);
     return ZL_OK;
 }
 
@@ -1320,12 +1311,12 @@ int stage_random(zl_llama* m, const std::string& name, int rows, int cols, int e
     uint64_t h = seed;
     for (char ch : name) h = h * 1099511628211ull + (unsigned char)ch;
     if (kind == 0)
-        RCHECK(zl_fill_random_u32((uint32_t*)s.ptr, n, h, m->stream));
+        RCHECK(zl_fill_random_u32((uint32_t*)s.ptr.get(), n, h, m->stream));
     else if (kind == 1)
-        RCHECK(zl_fill_const_u32((uint32_t*)s.ptr, n, 0x77777777u, m->stream));
+        RCHECK(zl_fill_const_u32((uint32_t*)s.ptr.get(), n, 0x77777777u, m->stream));
     else
-        RCHECK(zl_fill_uniform(s.ptr, n, lo, hi, h, m->cfg.dtype, m->stream));
-    m->staged[name] = s;
+        RCHECK(zl_fill_uniform(s.ptr.get(), n, lo, hi, h, m->cfg.dtype, m->stream));
+    m->staged[name] = std::move(s);
     return ZL_OK;
 }
 
@@ -1337,7 +1328,7 @@ int stage_random_linear(zl_llama* m, const std::string& prefix, int K, int N, ui
         if (c.sym) {
             const size_t words = (size_t)(K / 8) * N;
             k_recentre_nibbles<<<(unsigned)((words + 255) / 256), 256, 0, m->stream>>>(
-                static_cast<uint32_t*>(m->staged[prefix + ".qweight"].ptr), words);
+                static_cast<uint32_t*>(m->staged[prefix + ".qweight"].ptr.get()), words);
             ZL_CHECK_LAUNCH();
         }
         RCHECK(stage_random(m, prefix + ".qzeros", G, N / 8, 4, c.sym ? 1 : 0, 0, 0, seed));
@@ -1352,7 +1343,7 @@ int stage_random_linear(zl_llama* m, const std::string& prefix, int K, int N, ui
         RCHECK(stage_random(m, prefix + ".weight", N, K / 4, 4, 0, 0, 0, seed));
         Staged& w = m->staged[prefix + ".weight"];
         const size_t words = (size_t)N * K / 4;
-        k_and_u32<<<(unsigned)((words + 255) / 256), 256, 0, m->stream>>>(static_cast<uint32_t*>(w.ptr), words, 0xBFBFBFBFu);
+        k_and_u32<<<(unsigned)((words + 255) / 256), 256, 0, m->stream>>>(static_cast<uint32_t*>(w.ptr.get()), words, 0xBFBFBFBFu);
         ZL_CHECK_LAUNCH();
         w.cols = K;
         w.elem = 1;
@@ -1360,9 +1351,9 @@ int stage_random_linear(zl_llama* m, const std::string& prefix, int K, int N, ui
         sc.rows = sc.cols = 1;
         sc.elem = 4;
         RCHECK(dmalloc(&sc.ptr, 4));
-        k_set_f32<<<1, 1, 0, m->stream>>>(static_cast<float*>(sc.ptr), 0.03f);
+        k_set_f32<<<1, 1, 0, m->stream>>>(static_cast<float*>(sc.ptr.get()), 0.03f);
         ZL_CHECK_LAUNCH();
-        m->staged[prefix + ".weight_scale"] = sc;
+        m->staged[prefix + ".weight_scale"] = std::move(sc);
     } else {
         RCHECK(stage_random(m, prefix + ".weight", N, K, 2, 2, -0.035f, 0.035f, seed));   // ~ randn*0.02
     }
@@ -1412,7 +1403,7 @@ extern "C" int zl_llama_set_state(zl_llama_t* m, const int32_t* tokens_host, con
     const int slot = m->ring_next;
     m->ring_next = (slot + 1) % zl_llama::kStageSlots;
     if (m->ring_used[slot]) ZL_CHECK_CUDA(cudaEventSynchronize(m->ring_ev[slot]));   // its previous copies have executed
-    int32_t* hs = m->h_ring + (size_t)slot * 2 * m->cfg.max_batch;
+    int32_t* hs = m->h_ring.get() + (size_t)slot * 2 * m->cfg.max_batch;
     int mx = 0;
     for (int i = 0; i < B; ++i) {
         ZL_CHECK_ARG(positions_host[i] >= 0 && positions_host[i] < m->cfg.max_seq);
@@ -1422,8 +1413,8 @@ extern "C" int zl_llama_set_state(zl_llama_t* m, const int32_t* tokens_host, con
         if (positions_host[i] + 1 > mx) mx = positions_host[i] + 1;
     }
     m->cur_max_len = mx;
-    ZL_CHECK_CUDA(cudaMemcpyAsync(m->d_tokens, hs, B * 4, cudaMemcpyHostToDevice, m->stream));
-    ZL_CHECK_CUDA(cudaMemcpyAsync(m->d_pos, hs + B, B * 4, cudaMemcpyHostToDevice, m->stream));
+    ZL_CHECK_CUDA(cudaMemcpyAsync(m->d_tokens.get(), hs, B * 4, cudaMemcpyHostToDevice, m->stream));
+    ZL_CHECK_CUDA(cudaMemcpyAsync(m->d_pos.get(), hs + B, B * 4, cudaMemcpyHostToDevice, m->stream));
     ZL_CHECK_CUDA(cudaEventRecord(m->ring_ev[slot], m->stream));
     m->ring_used[slot] = true;
     return ZL_OK;
@@ -1436,7 +1427,7 @@ extern "C" int zl_llama_step_device(zl_llama_t* m, int B) {
         return ZL_ERR_STATE;
     }
     RCHECK(run_step(m, B));
-    k_advance<<<cdiv(B, 64), 64, 0, m->stream>>>(m->d_tokens, m->d_pos, m->d_next, B, g_w4_trace);
+    k_advance<<<cdiv(B, 64), 64, 0, m->stream>>>(m->d_tokens.get(), m->d_pos.get(), m->d_next.get(), B, g_w4_trace);
     ZL_CHECK_LAUNCH();
     m->cur_max_len += 1;
     return ZL_OK;
@@ -1447,30 +1438,30 @@ extern "C" int zl_llama_decode(zl_llama_t* m, const int32_t* tokens_host, const 
     ZL_CHECK_ARG(next_tokens_host != nullptr);
     RCHECK(zl_llama_set_state(m, tokens_host, positions_host, B));
     RCHECK(run_step(m, B));
-    ZL_CHECK_CUDA(cudaMemcpyAsync(m->h_stage + 3 * B, m->d_next, B * 4, cudaMemcpyDeviceToHost, m->stream));
+    ZL_CHECK_CUDA(cudaMemcpyAsync(m->h_stage.get() + 3 * B, m->d_next.get(), B * 4, cudaMemcpyDeviceToHost, m->stream));
     if (logits_host)   // (B, vocab/tp) of this rank's shard
-        ZL_CHECK_CUDA(cudaMemcpyAsync(logits_host, m->logits, (size_t)B * m->vshard * 4, cudaMemcpyDeviceToHost,
+        ZL_CHECK_CUDA(cudaMemcpyAsync(logits_host, m->logits.get(), (size_t)B * m->vshard * 4, cudaMemcpyDeviceToHost,
                                       m->stream));
     ZL_CHECK_CUDA(cudaStreamSynchronize(m->stream));
-    for (int i = 0; i < B; ++i) next_tokens_host[i] = m->h_stage[3 * B + i];
+    for (int i = 0; i < B; ++i) next_tokens_host[i] = m->h_stage.get()[3 * B + i];
     return ZL_OK;
 }
 
 extern "C" int zl_llama_get_state(zl_llama_t* m, int32_t* tokens_host, int32_t* positions_host, int B) {
     ZL_CHECK_ARG(m && tokens_host && positions_host && B > 0 && B <= m->cfg.max_batch);
-    ZL_CHECK_CUDA(cudaMemcpyAsync(m->h_stage, m->d_tokens, B * 4, cudaMemcpyDeviceToHost, m->stream));
-    ZL_CHECK_CUDA(cudaMemcpyAsync(m->h_stage + B, m->d_pos, B * 4, cudaMemcpyDeviceToHost, m->stream));
+    ZL_CHECK_CUDA(cudaMemcpyAsync(m->h_stage.get(), m->d_tokens.get(), B * 4, cudaMemcpyDeviceToHost, m->stream));
+    ZL_CHECK_CUDA(cudaMemcpyAsync(m->h_stage.get() + B, m->d_pos.get(), B * 4, cudaMemcpyDeviceToHost, m->stream));
     ZL_CHECK_CUDA(cudaStreamSynchronize(m->stream));
     for (int i = 0; i < B; ++i) {
-        tokens_host[i] = m->h_stage[i];
-        positions_host[i] = m->h_stage[B + i];
+        tokens_host[i] = m->h_stage.get()[i];
+        positions_host[i] = m->h_stage.get()[B + i];
     }
     return ZL_OK;
 }
 
 extern "C" int zl_llama_get_logits(zl_llama_t* m, float* logits_host, int B) {
     ZL_CHECK_ARG(m && logits_host && B > 0 && B <= m->cfg.max_batch);
-    ZL_CHECK_CUDA(cudaMemcpyAsync(logits_host, m->logits, (size_t)B * m->vshard * 4, cudaMemcpyDeviceToHost, m->stream));
+    ZL_CHECK_CUDA(cudaMemcpyAsync(logits_host, m->logits.get(), (size_t)B * m->vshard * 4, cudaMemcpyDeviceToHost, m->stream));
     ZL_CHECK_CUDA(cudaStreamSynchronize(m->stream));
     return ZL_OK;
 }
@@ -1478,10 +1469,18 @@ extern "C" int zl_llama_get_logits(zl_llama_t* m, float* logits_host, int B) {
 extern "C" int zl_llama_bench_gemms(zl_llama_t* m, int B, int iters, float* ms, int* launches, double* bytes) {
     ZL_CHECK_ARG(m && B > 0 && B <= m->cfg.max_batch && iters > 0 && ms);
     const auto& c = m->cfg;
-    const int D = c.dim_model, d = c.dim_head, dt = c.dtype, pdl = c.use_pdl;
+    const int D = c.dim_model, d = c.dim_head, pdl = c.use_pdl;
     const bool w4 = c.quant_type == 5 || c.quant_type == 6;
     cudaStream_t st = m->stream;
-    (void)pdl;
+    // the decode step's W4 GEMMs, launched by the same functions (fused RMSNorm, qkv RoPE + KV append, SwiGLU and residual
+    // epilogues, PDL policy).  Rewrites the KV rows of the current positions and the residual stream: call it after the
+    // measurements that need the decode state.
+    Chain ch;
+    ch.n = B;
+    ch.gemm_only = true;
+    ch.h = m->h.get();
+    m->cur_tb = m->d_iota.get();
+    m->cur_pos = m->d_pos.get();
     cudaEvent_t e0, e1;
     ZL_CHECK_CUDA(cudaEventCreate(&e0));
     ZL_CHECK_CUDA(cudaEventCreate(&e1));
@@ -1492,20 +1491,10 @@ extern "C" int zl_llama_bench_gemms(zl_llama_t* m, int B, int iters, float* ms, 
         for (int l = 0; l < c.num_layers; ++l) {
             Layer& L = m->layers[l];
             if (w4) {
-                // the SAME kernel variants as the decode step (enqueue_step): fused RMSNorm prologue, qkv RoPE + KV-append
-                // epilogue, SwiGLU, residual epilogues, per-kernel PDL policy.  (Rewrites the KV rows of the current
-                // positions and the residual stream: call it after the measurements that need the decode state.)
-                const void* ln1 = c.fuse >= 1 ? L.ln_attn : nullptr;
-                const void* ln2 = c.fuse >= 1 ? L.ln_ff : nullptr;
-                m->cur_tb = m->d_iota;
-                m->cur_pos = m->d_pos;
-                if (c.fuse >= 2)
-                    RCHECK(w4_gemm(m, m->h, D, L.q_qkv, nullptr, nullptr, B, ZL_EPI_QKV_ROPE, ln1, &L, l, 0));
-                else
-                    RCHECK(w4_gemm(m, ln1 ? m->h : m->xn, D, L.q_qkv, nullptr, m->qkv, B, ZL_EPI_NONE, ln1, nullptr, l, 0));
-                RCHECK(w4_gemm(m, m->ao, m->hq * d, L.q_o, m->h, m->h, B, ZL_EPI_RESIDUAL, nullptr, nullptr, l, 2));
-                RCHECK(w4_gemm(m, ln2 ? m->h : m->xn, D, L.q_gu, nullptr, m->act, B, ZL_EPI_SWIGLU, ln2, nullptr, l, 3));
-                RCHECK(w4_gemm(m, m->act, m->ff, L.q_down, m->h, m->h, B, ZL_EPI_RESIDUAL, nullptr, nullptr, l, 4));
+                RCHECK(qkv_gemm(m, l, ch));
+                RCHECK(o_gemm(m, l, ch));
+                RCHECK(gate_up_gemm(m, l, ch));
+                RCHECK(down_gemm(m, l, ch));
                 if (it == 0) {
                     nbytes += (double)zl_w4_packed_bytes(L.q_qkv.N, D, c.group_size) +
                               (double)zl_w4_packed_bytes(D, m->hq * d, c.group_size) +
@@ -1515,10 +1504,10 @@ extern "C" int zl_llama_bench_gemms(zl_llama_t* m, int B, int iters, float* ms, 
                     nbytes += 2.0 * B * (D + L.q_qkv.N + m->hq * d + 2 * D + D + m->ff + m->ff + 2 * D);
                 }
             } else {
-                RCHECK(dense_or_w8(m, m->xn, L.d_qkv, m->qkv, B, pdl));
-                RCHECK(dense_or_w8(m, m->ao, L.d_o, m->pend, B, pdl));
-                RCHECK(dense_or_w8(m, m->xn, L.d_gu, m->gu, B, pdl));
-                RCHECK(dense_or_w8(m, m->act, L.d_down, m->pend, B, pdl));
+                RCHECK(dense_or_w8(m, m->xn.get(), L.d_qkv, m->qkv.get(), B, pdl));
+                RCHECK(dense_or_w8(m, m->ao.get(), L.d_o, m->pend.get(), B, pdl));
+                RCHECK(dense_or_w8(m, m->xn.get(), L.d_gu, m->gu.get(), B, pdl));
+                RCHECK(dense_or_w8(m, m->act.get(), L.d_down, m->pend.get(), B, pdl));
                 if (it == 0) {
                     // weight bytes: 2 per element dense, 1 (+ per-row scale) for W8A8 (SURVEY 8d)
                     const double wb = L.d_qkv.w8 ? 1.0 : 2.0;
@@ -1558,7 +1547,7 @@ extern "C" int zl_llama_prefill(zl_llama_t* m, int task, const int32_t* tokens_h
         zl_set_last_error(__FILE__, __LINE__, "prompt does not fit the KV buffers (max_seq)");
         return ZL_ERR_STATE;
     }
-    int32_t* h_tok = m->h_stage + 4 * m->cfg.max_batch + 4;   // pinned staging for one chunk of token ids
+    int32_t* h_tok = m->h_stage.get() + 4 * m->cfg.max_batch + 4;   // pinned staging for one chunk of token ids
     for (int c0 = 0; c0 < n; c0 += chunk) {
         const int cn = (n - c0) < chunk ? (n - c0) : chunk;
         if (c0 > 0) ZL_CHECK_CUDA(cudaStreamSynchronize(m->stream));   // staging buffer reuse
@@ -1566,15 +1555,15 @@ extern "C" int zl_llama_prefill(zl_llama_t* m, int task, const int32_t* tokens_h
             ZL_CHECK_ARG(tokens_host[c0 + i] >= 0 && tokens_host[c0 + i] < m->cfg.vocab_size);
             h_tok[i] = tokens_host[c0 + i];
         }
-        ZL_CHECK_CUDA(cudaMemcpyAsync(m->d_pf_tokens, h_tok, cn * 4, cudaMemcpyHostToDevice, m->stream));
+        ZL_CHECK_CUDA(cudaMemcpyAsync(m->d_pf_tokens.get(), h_tok, cn * 4, cudaMemcpyHostToDevice, m->stream));
         PrefillChunk pc{task, pos0 + c0, cn, c0 + cn == n};
         RCHECK(enqueue_step(m, 1, 0, &pc, sampler_on(m, task, 1)));
     }
-    ZL_CHECK_CUDA(cudaMemcpyAsync(m->h_stage + 3 * m->cfg.max_batch, m->d_next, 4, cudaMemcpyDeviceToHost, m->stream));
+    ZL_CHECK_CUDA(cudaMemcpyAsync(m->h_stage.get() + 3 * m->cfg.max_batch, m->d_next.get(), 4, cudaMemcpyDeviceToHost, m->stream));
     if (logits_host)
-        ZL_CHECK_CUDA(cudaMemcpyAsync(logits_host, m->logits, (size_t)m->vshard * 4, cudaMemcpyDeviceToHost, m->stream));
+        ZL_CHECK_CUDA(cudaMemcpyAsync(logits_host, m->logits.get(), (size_t)m->vshard * 4, cudaMemcpyDeviceToHost, m->stream));
     ZL_CHECK_CUDA(cudaStreamSynchronize(m->stream));
-    *next_token_host = m->h_stage[3 * m->cfg.max_batch];
+    *next_token_host = m->h_stage.get()[3 * m->cfg.max_batch];
     if (pos0 + n > m->cur_max_len) m->cur_max_len = pos0 + n;
     return ZL_OK;
 }
@@ -1591,8 +1580,8 @@ extern "C" int zl_llama_set_sampling(zl_llama_t* m, int task, const zl_sample_pa
     }
     const zl_sample_params_t q = p ? *p : zl_sample_params_t{0.f, 1.f, 1.f, 0.f, 0, 0};
     // stream-ordered after every step already enqueued; the pageable source is staged before the call returns
-    ZL_CHECK_CUDA(cudaMemcpyAsync(m->d_sparams + task, &q, sizeof(q), cudaMemcpyHostToDevice, m->stream));
-    ZL_CHECK_CUDA(cudaMemsetAsync(m->d_hist + (size_t)task * m->hwords, 0, (size_t)m->hwords * 4, m->stream));
+    ZL_CHECK_CUDA(cudaMemcpyAsync(m->d_sparams.get() + task, &q, sizeof(q), cudaMemcpyHostToDevice, m->stream));
+    ZL_CHECK_CUDA(cudaMemsetAsync(m->d_hist.get() + (size_t)task * m->hwords, 0, (size_t)m->hwords * 4, m->stream));
     m->samp_on[task] = on ? 1 : 0;
     return ZL_OK;
 }

@@ -147,6 +147,13 @@ typedef struct zl_w4_fused_args {
     int variant; /* layout of `packed`: 0 ZLW4, 1 ZLW4I (integer kernel; needs the staged activations to fit smem) */
     zl_comm_t* tp_comm; int tp_mode; void* tp_h_out; int tp_index;
     const int32_t* k_perm; /* act-order activation permutation (K), or NULL */
+    /* int8 KV cache (ZL_EPI_QKV_ROPE on the exact-integer route only; the wgmma and fp16 routes and k_perm return
+     * ZL_ERR_UNSUPPORTED): kv_int8 != 0 appends every K (after RoPE) / V row in the contract of zl_decode_attention_kv8 --
+     * k_addrs / v_addrs are the tasks' uint8 code buffers, scale_k_addrs / scale_v_addrs their fp32 scale buffers -- with
+     * the arithmetic of zl_kv_int8_quant_append, bit for bit.  kv8_stage: (M, 2, num_kv_heads, dim_head) fp16 scratch;
+     * kv8_counters: (M, 2, num_kv_heads) uint32, zero before the first launch; each launch leaves them zero.  Launches that
+     * share the counters must be stream-ordered. */
+    int kv_int8; void* const* scale_k_addrs; void* const* scale_v_addrs; void* kv8_stage; uint32_t* kv8_counters;
 } zl_w4_fused_args_t;
 /* sizeof(zl_w4_fused_args_t) and offsetof(zl_w4_fused_args_t, k_perm), so that bindings can check their mirror. */
 int zl_w4_fused_args_layout(size_t* size, size_t* k_perm_offset);
@@ -416,7 +423,14 @@ typedef struct zl_llama_config {
                         * (chunked prefill, zhilight/config/adapter.py:47-48) */
     int qkv_bias; /* zl_llama_init_synthetic: also create q/k/v biases (Qwen2: attention.cpp:105-109); loaded checkpoints
                    * carry their ".bias" tensors regardless of this flag */
+    int kv_int8; /* 0: KV cache in the activation dtype.  1: int8 KV cache (KV_CACHE_DTYPE=int8, model_context.cpp:61-79) in
+                  * the contract of zl_decode_attention_kv8: every appended K (after RoPE) / V row is quantised per
+                  * (token, kv head) and decode, chunked prefill and the dual-stream prefill attend over the quantised
+                  * cache with zl_decode_attention_kv8 (the reference attends a prompt over an fp16 copy of its own K/V).
+                  * fp16 only, dim_head 64 or 128, max_seq <= 65536: other configurations return ZL_ERR_UNSUPPORTED */
 } zl_llama_config_t;
+/* sizeof(zl_llama_config_t) and offsetof(zl_llama_config_t, kv_int8), so that bindings can check their mirror. */
+int zl_llama_config_layout(size_t* size, size_t* kv_int8_offset);
 
 int zl_llama_create(const zl_llama_config_t* cfg, zl_llama_t** out);
 /* tensor parallel: hand the driver its exchange object (zl_comm_create + open_peers) before the first step. */
@@ -459,6 +473,12 @@ int zl_llama_prefill(zl_llama_t* m, int task, const int32_t* tokens_host, int n,
  * samples or has penalties (counter = the input token's position; prefill: pos0 + n - 1), so a task draws the same
  * tokens with host or device-resident stepping, with or without the graph.  The logits stay the raw lm_head output. */
 int zl_llama_set_sampling(zl_llama_t* m, int task, const zl_sample_params_t* p);
+/* Copy rows row0 .. row0 + n of task `task`'s layer-`layer` KV cache to the host (the reference's dump_task_buf,
+ * rag_buffer_context.h:199-233).  Synchronous.  Plain cache: k_host / v_host get (n, H_kv, d) activation-dtype values and
+ * sk_host / sv_host must be NULL.  kv_int8: k_host / v_host get (n, H_kv, d) uint8 codes and sk_host / sv_host (n, H_kv)
+ * fp32 scales (either may be NULL to skip it).  H_kv is this rank's kv heads. */
+int zl_llama_read_kv(zl_llama_t* m, int layer, int task, int row0, int n, void* k_host, void* v_host, float* sk_host,
+                     float* sv_host);
 zl_stream_t zl_llama_stream(zl_llama_t* m);
 /* bytes the step must read from HBM per rank (weights + lm_head + norms), kernel launches per step. */
 int zl_llama_stats(zl_llama_t* m, int B, double* weight_bytes, int* kernels_per_step);

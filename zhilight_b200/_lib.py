@@ -34,7 +34,7 @@ class LlamaConfig(ctypes.Structure):
         ("dtype", ctypes.c_int), ("max_batch", ctypes.c_int), ("max_seq", ctypes.c_int),
         ("tp_rank", ctypes.c_int), ("tp_size", ctypes.c_int),
         ("use_pdl", ctypes.c_int), ("use_graph", ctypes.c_int), ("tp_int8", ctypes.c_int), ("fuse", ctypes.c_int), ("prefill_chunk", ctypes.c_int),
-        ("qkv_bias", ctypes.c_int),
+        ("qkv_bias", ctypes.c_int), ("kv_int8", ctypes.c_int),
     ]
 
 
@@ -54,6 +54,8 @@ class W4FusedArgs(ctypes.Structure):
         ("variant", ctypes.c_int),
         ("tp_comm", ctypes.c_void_p), ("tp_mode", ctypes.c_int), ("tp_h_out", ctypes.c_void_p), ("tp_index", ctypes.c_int),
         ("k_perm", ctypes.c_void_p),
+        ("kv_int8", ctypes.c_int), ("scale_k_addrs", ctypes.c_void_p), ("scale_v_addrs", ctypes.c_void_p),
+        ("kv8_stage", ctypes.c_void_p), ("kv8_counters", ctypes.c_void_p),
     ]
 
 

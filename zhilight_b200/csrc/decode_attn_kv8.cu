@@ -15,6 +15,7 @@
 // to the exact result.  Half the algorithmic bytes of the fp16 cache: 2 * H_kv * d * ctx + 8 * H_kv * ctx per task per layer.
 #include "common.cuh"
 #include "decode_attn_short.cuh"
+#include "kv8_quant.cuh"
 
 namespace zl {
 
@@ -279,11 +280,9 @@ __global__ void k_kv8_quant_append(const T* __restrict__ k_src, const T* __restr
     const int pl = placement[tok];
     if (pl < 0) return;
     const int b = token_batch[tok];
-    const float block_scale = 127.0f / amax;                      // quant_kernel.cu:31
-    const float r = nearbyintf(x * block_scale);
     uint8_t* dst = (is_v ? v_addrs : k_addrs)[b] + ((size_t)pl * num_kv_heads + hk) * d;
-    dst[c] = (uint8_t)(128.f + r);
-    if (c == 0) (is_v ? sv_addrs : sk_addrs)[b][(size_t)pl * num_kv_heads + hk] = amax / 127.0f;
+    dst[c] = kv8_code(x, kv8_row_mul(amax));
+    if (c == 0) (is_v ? sv_addrs : sk_addrs)[b][(size_t)pl * num_kv_heads + hk] = kv8_row_scale(amax);
 }
 
 // dense form of the same quantisation: int8_op::quant_calc_scale(x, 127, 128) on (M, K) rows -> uint8 codes + fp32 scales
@@ -298,10 +297,9 @@ __global__ void k_int8_quant_rows_u8(const T* __restrict__ x, uint8_t* __restric
     __syncthreads();
     amax = 0.f;
     for (int w = 0; w < (int)(blockDim.x + 31) / 32; ++w) amax = fmaxf(amax, s_max[w]);
-    const float block_scale = 127.0f / amax;
-    for (int i = threadIdx.x; i < K; i += blockDim.x)
-        q[off + i] = (uint8_t)(128.f + nearbyintf(to_f32<T>(x[off + i]) * block_scale));
-    if (threadIdx.x == 0) scale[blockIdx.x] = amax / 127.0f;
+    const float mul = kv8_row_mul(amax);
+    for (int i = threadIdx.x; i < K; i += blockDim.x) q[off + i] = kv8_code(to_f32<T>(x[off + i]), mul);
+    if (threadIdx.x == 0) scale[blockIdx.x] = kv8_row_scale(amax);
 }
 
 }  // namespace zl

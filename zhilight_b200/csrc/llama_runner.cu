@@ -62,10 +62,14 @@ struct Layer {
     dev_ptr<> ln_ff;
     W4Lin q_qkv, q_o, q_gu, q_down;
     DenseLin d_qkv, d_o, d_gu, d_down;
-    dev_ptr<> kbuf;   // (max_batch, max_seq, Hkv, d)
+    dev_ptr<> kbuf;   // (max_batch, max_seq, Hkv, d): activation dtype, or uint8 codes at kv_int8
     dev_ptr<> vbuf;
     dev_ptr<void*> k_addrs;   // (max_batch)
     dev_ptr<void*> v_addrs;
+    dev_ptr<> skbuf;          // kv_int8: (max_batch, max_seq, Hkv) fp32 scales
+    dev_ptr<> svbuf;
+    dev_ptr<void*> sk_addrs;  // (max_batch)
+    dev_ptr<void*> sv_addrs;
 };
 
 }  // namespace
@@ -130,6 +134,16 @@ struct zl_llama {
     dev_ptr<uint32_t> d_hist;                // (max_batch, hwords)
     int hwords = 0;
     std::vector<char> samp_on;
+    // int8 KV cache: the rotated fp16 K / V rows of the launch sequence are staged in kv_stage (k: tok_cap x Hkv x d, then
+    // v) and quantised into the cache from there.  A qkv GEMM with the RoPE / KV-append epilogue appends into the staging
+    // rows as into the cache of one task: stage_addrs = {k rows, v rows}, token -> task map d_zeros, placement d_rowidx.
+    dev_ptr<> kv_stage;
+    dev_ptr<void*> stage_addrs;
+    dev_ptr<int32_t> d_zeros, d_rowidx;      // (tok_cap): 0 ..., and 0, 1, 2, ...
+    // the integer qkv GEMM's int8-cache epilogue: fp16 rows (16, 2, Hkv, d) and last-arriver counters (16, 2, Hkv), zero
+    // between launches (every qkv GEMM of the model runs in stream order on the compute stream)
+    dev_ptr<__half> kv8_rows;
+    dev_ptr<uint32_t> kv8_cnt;
 };
 
 namespace {
@@ -620,22 +634,44 @@ int finalize_globals(zl_llama* m) {
 int alloc_runtime(zl_llama* m) {
     const auto& c = m->cfg;
     const int B = c.max_batch, D = c.dim_model, d = c.dim_head;
-    const size_t kv_task = (size_t)c.max_seq * m->hkv * d * 2;
-    for (auto& L : m->layers) {
-        RCHECK(dmalloc(&L.kbuf, kv_task * B));
-        RCHECK(dmalloc(&L.vbuf, kv_task * B));
-        // never-written rows must be finite: masked keys still multiply their V rows by an exact 0, and with the
-        // dual-stream prefill one half's attention sees the other half's rows before they are appended
-        ZL_CHECK_CUDA(cudaMemsetAsync(L.kbuf.get(), 0, kv_task * B, m->stream));
-        ZL_CHECK_CUDA(cudaMemsetAsync(L.vbuf.get(), 0, kv_task * B, m->stream));
-        RCHECK(dmalloc(&L.k_addrs, sizeof(void*) * B));
-        RCHECK(dmalloc(&L.v_addrs, sizeof(void*) * B));
-        k_ptr_table<<<cdiv(B, 256), 256, 0, m->stream>>>(L.k_addrs.get(), (char*)L.kbuf.get(), kv_task, B);
-        k_ptr_table<<<cdiv(B, 256), 256, 0, m->stream>>>(L.v_addrs.get(), (char*)L.vbuf.get(), kv_task, B);
+    // bytes per task: codes (1 byte per value) + one fp32 scale per (token, kv head) at kv_int8, else 2 bytes per value
+    const size_t kv_task = (size_t)c.max_seq * m->hkv * d * (c.kv_int8 ? 1 : 2);
+    const size_t sc_task = (size_t)c.max_seq * m->hkv * 4;
+    // never-written rows must be finite: masked keys still multiply their V rows by an exact 0, and with the dual-stream
+    // prefill one half's attention sees the other half's rows before they are appended.  Zero codes with zero scales
+    // decode to 0.
+    auto cache = [&](dev_ptr<>* buf, dev_ptr<void*>* tab, size_t per_task) -> int {
+        RCHECK(dmalloc(buf, per_task * B));
+        ZL_CHECK_CUDA(cudaMemsetAsync(buf->get(), 0, per_task * B, m->stream));
+        RCHECK(dmalloc(tab, sizeof(void*) * B));
+        k_ptr_table<<<cdiv(B, 256), 256, 0, m->stream>>>(tab->get(), (char*)buf->get(), per_task, B);
         ZL_CHECK_LAUNCH();
+        return ZL_OK;
+    };
+    for (auto& L : m->layers) {
+        RCHECK(cache(&L.kbuf, &L.k_addrs, kv_task));
+        RCHECK(cache(&L.vbuf, &L.v_addrs, kv_task));
+        if (c.kv_int8) {
+            RCHECK(cache(&L.skbuf, &L.sk_addrs, sc_task));
+            RCHECK(cache(&L.svbuf, &L.sv_addrs, sc_task));
+        }
     }
     const int T = c.prefill_chunk > B ? c.prefill_chunk : B;   // tokens per launch: decode batch or prefill chunk
     m->tok_cap = T;
+    if (c.kv_int8) {
+        const size_t rows_bytes = (size_t)T * m->hkv * d * 2;
+        RCHECK(dmalloc(&m->kv_stage, 2 * rows_bytes));
+        RCHECK(dmalloc(&m->stage_addrs, sizeof(void*) * 2));
+        k_ptr_table<<<1, 32, 0, m->stream>>>(m->stage_addrs.get(), (char*)m->kv_stage.get(), rows_bytes, 2);
+        RCHECK(dmalloc(&m->d_zeros, (size_t)T * 4));
+        ZL_CHECK_CUDA(cudaMemsetAsync(m->d_zeros.get(), 0, (size_t)T * 4, m->stream));
+        RCHECK(dmalloc(&m->d_rowidx, (size_t)T * 4));
+        k_iota<<<cdiv(T, 256), 256, 0, m->stream>>>(m->d_rowidx.get(), T);
+        ZL_CHECK_LAUNCH();
+        RCHECK(dmalloc(&m->kv8_rows, (size_t)16 * 2 * m->hkv * d * 2));
+        RCHECK(dmalloc(&m->kv8_cnt, (size_t)16 * 2 * m->hkv * 4));
+        ZL_CHECK_CUDA(cudaMemsetAsync(m->kv8_cnt.get(), 0, (size_t)16 * 2 * m->hkv * 4, m->stream));
+    }
     RCHECK(dmalloc(&m->h, (size_t)T * D * 2));
     RCHECK(dmalloc(&m->xn, (size_t)T * D * 2));
     if (c.tp_size > 1) RCHECK(dmalloc(&m->h2, (size_t)T * D * 2));
@@ -672,6 +708,8 @@ int alloc_runtime(zl_llama* m) {
     RCHECK(dmalloc(&m->d_iota, B * 4));
     k_iota<<<cdiv(B, 256), 256, 0, m->stream>>>(m->d_iota.get(), B);
     ZL_CHECK_LAUNCH();
+    // also bounds zl_decode_attention_kv8: it splits the keys into at most 64 pieces (kA8MaxSplits, at least
+    // cdiv(max_len, 1024)) over B * len_q <= T query rows, and this reserves T * Hq * max(64, cdiv(max_seq, 1024)) pieces
     m->attn_ws_bytes = zl_decode_attention_workspace_bytes(T, 1, m->hq, d, c.max_seq);
     RCHECK(dmalloc(&m->attn_ws, m->attn_ws_bytes));
     RCHECK(dmalloc(&m->argmax_ws, zl_argmax_workspace_bytes(B)));
@@ -854,8 +892,34 @@ int w4_gemm(zl_llama* m, int l, Stage s, const Chain& ch, const W4Lin& w, const 
     return w4a16_gemm_fused_l2(&a, &l2, m->stream);
 }
 
+// int8 KV cache: the staged rotated K / V rows of ch's tokens -> codes and scales at their placement in their task's cache
+// (int8_op::quant_calc_scale(x, 127, 128) + copy_to_rag_buffer2, attention.cpp:656-676)
+int kv8_append(zl_llama* m, int l, const Chain& ch, int pdl) {
+    const auto& c = m->cfg;
+    const Layer& L = m->layers[l];
+    const size_t row = (size_t)m->hkv * c.dim_head;
+    const __half* ks = static_cast<const __half*>(m->kv_stage.get()) + ch.row0 * row;
+    const __half* vs = static_cast<const __half*>(m->kv_stage.get()) + ((size_t)m->tok_cap + ch.row0) * row;
+    return zl_kv_int8_quant_append(ks, vs, m->cur_tb + ch.row0, m->cur_pos + ch.row0, L.k_addrs.get(), L.v_addrs.get(),
+                                   L.sk_addrs.get(), L.sv_addrs.get(), ch.n, m->hkv, c.dim_head, c.dtype, pdl, m->stream);
+}
+
+// int8 KV cache after a GEMM that wrote the fused qkv rows of ch: split + RoPE (zl_rope_qk_cache) into q and the staging
+// rows, then quantise those into the cache -- the reference's own operator sequence (attention.cpp:636-676)
+int kv8_rope_append(zl_llama* m, int l, const Chain& ch, const void* qkv, void* q, int pdl) {
+    const auto& c = m->cfg;
+    const int d = c.dim_head;
+    const size_t row = (size_t)m->hkv * d;
+    __half* ks = static_cast<__half*>(m->kv_stage.get()) + ch.row0 * row;
+    __half* vs = static_cast<__half*>(m->kv_stage.get()) + ((size_t)m->tok_cap + ch.row0) * row;
+    RCHECK(zl_rope_qk_cache(m->cosb.get() + (size_t)ch.row0 * d, m->sinb.get() + (size_t)ch.row0 * d, qkv, q, ks, vs, ch.n,
+                            m->hq, m->hkv, d, 1, c.dtype, m->stream));
+    return kv8_append(m, l, ch, pdl);
+}
+
 // qkv: RMSNorm + GEMM; at fuse >= 2 the epilogue splits q / k / v, applies RoPE and appends K / V, otherwise
-// zl_qkv_rope_append does
+// zl_qkv_rope_append does.  int8 KV cache: the epilogue appends to the staging rows instead (fuse >= 2) or
+// zl_rope_qk_cache writes them (fuse < 2), and kv8_append quantises them into the cache.
 int qkv_gemm(zl_llama* m, int l, Chain& ch) {
     const auto& c = m->cfg;
     const Layer& L = m->layers[l];
@@ -868,6 +932,9 @@ int qkv_gemm(zl_llama* m, int l, Chain& ch) {
     void* q = rows(m->q.get(), ch.row0, m->hq * d);
     const int32_t* tb = m->cur_tb + ch.row0;
     const int32_t* pos = m->cur_pos + ch.row0;
+    // int8 cache at fuse >= 2 on the exact-integer route (M <= 16): the epilogue quantises K / V into the cache.  The wgmma
+    // and fp16 routes, and act-order qkv, append fp16 rows to the staging rows and kv8_append quantises them.
+    const bool fused_kv8 = c.kv_int8 && c.fuse >= 2 && !L.q_qkv.k_perm && route_of(L.q_qkv, ch.n) == 3;
     if (c.fuse >= 2) {
         a.epilogue = ZL_EPI_QKV_ROPE;
         a.cos = cos;
@@ -880,14 +947,47 @@ int qkv_gemm(zl_llama* m, int l, Chain& ch) {
         a.num_heads = m->hq;
         a.num_kv_heads = m->hkv;
         a.dim_head = d;
+        if (fused_kv8) {   // the exact-integer kernel quantises the rows into the cache itself
+            a.kv_int8 = 1;
+            a.scale_k_addrs = L.sk_addrs.get();
+            a.scale_v_addrs = L.sv_addrs.get();
+            a.kv8_stage = m->kv8_rows.get();
+            a.kv8_counters = m->kv8_cnt.get();
+        } else if (c.kv_int8) {   // staging row of token i = row row0 + i of the one "task" stage_addrs
+            a.token_batch = m->d_zeros.get();
+            a.placement = m->d_rowidx.get() + ch.row0;
+            a.k_addrs = m->stage_addrs.get();
+            a.v_addrs = m->stage_addrs.get() + 1;
+        }
     } else {
         a.y = rows(m->qkv.get(), ch.row0, hqkv);
     }
     ch.reduce_in(&a);
     RCHECK(w4_gemm(m, l, kQkv, ch, L.q_qkv, L.ln_attn.get(), a));
-    if (c.fuse >= 2 || ch.gemm_only) return ZL_OK;
+    if (ch.gemm_only) return ZL_OK;
+    const int pdl = ch.no_pdl ? 0 : c.use_pdl;
+    if (fused_kv8) return ZL_OK;
+    if (c.kv_int8) return c.fuse >= 2 ? kv8_append(m, l, ch, pdl) : kv8_rope_append(m, l, ch, a.y, q, pdl);
+    if (c.fuse >= 2) return ZL_OK;
     return zl_qkv_rope_append(cos, sin, a.y, q, tb, pos, L.k_addrs.get(), L.v_addrs.get(), ch.n, m->hq, m->hkv, d, 1, 1,
-                              m->d_lens.get(), c.dtype, ch.no_pdl ? 0 : c.use_pdl, m->stream);
+                              m->d_lens.get(), c.dtype, pdl, m->stream);
+}
+
+// attention of B tasks x len_q query rows (tasks task0 .. task0 + B - 1) over layer l's cache: zl_decode_attention, or
+// zl_decode_attention_kv8 over the int8 cache
+int attention(zl_llama* m, int l, const void* q, int task0, const int8_t* mask, int max_len, void* out, int B, int len_q,
+              int pdl, cudaStream_t st) {
+    const auto& c = m->cfg;
+    const Layer& L = m->layers[l];
+    const float scale = 1.0f / sqrtf((float)c.dim_head);   // attention.cpp:89
+    if (c.kv_int8)
+        return zl_decode_attention_kv8(q, m->d_lens.get() + task0, L.k_addrs.get() + task0, L.v_addrs.get() + task0,
+                                       L.sk_addrs.get() + task0, L.sv_addrs.get() + task0, mask, scale, max_len, out, B,
+                                       len_q, m->hq, m->hkv, c.dim_head, m->attn_ws.get(), m->attn_ws_bytes, c.dtype, pdl,
+                                       st);
+    return zl_decode_attention(q, m->d_lens.get() + task0, L.k_addrs.get() + task0, L.v_addrs.get() + task0, mask, scale,
+                               max_len, out, B, len_q, m->hq, m->hkv, c.dim_head, 1, m->attn_ws.get(), m->attn_ws_bytes,
+                               c.dtype, pdl, st);
 }
 
 // gate_up: RMSNorm + GEMM + SwiGLU epilogue into act
@@ -983,7 +1083,6 @@ int prefill_layers_dual(zl_llama* m, const PrefillChunk& pf) {
     const int D = c.dim_model, d = c.dim_head, dt = c.dtype;
     const bool tp = c.tp_size > 1;
     cudaStream_t cs = m->stream, rs = m->reduce_stream;
-    const float scale = 1.0f / sqrtf((float)d);
     const int n0 = (pf.n / 2 + 7) / 8 * 8 < pf.n ? (pf.n / 2 + 7) / 8 * 8 : pf.n / 2;   // rows of half 0
     const int len_buf = pf.pos0 + pf.n;
     Chain half[2];
@@ -1001,17 +1100,14 @@ int prefill_layers_dual(zl_llama* m, const PrefillChunk& pf) {
         return zl_element_add_scale(hp, pp, hp, (size_t)ch.n * D, 1.0f, dt, rs);
     };
     for (int l = 0; l < c.num_layers; ++l) {
-        Layer& L = m->layers[l];
         for (int h = 0; h < 2; ++h) {   // S1
             if (l > 0) ZL_CHECK_CUDA(cudaStreamWaitEvent(cs, m->ev_r2[h], 0));
             const int r0 = half[h].row0;
             RCHECK(qkv_gemm(m, l, half[h]));
             // causal rows r0.. of the chunk's mask; keys of BOTH halves are visible as far as the mask allows, so half 1
             // needs half 0's K/V rows, which the same stream appended just before
-            RCHECK(zl_decode_attention(rows(m->q.get(), r0, m->hq * d), m->d_lens.get() + pf.task,
-                                       L.k_addrs.get() + pf.task, L.v_addrs.get() + pf.task,
-                                       m->d_mask.get() + (size_t)r0 * len_buf, scale, len_buf, rows(m->ao.get(), r0, m->hq * d),
-                                       1, half[h].n, m->hq, m->hkv, d, 1, m->attn_ws.get(), m->attn_ws_bytes, dt, 0, cs));
+            RCHECK(attention(m, l, rows(m->q.get(), r0, m->hq * d), pf.task, m->d_mask.get() + (size_t)r0 * len_buf, len_buf,
+                             rows(m->ao.get(), r0, m->hq * d), 1, half[h].n, 0, cs));
             RCHECK(o_gemm(m, l, half[h]));
             ZL_CHECK_CUDA(cudaEventRecord(m->ev_o[h], cs));
             ZL_CHECK_CUDA(cudaStreamWaitEvent(rs, m->ev_o[h], 0));   // R1
@@ -1043,7 +1139,6 @@ int enqueue_step(zl_llama* m, int n_tasks, int len_bucket, const PrefillChunk* p
         zl_set_last_error(__FILE__, __LINE__, "tp_size > 1 but zl_llama_set_comm was not called");
         return ZL_ERR_STATE;
     }
-    const float scale = 1.0f / sqrtf((float)d);   // attention.cpp:89
 
     if (pf) {
         k_prefill_setup<<<8, 256, 0, st>>>(m->d_pf_pos.get(), m->d_tb.get(), m->d_lens.get(), m->d_mask.get(), pf->task,
@@ -1086,19 +1181,19 @@ int enqueue_step(zl_llama* m, int n_tasks, int len_bucket, const PrefillChunk* p
             RCHECK(zl_add_rmsnorm(m->h.get(), l == 0 ? nullptr : m->pend.get(), L.ln_attn.get(), m->h.get(), m->xn.get(),
                                   B, D, c.eps, 1.f, 0, dt, pdl, st));
             RCHECK(dense_or_w8(m, m->xn.get(), L.d_qkv, m->qkv.get(), B, pdl));
-            RCHECK(zl_qkv_rope_append(m->cosb.get(), m->sinb.get(), m->qkv.get(), m->q.get(), m->cur_tb, m->cur_pos,
-                                      L.k_addrs.get(), L.v_addrs.get(), B, m->hq, m->hkv, d, 1, 1, m->d_lens.get(), dt,
-                                      pdl, st));
+            if (c.kv_int8) {
+                RCHECK(kv8_rope_append(m, l, ch, m->qkv.get(), m->q.get(), pdl));
+            } else {
+                RCHECK(zl_qkv_rope_append(m->cosb.get(), m->sinb.get(), m->qkv.get(), m->q.get(), m->cur_tb, m->cur_pos,
+                                          L.k_addrs.get(), L.v_addrs.get(), B, m->hq, m->hkv, d, 1, 1, m->d_lens.get(), dt,
+                                          pdl, st));
+            }
         }
         if (pf) {
             // one task, len_q = chunk, causal int8 mask (Attention::dynamic_batch_forward with len_q > 1, attention.cpp:846-964)
-            RCHECK(zl_decode_attention(m->q.get(), m->d_lens.get() + pf->task, L.k_addrs.get() + pf->task,
-                                       L.v_addrs.get() + pf->task, m->d_mask.get(), scale, pf->pos0 + pf->n, m->ao.get(),
-                                       1, pf->n, m->hq, m->hkv, d, 1, m->attn_ws.get(), m->attn_ws_bytes, dt, pdl, st));
+            RCHECK(attention(m, l, m->q.get(), pf->task, m->d_mask.get(), pf->pos0 + pf->n, m->ao.get(), 1, pf->n, pdl, st));
         } else {
-            RCHECK(zl_decode_attention(m->q.get(), m->d_lens.get(), L.k_addrs.get(), L.v_addrs.get(), nullptr, scale,
-                                       len_bucket, m->ao.get(), B, 1, m->hq, m->hkv, d, 1, m->attn_ws.get(),
-                                       m->attn_ws_bytes, dt, stage_pdl(m, kAttn), st));
+            RCHECK(attention(m, l, m->q.get(), 0, nullptr, len_bucket, m->ao.get(), B, 1, stage_pdl(m, kAttn), st));
         }
         if (w4) {
             RCHECK(o_gemm(m, l, ch));
@@ -1230,6 +1325,13 @@ extern "C" int zl_llama_create(const zl_llama_config_t* cfg, zl_llama_t** out) {
     ZL_CHECK_ARG(cfg->fuse >= 0 && cfg->fuse <= 3);
     ZL_CHECK_ARG(cfg->prefill_chunk >= 0 && cfg->prefill_chunk <= 2048);
     ZL_CHECK_SUPPORTED(cfg->fuse < 2 || cfg->dim_head % 32 == 0);
+    ZL_CHECK_ARG(cfg->kv_int8 == 0 || cfg->kv_int8 == 1);
+    if (cfg->kv_int8) {
+        // zl_decode_attention_kv8 takes fp16 q, d = 64 or 128, and at most 64 key splits of 1024 keys
+        if (cfg->dtype != ZL_F16 || (cfg->dim_head != 64 && cfg->dim_head != 128) || cfg->max_seq > 65536)
+            return fail_state(__LINE__, "kv_int8 needs dtype fp16, dim_head 64 or 128 and max_seq <= 65536",
+                              ZL_ERR_UNSUPPORTED);
+    }
     RCHECK(zl_prepare());
     zl_llama* m = new zl_llama();
     m->cfg = *cfg;
@@ -1583,6 +1685,31 @@ extern "C" int zl_llama_set_sampling(zl_llama_t* m, int task, const zl_sample_pa
     ZL_CHECK_CUDA(cudaMemcpyAsync(m->d_sparams.get() + task, &q, sizeof(q), cudaMemcpyHostToDevice, m->stream));
     ZL_CHECK_CUDA(cudaMemsetAsync(m->d_hist.get() + (size_t)task * m->hwords, 0, (size_t)m->hwords * 4, m->stream));
     m->samp_on[task] = on ? 1 : 0;
+    return ZL_OK;
+}
+
+extern "C" int zl_llama_read_kv(zl_llama_t* m, int layer, int task, int row0, int n, void* k_host, void* v_host,
+                                float* sk_host, float* sv_host) {
+    ZL_CHECK_ARG(m && m->finalized && layer >= 0 && layer < m->cfg.num_layers && task >= 0 && task < m->cfg.max_batch);
+    ZL_CHECK_ARG(row0 >= 0 && n > 0 && row0 + n <= m->cfg.max_seq);
+    ZL_CHECK_ARG(m->cfg.kv_int8 || (!sk_host && !sv_host));
+    const Layer& L = m->layers[layer];
+    const size_t row = (size_t)m->hkv * m->cfg.dim_head;   // values per token
+    const size_t vb = m->cfg.kv_int8 ? 1 : 2;               // bytes per value
+    const size_t off = ((size_t)task * m->cfg.max_seq + row0) * row * vb;
+    const size_t soff = ((size_t)task * m->cfg.max_seq + row0) * m->hkv * 4;
+    ZL_CHECK_CUDA(cudaStreamSynchronize(m->stream));   // the steps that wrote the rows
+    if (k_host) ZL_CHECK_CUDA(cudaMemcpy(k_host, (char*)L.kbuf.get() + off, n * row * vb, cudaMemcpyDeviceToHost));
+    if (v_host) ZL_CHECK_CUDA(cudaMemcpy(v_host, (char*)L.vbuf.get() + off, n * row * vb, cudaMemcpyDeviceToHost));
+    if (sk_host) ZL_CHECK_CUDA(cudaMemcpy(sk_host, (char*)L.skbuf.get() + soff, (size_t)n * m->hkv * 4, cudaMemcpyDeviceToHost));
+    if (sv_host) ZL_CHECK_CUDA(cudaMemcpy(sv_host, (char*)L.svbuf.get() + soff, (size_t)n * m->hkv * 4, cudaMemcpyDeviceToHost));
+    return ZL_OK;
+}
+
+extern "C" int zl_llama_config_layout(size_t* size, size_t* kv_int8_offset) {
+    ZL_CHECK_ARG(size && kv_int8_offset);
+    *size = sizeof(zl_llama_config_t);
+    *kv_int8_offset = offsetof(zl_llama_config_t, kv_int8);
     return ZL_OK;
 }
 

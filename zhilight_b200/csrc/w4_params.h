@@ -53,6 +53,14 @@ struct W4Params {
     __half* tp_h_out = nullptr;
     // act-order: the staging loop reads x[k_perm[i]] and ln_w[k_perm[i]] (integer kernel only; zl_w4_fused_args_t.k_perm)
     const int32_t* k_perm = nullptr;
+    // int8 KV cache (integer kernel, ZL_EPI_QKV_ROPE; zl_w4_fused_args_t.kv_int8): k_addrs / v_addrs point at uint8 code
+    // buffers, kv8_sk / kv8_sv at the fp32 scale buffers; kv8_stage (mc, 2, H_kv, d) fp16 scratch, kv8_cnt (mc, 2, H_kv)
+    // counters that are 0 on entry and on exit
+    int kv8 = 0;
+    float* const* kv8_sk = nullptr;
+    float* const* kv8_sv = nullptr;
+    __half* kv8_stage = nullptr;
+    unsigned* kv8_cnt = nullptr;
 };
 
 // zl_w4a16_gemm_fused with the L2 head of the successor GEMM as a descriptor (l2 == nullptr: the public whole-range

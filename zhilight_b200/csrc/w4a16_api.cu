@@ -130,6 +130,11 @@ int zl::w4a16_gemm_fused_l2(const zl_w4_fused_args_t* a, const W4L2Head* l2, zl_
         ZL_CHECK_SUPPORTED(a->dim_head % 32 == 0);
         ZL_CHECK_ARG(a->N == (a->num_heads + 2 * a->num_kv_heads) * a->dim_head);
     }
+    if (a->kv_int8) {
+        ZL_CHECK_ARG(a->epilogue == ZL_EPI_QKV_ROPE && a->scale_k_addrs && a->scale_v_addrs && a->kv8_stage &&
+                     a->kv8_counters);
+        ZL_CHECK_SUPPORTED(!a->k_perm && "the int8-cache epilogue is not combined with k_perm");
+    }
     const void* tp_cd = nullptr;
     if (a->tp_mode != 0) {
         ZL_CHECK_ARG(a->tp_mode == 1 || a->tp_mode == 2);
@@ -156,6 +161,8 @@ int zl::w4a16_gemm_fused_l2(const zl_w4_fused_args_t* a, const W4L2Head* l2, zl_
     ZL_CHECK_SUPPORTED(!(route == 4 && a->ln_weight) && "the wgmma kernel has no fused RMSNorm prologue: run zl_rmsnorm first");
     ZL_CHECK_SUPPORTED(!(route != 3 && a->k_perm) &&
                        "only the exact-integer kernel gathers k_perm: permute x with zl_gather_cols_16 first");
+    ZL_CHECK_SUPPORTED(!(route != 3 && a->kv_int8) &&
+                       "only the exact-integer kernel (M <= 16) quantises an int8 KV cache: use zl_kv_int8_quant_append");
     const int step = route == 4 ? 256 : 32;
     for (int m0 = 0; m0 < a->M; m0 += step) {
         W4Params p;
@@ -196,6 +203,13 @@ int zl::w4a16_gemm_fused_l2(const zl_w4_fused_args_t* a, const W4L2Head* l2, zl_
         p.tp_index = a->tp_index;
         p.tp_h_out = static_cast<__half*>(a->tp_h_out);
         p.k_perm = a->k_perm;
+        if (a->kv_int8) {   // route 3: M <= 16, one pass
+            p.kv8 = 1;
+            p.kv8_sk = reinterpret_cast<float* const*>(a->scale_k_addrs);
+            p.kv8_sv = reinterpret_cast<float* const*>(a->scale_v_addrs);
+            p.kv8_stage = static_cast<__half*>(a->kv8_stage);
+            p.kv8_cnt = a->kv8_counters;
+        }
         if (l2) {
             p.l2 = *l2;
         } else if (a->prefetch_ptr && a->prefetch_bytes) {

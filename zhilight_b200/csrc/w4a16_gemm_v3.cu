@@ -19,6 +19,7 @@
 #include "w4_layout.cuh"
 #include "w4_params.h"
 #include "comm_dev.cuh"
+#include "kv8_quant.cuh"
 
 #include <cstdlib>
 
@@ -216,8 +217,32 @@ __device__ __forceinline__ void v3_gather_row(const __half* src, int K, const in
 // of its own first (permute_input, gptq/utils.cu:322-398); here the activations are read once either way, so the gather
 // costs no launch and no extra pass over x: each token's row is read coalesced into shared memory and permuted from
 // there (v3_gather_row).  The RMSNorm weights are gathered the same way before pdl_wait (they and k_perm are constants).
+// The last arriver's half of the int8-cache epilogue, for one warp (lane = stid): the staged rows (token, k|v, hk) of the
+// tokens set in `todo` -> codes and scale at the token's placement.  Out of line: it runs once per row, and inlined it
+// made the 16-token variants spill.
+__device__ __noinline__ void kv8_quant_rows(const __half* __restrict__ stage, const int32_t* __restrict__ placement,
+                                           const int32_t* __restrict__ token_batch, uint8_t* const* codes,
+                                           float* const* scales, unsigned todo, int is_v, int hk, int hkv, int d, int lane) {
+    while (todo) {
+        const int tok = __ffs(todo) - 1;
+        todo &= todo - 1;
+        const __half* row = stage + (((size_t)tok * 2 + is_v) * hkv + hk) * d;
+        float amax = 0.f;
+        for (int i = lane; i < d; i += 32) amax = fmaxf(amax, fabsf(__half2float(__ldcg(row + i))));
+        amax = warp_max(amax);
+        const float mul = kv8_row_mul(amax);
+        const int b = token_batch[tok];
+        const size_t off = (size_t)placement[tok] * hkv + hk;
+        uint8_t* dst = codes[b] + off * d;
+        for (int i = lane; i < d; i += 32) dst[i] = kv8_code(__half2float(__ldcg(row + i)), mul);
+        if (lane == 0) scales[b][off] = kv8_row_scale(amax);
+    }
+}
+
+// KV8 (int8 KV cache, p.kv8 != 0, ZL_EPI_QKV_ROPE only): the epilogue quantises the K / V rows into the int8 cache instead
+// of storing fp16 rows -- see the epilogue.
 template <int NT, bool NORM, int WARPS, int SUBS, int STAGES, int RT = NT * 8, bool PACK = false, int TPX = 0,
-          bool GATHER = false>
+          bool GATHER = false, bool KV8 = false>
 __global__ void __launch_bounds__(WARPS * SUBS * 32, 1) k_w4a16_v3(const W4Params p) {
     using S = V3Smem<NT, WARPS, SUBS, STAGES, RT>;
     // the tensor-parallel exchange code is compiled only into the TPX instantiations: carried as a run-time branch it cost
@@ -704,10 +729,44 @@ __global__ void __launch_bounds__(WARPS * SUBS * 32, 1) k_w4a16_v3(const W4Param
                     if (pl >= 0) {
                         const bool is_k = !is_v;
                         const int hk = is_k ? head - p.num_heads : head - p.num_heads - p.num_kv_heads;
-                        __half* base = (is_k ? p.k_addrs : p.v_addrs)[p.token_batch[tok]];
-                        __half* dst = base + ((size_t)pl * p.num_kv_heads + hk) * d;
+                        __half* dst;
+                        if constexpr (KV8)   // staging row (tok, k|v, hk) of p.kv8_stage (M, 2, H_kv, d)
+                            dst = p.kv8_stage + (((size_t)tok * 2 + is_v) * p.num_kv_heads + hk) * d;
+                        else
+                            dst = (is_k ? p.k_addrs : p.v_addrs)[p.token_batch[tok]] + ((size_t)pl * p.num_kv_heads + hk) * d;
                         dst[c] = olo;
                         dst[c + half_dim] = ohi;
+                    }
+                }
+            }
+            if constexpr (KV8) {
+                // A (token, K|V, kv head) row of d values spans d / 32 tiles, which the plan puts on different sub-CTAs, so
+                // no one sub-CTA sees the row's absmax.  Last-arriver protocol, without waiting or spinning: each tile owner
+                // has staged its 32 values above; it fences them, and one atomicAdd per row on p.kv8_cnt counts the tile in.
+                // The owner that sees d / 32 - 1 re-reads the whole row from the staging buffer past L1, quantises it
+                // (kv8_quant.cuh, the same arithmetic as zl_kv_int8_quant_append), writes codes and scale at the row's
+                // placement, and puts the counter back to 0.  Rows with placement < 0 are neither staged nor counted.
+                // Invariant: every counter is 0 between launches.  Each launch returns the counters it touched to 0, and
+                // the qkv GEMMs that share them run in stream order on one stream; with programmatic dependent launch,
+                // griddepcontrol.wait in the next kernel of the chain waits for this grid to complete, so the ordering
+                // is transitive along the chain.
+                if (head >= p.num_heads) {   // uniform over the sub-CTA: one tile, one head
+                    __threadfence();
+                    sub_barrier(1 + sub, kSubThreads);
+                    if (stid < 32) {        // the sub-CTA's first warp: lane = token
+                        const bool is_v = head >= p.num_heads + p.num_kv_heads;
+                        const int hk = is_v ? head - p.num_heads - p.num_kv_heads : head - p.num_heads;
+                        unsigned* cnt = p.kv8_cnt + ((size_t)stid * 2 + is_v) * p.num_kv_heads + hk;
+                        const bool mine = stid < p.mc && p.placement[stid] >= 0;
+                        const bool last = mine && atomicAdd(cnt, 1u) == (unsigned)(tiles_per_head - 1);
+                        const unsigned todo = __ballot_sync(0xffffffffu, last);
+                        if (todo) {
+                            __threadfence();
+                            kv8_quant_rows(p.kv8_stage, p.placement, p.token_batch,
+                                           reinterpret_cast<uint8_t* const*>(is_v ? p.v_addrs : p.k_addrs),
+                                           is_v ? p.kv8_sv : p.kv8_sk, todo, is_v, hk, p.num_kv_heads, d, stid);
+                        }
+                        if (last) *cnt = 0u;
                     }
                 }
             }
@@ -764,6 +823,9 @@ static cudaError_t launch_v3_t(const W4Params& params, const V3Plan& pl, bool pd
     if (p.tp_mode != 0) {
         // exchange variants exist for the 4-stage rings only (w4_v3_plan routes tensor-parallel launches there)
         if constexpr (STAGES == 4 && RT == NT * 8) {
+            if (p.tp_mode == 1 && p.kv8)   // reduce-in on the qkv GEMM of an int8-cache model
+                return launch(k_w4a16_v3<NT, NORM, WARPS, SUBS, STAGES, RT, PACK, 1, false, true>, grid, block,
+                              (size_t)pl.smem, stream, pdl, p);
             if (p.tp_mode == 1)
                 return launch(k_w4a16_v3<NT, NORM, WARPS, SUBS, STAGES, RT, PACK, 1>, grid, block, (size_t)pl.smem, stream,
                               pdl, p);
@@ -773,9 +835,12 @@ static cudaError_t launch_v3_t(const W4Params& params, const V3Plan& pl, bool pd
             return cudaErrorNotSupported;
         }
     }
-    if (p.k_perm)   // act-order (the front end rejects k_perm with tp_mode)
+    if (p.k_perm)   // act-order (the front end rejects k_perm with tp_mode and with kv8)
         return launch(k_w4a16_v3<NT, NORM, WARPS, SUBS, STAGES, RT, PACK, 0, true>, grid, block, (size_t)pl.smem, stream, pdl,
                       p);
+    if (p.kv8)
+        return launch(k_w4a16_v3<NT, NORM, WARPS, SUBS, STAGES, RT, PACK, 0, false, true>, grid, block, (size_t)pl.smem,
+                      stream, pdl, p);
     return launch(k_w4a16_v3<NT, NORM, WARPS, SUBS, STAGES, RT, PACK>, grid, block, (size_t)pl.smem, stream, pdl, p);
 }
 
@@ -942,13 +1007,16 @@ bool w4_v3_fits(int mc, int N, int K) {
     return false;
 }
 
-// opt-in shared memory of one single-GPU variant, with and without the act-order gather
+// opt-in shared memory of one single-GPU variant, with and without the act-order gather, and with the int8-cache epilogue
 template <int NT, bool NORM, int W, int SB, int ST, int RT = NT * 8, bool PK = false>
 static cudaError_t v3_set_smem() {
     cudaError_t e = cudaFuncSetAttribute(k_w4a16_v3<NT, NORM, W, SB, ST, RT, PK>,
                                          cudaFuncAttributeMaxDynamicSharedMemorySize, kV3Budget);
     if (e != cudaSuccess) return e;
-    return cudaFuncSetAttribute(k_w4a16_v3<NT, NORM, W, SB, ST, RT, PK, 0, true>,
+    e = cudaFuncSetAttribute(k_w4a16_v3<NT, NORM, W, SB, ST, RT, PK, 0, true>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                             kV3Budget);
+    if (e != cudaSuccess) return e;
+    return cudaFuncSetAttribute(k_w4a16_v3<NT, NORM, W, SB, ST, RT, PK, 0, false, true>,
                                 cudaFuncAttributeMaxDynamicSharedMemorySize, kV3Budget);
 }
 
@@ -978,6 +1046,9 @@ cudaError_t prepare_w4_v3() {
                              cudaFuncAttributeMaxDynamicSharedMemorySize, kV3Budget);                           \
     if (e != cudaSuccess) return e;                                                                             \
     e = cudaFuncSetAttribute(k_w4a16_v3<NT, NORM, W, SB, 4, NT * 8, PK, 2>,                                     \
+                             cudaFuncAttributeMaxDynamicSharedMemorySize, kV3Budget);                           \
+    if (e != cudaSuccess) return e;                                                                             \
+    e = cudaFuncSetAttribute(k_w4a16_v3<NT, NORM, W, SB, 4, NT * 8, PK, 1, false, true>,                        \
                              cudaFuncAttributeMaxDynamicSharedMemorySize, kV3Budget);                           \
     if (e != cudaSuccess) return e;
     ZL_SETX(1, false, 8, 2, false) ZL_SETX(1, true, 8, 2, false) ZL_SETX(1, false, 16, 1, false) ZL_SETX(1, true, 16, 1, false)

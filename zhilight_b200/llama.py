@@ -37,17 +37,25 @@ class LlamaDecoder:
     def __init__(self, num_layers, dim_model, num_heads, num_kv_heads, dim_head, dim_ff, vocab_size, eps=1e-5,
                  rope_theta=10000.0, rope_llama3=None, quant_type=QUANT_NONE, group_size=128, sym=False,
                  dtype="f16", max_batch=1, max_seq=512, use_pdl=True, use_graph=True, tp_rank=0, tp_size=1, fuse=2, tp_int8=False,
-                 prefill_chunk=0, qkv_bias=False):
+                 prefill_chunk=0, qkv_bias=False, kv_cache_dtype=None):
+        """kv_cache_dtype: None keeps K/V in the activation dtype; "int8" stores them as per-(token, kv head) int8 codes
+        with fp32 scales (the reference's KV_CACHE_DTYPE=int8; fp16 models with dim_head 64 or 128)."""
+        if kv_cache_dtype not in (None, "int8"):
+            raise ValueError("kv_cache_dtype must be None or 'int8', not %r" % (kv_cache_dtype,))
         self.lib = _lib.load()
         l3 = rope_llama3 or {}
         self.cfg = _lib.LlamaConfig(
             num_layers, dim_model, num_heads, num_kv_heads, dim_head, dim_ff, vocab_size, eps, rope_theta,
             float(l3.get("factor", 0.0)), float(l3.get("low", 1.0)), float(l3.get("high", 4.0)),
             float(l3.get("orig", 8192.0)), quant_type, group_size, int(sym), {"f16": 0, "bf16": 1}[dtype],
-            max_batch, max_seq, tp_rank, tp_size, int(use_pdl), int(use_graph), int(tp_int8), int(fuse), int(prefill_chunk), int(qkv_bias))
+            max_batch, max_seq, tp_rank, tp_size, int(use_pdl), int(use_graph), int(tp_int8), int(fuse), int(prefill_chunk), int(qkv_bias),
+            int(kv_cache_dtype == "int8"))
         self.vocab_size = vocab_size
         self.vocab_shard = vocab_size // tp_size      # lm_head is vocab-parallel: logits come back per rank shard
         self.max_batch = max_batch
+        self.kv_cache_dtype = kv_cache_dtype
+        self.kv_row = (num_kv_heads // tp_size, dim_head)     # this rank's (H_kv, d) of one cached token
+        self.dtype = dtype
         h = ctypes.c_void_p()
         _lib.check(self.lib.zl_llama_create(ctypes.byref(self.cfg), ctypes.byref(h)))
         self.h = h
@@ -111,6 +119,22 @@ class LlamaDecoder:
         The defaults are plain greedy."""
         p = _lib.sample_params(temperature, top_p, top_k, repetition_penalty, presence_penalty, seed)
         _lib.check(self.lib.zl_llama_set_sampling(self.h, int(task), ctypes.byref(p)))
+
+    def read_kv(self, layer, task, row0, n):
+        """Rows row0 .. row0 + n of a task's layer-`layer` KV cache (zl_llama_read_kv), each (n, H_kv, d).
+        Plain cache: (k, v) as float16 (bf16 models: uint16 bit patterns).  int8 cache: (k, v, scale_k, scale_v) with
+        uint8 codes and (n, H_kv) float32 scales; a value is (code - 128) * scale."""
+        hkv, d = self.kv_row
+        p = lambda a: a.ctypes.data_as(ctypes.c_void_p)
+        if self.kv_cache_dtype == "int8":
+            k, v = np.empty((n, hkv, d), np.uint8), np.empty((n, hkv, d), np.uint8)
+            sk, sv = np.empty((n, hkv), np.float32), np.empty((n, hkv), np.float32)
+            _lib.check(self.lib.zl_llama_read_kv(self.h, layer, task, row0, n, p(k), p(v), p(sk), p(sv)))
+            return k, v, sk, sv
+        dt = np.float16 if self.dtype == "f16" else np.uint16
+        k, v = np.empty((n, hkv, d), dt), np.empty((n, hkv, d), dt)
+        _lib.check(self.lib.zl_llama_read_kv(self.h, layer, task, row0, n, p(k), p(v), None, None))
+        return k, v
 
     def set_state(self, tokens, positions):
         t = np.ascontiguousarray(tokens, dtype=np.int32)

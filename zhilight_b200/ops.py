@@ -205,10 +205,13 @@ def gather_rows_16(src, row_map):
 
 
 def w4a16_gemm_fused(x, packed, n, k, group_size=128, bias=None, residual=None, epilogue=EPI_NONE, pdl=False, out=None,
-                     ln_weight=None, eps=1e-5, rope=None, variant=0, k_perm=None):
+                     ln_weight=None, eps=1e-5, rope=None, variant=0, k_perm=None, kv8=None):
     """zl_w4a16_gemm_fused.  rope = dict(cos, sin, token_batch, placement, k_bufs, v_bufs, num_heads, num_kv_heads,
     dim_head) for EPI_QKV_ROPE (returns q); bias must be in packed-row order.  k_perm (K int32, act-order): y = W . x[:, k_perm]
-    with W packed from the sequentialised weights (exact-integer route only; elsewhere gather_cols first)."""
+    with W packed from the sequentialised weights (exact-integer route only; elsewhere gather_cols first).
+    kv8 = dict(sk_bufs, sv_bufs, stage, counters) with EPI_QKV_ROPE: k_bufs / v_bufs are uint8 code buffers and the epilogue
+    quantises the K / V rows into them (int8 KV cache; exact-integer route only).  stage: fp16 (M, 2, H_kv, d) scratch,
+    counters: int32 (M, 2, H_kv), zero before the first launch and left zero."""
     if x.dtype != torch.float16:
         raise _lib.ZLError(-2, "A must be half")
     m = x.shape[0]
@@ -228,6 +231,11 @@ def w4a16_gemm_fused(x, packed, n, k, group_size=128, bias=None, residual=None, 
         a.token_batch, a.placement = r["token_batch"].data_ptr(), r["placement"].data_ptr()
         a.k_addrs, a.v_addrs = ka.data_ptr(), va.data_ptr()
         a.num_heads, a.num_kv_heads, a.dim_head = r["num_heads"], r["num_kv_heads"], r["dim_head"]
+        if kv8 is not None:
+            ska, sva = _ptr_table(kv8["sk_bufs"], x.device), _ptr_table(kv8["sv_bufs"], x.device)
+            keep += [ska, sva]
+            a.kv_int8, a.scale_k_addrs, a.scale_v_addrs = 1, ska.data_ptr(), sva.data_ptr()
+            a.kv8_stage, a.kv8_counters = kv8["stage"].data_ptr(), kv8["counters"].data_ptr()
         ret = q
     else:
         n_out = n // 2 if epilogue == EPI_SWIGLU else n

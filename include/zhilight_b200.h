@@ -283,6 +283,21 @@ int zl_decode_attention(const void* q, const int32_t* buf_lens, void* const* k_a
                         int num_heads, int num_kv_heads, int dim_head, int bshd, void* workspace,
                         size_t workspace_bytes, int dtype, int pdl, zl_stream_t stream);
 
+/* Causal variable-length attention: every row of a joined chunked-prefill step (encode and search tokens of
+ * SearcherImplV1::join_forward, src/generator/batch_generator.cpp:1337-1422, attended by Attention::dynamic_batch_forward,
+ * src/nn/attention/attention.cpp:924-961, beam_size 1) in one launch, with no materialised mask.
+ * seg (nseg, 4) int32 DEVICE array, 16-byte aligned, of segments {task, row0, pos0, n}: rows row0 .. row0 + n - 1 of q
+ * hold positions pos0 .. pos0 + n - 1 of task `task`, and the row at position p attends keys 0 ..= p of that task's cache.
+ * A decode row is a segment with n = 1.  q / out (rows, H_q, d); k_addrs / v_addrs per-task BSHD caches (len, H_kv, d)
+ * as for zl_decode_attention; every segment needs pos0 + n <= max_keys; keys past a row's position are never read.
+ * fp16 / bf16, d = 64 or 128, H_q % H_kv == 0.  Splits cover fixed 512-key ranges, so a row's output bits depend only on
+ * its q, its task's cache and its position, not on the other segments.  workspace: zl_varlen_attention_workspace_bytes
+ * (0 when max_keys <= 512). */
+size_t zl_varlen_attention_workspace_bytes(int rows, int nseg, int num_heads, int dim_head, int max_keys);
+int zl_varlen_attention(const void* q, const int32_t* seg, int nseg, int rows, void* const* k_addrs, void* const* v_addrs,
+                        float scale, int max_keys, void* out, int num_heads, int num_kv_heads, int dim_head, void* ws,
+                        size_t ws_bytes, int dtype, int pdl, zl_stream_t stream);
+
 /* int8 KV cache (KV_CACHE_DTYPE=int8 of the reference): KERNEL_mqa_rag_buffer_split_kv_quant
  * (src/nn/attention/attention_kernel.cu:804-880, src/nn/attention/quant_attention.cuh:10-123).  K / V buffers per task are
  * (len_buf, H_kv, d) uint8 = round(x * 127 / absmax) + 128, scale buffers (len_buf, H_kv) fp32 = absmax / 127 (BSHD only,
@@ -466,6 +481,17 @@ int zl_llama_sync(zl_llama_t* m);
  * overwrites the next-token / logits row 0 outputs, which zl_llama_step_device consumes before it returns. */
 int zl_llama_prefill(zl_llama_t* m, int task, const int32_t* tokens_host, int n, int pos0, int32_t* next_token_host,
                      float* logits_host);
+/* One forward over nseg segments, the joined step of chunked-prefill scheduling (SearcherImplV1::join_forward,
+ * src/generator/batch_generator.cpp:1337-1422): prompt chunks and decode rows of different tasks stream the weights once.
+ * seg_host (nseg x 4, HOST) = {task, pos0, n, emit}; tokens_host = the segments' tokens concatenated.  Rows sum(n) <=
+ * max(max_batch, prefill_chunk); distinct tasks; pos0 + n <= max_seq.  Each segment appends its n K/V rows at pos0.. of its
+ * task and attends causally (zl_varlen_attention).  For each segment with emit != 0 its LAST row goes through the final
+ * norm, lm_head and the pick (greedy, or per-task sampling with counter = that row's position, recorded in the task's
+ * history); next_host (nseg) gets the pick or -1, logits_host (n_emit x vocab, segment order) may be NULL.  The
+ * device-resident decode state (zl_llama_set_state) survives the call, as it survives a prefill.  Synchronous, no graph.
+ * prefill_chunk == 0: ZL_ERR_STATE; malformed segments: ZL_ERR_INVALID_ARG; kv_int8 or tp_size > 1: ZL_ERR_UNSUPPORTED. */
+int zl_llama_step_joined(zl_llama_t* m, const int32_t* tokens_host, const int32_t* seg_host, int nseg, int32_t* next_host,
+                         float* logits_host);
 /* Per-task sampling (zl_sample's contract) for the picks of zl_llama_decode / step_device / prefill.  Copies *p (HOST
  * pointer) to the device and clears the task's history; p == NULL returns the task to plain greedy.  Invalid values:
  * ZL_ERR_INVALID_ARG; anything but plain greedy under tp_size > 1: ZL_ERR_UNSUPPORTED (vocabulary shards would need a

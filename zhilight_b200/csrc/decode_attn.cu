@@ -11,6 +11,7 @@
 // P.V runs in fp32 on the CUDA cores with 16-byte coalesced V loads (each V element feeds all heads).
 // Splits are merged with the reference's LSE rule (attention_kernel.cu:881-923).
 #include "common.cuh"
+#include "attn_combine.cuh"
 #include "decode_attn_short.cuh"
 #include "decode_attn_warp.cuh"
 
@@ -313,26 +314,7 @@ k_decode_attn_short(const T* __restrict__ q, const int32_t* __restrict__ buf_len
 }
 
 
-// grid (B*len_q*num_heads), block D
-template <typename T>
-__global__ void k_attn_combine(const float* __restrict__ part_o, const float* __restrict__ part_m,
-                               const float* __restrict__ part_l, T* __restrict__ out, int num_splits) {
-    const int vh = blockIdx.x, D = blockDim.x, d = threadIdx.x;
-    pdl_trigger();
-    pdl_wait();
-    const float* pm = part_m + (size_t)vh * num_splits;
-    const float* pl = part_l + (size_t)vh * num_splits;
-    float gm = -1e20f;
-    for (int i = 0; i < num_splits; ++i) gm = fmaxf(gm, pm[i]);
-    float gs = 0.f;
-    for (int i = 0; i < num_splits; ++i) gs += pl[i] * expf(pm[i] - gm);
-    float res = 0.f;
-    for (int i = 0; i < num_splits; ++i) {
-        const float w = pl[i] / gs * expf(pm[i] - gm);
-        res += part_o[((size_t)vh * num_splits + i) * D + d] * w;
-    }
-    out[(size_t)vh * D + d] = from_f32<T>(res);
-}
+// k_attn_combine (attn_combine.cuh): grid (B*len_q*num_heads), block D
 
 static int attn_num_splits(int B, int len_q, int num_kv_heads, int m_query, int max_len_buf) {
     const int hgroups = (m_query + 7) / 8;

@@ -127,6 +127,11 @@ struct zl_llama {
     dev_ptr<int32_t> d_tb;     // token -> task map of the chunk being prefilled
     const int32_t* cur_tb = nullptr;   // token -> task map of the launch sequence being enqueued (d_iota at decode)
     dev_ptr<int8_t> d_mask;    // (chunk, max_seq) causal mask of the chunk
+    // joined steps (zl_llama_step_joined): segments {task, row0, pos0, n} for zl_varlen_attention, then per emitting
+    // segment its last row | its task | that row's position (max_batch each); h_join stages them with the tokens,
+    // positions and token -> task map of the rows (tok_cap each) for the copies into d_pf_tokens / d_pf_pos / d_tb
+    dev_ptr<int32_t> d_join;
+    host_ptr<int32_t> h_join;
     dev_ptr<> xperm;           // act-order: activations permuted for the GEMM routes that cannot gather (tok_cap x max K)
     // sampling (zl_llama_set_sampling): per-task parameters and generated-token bitmaps on the device; samp_on[t] is set
     // while task t samples or has penalties, and the step then runs zl_sample instead of zl_argmax
@@ -197,6 +202,14 @@ __global__ void k_prefill_setup(int32_t* __restrict__ pos, int32_t* __restrict__
         }
         if (threadIdx.x == 0) lens[task] = len_buf;
     }
+}
+
+// dst row i = src row idx[i] of a 16-bit (rows, D) matrix; grid = rows of dst
+__global__ void k_gather_rows(const uint16_t* __restrict__ src, const int32_t* __restrict__ idx, uint16_t* __restrict__ dst,
+                              int D) {
+    const uint16_t* s = src + (size_t)idx[blockIdx.x] * D;
+    uint16_t* o = dst + (size_t)blockIdx.x * D;
+    for (int i = threadIdx.x; i < D; i += blockDim.x) o[i] = s[i];
 }
 
 template <typename T>
@@ -703,6 +716,10 @@ int alloc_runtime(zl_llama* m) {
         RCHECK(dmalloc(&m->d_pf_tokens, T * 4));
         RCHECK(dmalloc(&m->d_pf_pos, T * 4));
         RCHECK(dmalloc(&m->d_mask, (size_t)c.prefill_chunk * c.max_seq));
+        RCHECK(dmalloc(&m->d_join, (size_t)7 * B * 4));
+        int32_t* hj = nullptr;
+        ZL_CHECK_CUDA(cudaMallocHost((void**)&hj, sizeof(int32_t) * ((size_t)3 * T + 7 * B)));
+        m->h_join.reset(hj);
     }
     RCHECK(dmalloc(&m->d_next, B * 4));
     RCHECK(dmalloc(&m->d_iota, B * 4));
@@ -711,6 +728,10 @@ int alloc_runtime(zl_llama* m) {
     // also bounds zl_decode_attention_kv8: it splits the keys into at most 64 pieces (kA8MaxSplits, at least
     // cdiv(max_len, 1024)) over B * len_q <= T query rows, and this reserves T * Hq * max(64, cdiv(max_seq, 1024)) pieces
     m->attn_ws_bytes = zl_decode_attention_workspace_bytes(T, 1, m->hq, d, c.max_seq);
+    if (c.prefill_chunk > 0) {   // joined steps: zl_varlen_attention over at most T rows of at most max_seq keys
+        const size_t va = zl_varlen_attention_workspace_bytes(T, 1, m->hq, d, c.max_seq);
+        if (va > m->attn_ws_bytes) m->attn_ws_bytes = va;
+    }
     RCHECK(dmalloc(&m->attn_ws, m->attn_ws_bytes));
     RCHECK(dmalloc(&m->argmax_ws, zl_argmax_workspace_bytes(B)));
     m->hwords = cdiv(m->vshard, 32);
@@ -1043,10 +1064,17 @@ int dense_or_w8(zl_llama* m, const void* x, const DenseLin& L, void* y, int B, i
                         ZL_W8_FP8_ROWS, c.dtype, pdl, st);
 }
 
-// pf != nullptr: one chunk of a prompt (tokens of ONE task at consecutive positions) instead of one token per task
-struct PrefillChunk {
-    int task, pos0, n;
-    bool last;   // run final norm + lm_head + pick on the chunk's last token
+// pf != nullptr: a list of segments -- rows of one task at consecutive positions -- instead of one token per task.  Their
+// tokens, positions and token -> task map are staged in d_pf_tokens / d_pf_pos / d_tb.
+//   prefill chunk (joined = false): ONE segment (task, pos0, n), attended with the masked decode kernel; last = run the
+//                                   final norm + lm_head + pick on its last row
+//   joined step (joined = true):    nseg segments of distinct tasks (d_join), attended with zl_varlen_attention; the last
+//                                   rows of the n_emit emitting segments feed the head
+struct Segments {
+    int task = 0, pos0 = 0, n = 0;   // n: rows of the whole launch sequence
+    bool last = false;
+    bool joined = false;
+    int nseg = 1, n_emit = 0, max_keys = 0;
 };
 
 // ------------------------------------------------------------------------------------------------------------------
@@ -1077,7 +1105,7 @@ static bool prefill_dual_enabled(const zl_llama* m, int n) {
     return force == 1 || (force == 2 && c.tp_size > 1);
 }
 
-int prefill_layers_dual(zl_llama* m, const PrefillChunk& pf) {
+int prefill_layers_dual(zl_llama* m, const Segments& pf) {
     const auto& c = m->cfg;
     RCHECK(ensure_dual_resources(m));
     const int D = c.dim_model, d = c.dim_head, dt = c.dtype;
@@ -1128,23 +1156,30 @@ int prefill_layers_dual(zl_llama* m, const PrefillChunk& pf) {
     return ZL_OK;
 }
 
-int enqueue_step(zl_llama* m, int n_tasks, int len_bucket, const PrefillChunk* pf = nullptr, bool sampler = false) {
+int enqueue_step(zl_llama* m, int n_tasks, int len_bucket, const Segments* pf = nullptr, bool sampler = false) {
     const auto& c = m->cfg;
     const int B = pf ? pf->n : n_tasks;   // rows (tokens) of every activation matrix in this launch sequence
     const int D = c.dim_model, d = c.dim_head, dt = c.dtype, pdl = c.use_pdl;
     cudaStream_t st = m->stream;
     const bool w4 = c.quant_type == 5 || c.quant_type == 6;
     const bool tp = c.tp_size > 1;
+    const bool joined = pf && pf->joined;
     if (tp && !m->comm) {
         zl_set_last_error(__FILE__, __LINE__, "tp_size > 1 but zl_llama_set_comm was not called");
         return ZL_ERR_STATE;
     }
+    // joined steps: d_join = segments (nseg x 4) | emitting rows | their tasks | their positions (max_batch each)
+    const int32_t* j_seg = joined ? m->d_join.get() : nullptr;
+    const int32_t* j_rows = joined ? j_seg + 4 * c.max_batch : nullptr;
+    const int32_t* j_task = joined ? j_rows + c.max_batch : nullptr;
+    const int32_t* j_pos = joined ? j_task + c.max_batch : nullptr;
 
-    if (pf) {
+    // (a joined step's positions and token -> task map were staged by zl_llama_step_joined with its tokens)
+    if (pf && !joined) {
         k_prefill_setup<<<8, 256, 0, st>>>(m->d_pf_pos.get(), m->d_tb.get(), m->d_lens.get(), m->d_mask.get(), pf->task,
                                            pf->pos0, pf->n);
         ZL_CHECK_LAUNCH();
-    } else {
+    } else if (!pf) {
         ZL_CHECK_CUDA(launch(k_lens_from_pos, dim3(cdiv(B, 64)), dim3(64), 0, st, false, (const int32_t*)m->d_pos.get(),
                              m->d_lens.get(), B, g_w4_trace));
     }
@@ -1154,7 +1189,7 @@ int enqueue_step(zl_llama* m, int n_tasks, int len_bucket, const PrefillChunk* p
     RCHECK(zl_rope_cos_sin(m->cur_pos, m->cosb.get(), m->sinb.get(), B, d, c.rope_theta, c.rope_llama3_factor,
                            c.rope_low_freq_factor, c.rope_high_freq_factor, c.rope_orig_ctx, 1, st));
     RCHECK(zl_embedding(m->cur_tokens, m->emb.get(), m->h.get(), B, D, c.vocab_size, dt, 0, st));
-    const bool dual = pf && prefill_dual_enabled(m, pf->n);
+    const bool dual = pf && !joined && prefill_dual_enabled(m, pf->n);
     if (dual) RCHECK(prefill_layers_dual(m, *pf));
     Chain ch;
     ch.n = B;
@@ -1189,7 +1224,12 @@ int enqueue_step(zl_llama* m, int n_tasks, int len_bucket, const PrefillChunk* p
                                           pdl, st));
             }
         }
-        if (pf) {
+        if (joined) {
+            // every segment causally over its own task's cache, one launch (attention.cpp:924-961)
+            RCHECK(zl_varlen_attention(m->q.get(), j_seg, pf->nseg, B, L.k_addrs.get(), L.v_addrs.get(),
+                                       1.0f / sqrtf((float)d), pf->max_keys, m->ao.get(), m->hq, m->hkv, d, m->attn_ws.get(),
+                                       m->attn_ws_bytes, dt, pdl, st));
+        } else if (pf) {
             // one task, len_q = chunk, causal int8 mask (Attention::dynamic_batch_forward with len_q > 1, attention.cpp:846-964)
             RCHECK(attention(m, l, m->q.get(), pf->task, m->d_mask.get(), pf->pos0 + pf->n, m->ao.get(), 1, pf->n, pdl, st));
         } else {
@@ -1215,7 +1255,21 @@ int enqueue_step(zl_llama* m, int n_tasks, int len_bucket, const PrefillChunk* p
                                              pdl, st));
         }
     }
-    if (pf) {
+    const void* head_x = m->xn.get();   // rows that reach lm_head
+    if (joined) {
+        if (pf->n_emit == 0) return ZL_OK;
+        // the final norm is row-wise: norm every row, then gather the emitting segments' last rows into rows
+        // 0 .. n_emit - 1 of pend (free after the norm), so that only they reach lm_head
+        if (w4)
+            RCHECK(zl_rmsnorm(m->h.get(), m->ln_f.get(), m->xn.get(), B, D, c.eps, 1.f, dt, pdl, st));
+        else
+            RCHECK(zl_add_rmsnorm(m->h.get(), m->pend.get(), m->ln_f.get(), m->h.get(), m->xn.get(), B, D, c.eps, 1.f, 0,
+                                  dt, pdl, st));
+        k_gather_rows<<<pf->n_emit, 256, 0, st>>>(static_cast<const uint16_t*>(m->xn.get()), j_rows,
+                                                 static_cast<uint16_t*>(m->pend.get()), D);
+        ZL_CHECK_LAUNCH();
+        head_x = m->pend.get();
+    } else if (pf) {
         if (!pf->last) return ZL_OK;
         // only the last prompt position feeds the head: move it to row 0 semantics by pointing at its row
         void* hl = rows(m->h.get(), pf->n - 1, D);
@@ -1231,15 +1285,16 @@ int enqueue_step(zl_llama* m, int n_tasks, int len_bucket, const PrefillChunk* p
         RCHECK(zl_add_rmsnorm(m->h.get(), m->pend.get(), m->ln_f.get(), m->h.get(), m->xn.get(), B, D, c.eps, 1.f, 0, dt,
                               stage_pdl(m, kFinalNorm), st));
     }
-    const int HB = pf ? 1 : B;   // rows that reach lm_head
+    const int HB = joined ? pf->n_emit : pf ? 1 : B;   // rows that reach lm_head
     // vocab-parallel lm_head (embedding.cu:353-392): each rank owns vshard rows
-    RCHECK(zl_dense_gemm_skinny(m->xn.get(), D, m->lm_head, nullptr, m->logits.get(), HB, m->vshard, D, dt, ZL_F32,
+    RCHECK(zl_dense_gemm_skinny(head_x, D, m->lm_head, nullptr, m->logits.get(), HB, m->vshard, D, dt, ZL_F32,
                                 stage_pdl(m, kLmHead), st));
     if (sampler) {
         // one row per task at decode (row b = task b, counter = its input position); prefill: the task's last prompt
-        // position.  set_sampling keeps this off under tensor parallelism.
-        const int32_t* row_task = pf ? m->d_iota.get() + pf->task : m->d_iota.get();
-        const int32_t* counter = pf ? m->d_pf_pos.get() + (pf->n - 1) : m->d_pos.get();
+        // position; joined: each emitting segment's task and last position.  set_sampling keeps this off under tensor
+        // parallelism.
+        const int32_t* row_task = joined ? j_task : pf ? m->d_iota.get() + pf->task : m->d_iota.get();
+        const int32_t* counter = joined ? j_pos : pf ? m->d_pf_pos.get() + (pf->n - 1) : m->d_pos.get();
         RCHECK(zl_sample(m->logits.get(), HB, m->vshard, m->d_sparams.get(), row_task, counter, m->d_hist.get(), m->hwords,
                          m->d_next.get(), nullptr, 0, stage_pdl(m, kPick), st));
     } else if (!tp) {
@@ -1658,7 +1713,11 @@ extern "C" int zl_llama_prefill(zl_llama_t* m, int task, const int32_t* tokens_h
             h_tok[i] = tokens_host[c0 + i];
         }
         ZL_CHECK_CUDA(cudaMemcpyAsync(m->d_pf_tokens.get(), h_tok, cn * 4, cudaMemcpyHostToDevice, m->stream));
-        PrefillChunk pc{task, pos0 + c0, cn, c0 + cn == n};
+        Segments pc;
+        pc.task = task;
+        pc.pos0 = pos0 + c0;
+        pc.n = cn;
+        pc.last = c0 + cn == n;
         RCHECK(enqueue_step(m, 1, 0, &pc, sampler_on(m, task, 1)));
     }
     ZL_CHECK_CUDA(cudaMemcpyAsync(m->h_stage.get() + 3 * m->cfg.max_batch, m->d_next.get(), 4, cudaMemcpyDeviceToHost, m->stream));
@@ -1667,6 +1726,87 @@ extern "C" int zl_llama_prefill(zl_llama_t* m, int task, const int32_t* tokens_h
     ZL_CHECK_CUDA(cudaStreamSynchronize(m->stream));
     *next_token_host = m->h_stage.get()[3 * m->cfg.max_batch];
     if (pos0 + n > m->cur_max_len) m->cur_max_len = pos0 + n;
+    return ZL_OK;
+}
+
+extern "C" int zl_llama_step_joined(zl_llama_t* m, const int32_t* tokens_host, const int32_t* seg_host, int nseg,
+                                    int32_t* next_host, float* logits_host) {
+    ZL_CHECK_ARG(m && tokens_host && seg_host && next_host && nseg > 0);
+    const auto& c = m->cfg;
+    if (c.prefill_chunk <= 0) {
+        zl_set_last_error(__FILE__, __LINE__, "zl_llama_step_joined needs cfg.prefill_chunk > 0");
+        return ZL_ERR_STATE;
+    }
+    // zl_varlen_attention reads the activation-dtype cache of one rank
+    if (c.kv_int8 || c.tp_size > 1)
+        return fail_state(__LINE__, "joined steps are not available with an int8 KV cache or tensor parallelism",
+                          ZL_ERR_UNSUPPORTED);
+    if (!m->finalized) return fail_state(__LINE__, "model not finalized");
+    ZL_CHECK_ARG(nseg <= c.max_batch);
+    // every check before any work is enqueued
+    std::vector<char> seen(c.max_batch, 0);
+    int rows = 0;
+    for (int s = 0; s < nseg; ++s) {
+        const int32_t* s4 = seg_host + 4 * s;   // {task, pos0, n, emit}
+        ZL_CHECK_ARG(s4[0] >= 0 && s4[0] < c.max_batch && !seen[s4[0]]);
+        ZL_CHECK_ARG(s4[2] >= 1 && s4[1] >= 0 && s4[1] <= c.max_seq - s4[2]);
+        seen[s4[0]] = 1;
+        rows += s4[2];
+        ZL_CHECK_ARG(rows <= m->tok_cap);
+    }
+    for (int i = 0; i < rows; ++i) ZL_CHECK_ARG(tokens_host[i] >= 0 && tokens_host[i] < c.vocab_size);
+
+    // host staging: tokens | positions | token -> task (tok_cap each) | segments | emitting rows | tasks | positions
+    const int T = m->tok_cap, MB = c.max_batch;
+    int32_t* h_tok = m->h_join.get();
+    int32_t* h_pos = h_tok + T;
+    int32_t* h_tb = h_pos + T;
+    int32_t* h_seg = h_tb + T;
+    int32_t* h_erow = h_seg + 4 * MB;
+    int32_t* h_etask = h_erow + MB;
+    int32_t* h_epos = h_etask + MB;
+    Segments sg;
+    sg.joined = true;
+    sg.n = rows;
+    sg.nseg = nseg;
+    bool sampler = false;
+    for (int s = 0, row0 = 0; s < nseg; ++s) {
+        const int task = seg_host[4 * s], pos0 = seg_host[4 * s + 1], n = seg_host[4 * s + 2];
+        for (int i = 0; i < n; ++i) {
+            h_tok[row0 + i] = tokens_host[row0 + i];
+            h_pos[row0 + i] = pos0 + i;
+            h_tb[row0 + i] = task;
+        }
+        h_seg[4 * s] = task;
+        h_seg[4 * s + 1] = row0;
+        h_seg[4 * s + 2] = pos0;
+        h_seg[4 * s + 3] = n;
+        if (seg_host[4 * s + 3]) {
+            h_erow[sg.n_emit] = row0 + n - 1;
+            h_etask[sg.n_emit] = task;
+            h_epos[sg.n_emit] = pos0 + n - 1;
+            ++sg.n_emit;
+            sampler |= m->samp_on[task] != 0;
+        }
+        if (pos0 + n > sg.max_keys) sg.max_keys = pos0 + n;
+        row0 += n;
+    }
+    cudaStream_t st = m->stream;
+    ZL_CHECK_CUDA(cudaMemcpyAsync(m->d_pf_tokens.get(), h_tok, (size_t)rows * 4, cudaMemcpyHostToDevice, st));
+    ZL_CHECK_CUDA(cudaMemcpyAsync(m->d_pf_pos.get(), h_pos, (size_t)rows * 4, cudaMemcpyHostToDevice, st));
+    ZL_CHECK_CUDA(cudaMemcpyAsync(m->d_tb.get(), h_tb, (size_t)rows * 4, cudaMemcpyHostToDevice, st));
+    ZL_CHECK_CUDA(cudaMemcpyAsync(m->d_join.get(), h_seg, (size_t)7 * MB * 4, cudaMemcpyHostToDevice, st));
+    RCHECK(enqueue_step(m, 0, 0, &sg, sampler));
+    int32_t* h_next = m->h_stage.get() + 3 * MB;
+    if (sg.n_emit) {
+        ZL_CHECK_CUDA(cudaMemcpyAsync(h_next, m->d_next.get(), (size_t)sg.n_emit * 4, cudaMemcpyDeviceToHost, st));
+        if (logits_host)
+            ZL_CHECK_CUDA(cudaMemcpyAsync(logits_host, m->logits.get(), (size_t)sg.n_emit * m->vshard * 4,
+                                          cudaMemcpyDeviceToHost, st));
+    }
+    ZL_CHECK_CUDA(cudaStreamSynchronize(st));   // also frees the pinned staging for the next call
+    for (int s = 0, e = 0; s < nseg; ++s) next_host[s] = seg_host[4 * s + 3] ? h_next[e++] : -1;
+    if (sg.max_keys > m->cur_max_len) m->cur_max_len = sg.max_keys;
     return ZL_OK;
 }
 

@@ -33,6 +33,35 @@ MODEL_PRESETS = {
 QUANT_NONE, QUANT_AUTO_INT8, QUANT_GPTQ, QUANT_AWQ, QUANT_FP8 = 0, 2, 5, 6, 7     # model_config.hpp:132-144
 
 
+def pack_joined_segments(segments, max_batch, max_seq, vocab_size):
+    """Validate the segments of a joined step, [(task, tokens, pos0, emit), ...], and pack them for zl_llama_step_joined:
+    -> (tokens (sum n) int32, seg (nseg, 4) int32 {task, pos0, n, emit}).  Raises ValueError for a malformed list."""
+    segments = list(segments)
+    if not segments or len(segments) > max_batch:
+        raise ValueError("a joined step takes 1 .. max_batch (%d) segments, not %d" % (max_batch, len(segments)))
+    seg = np.zeros((len(segments), 4), dtype=np.int32)
+    toks, seen = [], set()
+    for i, s in enumerate(segments):
+        if len(s) != 4:
+            raise ValueError("segment %d: expected (task, tokens, pos0, emit)" % i)
+        task, tokens, pos0, emit = s
+        t = np.asarray(tokens)
+        if t.ndim != 1 or t.size == 0 or not np.issubdtype(t.dtype, np.integer):
+            raise ValueError("segment %d: tokens must be a non-empty 1-D integer array" % i)
+        task, pos0 = int(task), int(pos0)
+        if not 0 <= task < max_batch or task in seen:
+            raise ValueError("segment %d: task %d out of range or repeated" % (i, task))
+        if pos0 < 0 or pos0 + t.size > max_seq:
+            raise ValueError("segment %d: positions %d .. %d outside the KV buffers (max_seq %d)"
+                             % (i, pos0, pos0 + t.size - 1, max_seq))
+        if t.min() < 0 or t.max() >= vocab_size:
+            raise ValueError("segment %d: token id out of range" % i)
+        seen.add(task)
+        seg[i] = (task, pos0, t.size, 1 if emit else 0)
+        toks.append(t.astype(np.int32))
+    return np.ascontiguousarray(np.concatenate(toks)), seg
+
+
 class LlamaDecoder:
     def __init__(self, num_layers, dim_model, num_heads, num_kv_heads, dim_head, dim_ff, vocab_size, eps=1e-5,
                  rope_theta=10000.0, rope_llama3=None, quant_type=QUANT_NONE, group_size=128, sym=False,
@@ -112,6 +141,22 @@ class LlamaDecoder:
             self.h, int(task), t.ctypes.data_as(ctypes.c_void_p), t.size, int(pos0),
             nxt.ctypes.data_as(ctypes.c_void_p), logits.ctypes.data_as(ctypes.c_void_p) if want_logits else None))
         return (int(nxt[0]), logits) if want_logits else int(nxt[0])
+
+    def step_joined(self, segments, want_logits=False):
+        """One joined step (zl_llama_step_joined): segments = [(task, tokens, pos0, emit), ...] of distinct tasks -- prompt
+        chunks and decode rows (one token) alike -- run through one forward; rows sum(len(tokens)) <= max(max_batch,
+        prefill_chunk).  Returns the next tokens (nseg,) int32, -1 where emit is false [, logits (n_emit, V/tp) fp32 of
+        the emitting segments' last rows, in segment order]."""
+        cfg = self.cfg
+        tokens, seg = pack_joined_segments(segments, cfg.max_batch, cfg.max_seq, cfg.vocab_size)
+        n_emit = int(seg[:, 3].sum())
+        nxt = np.empty(seg.shape[0], dtype=np.int32)
+        logits = np.empty((n_emit, self.vocab_shard), dtype=np.float32) if want_logits else None
+        _lib.check(self.lib.zl_llama_step_joined(
+            self.h, tokens.ctypes.data_as(ctypes.c_void_p), seg.ctypes.data_as(ctypes.c_void_p), seg.shape[0],
+            nxt.ctypes.data_as(ctypes.c_void_p),
+            logits.ctypes.data_as(ctypes.c_void_p) if want_logits and n_emit else None))
+        return (nxt, logits) if want_logits else nxt
 
     def set_sampling(self, task, temperature=0.0, top_p=1.0, top_k=0, repetition_penalty=1.0, presence_penalty=0.0,
                      seed=0):

@@ -405,6 +405,30 @@ def decode_attention(q, buf_lens, k_bufs, v_bufs, mask, scale, max_len_buf, num_
     return out
 
 
+def varlen_attention(q, segments, k_bufs, v_bufs, scale, num_kv_heads, max_keys=None, pdl=False):
+    """Causal variable-length attention: q (rows, H_q, d); segments (nseg, 4) int32 {task, row0, pos0, n} (host or device;
+    rows row0 .. row0 + n - 1 are positions pos0 .. pos0 + n - 1 of task `task`, each attending keys 0 ..= its position);
+    k_bufs / v_bufs lists of per-task (len, H_kv, d) tensors.  max_keys defaults to max(pos0 + n)."""
+    if q.dim() != 3:
+        raise _lib.ZLError(-1, "q must be (rows, H_q, d)")
+    rows, hq, d = q.shape
+    seg = torch.as_tensor(segments, dtype=torch.int32)
+    if seg.dim() != 2 or seg.shape[1] != 4:
+        raise _lib.ZLError(-1, "segments must be (nseg, 4) {task, row0, pos0, n}")
+    if max_keys is None:
+        max_keys = int((seg[:, 2] + seg[:, 3]).max().item())
+    seg = seg.to(q.device).contiguous()
+    nseg = seg.shape[0]
+    out = torch.empty_like(q)
+    ws_bytes = _lib.load().zl_varlen_attention_workspace_bytes(rows, nseg, hq, d, max_keys)
+    ws = torch.empty(ws_bytes, dtype=torch.uint8, device=q.device)
+    ka, va = _ptr_table(k_bufs, q.device), _ptr_table(v_bufs, q.device)
+    _lib.call("zl_varlen_attention", _p(q), _p(seg), nseg, rows, _p(ka), _p(va), float(scale), int(max_keys), _p(out), hq,
+              num_kv_heads, d, _p(ws), ws_bytes, _dt(q), int(pdl), _stream())
+    torch.cuda.current_stream().synchronize()
+    return out
+
+
 def decode_attention_kv8(q, buf_lens, k_bufs, v_bufs, sk_bufs, sv_bufs, mask, scale, max_len_buf, num_kv_heads, out_dtype=None,
                          pdl=False):
     """int8 KV cache attention: q (B, len_q, H_q, d) f16; k/v lists of (len_buf, H_kv, d) uint8; sk/sv lists of

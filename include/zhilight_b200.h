@@ -298,6 +298,22 @@ int zl_varlen_attention(const void* q, const int32_t* seg, int nseg, int rows, v
                         float scale, int max_keys, void* out, int num_heads, int num_kv_heads, int dim_head, void* ws,
                         size_t ws_bytes, int dtype, int pdl, zl_stream_t stream);
 
+/* MLA decode attention over per-task latent caches: nn::multi_query_attention_rag_buffer with dim_head 576 and a
+ * 512-wide output, as the reference's MLA search path calls it (src/nn/attention/multi_head_latent_attention.cpp:1053-1068;
+ * kernels attention_kernel.cu:1281-1284, 1347-1348, 1390-1391, 1429-1435), and the per-task GEMM / softmax / GEMM of its
+ * attn_by_gemm (multi_head_latent_attention.cpp:834-874).
+ * q (B, len_q, H, 576); kv_addrs (B) device array of device pointers, task b's latent rows (len_buf_b, 576): the first 512
+ * elements of a row are its value, the whole row its key, shared by all H heads; buf_lens (B); mask optional int8 ragged
+ * concat of (len_q, len_buf_b) as for zl_decode_attention; out (B, len_q, H, 512).  Row (b, i, h) attends keys
+ * 0 .. buf_lens[b] - 1: logit = mask ? scale * q.k : -inf, o = softmax . v (max seeded -1e20, sum seeded 1e-20), so a row
+ * with every key masked gives 0.  Rows past buf_lens[b] are never read.  fp16 / bf16, 1 <= H <= 128 (ZL_ERR_UNSUPPORTED
+ * above).  workspace: at least zl_mla_decode_attention_workspace_bytes (0 when max_len_buf <= 256); two launches give
+ * bit-identical output. */
+size_t zl_mla_decode_attention_workspace_bytes(int B, int len_q, int num_heads, int max_len_buf);
+int zl_mla_decode_attention(const void* q, const int32_t* buf_lens, void* const* kv_addrs, const int8_t* mask,
+                            float scale, int max_len_buf, void* out, int B, int len_q, int num_heads,
+                            void* workspace, size_t workspace_bytes, int dtype, int pdl, zl_stream_t stream);
+
 /* int8 KV cache (KV_CACHE_DTYPE=int8 of the reference): KERNEL_mqa_rag_buffer_split_kv_quant
  * (src/nn/attention/attention_kernel.cu:804-880, src/nn/attention/quant_attention.cuh:10-123).  K / V buffers per task are
  * (len_buf, H_kv, d) uint8 = round(x * 127 / absmax) + 128, scale buffers (len_buf, H_kv) fp32 = absmax / 127 (BSHD only,

@@ -25,6 +25,7 @@
 
 #include "zhilight_b200.h"
 
+#include <algorithm>
 #include <string>
 #include <tuple>
 
@@ -298,6 +299,21 @@ void multi_query_attention_rag_buffer(const core::Context& ctx, const Tensor& ba
     (void)algo_id;
     (void)ws;
     const int B = (int)batch_q.size(0), len_q = (int)batch_q.size(1), Hq = (int)batch_q.size(2), d = (int)batch_q.size(3);
+    if (d == 576) {
+        // MLA (multi_head_latent_attention.cpp:1053-1068): one latent head whose 576-wide rows are K and whose first 512
+        // elements are V; the reference passes the same address table as keys and values
+        BM_ASSERT_EQ(output.size(-1), 512, "dim_head mismatch");
+        BM_ASSERT_EQ(m_query, Hq, "MLA attends one latent head");
+        BM_ASSERT(key_buf_addrs.data() == val_buf_addrs.data(), "MLA keys and values share one latent cache");
+        BM_ASSERT(!scale_key_addrs.numel(), "no int8 latent cache");
+        const size_t mwsb = zl_mla_decode_attention_workspace_bytes(B, len_q, Hq, max_len_buf);
+        Tensor mwork = ctx.tensor({std::max<size_t>(mwsb, 16)}, DataType::kInt8);
+        ZL_THROW_IF(zl_mla_decode_attention(batch_q.data(), buf_lens.data<int32_t>(), key_buf_addrs.data<void*>(),
+                                            mask.numel() ? mask.data<int8_t>() : nullptr, scale, max_len_buf,
+                                            output.data(), B, len_q, Hq, mwork.data(), mwsb, zl_dt(batch_q.dtype()), 0,
+                                            st(ctx)));
+        return;
+    }
     const size_t wsb = zl_decode_attention_workspace_bytes(B, len_q, Hq, d, max_len_buf);
     Tensor work = ctx.tensor({wsb}, DataType::kInt8);
     if (scale_key_addrs.numel()) {

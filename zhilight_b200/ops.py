@@ -405,6 +405,30 @@ def decode_attention(q, buf_lens, k_bufs, v_bufs, mask, scale, max_len_buf, num_
     return out
 
 
+def mla_decode_attention(q, buf_lens, kv_bufs, mask, scale, max_len_buf, pdl=False):
+    """MLA decode attention (nn::multi_query_attention_rag_buffer with dim_head 576): q (B, len_q, H, 576); kv_bufs a list
+    of B per-task latent caches (len, 576) or (len, 1, 576), each row the key of every head and its first 512 elements
+    the value; mask None or the int8 ragged concat of (len_q, len_buf_b).  Returns (B, len_q, H, 512)."""
+    if q.dim() != 4 or q.shape[-1] != 576:
+        raise _lib.ZLError(-1, "q must be (B, len_q, H, 576)")
+    b, len_q, hq, _ = q.shape
+    if len(kv_bufs) != b:
+        raise _lib.ZLError(-1, "one latent cache per task expected")
+    for t in kv_bufs:
+        if not (t.dim() == 2 and t.shape[1] == 576) and not (t.dim() == 3 and t.shape[1:] == (1, 576)):
+            raise _lib.ZLError(-1, "latent cache must be (len, 576) or (len, 1, 576)")
+        if t.dtype != q.dtype:
+            raise _lib.ZLError(-1, "latent cache dtype differs from q")
+    out = torch.empty((b, len_q, hq, 512), dtype=q.dtype, device=q.device)
+    ws_bytes = _lib.load().zl_mla_decode_attention_workspace_bytes(b, len_q, hq, max_len_buf)
+    ws = torch.empty(ws_bytes, dtype=torch.uint8, device=q.device)
+    ka = _ptr_table(kv_bufs, q.device)
+    _lib.call("zl_mla_decode_attention", _p(q), _p(buf_lens), _p(ka), _p(mask), float(scale), int(max_len_buf), _p(out), b,
+              len_q, hq, _p(ws), ws_bytes, _dt(q), int(pdl), _stream())
+    torch.cuda.current_stream().synchronize()
+    return out
+
+
 def varlen_attention(q, segments, k_bufs, v_bufs, scale, num_kv_heads, max_keys=None, pdl=False):
     """Causal variable-length attention: q (rows, H_q, d); segments (nseg, 4) int32 {task, row0, pos0, n} (host or device;
     rows row0 .. row0 + n - 1 are positions pos0 .. pos0 + n - 1 of task `task`, each attending keys 0 ..= its position);

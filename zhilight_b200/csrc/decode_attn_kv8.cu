@@ -55,7 +55,8 @@ k_decode_attn_kv8(const __half* __restrict__ q, const int32_t* __restrict__ buf_
     constexpr int DC = D / 8;                  // threads covering one V row (8 bytes each)
     constexpr int NSUB = kA8Threads / DC;
     __shared__ __align__(16) float s_logit[8 * kA8RowStride];
-    __shared__ float s_m[8], s_l[8];
+    __shared__ float s_sv[kA8MaxRange];        // V scales of the split's keys
+    __shared__ float s_m[8], s_l[8], s_w[8];
 
     const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
     const int g = lane >> 2, t = lane & 3;
@@ -107,6 +108,10 @@ k_decode_attn_kv8(const __half* __restrict__ q, const int32_t* __restrict__ buf_
             kb[i] = ld_cg_b8(pb + i * 32);
         }
         const float sa = __ldcg(skb + (size_t)ra * num_kv_heads), sb = __ldcg(skb + (size_t)rb * num_kv_heads);
+        if (t == 0) {   // the V scales ride along with the K loads, so that phase 2 reads them from shared memory
+            s_sv[tile * 16 + g] = __ldcg(svb + (size_t)ra * num_kv_heads);
+            s_sv[tile * 16 + g + 8] = __ldcg(svb + (size_t)rb * num_kv_heads);
+        }
         float acc[4] = {0.f, 0.f, 0.f, 0.f};
 #pragma unroll
         for (int i = 0; i < NI; ++i) {
@@ -135,30 +140,36 @@ k_decode_attn_kv8(const __half* __restrict__ q, const int32_t* __restrict__ buf_
     }
     __syncthreads();
 
-    // ---- phase 2: masked softmax statistics per head; the V scale is folded into the stored weights ----
+    // ---- phase 2: masked softmax statistics per head; the V scale is folded into the stored weights w = e * scale_v,
+    // and s_w keeps the split's largest weight per head (floored at 1e-30 so that 1024 / s_w stays finite) ----
     for (int h = warp; h < mq; h += kA8Warps) {
         float* row = s_logit + h * kA8RowStride;
         float mx = -1e20f;
         for (int i = lane; i < n; i += 32) mx = fmaxf(mx, row[i]);
         mx = warp_max(mx);
-        float sum = 0.f;
+        float sum = 0.f, wmax = 0.f;
         for (int i = lane; i < n; i += 32) {
             const float e = expf(row[i] - mx);
+            const float w = e * s_sv[i];
             sum += e;
-            row[i] = e * __ldcg(svb + (size_t)(k0 + i) * num_kv_heads);
+            row[i] = w;
+            wmax = fmaxf(wmax, w);
         }
         sum = warp_sum(sum) + 1e-20f;
+        wmax = warp_max(wmax);
         if (lane == 0) {
             s_m[h] = mx;
             s_l[h] = sum;
+            s_w[h] = fmaxf(wmax, 1e-30f);
         }
     }
     __syncthreads();
 
     // ---- phase 3: O = (P * scale_v) . (V - 128) on the tensor cores (mma.sync m16n8k16, fp32 accumulate) ----
-    // A = weights [head (8 of 16 rows) x 16 keys] as fp16 (scaled by 2^10 so that small probabilities stay normal numbers),
-    // B = V [16 keys x 8 columns] as exact fp16 integers.  A B fragment register holds TWO KEYS of one column, V is stored
-    // key-major: lane (g, t) loads D/8 contiguous bytes (columns NJ g .. NJ g + NJ - 1) of its four keys 2t, 2t+1, 2t+8,
+    // A = weights [head (8 of 16 rows) x 16 keys] as fp16 w * 2^10 / s_w: at most 1024, so a V row with a large absmax
+    // cannot overflow fp16, and small weights stay normal numbers; s_w / 2^10 is multiplied back in when the accumulators
+    // are written out.  B = V [16 keys x 8 columns] as exact fp16 integers.  A B fragment register holds TWO KEYS of one
+    // column, V is stored key-major: lane (g, t) loads D/8 contiguous bytes (columns NJ g .. NJ g + NJ - 1) of its four keys 2t, 2t+1, 2t+8,
     // 2t+9 and byte-interleaves row pairs with PRMT; n-tile j column c then stands for column d = NJ c + j of V (any
     // permutation of the columns is as good as another -- it is undone when the accumulators are written out).
     constexpr int NJ = D / 8;                        // n-tiles = V columns per lane and key row
@@ -167,6 +178,7 @@ k_decode_attn_kv8(const __half* __restrict__ q, const int32_t* __restrict__ buf_
 #pragma unroll
     for (int j = 0; j < NJ; ++j) o[j][0] = o[j][1] = o[j][2] = o[j][3] = 0.f;
     const __half2 voff = __float2half2_rn(1152.f);   // 1024 (magic) + 128 (zero point of the cache)
+    const float wenc = g < mq ? 1024.f / s_w[g] : 0.f;
     for (int tile = warp; tile < ntiles; tile += kA8Warps) {
         const int kb = tile * 16;                    // first key of the tile, relative to k0
         uint32_t vw[4][NW];
@@ -191,8 +203,8 @@ k_decode_attn_kv8(const __half* __restrict__ q, const int32_t* __restrict__ buf_
             const float* pr = s_logit + g * kA8RowStride + kb + 2 * t;
             const float2 p0 = *reinterpret_cast<const float2*>(pr), p1 = *reinterpret_cast<const float2*>(pr + 8);
             const bool in0 = kb + 2 * t < n, in1 = kb + 2 * t + 1 < n, in2 = kb + 2 * t + 8 < n, in3 = kb + 2 * t + 9 < n;
-            const __half2 h0 = __floats2half2_rn(in0 ? p0.x * 1024.f : 0.f, in1 ? p0.y * 1024.f : 0.f);
-            const __half2 h1 = __floats2half2_rn(in2 ? p1.x * 1024.f : 0.f, in3 ? p1.y * 1024.f : 0.f);
+            const __half2 h0 = __floats2half2_rn(in0 ? p0.x * wenc : 0.f, in1 ? p0.y * wenc : 0.f);
+            const __half2 h1 = __floats2half2_rn(in2 ? p1.x * wenc : 0.f, in3 ? p1.y * wenc : 0.f);
             af[0] = *reinterpret_cast<const uint32_t*>(&h0);   // (head g, keys 2t, 2t+1)
             af[2] = *reinterpret_cast<const uint32_t*>(&h1);   // (head g, keys 2t+8, 2t+9); rows g+8 (a1, a3) stay zero
         }
@@ -215,10 +227,11 @@ k_decode_attn_kv8(const __half* __restrict__ q, const int32_t* __restrict__ buf_
     float* s_red = s_logit;   // [warp][h][D]
     if (g < mq) {
         // accumulator (n-tile j, column c = 2t + i) = head g, V column NJ c + j; rows g + 8 (o[j][2..3]) are padding
+        const float wdec = s_w[g] * (1.f / 1024.f);
 #pragma unroll
         for (int j = 0; j < NJ; ++j) {
-            s_red[(warp * 8 + g) * D + NJ * (2 * t) + j] = o[j][0] * (1.f / 1024.f);
-            s_red[(warp * 8 + g) * D + NJ * (2 * t + 1) + j] = o[j][1] * (1.f / 1024.f);
+            s_red[(warp * 8 + g) * D + NJ * (2 * t) + j] = o[j][0] * wdec;
+            s_red[(warp * 8 + g) * D + NJ * (2 * t + 1) + j] = o[j][1] * wdec;
         }
     }
     __syncthreads();

@@ -5,6 +5,8 @@ import pytest
 import torch
 
 from oracle import ops as oops
+from tests.attn_check import assert_close as _assert_close
+from tests.attn_check import launched as _launched
 from tests.helpers import rel_l2
 
 pytestmark = pytest.mark.gpu
@@ -137,20 +139,6 @@ def _hot_keys(len_buf, split_counts):
     return sorted(hot)
 
 
-def _launched(fn):
-    """fn()'s result and the names of the kernels it launched.  The profiler now and then delivers a session's runtime
-    calls without the kernels' device records; such a session is run again (fn is deterministic)."""
-    from torch.profiler import ProfilerActivity, profile
-    for _ in range(3):
-        with profile(activities=[ProfilerActivity.CUDA]) as prof:
-            out = fn()
-            torch.cuda.synchronize()
-        names = [e.key for e in prof.key_averages()]
-        if any("cudaLaunchKernel" not in n and "k_" in n for n in names) or not any("cudaLaunchKernel" in n for n in names):
-            break
-    return out, names
-
-
 def _assert_route(names, route, splits):
     for r, k in KERNEL.items():
         assert any(k in n for n in names) == (r == route), (route, splits, names)
@@ -263,24 +251,6 @@ class _Kv8Cache:
 
     def run(self, inp, max_len_buf, out_dtype):
         return _launched(lambda: self.launch(inp, max_len_buf, out_dtype))
-
-
-def _assert_close(out, ref, tol, what=""):
-    """rel L2 <= tol over everything and <= 4 tol on each (task, query, head) row; rows whose reference is 0 (fully
-    masked) must be exactly 0."""
-    o = out.double()
-    assert torch.isfinite(o).all(), what
-    assert ((o - ref).norm() / ref.norm()).item() <= tol, (what, ((o - ref).norm() / ref.norm()).item())
-    d = ref.shape[-1]
-    rn, en = ref.reshape(-1, d).norm(dim=1), (o - ref).reshape(-1, d).norm(dim=1)
-    dead = rn == 0
-    assert (en[dead] == 0).all(), what
-    if (~dead).any():
-        rel = en[~dead] / rn[~dead]
-        worst = int(rel.argmax())
-        row = int(torch.nonzero(~dead)[worst])
-        assert rel[worst].item() <= 4 * tol, (what, "row (task, query, head)", np.unravel_index(row, ref.shape[:-1]),
-                                              rel[worst].item())
 
 
 def _tasks(route, lens, len_q, hkv, mq, splits=None, kv8=False):

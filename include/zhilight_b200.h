@@ -217,6 +217,24 @@ int zl_int8_scale_back(const int32_t* acc, const float* x_scale, const void* w_s
 int zl_w8a8_gemm(const void* xq, const float* x_scale, const void* w, const void* w_scale, int w_scale_dtype,
                  const void* bias, void* y, int M, int N, int K, int kind, int dtype, int pdl, zl_stream_t stream);
 
+/* ---- FP8 block-scaled Linear (QuantType 10, Fp8Block, src/nn/linear/linear.cpp:1697-1960): e4m3 weights (N,K) with
+ * one f32 weight_scale_inv per 128x128 block, activations quantised per token in groups of 128 along K ---------- */
+/* nn::fp8::per_token_cast_to_fp8 (src/nn/quant/fp8/fp8_util.cu:231-322), bit for bit: per (token m, 128-column group kb)
+ * amax = max(max|x|, 1e-4), q = e4m3(satfinite(x * (448/amax))) with the f32 product, scale[kb * scale_ld + m] =
+ * amax/448 (column-major (K/128, scale_ld); the reference and DeepGEMM use scale_ld = round_up(M, 4)).
+ * x (M,K) f16/bf16 with row stride ldx (ldx % 4 == 0, 8-byte aligned); q (M,K) e4m3 bytes.
+ * K % 128 != 0 -> ZL_ERR_UNSUPPORTED. */
+int zl_fp8_quant_per_token_group(const void* x, int ldx, void* q, float* scale, int scale_ld, int M, int K, int dtype,
+                                 int pdl, zl_stream_t stream);
+/* Fp8Block::forward's GEMM (deep_gemm_fp8_block_h20_group, linear.cpp:1697-1960) on the W8A8 kernels:
+ * y[m,n] = T( sum_kb (sum_{k in kb} xq[m,k] * w[n,k]) * x_scale[kb * x_scale_ld + m] * w_scale[(n/128) * (K/128) + kb] ).
+ * xq (M,K) e4m3 and w (N,K) e4m3 row-major, 16-byte aligned; x_scale as written by zl_fp8_quant_per_token_group;
+ * w_scale (ceil(N/128), K/128) f32 row-major (N need not be a multiple of 128).  Output f16 or bf16, no bias.
+ * mma.sync kernel up to M = 32, wgmma kernel in 256-row chunks above; each 128-k block's sum is promoted to f32 before
+ * it is scaled.  K % 128 != 0 -> ZL_ERR_UNSUPPORTED. */
+int zl_fp8_block_gemm(const void* xq, const float* x_scale, int x_scale_ld, const void* w, const float* w_scale, void* y,
+                      int M, int N, int K, int dtype, int pdl, zl_stream_t stream);
+
 /* functions::Gemm / NormalLinear for skinny M (lm_head, bf16 models; src/nn/linear/linear.cpp:150-430,
  * src/nn/embedding/embedding.cu:353-392): y(M,N) = x(M,K) @ W(N,K)^T (+bias), dtype f16/bf16,
  * out_dtype f16/bf16/f32. */
@@ -441,7 +459,9 @@ typedef struct zl_llama_config {
     float rope_llama3_factor; /* <= 0: plain rope */
     float rope_low_freq_factor, rope_high_freq_factor, rope_orig_ctx;
     int quant_type; /* model_config.hpp:132-144 QuantType: 0 none, 2 AutoInt8 (fp weights quantised per row at load),
-                     * 5 GPTQ, 6 AWQ, 7 FP8 (e4m3 weights + per-tensor weight_scale), 8 GPTQ_Marlin (= 5 with sym) */
+                     * 5 GPTQ, 6 AWQ, 7 FP8 (e4m3 weights + per-tensor weight_scale), 8 GPTQ_Marlin (= 5 with sym),
+                     * 10 FP8_Block (e4m3 weights + weight_scale_inv (ceil(N/128), K/128) f32; tp_size 1, no qkv_bias,
+                     * dim_model, q/k/v widths and dim_ff multiples of 128, else ZL_ERR_UNSUPPORTED) */
     int group_size, sym;
     int dtype; /* ZL_F16 / ZL_BF16 (W4 paths are fp16-only like the reference, q_gemm_k_major.cu:989) */
     int max_batch, max_seq;

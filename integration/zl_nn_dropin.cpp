@@ -8,7 +8,7 @@
 // Signatures: src/nn/quant/gptq/gptq.h:24-110, src/nn/attention/attention_kernel.h:64-80,
 // src/nn/layernorm/layernorm.h:7-34, src/nn/block/block_kernel.h, src/nn/linear/activation_kernel.h:12-16,
 // src/nn/position/rotary_embedding.h:52-65, src/kvcache/ragged_buffer_kernel.h:27-36,
-// src/nn/quant/int8/quant_kernel.h:15-128, src/nn/quant/fp8/fp8.h:13-23.
+// src/nn/quant/int8/quant_kernel.h:15-128, src/nn/quant/fp8/fp8.h:13-30, 3rd/deep_gemm/deep_gemm_api.h.
 #include <bmengine/core/core.h>
 #include <bmengine/functions/typecast.h>
 
@@ -467,4 +467,39 @@ Tensor dynamic_scaled_quant(const core::Context& ctx, const Tensor& input, float
     return out;
 }
 
+// fp8_util.cu:231-322: one scale per (token, 128 columns), (K/128, round_up(M, 4)) column-major or (round_up(M, 4),
+// K/128) row-major.  The kernel writes column-major; the row-major form is its transpose.
+Tensor per_token_cast_to_fp8(const core::Context& ctx, const Tensor& input, bool scale_col_major, float MAX_E4M3) {
+    BM_ASSERT(MAX_E4M3 == 448.f, "e4m3 max");
+    BM_ASSERT_EQ(input.ndim(), 2, "FP8 block_scale: input is not 2D");
+    BM_ASSERT_EQ(input.size(1) % 128, 0, "FP8 block_scale: input.size(1) can't divide 128");
+    const size_t m = input.size(0), n = input.size(1), aligned_m = (m + 3) / 4 * 4;
+    Tensor out = ctx.tensor(input.shape(), DataType::kFP8_E4M3, "", std::max<size_t>(32 * n, 1024));
+    Tensor col = ctx.tensor({n / 128, aligned_m}, DataType::kFloat);
+    ZL_THROW_IF(zl_fp8_quant_per_token_group(input.data(), (int)input.stride(0), out.data(), col.mutable_data<float>(),
+                                             (int)aligned_m, (int)m, (int)n, zl_dt(input.dtype()), 0, st(ctx)));
+    Tensor scale = col;
+    if (!scale_col_major) {
+        scale = ctx.tensor({aligned_m, n / 128}, DataType::kFloat);
+        ZL_THROW_IF(zl_transpose_2d(col.data(), scale.mutable_data(), (int)(n / 128), (int)aligned_m, 4, st(ctx)));
+    }
+    out.set_quant_scale(scale);
+    return out;
+}
+
 }  // namespace nn::fp8
+
+// DeepGEMM's entry point (3rd/deep_gemm/deep_gemm_api.h), called by Fp8Block::forward (linear.cpp:1880-1945) with
+// lhs = per_token_cast_to_fp8's codes and column-major scales (leading dimension round_up(m, 4)), rhs = the (n, k) e4m3
+// weight with (ceil(n/128), k/128) f32 weight_scale_inv, bf16 out.  Plain GEMMs (num_groups == 1) run on
+// zl_fp8_block_gemm; the grouped (MoE) form returns -1, which the caller reports as an unsupported shape.
+extern "C" int deep_gemm_fp8_block_h20_group(void* lhs, void* lhs_scales, void* rhs, void* rhs_scales, void* out,
+                                             void* grouped_layout, void* stream, int m, int n, int k, int block_m,
+                                             int num_groups) {
+    (void)block_m;
+    if (num_groups != 1 || grouped_layout != nullptr) return -1;
+    const int rc = zl_fp8_block_gemm(lhs, static_cast<const float*>(lhs_scales), (m + 3) / 4 * 4, rhs,
+                                     static_cast<const float*>(rhs_scales), out, m, n, k, ZL_BF16, 0,
+                                     static_cast<zl_stream_t>(stream));
+    return rc == ZL_OK ? 0 : -1;
+}

@@ -51,11 +51,13 @@ struct DenseLin {
     dev_ptr<> w;
     dev_ptr<> bias;
     int N = 0, K = 0;
-    // W8A8 (quant_type 2 / 7): 8-bit weights (N, K) + per-row scales; w is released
+    // W8A8 (quant_type 2 / 7 / 10): 8-bit weights (N, K) + scales; w is released
     dev_ptr<> w8;
-    dev_ptr<> w_scale;   // int8: (N) in the activation dtype (linear.cpp:541); fp8: (N) f32 rows
-    int w8_kind = -1;    // ZL_W8_INT8 or ZL_W8_FP8_ROWS
+    dev_ptr<> w_scale;   // int8: (N) in the activation dtype (linear.cpp:541); fp8: (N) f32 rows;
+                         // fp8 block: (N/128, K/128) f32 weight_scale_inv
+    int w8_kind = -1;    // ZL_W8_INT8, ZL_W8_FP8_ROWS or kW8Block
 };
+constexpr int kW8Block = 10;   // QuantType 10 (Fp8Block): served by zl_fp8_block_gemm, not a zl_w8a8_gemm kind
 
 struct Layer {
     dev_ptr<> ln_attn;
@@ -123,7 +125,7 @@ struct zl_llama {
     cudaEvent_t ev_o[2] = {nullptr, nullptr}, ev_r1[2] = {nullptr, nullptr}, ev_dn[2] = {nullptr, nullptr},
                 ev_r2[2] = {nullptr, nullptr};
     dev_ptr<> xq;              // W8A8: quantised activations of the Linear being run (tok_cap x max K bytes)
-    dev_ptr<float> xs;         //       their scales (tok_cap)
+    dev_ptr<float> xs;         //       their scales (tok_cap; fp8 block: (max K/128, round_up(tok_cap, 4)))
     dev_ptr<int32_t> d_tb;     // token -> task map of the chunk being prefilled
     const int32_t* cur_tb = nullptr;   // token -> task map of the launch sequence being enqueued (d_iota at decode)
     dev_ptr<int8_t> d_mask;    // (chunk, max_seq) causal mask of the chunk
@@ -226,6 +228,11 @@ __global__ void k_and_u32(uint32_t* __restrict__ p, size_t n, uint32_t mask) {
     if (i < n) p[i] &= mask;
 }
 __global__ void k_set_f32(float* p, float v) { *p = v; }
+// in place: random u32 words -> f32 lo * (hi/lo)^u with u uniform in [0, 1)
+__global__ void k_u32_to_log_uniform(uint32_t* __restrict__ p, int n, float lo, float hi) {
+    const int i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i < n) p[i] = __float_as_uint(lo * powf(hi / lo, (float)(p[i] >> 8) * (1.f / 16777216.f)));
+}
 // synthetic symmetric checkpoints: a uniformly random nibble minus the fixed zero point 8 has mean -0.5, and with thousands
 // of such weights per row every layer adds a common-mode offset to the residual stream that overflows fp16 after ~30
 // layers (measured: NaN logits on the 32-layer model).  Nibble 0 -> 8 makes q - 8 symmetric around zero (-7 .. 7).
@@ -580,6 +587,56 @@ int build_fp8(zl_llama* m, const std::vector<std::string>& prefixes, const std::
     return ZL_OK;
 }
 
+// quant_type 10 (Fp8Block, linear.cpp:1697-1960): e4m3 weights + weight_scale_inv with one f32 per 128x128 block.
+// Projections that share an input are fused along N by concatenating both their weight rows and their scale rows,
+// which needs every part's N to be a multiple of 128.  Fp8Block has no bias (set_has_bias throws).
+int build_fp8_block(zl_llama* m, const std::vector<std::string>& prefixes, const std::vector<int>& ns, int K,
+                    DenseLin* out) {
+    int N = 0;
+    for (int n : ns) N += n;
+    if (K % 128 != 0 || (prefixes.size() > 1 && N % 128 != 0))
+        return fail_state(__LINE__, "fp8 block weights need K % 128 == 0 and every fused part's N % 128 == 0",
+                          ZL_ERR_UNSUPPORTED);
+    for (size_t i = 0; i < prefixes.size(); ++i) {
+        if (prefixes.size() > 1 && ns[i] % 128 != 0)
+            return fail_state(__LINE__, "fp8 block weights: fused part " + prefixes[i] + " has N % 128 != 0",
+                              ZL_ERR_UNSUPPORTED);
+        if (find(m, prefixes[i] + ".bias"))
+            return fail_state(__LINE__, "fp8 block Linear " + prefixes[i] + " has a bias (Fp8Block has none)",
+                              ZL_ERR_UNSUPPORTED);
+    }
+    const int KB = K / 128, NB = (N + 127) / 128;
+    RCHECK(dmalloc(&out->w8, (size_t)N * K));
+    RCHECK(dmalloc(&out->w_scale, (size_t)NB * KB * 4));
+    int off = 0;
+    for (size_t i = 0; i < prefixes.size(); ++i) {
+        const Staged* w = find(m, prefixes[i] + ".weight");
+        const Staged* ws = find(m, prefixes[i] + ".weight_scale_inv");
+        const int nb = (ns[i] + 127) / 128;
+        if (!w || w->rows != ns[i] || w->cols != K || w->elem != 1 || !ws || ws->elem != 4 || ws->rows != nb ||
+            ws->cols != KB) {
+            zl_set_last_error(__FILE__, __LINE__,
+                              ("missing/ill-shaped fp8 block weight or weight_scale_inv " + prefixes[i]).c_str());
+            return ZL_ERR_STATE;
+        }
+        ZL_CHECK_CUDA(cudaMemcpyAsync((char*)out->w8.get() + (size_t)off * K, w->ptr.get(), (size_t)ns[i] * K,
+                                      cudaMemcpyDeviceToDevice, m->stream));
+        ZL_CHECK_CUDA(cudaMemcpyAsync((char*)out->w_scale.get() + (size_t)(off / 128) * KB * 4, ws->ptr.get(),
+                                      (size_t)nb * KB * 4, cudaMemcpyDeviceToDevice, m->stream));
+        off += ns[i];
+    }
+    ZL_CHECK_CUDA(cudaStreamSynchronize(m->stream));
+    for (auto& p : prefixes) {
+        drop(m, p + ".weight");
+        drop(m, p + ".weight_scale_inv");
+    }
+    out->N = N;
+    out->K = K;
+    out->w8_kind = kW8Block;
+    m->weight_bytes += (double)N * K + (double)NB * KB * 4;
+    return ZL_OK;
+}
+
 int take_vector(zl_llama* m, const std::string& name, int n, dev_ptr<>* out) {
     auto it = m->staged.find(name);
     if (it == m->staged.end() || (size_t)it->second.rows * it->second.cols != (size_t)n || it->second.elem != 2) {
@@ -617,6 +674,11 @@ int finalize_layer(zl_llama* m, int l) {
         RCHECK(build_fp8(m, {p + "attn.attn_out"}, {D}, m->hq * d, &L.d_o));
         RCHECK(build_fp8(m, gu, gu_n, D, &L.d_gu));
         RCHECK(build_fp8(m, {p + "ff.w_out"}, {D}, m->ff, &L.d_down));
+    } else if (c.quant_type == 10) {
+        RCHECK(build_fp8_block(m, qkv, qkv_n, D, &L.d_qkv));
+        RCHECK(build_fp8_block(m, {p + "attn.attn_out"}, {D}, m->hq * d, &L.d_o));
+        RCHECK(build_fp8_block(m, gu, gu_n, D, &L.d_gu));
+        RCHECK(build_fp8_block(m, {p + "ff.w_out"}, {D}, m->ff, &L.d_down));
     } else {
         RCHECK(build_dense(m, qkv, qkv_n, D, &L.d_qkv));
         RCHECK(build_dense(m, {p + "attn.attn_out"}, {D}, m->hq * d, &L.d_o));
@@ -705,11 +767,12 @@ int alloc_runtime(zl_llama* m) {
     RCHECK(dmalloc(&m->d_tokens, B * 4));
     RCHECK(dmalloc(&m->d_pos, B * 4));
     RCHECK(dmalloc(&m->d_lens, B * 4));
-    if (c.quant_type == 2 || c.quant_type == 7) {
+    if (c.quant_type == 2 || c.quant_type == 7 || c.quant_type == 10) {
         int kmax = D > m->ff ? D : m->ff;
         kmax = kmax > m->hq * d ? kmax : m->hq * d;
         RCHECK(dmalloc(&m->xq, (size_t)T * kmax));
-        RCHECK(dmalloc(&m->xs, (size_t)T * 4));
+        // fp8 block: one scale per (token, 128 columns), column-major with leading dimension round_up(tokens, 4)
+        RCHECK(dmalloc(&m->xs, c.quant_type == 10 ? (size_t)(kmax / 128 + 1) * ((T + 3) / 4 * 4) * 4 : (size_t)T * 4));
     }
     if (c.prefill_chunk > 0) {
         RCHECK(dmalloc(&m->d_tb, T * 4));
@@ -1059,6 +1122,12 @@ int dense_or_w8(zl_llama* m, const void* x, const DenseLin& L, void* y, int B, i
         return zl_w8a8_gemm(m->xq.get(), m->xs.get(), L.w8.get(), L.w_scale.get(), c.dtype, L.bias.get(), y, B, L.N, L.K,
                             ZL_W8_INT8, c.dtype, pdl, st);
     }
+    if (L.w8_kind == kW8Block) {   // Fp8Block::forward: per_token_cast_to_fp8 + the block-scaled GEMM
+        const int ld = (B + 3) / 4 * 4;
+        RCHECK(zl_fp8_quant_per_token_group(x, L.K, m->xq.get(), m->xs.get(), ld, B, L.K, c.dtype, pdl, st));
+        return zl_fp8_block_gemm(m->xq.get(), m->xs.get(), ld, L.w8.get(), static_cast<const float*>(L.w_scale.get()), y,
+                                 B, L.N, L.K, c.dtype, pdl, st);
+    }
     RCHECK(zl_fp8_quant_per_tensor(x, m->xq.get(), m->xs.get(), (size_t)B * L.K, c.dtype, pdl, st));
     return zl_w8a8_gemm(m->xq.get(), m->xs.get(), L.w8.get(), L.w_scale.get(), ZL_F32, L.bias.get(), y, B, L.N, L.K,
                         ZL_W8_FP8_ROWS, c.dtype, pdl, st);
@@ -1369,7 +1438,13 @@ extern "C" int zl_llama_create(const zl_llama_config_t* cfg, zl_llama_t** out) {
     }
     cfg = &norm_cfg;
     ZL_CHECK_SUPPORTED(cfg->quant_type == 0 || cfg->quant_type == 2 || cfg->quant_type == 5 || cfg->quant_type == 6 ||
-                       cfg->quant_type == 7);
+                       cfg->quant_type == 7 || cfg->quant_type == 10);
+    // Fp8Block (QuantType 10): single rank, no bias (Fp8Block::set_has_bias throws)
+    ZL_CHECK_SUPPORTED(cfg->quant_type != 10 || (cfg->tp_size == 1 && !cfg->qkv_bias));
+    // ... and 128-wide scale blocks: every K is a multiple of 128, and so is every part of the fused q/k/v and gate/up
+    ZL_CHECK_SUPPORTED(cfg->quant_type != 10 ||
+                       (cfg->dim_model % 128 == 0 && (cfg->num_heads * cfg->dim_head) % 128 == 0 &&
+                        (cfg->num_kv_heads * cfg->dim_head) % 128 == 0 && cfg->dim_ff % 128 == 0));
     ZL_CHECK_SUPPORTED(!(cfg->quant_type == 5 || cfg->quant_type == 6) || cfg->dtype == ZL_F16);
     ZL_CHECK_SUPPORTED(!(cfg->quant_type == 2 || cfg->quant_type == 7) || cfg->tp_size == 1);   // "A must be half" q_gemm_k_major.cu:989
     ZL_CHECK_SUPPORTED(cfg->dtype == ZL_F16 || cfg->dtype == ZL_BF16);
@@ -1511,6 +1586,22 @@ int stage_random_linear(zl_llama* m, const std::string& prefix, int K, int N, ui
         k_set_f32<<<1, 1, 0, m->stream>>>(static_cast<float*>(sc.ptr.get()), 0.03f);
         ZL_CHECK_LAUNCH();
         m->staged[prefix + ".weight_scale"] = std::move(sc);
+    } else if (c.quant_type == 10) {
+        // e4m3 codes as for type 7, and one f32 scale per 128x128 block drawn log-uniformly over 0.0075 .. 0.12 (16x)
+        // so that a scale applied to the wrong block shows
+        RCHECK(stage_random(m, prefix + ".weight", N, K / 4, 4, 0, 0, 0, seed));
+        Staged& w = m->staged[prefix + ".weight"];
+        const size_t words = (size_t)N * K / 4;
+        k_and_u32<<<(unsigned)((words + 255) / 256), 256, 0, m->stream>>>(static_cast<uint32_t*>(w.ptr.get()), words, 0xBFBFBFBFu);
+        ZL_CHECK_LAUNCH();
+        w.cols = K;
+        w.elem = 1;
+        const int nb = (N + 127) / 128, kb = K / 128;
+        RCHECK(stage_random(m, prefix + ".weight_scale_inv", nb, kb, 4, 0, 0, 0, seed));
+        Staged& sc = m->staged[prefix + ".weight_scale_inv"];
+        k_u32_to_log_uniform<<<cdiv(nb * kb, 256), 256, 0, m->stream>>>(static_cast<uint32_t*>(sc.ptr.get()), nb * kb,
+                                                                        0.0075f, 0.12f);
+        ZL_CHECK_LAUNCH();
     } else {
         RCHECK(stage_random(m, prefix + ".weight", N, K, 2, 2, -0.035f, 0.035f, seed));   // ~ randn*0.02
     }

@@ -13,6 +13,10 @@
 // weight row g (and g+8) per 64-k step and the activation fragment uses the same k permutation -- every global
 // load is a full 16-byte vector, no shared-memory staging of the weights at all.
 // Small N is covered by splitting K across the warps of a CTA (int32 partial sums add exactly).
+//
+// Block-scaled FP8 (BLK, QuantType 10 / Fp8Block, linear.cpp:1697-1960): each warp's K range is whole 128-k blocks,
+// the 64-k steps of one block are steps 2 kb and 2 kb + 1 (the lane permutation stays inside a step), and after
+// every block the QMMA sum is folded into an fp32 sum times sx[kb, token] * sw[row / 128, kb].
 #include "common.cuh"
 
 #include <cstdlib>
@@ -22,7 +26,7 @@ namespace zl {
 bool w8_tc_supports(int N, int K);
 template <typename T, bool FP8>
 cudaError_t launch_w8_tc(const uint8_t* xq, const float* sx, const uint8_t* w, const void* sw, int sw_mode, const T* bias, T* y,
-                         int mc, int N, int K, bool pdl, cudaStream_t stream);
+                         int mc, int N, int K, bool pdl, cudaStream_t stream, int sx_ld = 0);
 }  // namespace zl
 
 #include <cuda_fp8.h>
@@ -185,6 +189,43 @@ k_fp8_quant_per_tensor(const T* __restrict__ x, uint8_t* __restrict__ q, float* 
     }
 }
 
+// nn::fp8::per_token_cast_to_fp8 (fp8_util.cu:231-322): one warp per (token, 128-column group), 4 values per lane;
+// amax clamped to 1e-4, q = e4m3(x * (448/amax)) with the fp32 product, scale = amax/448 stored column-major
+// (K/128, scale_ld).  Each warp of a 256-thread CTA takes one group.
+template <typename T>
+__global__ void __launch_bounds__(256)
+k_fp8_quant_per_token_group(const T* __restrict__ x, int ldx, uint8_t* __restrict__ q, float* __restrict__ scale,
+                            int scale_ld, int M, int K) {
+    pdl_trigger();
+    pdl_wait();
+    const int groups = K >> 7;
+    const long long gi = (long long)blockIdx.x * 8 + (threadIdx.x >> 5);
+    if (gi >= (long long)M * groups) return;
+    const int lane = threadIdx.x & 31;
+    const int m = (int)(gi / groups), kb = (int)(gi % groups);
+    const T* src = x + (size_t)m * ldx + kb * 128 + lane * 4;
+    const uint2 raw = __ldcg(reinterpret_cast<const uint2*>(src));
+    const T* h = reinterpret_cast<const T*>(&raw);
+    float v[4];
+    float amax = 0.f;
+#pragma unroll
+    for (int i = 0; i < 4; ++i) {
+        v[i] = to_f32<T>(h[i]);
+        amax = fmaxf(amax, fabsf(v[i]));
+    }
+    amax = warp_max(amax);
+    if (amax < 1e-4f) amax = 1e-4f;
+    const float mul = __fdiv_rn(448.f, amax);
+    uint32_t word = 0;
+#pragma unroll
+    for (int i = 0; i < 4; ++i) {
+        const __nv_fp8_storage_t c = __nv_cvt_float_to_fp8(__fmul_rn(v[i], mul), __NV_SATFINITE, __NV_E4M3);
+        word |= (uint32_t)c << (8 * i);
+    }
+    *reinterpret_cast<uint32_t*>(q + (size_t)m * K + kb * 128 + lane * 4) = word;
+    if (lane == 0) scale[(size_t)kb * scale_ld + m] = __fdiv_rn(amax, 448.f);
+}
+
 // quant_scale_back (quant_kernel.cu:231-246) for callers that still hold an int32 accumulator
 template <typename T>
 __global__ void k_int8_scale_back(const int32_t* __restrict__ acc, const float* __restrict__ sx, const void* __restrict__ sw,
@@ -199,11 +240,12 @@ __global__ void k_int8_scale_back(const int32_t* __restrict__ acc, const float* 
 // GEMM: y(M,N) = scale-back( xq(M,K) . wq(N,K)^T )
 // ---------------------------------------------------------------------------------------------
 // One CTA = kW8Warps warps = (kW8Warps / KS) row tiles of 16 weight rows, each split KS ways along K.
-template <typename T, bool FP8, int NT, int KS>
+template <typename T, bool FP8, int NT, int KS, bool BLK>
 __global__ void __launch_bounds__(kW8Warps * 32)
 k_w8a8_skinny(const uint8_t* __restrict__ xq, const float* __restrict__ sx, const uint8_t* __restrict__ w,
               const void* __restrict__ sw, int sw_f32, const T* __restrict__ bias, T* __restrict__ y, int mc, int N,
-              int K) {
+              int K, int sx_ld) {
+    static_assert(FP8 || !BLK, "block scales are fp8 only");
     using Acc = typename W8Acc<FP8>::type;
     constexpr int TPC = kW8Warps / KS;   // tiles per CTA
     __shared__ Acc red[KS > 1 ? kW8Warps : 1][NT][4][32];
@@ -216,7 +258,9 @@ k_w8a8_skinny(const uint8_t* __restrict__ xq, const float* __restrict__ sx, cons
     pdl_trigger();
 
     const int steps = K / 64;
-    const int s_lo = (int)((long long)steps * ks / KS), s_hi = (int)((long long)steps * (ks + 1) / KS);
+    // BLK: split by whole 128-k blocks, so s_lo is even and step s0 + u belongs to block (s0 + u) / 2 with parity u
+    const int s_lo = BLK ? 2 * (int)((long long)(steps / 2) * ks / KS) : (int)((long long)steps * ks / KS);
+    const int s_hi = BLK ? 2 * (int)((long long)(steps / 2) * (ks + 1) / KS) : (int)((long long)steps * (ks + 1) / KS);
     const int ra = min(row0 + g, N - 1), rb = min(row0 + g + 8, N - 1);
     const uint8_t* wa = w + (size_t)ra * K + t * 16;
     const uint8_t* wb = w + (size_t)rb * K + t * 16;
@@ -233,10 +277,17 @@ k_w8a8_skinny(const uint8_t* __restrict__ xq, const float* __restrict__ sx, cons
     pdl_wait();
 
     Acc acc[NT][4];
+    float accb[BLK ? NT : 1][4];
 #pragma unroll
     for (int nt = 0; nt < NT; ++nt)
 #pragma unroll
         for (int c = 0; c < 4; ++c) acc[nt][c] = 0;
+    if constexpr (BLK) {
+#pragma unroll
+        for (int nt = 0; nt < NT; ++nt)
+#pragma unroll
+            for (int c = 0; c < 4; ++c) accb[nt][c] = 0.f;
+    }
 
     if (live) {
         for (int s0 = s_lo; s0 < s_hi; s0 += kW8Unroll) {
@@ -276,8 +327,31 @@ k_w8a8_skinny(const uint8_t* __restrict__ xq, const float* __restrict__ sx, cons
                         }
                     }
                 }
+                if constexpr (BLK) {
+                    if ((u & 1) && s0 + u < s_hi) {   // end of block kb: rows row0 .. row0 + 15 share one weight scale
+                        const int kb = (s0 + u) >> 1;
+                        const float s_w = static_cast<const float*>(sw)[(size_t)(row0 >> 7) * (K >> 7) + kb];
+#pragma unroll
+                        for (int nt = 0; nt < NT; ++nt)
+#pragma unroll
+                            for (int e = 0; e < 2; ++e) {
+                                const int tok = nt * 8 + 2 * t + e;
+                                const float s = tok < mc ? __ldg(sx + (size_t)kb * sx_ld + tok) * s_w : 0.f;
+                                accb[nt][e] = fmaf(acc[nt][e], s, accb[nt][e]);
+                                accb[nt][e + 2] = fmaf(acc[nt][e + 2], s, accb[nt][e + 2]);
+                                acc[nt][e] = 0.f;
+                                acc[nt][e + 2] = 0.f;
+                            }
+                    }
+                }
             }
         }
+    }
+    if constexpr (BLK) {
+#pragma unroll
+        for (int nt = 0; nt < NT; ++nt)
+#pragma unroll
+            for (int c = 0; c < 4; ++c) acc[nt][c] = accb[nt][c];
     }
 
     if constexpr (KS > 1) {
@@ -307,7 +381,9 @@ k_w8a8_skinny(const uint8_t* __restrict__ xq, const float* __restrict__ sx, cons
             const int row = row0 + g + ((c >> 1) ? 8 : 0);
             if (tok < mc && row < N) {
                 float v;
-                if constexpr (FP8) {
+                if constexpr (BLK) {
+                    v = acc[nt][c];   // scaled block by block above; Fp8Block has no bias
+                } else if constexpr (FP8) {
                     // cuBLASLt fp8: D = (scaleA * scaleB) * acc (+ bias), functions::Gemm with A/B scales
                     // sw_f32 == 2: one scale per output row (several per-tensor-scaled projections fused along N)
                     const float s_w = sw_f32 == 2 ? static_cast<const float*>(sw)[row] : *static_cast<const float*>(sw);
@@ -325,9 +401,9 @@ k_w8a8_skinny(const uint8_t* __restrict__ xq, const float* __restrict__ sx, cons
     }
 }
 
-template <typename T, bool FP8, int NT>
+template <typename T, bool FP8, int NT, bool BLK>
 static cudaError_t launch_w8_ks(const uint8_t* xq, const float* sx, const uint8_t* w, const void* sw, int sw_f32,
-                                const T* bias, T* y, int mc, int N, int K, bool pdl, cudaStream_t st) {
+                                const T* bias, T* y, int mc, int N, int K, bool pdl, cudaStream_t st, int sx_ld) {
     const int tiles = cdiv(N, 16);
     // enough warps to keep ~13 MB of loads in flight chip-wide: aim for >= 16 warps per SM
     int dev = 0, sms = 132;
@@ -336,10 +412,12 @@ static cudaError_t launch_w8_ks(const uint8_t* xq, const float* sx, const uint8_
     const int steps = K / 64;
     int ks = 1;
     while (ks < kW8Warps && tiles * ks < sms * 16 && steps / (ks * 2) >= kW8Unroll) ks *= 2;
+    if (BLK)   // every warp needs at least one whole 128-k block
+        while (ks > 1 && (steps / 2) < ks) ks /= 2;
     dim3 block(kW8Warps * 32);
 #define ZL_W8_LAUNCH(KS_)                                                                                          \
-    return launch(k_w8a8_skinny<T, FP8, NT, KS_>, dim3(cdiv(tiles, kW8Warps / KS_)), block, 0, st, pdl, xq, sx, w, \
-                  sw, sw_f32, bias, y, mc, N, K)
+    return launch(k_w8a8_skinny<T, FP8, NT, KS_, BLK>, dim3(cdiv(tiles, kW8Warps / KS_)), block, 0, st, pdl, xq, sx, \
+                  w, sw, sw_f32, bias, y, mc, N, K, sx_ld)
     if (ks == 1) ZL_W8_LAUNCH(1);
     if (ks == 2) ZL_W8_LAUNCH(2);
     if (ks == 4) ZL_W8_LAUNCH(4);
@@ -347,12 +425,42 @@ static cudaError_t launch_w8_ks(const uint8_t* xq, const float* sx, const uint8_
 #undef ZL_W8_LAUNCH
 }
 
-template <typename T, bool FP8>
+template <typename T, bool FP8, bool BLK = false>
 static cudaError_t launch_w8(const uint8_t* xq, const float* sx, const uint8_t* w, const void* sw, int sw_f32,
-                             const T* bias, T* y, int mc, int N, int K, bool pdl, cudaStream_t st) {
-    if (mc <= 8) return launch_w8_ks<T, FP8, 1>(xq, sx, w, sw, sw_f32, bias, y, mc, N, K, pdl, st);
-    if (mc <= 16) return launch_w8_ks<T, FP8, 2>(xq, sx, w, sw, sw_f32, bias, y, mc, N, K, pdl, st);
-    return launch_w8_ks<T, FP8, 4>(xq, sx, w, sw, sw_f32, bias, y, mc, N, K, pdl, st);
+                             const T* bias, T* y, int mc, int N, int K, bool pdl, cudaStream_t st, int sx_ld = 0) {
+    if (mc <= 8) return launch_w8_ks<T, FP8, 1, BLK>(xq, sx, w, sw, sw_f32, bias, y, mc, N, K, pdl, st, sx_ld);
+    if (mc <= 16) return launch_w8_ks<T, FP8, 2, BLK>(xq, sx, w, sw, sw_f32, bias, y, mc, N, K, pdl, st, sx_ld);
+    return launch_w8_ks<T, FP8, 4, BLK>(xq, sx, w, sw, sw_f32, bias, y, mc, N, K, pdl, st, sx_ld);
+}
+
+// Routing shared by zl_w8a8_gemm and zl_fp8_block_gemm.  With the reference's row-major (N, K) layout every 128-byte row
+// segment of a TMA box comes from a different DRAM page, so at decode sizes the mma.sync kernel's 16-byte row-contiguous
+// loads are used; the wgmma kernel takes over where the mma.sync kernel would re-stream the weights (M > 32: prefill
+// chunks).  The crossover was not measured on H100.  tc(m0, mc, pdl) runs rows m0 .. m0 + mc - 1 (mc <= 256) on the
+// wgmma kernel, skinny(m0, mc, pdl) on the mma.sync kernel (mc <= 32); only the first launch is PDL-launched.
+template <typename TcFn, typename SkinnyFn>
+static int w8_route(int M, int N, int K, int pdl, TcFn tc, SkinnyFn skinny) {
+    static const int tc_min_m = getenv("ZL_W8_TC_MIN_M") ? atoi(getenv("ZL_W8_TC_MIN_M")) : 33;
+    if (M >= tc_min_m && w8_tc_supports(N, K)) {
+        static bool prepared[64] = {};   // zl_prepare() once per device: split-k workspace, opt-in shared memory
+        int dev = 0;
+        cudaGetDevice(&dev);
+        if (dev < 0 || dev >= 64 || !prepared[dev]) {
+            int rc = zl_prepare();
+            if (rc != ZL_OK) return rc;
+            if (dev >= 0 && dev < 64) prepared[dev] = true;
+        }
+        for (int m0 = 0; m0 < M; m0 += 256) {
+            const int mc = (M - m0) < 256 ? (M - m0) : 256;
+            ZL_CHECK_CUDA(tc(m0, mc, pdl != 0 && m0 == 0));
+        }
+        return ZL_OK;
+    }
+    for (int m0 = 0; m0 < M; m0 += 32) {
+        const int mc = (M - m0) < 32 ? (M - m0) : 32;
+        ZL_CHECK_CUDA(skinny(m0, mc, pdl != 0 && m0 == 0));
+    }
+    return ZL_OK;
 }
 
 }  // namespace zl
@@ -442,61 +550,81 @@ extern "C" int zl_w8a8_gemm(const void* xq, const float* x_scale, const void* w,
     const uint8_t* xq8 = static_cast<const uint8_t*>(xq);
     const uint8_t* w8 = static_cast<const uint8_t*>(w);
     const int sw_f32 = kind == ZL_W8_FP8_ROWS ? 2 : (w_scale_dtype == ZL_F32 ? 1 : 0);
-    // with the reference's row-major (N, K) layout every 128-byte row segment of a TMA box comes from a different DRAM page,
-    // so at decode sizes the mma.sync kernel's 16-byte row-contiguous loads are used; the wgmma kernel takes over where the
-    // mma.sync kernel would re-stream the weights (M > 32: prefill chunks).  The crossover was not measured on H100.
-    static const int tc_min_m = getenv("ZL_W8_TC_MIN_M") ? atoi(getenv("ZL_W8_TC_MIN_M")) : 33;
-    if (M >= tc_min_m && w8_tc_supports(N, K)) {
+    const bool fp8 = kind != ZL_W8_INT8;
+    const int sw_mode = fp8 ? (kind == ZL_W8_FP8_ROWS ? 2 : 3) : sw_f32;
+    auto tc = [&](int m0, int mc, bool p) -> cudaError_t {
         // wgmma path (w8_tc.cu): both operands through the TMA engine, s32 / f32 register accumulators
-        {
-            static bool prepared[64] = {};
-            int dev = 0;
-            cudaGetDevice(&dev);
-            if (dev < 0 || dev >= 64 || !prepared[dev]) {
-                int rc = zl_prepare();
-                if (rc != ZL_OK) return rc;
-                if (dev >= 0 && dev < 64) prepared[dev] = true;
-            }
-        }
-        const bool fp8 = kind != ZL_W8_INT8;
-        const int sw_mode = fp8 ? (kind == ZL_W8_FP8_ROWS ? 2 : 3) : sw_f32;
-        for (int m0 = 0; m0 < M; m0 += 256) {
-            const int mc = (M - m0) < 256 ? (M - m0) : 256;
-            const bool p = pdl != 0 && m0 == 0;
-            const float* sx = kind == ZL_W8_INT8 ? x_scale + m0 : x_scale;
-            cudaError_t e;
-            if (dtype == ZL_F16) {
-                const __half* b = static_cast<const __half*>(bias);
-                __half* yo = static_cast<__half*>(y) + (size_t)m0 * N;
-                e = fp8 ? launch_w8_tc<__half, true>(xq8 + (size_t)m0 * K, sx, w8, w_scale, sw_mode, b, yo, mc, N, K, p, stream)
-                        : launch_w8_tc<__half, false>(xq8 + (size_t)m0 * K, sx, w8, w_scale, sw_mode, b, yo, mc, N, K, p, stream);
-            } else {
-                const __nv_bfloat16* b = static_cast<const __nv_bfloat16*>(bias);
-                __nv_bfloat16* yo = static_cast<__nv_bfloat16*>(y) + (size_t)m0 * N;
-                e = fp8 ? launch_w8_tc<__nv_bfloat16, true>(xq8 + (size_t)m0 * K, sx, w8, w_scale, sw_mode, b, yo, mc, N, K, p, stream)
-                        : launch_w8_tc<__nv_bfloat16, false>(xq8 + (size_t)m0 * K, sx, w8, w_scale, sw_mode, b, yo, mc, N, K, p, stream);
-            }
-            ZL_CHECK_CUDA(e);
-        }
-        return ZL_OK;
-    }
-    for (int m0 = 0; m0 < M; m0 += 32) {
-        const int mc = (M - m0) < 32 ? (M - m0) : 32;
-        const bool p = pdl != 0 && m0 == 0;
         const float* sx = kind == ZL_W8_INT8 ? x_scale + m0 : x_scale;
-        cudaError_t e;
-#define ZL_W8_GO(TT, F8)                                                                                           \
-    e = launch_w8<TT, F8>(xq8 + (size_t)m0 * K, sx, w8, w_scale, sw_f32, static_cast<const TT*>(bias),              \
-                          static_cast<TT*>(y) + (size_t)m0 * N, mc, N, K, p, stream)
         if (dtype == ZL_F16) {
-            if (kind != ZL_W8_INT8) ZL_W8_GO(__half, true);
-            else ZL_W8_GO(__half, false);
-        } else {
-            if (kind != ZL_W8_INT8) ZL_W8_GO(__nv_bfloat16, true);
-            else ZL_W8_GO(__nv_bfloat16, false);
+            const __half* b = static_cast<const __half*>(bias);
+            __half* yo = static_cast<__half*>(y) + (size_t)m0 * N;
+            return fp8 ? launch_w8_tc<__half, true>(xq8 + (size_t)m0 * K, sx, w8, w_scale, sw_mode, b, yo, mc, N, K, p, stream)
+                       : launch_w8_tc<__half, false>(xq8 + (size_t)m0 * K, sx, w8, w_scale, sw_mode, b, yo, mc, N, K, p, stream);
         }
+        const __nv_bfloat16* b = static_cast<const __nv_bfloat16*>(bias);
+        __nv_bfloat16* yo = static_cast<__nv_bfloat16*>(y) + (size_t)m0 * N;
+        return fp8 ? launch_w8_tc<__nv_bfloat16, true>(xq8 + (size_t)m0 * K, sx, w8, w_scale, sw_mode, b, yo, mc, N, K, p, stream)
+                   : launch_w8_tc<__nv_bfloat16, false>(xq8 + (size_t)m0 * K, sx, w8, w_scale, sw_mode, b, yo, mc, N, K, p, stream);
+    };
+    auto skinny = [&](int m0, int mc, bool p) -> cudaError_t {
+        const float* sx = kind == ZL_W8_INT8 ? x_scale + m0 : x_scale;
+#define ZL_W8_GO(TT, F8)                                                                                           \
+    return launch_w8<TT, F8>(xq8 + (size_t)m0 * K, sx, w8, w_scale, sw_f32, static_cast<const TT*>(bias),           \
+                             static_cast<TT*>(y) + (size_t)m0 * N, mc, N, K, p, stream)
+        if (dtype == ZL_F16) {
+            if (fp8) ZL_W8_GO(__half, true);
+            ZL_W8_GO(__half, false);
+        }
+        if (fp8) ZL_W8_GO(__nv_bfloat16, true);
+        ZL_W8_GO(__nv_bfloat16, false);
 #undef ZL_W8_GO
-        ZL_CHECK_CUDA(e);
-    }
+    };
+    return w8_route(M, N, K, pdl, tc, skinny);
+}
+
+extern "C" int zl_fp8_quant_per_token_group(const void* x, int ldx, void* q, float* scale, int scale_ld, int M, int K,
+                                            int dtype, int pdl, zl_stream_t stream) {
+    ZL_CHECK_ARG(x && q && scale && M > 0 && K > 0 && ldx >= K && scale_ld >= M);
+    ZL_CHECK_ARG(dtype == ZL_F16 || dtype == ZL_BF16);
+    ZL_CHECK_SUPPORTED(K % 128 == 0 && ldx % 4 == 0);
+    ZL_CHECK_ARG((reinterpret_cast<uintptr_t>(x) & 7) == 0 && (reinterpret_cast<uintptr_t>(q) & 3) == 0);
+    const long long groups = (long long)M * (K / 128);
+    const dim3 grid((unsigned)((groups + 7) / 8));
+    cudaError_t e;
+    if (dtype == ZL_F16)
+        e = launch(k_fp8_quant_per_token_group<__half>, grid, dim3(256), 0, stream, pdl != 0, static_cast<const __half*>(x),
+                   ldx, static_cast<uint8_t*>(q), scale, scale_ld, M, K);
+    else
+        e = launch(k_fp8_quant_per_token_group<__nv_bfloat16>, grid, dim3(256), 0, stream, pdl != 0,
+                   static_cast<const __nv_bfloat16*>(x), ldx, static_cast<uint8_t*>(q), scale, scale_ld, M, K);
+    ZL_CHECK_CUDA(e);
     return ZL_OK;
+}
+
+extern "C" int zl_fp8_block_gemm(const void* xq, const float* x_scale, int x_scale_ld, const void* w, const float* w_scale,
+                                 void* y, int M, int N, int K, int dtype, int pdl, zl_stream_t stream) {
+    ZL_CHECK_ARG(xq && x_scale && w && w_scale && y && M > 0 && N > 0 && K > 0 && x_scale_ld >= M);
+    ZL_CHECK_ARG(dtype == ZL_F16 || dtype == ZL_BF16);
+    ZL_CHECK_SUPPORTED(K % 128 == 0);
+    ZL_CHECK_ARG((reinterpret_cast<uintptr_t>(xq) & 15) == 0 && (reinterpret_cast<uintptr_t>(w) & 15) == 0);
+    const uint8_t* xq8 = static_cast<const uint8_t*>(xq);
+    const uint8_t* w8 = static_cast<const uint8_t*>(w);
+    // routed like zl_w8a8_gemm; a chunk's x_scale is x_scale + m0 with the same leading dimension
+    auto tc = [&](int m0, int mc, bool p) -> cudaError_t {
+        if (dtype == ZL_F16)
+            return launch_w8_tc<__half, true>(xq8 + (size_t)m0 * K, x_scale + m0, w8, w_scale, 4, nullptr,
+                                              static_cast<__half*>(y) + (size_t)m0 * N, mc, N, K, p, stream, x_scale_ld);
+        return launch_w8_tc<__nv_bfloat16, true>(xq8 + (size_t)m0 * K, x_scale + m0, w8, w_scale, 4, nullptr,
+                                                 static_cast<__nv_bfloat16*>(y) + (size_t)m0 * N, mc, N, K, p, stream,
+                                                 x_scale_ld);
+    };
+    auto skinny = [&](int m0, int mc, bool p) -> cudaError_t {
+        if (dtype == ZL_F16)
+            return launch_w8<__half, true, true>(xq8 + (size_t)m0 * K, x_scale + m0, w8, w_scale, 0, nullptr,
+                                                 static_cast<__half*>(y) + (size_t)m0 * N, mc, N, K, p, stream, x_scale_ld);
+        return launch_w8<__nv_bfloat16, true, true>(xq8 + (size_t)m0 * K, x_scale + m0, w8, w_scale, 0, nullptr,
+                                                    static_cast<__nv_bfloat16*>(y) + (size_t)m0 * N, mc, N, K, p, stream,
+                                                    x_scale_ld);
+    };
+    return w8_route(M, N, K, pdl, tc, skinny);
 }

@@ -11,6 +11,8 @@
 //   warps 0-7  consumers : two warpgroups, warpgroup r owns weight rows 64 r .. 64 r + 63 of the tile and all NTOK tokens:
 //                          4 x wgmma m64 x NTOK x 32 per stage, then scale-back (+bias), or split-k partials + last-CTA reduce
 //   warp 8     producer  : per 128-byte k-stage one weight box (128 rows x 128 B) + one activation box (NTOK x 128 B)
+// Block-scaled fp8 (BLK, QuantType 10): a 128-byte k-stage is one 128-wide scale block and a 128-row tile is one weight-scale
+// row, so each stage's accumulator is folded into the fp32 sum times sx[kb, token] * sw[tile, kb].
 // INT8 results are bit-identical to the reference's three-kernel path (s32 accumulation is exact in any order).
 #include "common.cuh"
 #include "tc_common.cuh"
@@ -40,9 +42,10 @@ struct W8TcCfg {
 struct alignas(64) W8TcParams {
     CUtensorMap wmap;          // w (N, K) 8-bit row-major, box {128 B, 128 rows}
     CUtensorMap xmap;          // xq (M, K) 8-bit row-major, box {128 B, NTOK rows}
-    const float* sx;           // int8: (M) per-token scales; fp8: one scale
-    const void* sw;            // int8: (N) f32 or T; fp8: one f32 or (N) f32 rows
-    int sw_mode;               // 0: T per row, 1: f32 per row, 2: f32 per row (fp8 rows), 3: one f32 (fp8)
+    const float* sx;           // int8: (M) per-token scales; fp8: one scale; block: (K/128, sx_ld) column-major
+    const void* sw;            // int8: (N) f32 or T; fp8: one f32 or (N) f32 rows; block: (ceil(N/128), K/128) f32
+    int sw_mode;               // 0: T per row, 1: f32 per row, 2: f32 per row (fp8 rows), 3: one f32 (fp8), 4: block
+    int sx_ld;
     const void* bias;
     void* y;
     int M, N, K, S;
@@ -52,9 +55,13 @@ struct alignas(64) W8TcParams {
 };
 
 // one output element: acc is the s32 sum (int8) or the f32 sum (fp8)
-template <typename T, bool FP8>
+template <typename T, bool FP8, bool BLK>
 __device__ __forceinline__ void w8_epilogue1(const W8TcParams& p, int row, int tok, float acc) {
     if (row >= p.N || tok >= p.M) return;
+    if constexpr (BLK) {   // the block scales were applied per k-stage; no bias (Fp8Block has none)
+        static_cast<T*>(p.y)[(size_t)tok * p.N + row] = from_f32<T>(acc);
+        return;
+    }
     const T* bias = static_cast<const T*>(p.bias);
     float s_w;
     if (p.sw_mode == 0) s_w = to_f32<T>(static_cast<const T*>(p.sw)[row]);
@@ -72,8 +79,9 @@ __device__ __forceinline__ void w8_epilogue1(const W8TcParams& p, int row, int t
     static_cast<T*>(p.y)[(size_t)tok * p.N + row] = from_f32<T>(r);
 }
 
-template <typename T, bool FP8, int NTOK>
+template <typename T, bool FP8, int NTOK, bool BLK>
 __global__ void __launch_bounds__(kW8TcThreads, 1) k_w8a8_tc(const __grid_constant__ W8TcParams p) {
+    static_assert(FP8 || !BLK, "block scales are fp8 only");
     using C = W8TcCfg<NTOK>;
     using Acc = typename std::conditional<FP8, float, int>::type;
     extern __shared__ uint8_t smem_dyn[];
@@ -155,10 +163,26 @@ __global__ void __launch_bounds__(kW8TcThreads, 1) k_w8a8_tc(const __grid_consta
                 else wg_s8_ss<NTOK>(acc, ad + (uint64_t)(k32 * 2), xd + (uint64_t)(k32 * 2), accum);
             }
             wg_commit();
-            wg_wait_all();
-            if constexpr (FP8) {
+            if constexpr (BLK) {
+                // one weight scale for the tile, one x scale per token; the weight scale loads while the wgmmas run
+                const float s_w = static_cast<const float*>(p.sw)[(size_t)tile * KS + ks];
+                const float* sxk = p.sx + (size_t)ks * p.sx_ld;
+                wg_wait_all();
 #pragma unroll
-                for (int i = 0; i < NTOK / 2; ++i) accf[i] += acc[i];
+                for (int j = 0; j < NTOK / 8; ++j)
+#pragma unroll
+                    for (int e = 0; e < 2; ++e) {
+                        const int tok = 8 * j + 2 * tig + e;
+                        const float sc = tok < p.M ? __ldg(sxk + tok) * s_w : 0.f;
+                        accf[4 * j + e] = fmaf(acc[4 * j + e], sc, accf[4 * j + e]);
+                        accf[4 * j + e + 2] = fmaf(acc[4 * j + e + 2], sc, accf[4 * j + e + 2]);
+                    }
+            } else {
+                wg_wait_all();
+                if constexpr (FP8) {
+#pragma unroll
+                    for (int i = 0; i < NTOK / 2; ++i) accf[i] += acc[i];
+                }
             }
             __syncwarp();
             if (lane == 0) mbar_arrive(&empty[st]);
@@ -172,7 +196,7 @@ __global__ void __launch_bounds__(kW8TcThreads, 1) k_w8a8_tc(const __grid_consta
             for (int j = 0; j < NTOK / 8; ++j)
 #pragma unroll
                 for (int e = 0; e < 4; ++e)
-                    w8_epilogue1<T, FP8>(p, tile * kTcRows + m0 + (e >> 1) * 8, 8 * j + 2 * tig + (e & 1),
+                    w8_epilogue1<T, FP8, BLK>(p, tile * kTcRows + m0 + (e >> 1) * 8, 8 * j + 2 * tig + (e & 1),
                                         FP8 ? (float)accf[FP8 ? 4 * j + e : 0] : (float)acc[4 * j + e]);
             continue;
         }
@@ -209,7 +233,7 @@ __global__ void __launch_bounds__(kW8TcThreads, 1) k_w8a8_tc(const __grid_consta
                     for (int s = 0; s < S; ++s) a += __float_as_int(__ldcg(base + (size_t)s * p.M * kTcRows + idx));
                     v = (float)a;
                 }
-                w8_epilogue1<T, FP8>(p, tile * kTcRows + m, tok, v);
+                w8_epilogue1<T, FP8, BLK>(p, tile * kTcRows + m, tok, v);
             }
             if (ct == 0) p.counters[tile] = 0u;
         }
@@ -239,23 +263,26 @@ bool w8_tc_supports(int N, int K) {
     return !off && K % 128 == 0 && N >= 1 && (N + kTcRows - 1) / kTcRows <= kTcMaxTiles;
 }
 
-template <typename T, bool FP8, int NTOK>
+template <typename T, bool FP8, int NTOK, bool BLK>
 static cudaError_t launch_w8_tc_t(const W8TcParams& q, dim3 grid, bool pdl, cudaStream_t stream) {
-    return launch(k_w8a8_tc<T, FP8, NTOK>, grid, dim3(kW8TcThreads), (size_t)W8TcCfg<NTOK>::kBytes, stream, pdl, q);
+    return launch(k_w8a8_tc<T, FP8, NTOK, BLK>, grid, dim3(kW8TcThreads), (size_t)W8TcCfg<NTOK>::kBytes, stream, pdl, q);
 }
 
 // mc <= 256 rows of one pass (fp8: passes of <= 128 rows, its promoted accumulators take twice the registers).
+// sw_mode 4 (block scales, FP8 only): sx is (K/128, sx_ld) column-major, sw (ceil(N/128), K/128) row-major.
 // zl_prepare() must have run on this device (split-k workspace, opt-in shared memory).
 template <typename T, bool FP8>
 cudaError_t launch_w8_tc(const uint8_t* xq, const float* sx, const uint8_t* w, const void* sw, int sw_mode, const T* bias, T* y,
-                         int mc, int N, int K, bool pdl, cudaStream_t stream) {
+                         int mc, int N, int K, bool pdl, cudaStream_t stream, int sx_ld) {
     TcDeviceState* st = tc_state();
     if (!st || !st->ws) return cudaErrorNotSupported;
+    const bool blk = sw_mode == 4;
+    if (blk && !FP8) return cudaErrorInvalidValue;
     if (FP8 && mc > 128) {
-        for (int r0 = 0; r0 < mc; r0 += 128) {   // one scale for all tokens: only x and y move
+        for (int r0 = 0; r0 < mc; r0 += 128) {   // per-tensor: one scale for all tokens, only x and y move
             const int rows = mc - r0 < 128 ? mc - r0 : 128;
-            const cudaError_t e = launch_w8_tc<T, FP8>(xq + (size_t)r0 * K, sx, w, sw, sw_mode, bias, y + (size_t)r0 * N, rows,
-                                                       N, K, pdl, stream);
+            const cudaError_t e = launch_w8_tc<T, FP8>(xq + (size_t)r0 * K, blk ? sx + r0 : sx, w, sw, sw_mode, bias,
+                                                       y + (size_t)r0 * N, rows, N, K, pdl, stream, sx_ld);
             if (e != cudaSuccess) return e;
         }
         return cudaSuccess;
@@ -268,6 +295,7 @@ cudaError_t launch_w8_tc(const uint8_t* xq, const float* sx, const uint8_t* w, c
     q.sx = sx;
     q.sw = sw;
     q.sw_mode = sw_mode;
+    q.sx_ld = sx_ld;
     q.bias = bias;
     q.y = y;
     q.M = mc;
@@ -280,35 +308,46 @@ cudaError_t launch_w8_tc(const uint8_t* xq, const float* sx, const uint8_t* w, c
     q.err = st->err;
     const int items = n_tiles * q.S, sms = device_sm_count();
     const dim3 grid(items < sms ? items : sms);
+    if constexpr (FP8) {
+        if (blk) {
+            switch (ntok) {
+                case 32: return launch_w8_tc_t<T, true, 32, true>(q, grid, pdl, stream);
+                case 64: return launch_w8_tc_t<T, true, 64, true>(q, grid, pdl, stream);
+                case 128: return launch_w8_tc_t<T, true, 128, true>(q, grid, pdl, stream);
+                default: return cudaErrorInvalidValue;
+            }
+        }
+    }
     switch (ntok) {
-        case 32: return launch_w8_tc_t<T, FP8, 32>(q, grid, pdl, stream);
-        case 64: return launch_w8_tc_t<T, FP8, 64>(q, grid, pdl, stream);
-        case 128: return launch_w8_tc_t<T, FP8, 128>(q, grid, pdl, stream);
+        case 32: return launch_w8_tc_t<T, FP8, 32, false>(q, grid, pdl, stream);
+        case 64: return launch_w8_tc_t<T, FP8, 64, false>(q, grid, pdl, stream);
+        case 128: return launch_w8_tc_t<T, FP8, 128, false>(q, grid, pdl, stream);
         default:
             if constexpr (FP8) return cudaErrorInvalidValue;
-            else return launch_w8_tc_t<T, FP8, 256>(q, grid, pdl, stream);
+            else return launch_w8_tc_t<T, FP8, 256, false>(q, grid, pdl, stream);
     }
 }
 
 template cudaError_t launch_w8_tc<__half, false>(const uint8_t*, const float*, const uint8_t*, const void*, int, const __half*,
-                                                 __half*, int, int, int, bool, cudaStream_t);
+                                                 __half*, int, int, int, bool, cudaStream_t, int);
 template cudaError_t launch_w8_tc<__half, true>(const uint8_t*, const float*, const uint8_t*, const void*, int, const __half*,
-                                                __half*, int, int, int, bool, cudaStream_t);
+                                                __half*, int, int, int, bool, cudaStream_t, int);
 template cudaError_t launch_w8_tc<__nv_bfloat16, false>(const uint8_t*, const float*, const uint8_t*, const void*, int,
-                                                        const __nv_bfloat16*, __nv_bfloat16*, int, int, int, bool, cudaStream_t);
+                                                        const __nv_bfloat16*, __nv_bfloat16*, int, int, int, bool, cudaStream_t, int);
 template cudaError_t launch_w8_tc<__nv_bfloat16, true>(const uint8_t*, const float*, const uint8_t*, const void*, int,
-                                                       const __nv_bfloat16*, __nv_bfloat16*, int, int, int, bool, cudaStream_t);
+                                                       const __nv_bfloat16*, __nv_bfloat16*, int, int, int, bool, cudaStream_t, int);
 
 // opt-in shared-memory sizes must be set outside stream capture: called from zl_prepare
 cudaError_t prepare_w8_tc() {
     cudaError_t e;
-#define ZL_W8TC_SET(TT, F8, NT)                                                                                     \
-    if ((e = cudaFuncSetAttribute(k_w8a8_tc<TT, F8, NT>, cudaFuncAttributeMaxDynamicSharedMemorySize,               \
+#define ZL_W8TC_SET(TT, F8, NT, B)                                                                                  \
+    if ((e = cudaFuncSetAttribute(k_w8a8_tc<TT, F8, NT, B>, cudaFuncAttributeMaxDynamicSharedMemorySize,            \
                                   W8TcCfg<NT>::kBytes)) != cudaSuccess)                                            \
         return e;
-#define ZL_W8TC_ALL(TT, F8) ZL_W8TC_SET(TT, F8, 32) ZL_W8TC_SET(TT, F8, 64) ZL_W8TC_SET(TT, F8, 128)
-    ZL_W8TC_ALL(__half, false) ZL_W8TC_ALL(__half, true) ZL_W8TC_ALL(__nv_bfloat16, false) ZL_W8TC_ALL(__nv_bfloat16, true)
-    ZL_W8TC_SET(__half, false, 256) ZL_W8TC_SET(__nv_bfloat16, false, 256)
+#define ZL_W8TC_ALL(TT, F8, B) ZL_W8TC_SET(TT, F8, 32, B) ZL_W8TC_SET(TT, F8, 64, B) ZL_W8TC_SET(TT, F8, 128, B)
+    ZL_W8TC_ALL(__half, false, false) ZL_W8TC_ALL(__half, true, false) ZL_W8TC_ALL(__nv_bfloat16, false, false)
+    ZL_W8TC_ALL(__nv_bfloat16, true, false) ZL_W8TC_ALL(__half, true, true) ZL_W8TC_ALL(__nv_bfloat16, true, true)
+    ZL_W8TC_SET(__half, false, 256, false) ZL_W8TC_SET(__nv_bfloat16, false, 256, false)
 #undef ZL_W8TC_ALL
 #undef ZL_W8TC_SET
     return cudaSuccess;

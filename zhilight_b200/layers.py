@@ -4,7 +4,8 @@
 
 `Linear` restates `nn::Linear`'s dispatch by QuantType (src/nn/linear/linear.cpp:1952-2075,
 src/model/model_config.hpp:132-144): 0 Normal, 1/2 Int8 (2 = AutoInt8: quantise the fp weight at load,
-linear.cpp:521-550), 5 GPTQ, 6 AWQ, 7 FP8, 8 GPTQ_Marlin (same checkpoint as 5, symmetric u4b8).
+linear.cpp:521-550), 5 GPTQ, 6 AWQ, 7 FP8, 8 GPTQ_Marlin (same checkpoint as 5, symmetric u4b8), 10 FP8_Block
+(e4m3 weights with one weight_scale_inv per 128x128 block, activations quantised per token in groups of 128).
 Every code path ends in the C-ABI (zhilight_b200.ops); there is no torch fallback -- without the CUDA library the
 constructor raises."""
 import torch
@@ -12,6 +13,7 @@ import torch
 from . import _lib, ops
 
 QUANT_NONE, QUANT_INT8, QUANT_AUTO_INT8, QUANT_GPTQ, QUANT_AWQ, QUANT_FP8, QUANT_GPTQ_MARLIN = 0, 1, 2, 5, 6, 7, 8
+QUANT_FP8_BLOCK = 10
 _DTYPES = {"half": torch.float16, "float16": torch.float16, "bfloat": torch.bfloat16, "bfloat16": torch.bfloat16}
 
 
@@ -25,12 +27,14 @@ class Linear:
         if self.activation not in ("", "silu", "gelu"):
             raise ValueError("unsupported activation %r" % activation)
         self.quant = int(quant)                          # the reference's tests pass False for 0
-        if self.quant not in (0, 1, 2, 5, 6, 7, 8):
+        if self.quant not in (0, 1, 2, 5, 6, 7, 8, 10):
             raise _lib.ZLError(-2, "quant value error: %d" % self.quant)
         self.dtype = _DTYPES[dtype]
         self.group_size, self.sym = group_size, bool(sym) or self.quant == QUANT_GPTQ_MARLIN
         if self.quant in (QUANT_GPTQ, QUANT_AWQ, QUANT_GPTQ_MARLIN) and self.dtype != torch.float16:
             raise _lib.ZLError(-2, "A must be half")     # q_gemm_k_major.cu:989
+        if self.quant == QUANT_FP8_BLOCK and self.dim_in % 128 != 0:
+            raise _lib.ZLError(-2, "FP8 block_scale: dim_in can't divide 128")
         self._p = {}
         self.bias = None
 
@@ -55,6 +59,18 @@ class Linear:
             w = sd["weight"]
             w = w.view(torch.uint8) if w.dtype != torch.uint8 else w
             self._p = {"weight": w.contiguous(), "weight_scale": sd["weight_scale"].float().reshape(1).contiguous()}
+        elif q == QUANT_FP8_BLOCK:
+            if self.bias is not None:
+                raise _lib.ZLError(-2, "Fp8Block does not support bias")        # Fp8Block::set_has_bias throws
+            w = sd["weight"]
+            w = w.view(torch.uint8) if w.dtype != torch.uint8 else w
+            s = sd["weight_scale_inv"]
+            if tuple(w.shape) != (n, k):
+                raise _lib.ZLError(-1, "weight shape mismatch: %s, expected (%d, %d)" % (tuple(w.shape), n, k))
+            if s.dtype != torch.float32 or tuple(s.shape) != ((n + 127) // 128, k // 128):
+                raise _lib.ZLError(-1, "weight_scale_inv must be float32 (%d, %d), got %s %s"
+                                   % ((n + 127) // 128, k // 128, s.dtype, tuple(s.shape)))
+            self._p = {"weight": w.contiguous(), "weight_scale_inv": s.contiguous()}
         else:
             is_awq = q == QUANT_AWQ
             g_idx = sd.get("g_idx")
@@ -94,6 +110,8 @@ class Linear:
             y = ops.int8_linear(x2, self._p["weight"], self._p["weight_scale"], self.bias)
         elif q == QUANT_FP8:
             y = ops.fp8_linear(x2, self._p["weight"], self._p["weight_scale"], self.bias)
+        elif q == QUANT_FP8_BLOCK:
+            y = ops.fp8_block_linear(x2, self._p["weight"], self._p["weight_scale_inv"])
         else:
             kp = self._k_perm
             if kp is not None and not (self._variant == 1 and _lib.load().zl_w4_int_layout_route(x2.shape[0], n, k) == 3):

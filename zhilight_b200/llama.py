@@ -30,7 +30,7 @@ MODEL_PRESETS = {
                  vocab_size=512, eps=1e-5, rope_theta=10000.0, rope_llama3=None),
 }
 
-QUANT_NONE, QUANT_AUTO_INT8, QUANT_GPTQ, QUANT_AWQ, QUANT_FP8 = 0, 2, 5, 6, 7     # model_config.hpp:132-144
+QUANT_NONE, QUANT_AUTO_INT8, QUANT_GPTQ, QUANT_AWQ, QUANT_FP8, QUANT_FP8_BLOCK = 0, 2, 5, 6, 7, 10   # model_config.hpp:132-144
 
 
 def pack_joined_segments(segments, max_batch, max_seq, vocab_size):

@@ -312,6 +312,35 @@ def fp8_linear(x, w_fp8, w_scale, bias=None, pdl=False):
     return w8a8_gemm(q, s, w_fp8, w_scale, x.dtype, W8_FP8, bias, pdl)
 
 
+def fp8_quant_per_token_group(x, pdl=False):
+    """nn::fp8::per_token_cast_to_fp8: returns (q uint8 (M,K) holding e4m3 bits, scale f32 (K/128, round_up(M, 4)))
+    with one scale per (token, 128-column group), stored column-major like the reference."""
+    m, k = x.shape
+    ld = (m + 3) // 4 * 4
+    q = torch.empty((m, k), dtype=torch.uint8, device=x.device)
+    scale = torch.empty((k // 128 if k % 128 == 0 else 1, ld), dtype=torch.float32, device=x.device)
+    _lib.call("zl_fp8_quant_per_token_group", _p(x), x.stride(0), _p(q), _p(scale), ld, m, k, _dt(x), int(pdl),
+              _stream())
+    return q, scale
+
+
+def fp8_block_gemm(xq, x_scale, w, w_scale, out_dtype, pdl=False):
+    """deep_gemm_fp8_block_h20_group: xq (M,K) e4m3 bytes, x_scale (K/128, ld) f32, w (N,K) e4m3,
+    w_scale (ceil(N/128), K/128) f32 -> y (M,N) out_dtype."""
+    m, k = xq.shape
+    n = w.shape[0]
+    y = torch.empty((m, n), dtype=out_dtype, device=xq.device)
+    _lib.call("zl_fp8_block_gemm", _p(xq), _p(x_scale), x_scale.shape[-1], _p(w), _p(w_scale), _p(y), m, n, k, _dt(y),
+              int(pdl), _stream())
+    return y
+
+
+def fp8_block_linear(x, w_fp8, w_scale_inv, pdl=False):
+    """Fp8Block::forward (linear.cpp:1697-1960): per-token-group activation quant, then the block-scaled GEMM."""
+    q, s = fp8_quant_per_token_group(x, pdl)
+    return fp8_block_gemm(q, s, w_fp8, w_scale_inv, x.dtype, pdl)
+
+
 def rmsnorm(x, weight, eps, scale=1.0, pdl=False):
     t, d = x.shape
     y = torch.empty_like(x)

@@ -166,8 +166,7 @@ int zl_w4_int_layout_route(int M, int N, int K);
 /* last watchdog code published by a tensor-core kernel on the current device (0 = none); a bounded mbarrier wait that expires
  * records which pipeline barrier starved and traps instead of hanging the GPU. */
 unsigned zl_w4_tc_watchdog(void);
-/* debug / tests: at least `splits` pieces per weight-row tile in the wgmma kernel's stream-k schedule (0 = automatic; also
- * ZL_TC_SPLITS). */
+/* debug / tests: at least `splits` pieces per weight-row tile in the wgmma kernel's stream-k schedule (0 = automatic). */
 int zl_w4_tc_set_splits(int splits);
 /* tests: host view of the wgmma kernel's stream-k schedule (the kernel's own scheduling code): pieces of CTA `cta` of `ctas`
  * for n_tiles x G (tile, group) units; out[5 i ..] = tile, g0, g1, pieces of that tile, workspace slot (-1: whole tile);
@@ -289,9 +288,6 @@ int zl_qkv_rope_append(const float* cos, const float* sin, const void* qkv, void
  * Decode attention over per-task ragged KV buffers
  * nn::multi_query_attention_rag_buffer (src/nn/attention/attention_kernel.cu:1252-1457)
  * ------------------------------------------------------------------------------------------ */
-/* one-shot hint: the NEXT zl_decode_attention call on this thread also prefetches [ptr, ptr+bytes) into L2
- * (weights of a later GEMM; attention leaves HBM idle at small batch). */
-int zl_decode_attention_set_prefetch(const void* ptr, size_t bytes);
 size_t zl_decode_attention_workspace_bytes(int B, int len_q, int num_heads, int dim_head, int max_len_buf);
 /* q (B, len_q, H_q, d); buf_lens (B); k_addrs/v_addrs (B) device arrays of device pointers;
  * mask int8 ragged concat of (len_q, len_buf_b); out (B, len_q, H_q, d).  bshd: (len_buf, H_kv, d) else

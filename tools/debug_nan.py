@@ -44,9 +44,8 @@ if __name__ == "__main__":
         a = [int(x) for x in sys.argv[1:7]]
         run(*a)
         sys.exit(0)
-    variants = [({}, (32, 140, 2, 1, 1, 1)), ({"ZL_ATTN_OLD_SHORT": "1"}, (32, 140, 2, 1, 1, 1)), ({}, (32, 140, 0, 1, 1, 1)),
-                ({}, (32, 140, 2, 0, 0, 1)), ({}, (4, 140, 2, 1, 1, 1)), ({"ZL_W4_NO_ONE": "1"}, (32, 140, 2, 1, 1, 1)),
-                ({}, (32, 40, 2, 1, 1, 32))]
+    variants = [({}, (32, 140, 2, 1, 1, 1)), ({}, (32, 140, 0, 1, 1, 1)), ({}, (32, 140, 2, 0, 0, 1)),
+                ({}, (4, 140, 2, 1, 1, 1)), ({}, (32, 40, 2, 1, 1, 32))]
     for env, args in variants:
         e = dict(os.environ)
         e.update(env)

@@ -159,14 +159,6 @@ __device__ __forceinline__ void l2_prefetch_share(const uint8_t* base, size_t by
     }
 }
 
-// LSU-path variant (no TMA queue entries): every lane of every (cta, warp) touches its strided share of the 128-byte
-// lines of [base, base+bytes) with prefetch.global.L2.  Call from all 32 lanes.
-__device__ __forceinline__ void l2_prefetch_lines(const uint8_t* base, size_t bytes, int part, int parts, int lane) {
-    const size_t n_lines = (bytes + 127) >> 7;
-    for (size_t l = (size_t)part * 32 + lane; l < n_lines; l += (size_t)parts * 32)
-        asm volatile("prefetch.global.L2 [%0];" ::"l"(base + (l << 7)));
-}
-
 // ---------------------------------------------------------------------------------------------
 // loads
 // ---------------------------------------------------------------------------------------------

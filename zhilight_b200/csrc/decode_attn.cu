@@ -8,14 +8,13 @@
 // every K/V byte: K is read ONCE per kv-head straight into tensor-core A fragments (16 keys x 16 dims),
 // Q is the B operand (16 dims x 8 heads), so S = K.Q^T needs no shuffles; softmax is the reference's
 // exact two-pass fp32 form inside the split (mask ? scale*s : -inf, max seeded -1e20, sum seeded 1e-20);
-// P.V runs in fp32 on the CUDA cores with 16-byte coalesced V loads (each V element feeds all heads).
+// P.V runs on the tensor cores too, with fp32 accumulators.
 // Splits are merged with the reference's LSE rule (attention_kernel.cu:881-923).
 #include "common.cuh"
 #include "attn_combine.cuh"
 #include "decode_attn_short.cuh"
 #include "decode_attn_warp.cuh"
 
-#include <cstdlib>
 #include <type_traits>
 
 namespace zl {
@@ -26,16 +25,14 @@ constexpr int kAttnMaxRange = 1024;            // keys per CTA; logits live in s
 constexpr int kAttnRowStride = kAttnMaxRange + 4;
 constexpr int kAttnMaxSplits = 64;
 
-template <typename T, int D, bool PV_FP32>
+template <typename T, int D>
 __global__ void __launch_bounds__(kAttnThreads)
 k_decode_attn(const T* __restrict__ q, const int32_t* __restrict__ buf_lens, T* const* __restrict__ k_addrs,
               T* const* __restrict__ v_addrs, const int8_t* __restrict__ mask, float scale,
               T* __restrict__ out, float* __restrict__ part_o, float* __restrict__ part_m,
               float* __restrict__ part_l, int len_q, int num_heads, int num_kv_heads, int m_query,
-              int num_splits, int bshd, const uint8_t* __restrict__ pf_ptr, unsigned long long pf_bytes) {
+              int num_splits, int bshd) {
     constexpr int NI = D / 32;                 // 16-byte chunks per lane per key row
-    constexpr int DC = D / 8;                  // threads covering one V row
-    constexpr int NSUB = kAttnThreads / DC;    // key subsets in the PV phase
     __shared__ __align__(16) float s_logit[8 * kAttnRowStride];
     __shared__ float s_m[8], s_l[8];
 
@@ -50,13 +47,6 @@ k_decode_attn(const T* __restrict__ q, const int32_t* __restrict__ buf_lens, T* 
     const int head0 = hk * m_query + mq0;
 
     pdl_trigger();
-    // attention barely touches HBM at small batch: use the time to pull a later GEMM's weights into L2
-    if (pf_ptr) {
-        const int n_cta = gridDim.x * gridDim.y * gridDim.z;
-        const int cta = blockIdx.x + gridDim.x * (blockIdx.y + gridDim.y * blockIdx.z);
-        const int wpc = blockDim.x >> 5;
-        l2_prefetch_lines(pf_ptr, (size_t)pf_bytes, cta * wpc + warp, n_cta * wpc, lane);
-    }
     pdl_wait();
 
     const int len_buf = buf_lens[b];
@@ -138,8 +128,7 @@ k_decode_attn(const T* __restrict__ q, const int32_t* __restrict__ buf_lens, T* 
     }
     __syncthreads();
 
-    // ---- phase 3: O = P.V on the tensor cores (mma.sync m16n8k16, fp32 accumulate); ZL_ATTN_PV_FP32=1 keeps the CUDA-core
-    // loop of round 1 (every V element times every head in fp32) for A/B measurements ----
+    // ---- phase 3: O = P.V on the tensor cores (mma.sync m16n8k16, fp32 accumulate) ----
     // A = P [head (8 of 16 rows) x 16 keys]: fp16 models carry p * 2^10 in fp16 (11 significant bits, no subnormals); bf16
     // models carry p as bf16 hi + lo (two MMAs), so that the product keeps ~16 bits of p.  B = V [16 keys x 8 columns]: a B
     // register holds TWO KEYS of one column while V is key-major, so lane (g, t) loads D/8 contiguous elements (columns
@@ -149,118 +138,64 @@ k_decode_attn(const T* __restrict__ q, const int32_t* __restrict__ buf_lens, T* 
     constexpr int NW = NJ / 2;                // 32-bit words of a lane's column chunk (2 elements each)
     constexpr bool kHalf = sizeof(T) == 2 && std::is_same<T, __half>::value;
     float* s_red = s_logit;                   // [warp][h][D], valid after the barrier below
-    if constexpr (!PV_FP32) {
-        float o[NJ][4];
+    float o[NJ][4];
 #pragma unroll
-        for (int j = 0; j < NJ; ++j) o[j][0] = o[j][1] = o[j][2] = o[j][3] = 0.f;
-        for (int tile = warp; tile < ntiles; tile += kAttnWarps) {
-            const int kb = tile * 16;
-            uint32_t vw[4][NW];
+    for (int j = 0; j < NJ; ++j) o[j][0] = o[j][1] = o[j][2] = o[j][3] = 0.f;
+    for (int tile = warp; tile < ntiles; tile += kAttnWarps) {
+        const int kb = tile * 16;
+        uint32_t vw[4][NW];
 #pragma unroll
-            for (int r = 0; r < 4; ++r) {
-                const int kk = kb + 2 * t + (r & 1) + (r >> 1) * 8;
+        for (int r = 0; r < 4; ++r) {
+            const int kk = kb + 2 * t + (r & 1) + (r >> 1) * 8;
 #pragma unroll
-                for (int w = 0; w < NW; ++w) vw[r][w] = 0u;
-                if (kk < n) {
-                    const T* src = vbase + (size_t)(k0 + kk) * stride + g * NJ;
+            for (int w = 0; w < NW; ++w) vw[r][w] = 0u;
+            if (kk < n) {
+                const T* src = vbase + (size_t)(k0 + kk) * stride + g * NJ;
 #pragma unroll
-                    for (int w4 = 0; w4 < NW / 4; ++w4) {
-                        const uint4 v = ld_cg_u4(src + w4 * 8);
-                        vw[r][w4 * 4 + 0] = v.x, vw[r][w4 * 4 + 1] = v.y, vw[r][w4 * 4 + 2] = v.z, vw[r][w4 * 4 + 3] = v.w;
-                    }
-                }
-            }
-            uint32_t af[4] = {0u, 0u, 0u, 0u}, al[4] = {0u, 0u, 0u, 0u};
-            if (g < mq) {
-                const float* pr = s_logit + g * kAttnRowStride + kb + 2 * t;
-                const float2 p0 = *reinterpret_cast<const float2*>(pr), p1 = *reinterpret_cast<const float2*>(pr + 8);
-                const float q0 = kb + 2 * t < n ? p0.x : 0.f, q1 = kb + 2 * t + 1 < n ? p0.y : 0.f;
-                const float q2 = kb + 2 * t + 8 < n ? p1.x : 0.f, q3 = kb + 2 * t + 9 < n ? p1.y : 0.f;
-                if constexpr (kHalf) {
-                    const __half2 h0 = __floats2half2_rn(q0 * 1024.f, q1 * 1024.f), h1 = __floats2half2_rn(q2 * 1024.f, q3 * 1024.f);
-                    af[0] = *reinterpret_cast<const uint32_t*>(&h0);
-                    af[2] = *reinterpret_cast<const uint32_t*>(&h1);
-                } else {
-                    const __nv_bfloat162 h0 = __floats2bfloat162_rn(q0, q1), h1 = __floats2bfloat162_rn(q2, q3);
-                    const float2 f0 = __bfloat1622float2(h0), f1 = __bfloat1622float2(h1);
-                    const __nv_bfloat162 l0 = __floats2bfloat162_rn(q0 - f0.x, q1 - f0.y), l1 = __floats2bfloat162_rn(q2 - f1.x, q3 - f1.y);
-                    af[0] = *reinterpret_cast<const uint32_t*>(&h0);
-                    af[2] = *reinterpret_cast<const uint32_t*>(&h1);
-                    al[0] = *reinterpret_cast<const uint32_t*>(&l0);
-                    al[2] = *reinterpret_cast<const uint32_t*>(&l1);
-                }
-            }
-#pragma unroll
-            for (int w = 0; w < NW; ++w) {
-#pragma unroll
-                for (int e = 0; e < 2; ++e) {            // element 2 w + e of the chunk = n-tile j
-                    const uint32_t sel = e ? 0x7632u : 0x5410u;
-                    const uint32_t b0 = __byte_perm(vw[0][w], vw[1][w], sel), b1 = __byte_perm(vw[2][w], vw[3][w], sel);
-                    mma_attn<T>(o[2 * w + e], af, b0, b1);
-                    if constexpr (!kHalf) mma_attn<T>(o[2 * w + e], al, b0, b1);
+                for (int w4 = 0; w4 < NW / 4; ++w4) {
+                    const uint4 v = ld_cg_u4(src + w4 * 8);
+                    vw[r][w4 * 4 + 0] = v.x, vw[r][w4 * 4 + 1] = v.y, vw[r][w4 * 4 + 2] = v.z, vw[r][w4 * 4 + 3] = v.w;
                 }
             }
         }
-        __syncthreads();   // everyone is done reading probabilities; reuse s_logit as the reduction buffer
+        uint32_t af[4] = {0u, 0u, 0u, 0u}, al[4] = {0u, 0u, 0u, 0u};
         if (g < mq) {
-            const float sc = kHalf ? (1.f / 1024.f) : 1.f;
-#pragma unroll
-            for (int j = 0; j < NJ; ++j) {
-                s_red[(warp * 8 + g) * D + NJ * (2 * t) + j] = o[j][0] * sc;
-                s_red[(warp * 8 + g) * D + NJ * (2 * t + 1) + j] = o[j][1] * sc;
+            const float* pr = s_logit + g * kAttnRowStride + kb + 2 * t;
+            const float2 p0 = *reinterpret_cast<const float2*>(pr), p1 = *reinterpret_cast<const float2*>(pr + 8);
+            const float q0 = kb + 2 * t < n ? p0.x : 0.f, q1 = kb + 2 * t + 1 < n ? p0.y : 0.f;
+            const float q2 = kb + 2 * t + 8 < n ? p1.x : 0.f, q3 = kb + 2 * t + 9 < n ? p1.y : 0.f;
+            if constexpr (kHalf) {
+                const __half2 h0 = __floats2half2_rn(q0 * 1024.f, q1 * 1024.f), h1 = __floats2half2_rn(q2 * 1024.f, q3 * 1024.f);
+                af[0] = *reinterpret_cast<const uint32_t*>(&h0);
+                af[2] = *reinterpret_cast<const uint32_t*>(&h1);
+            } else {
+                const __nv_bfloat162 h0 = __floats2bfloat162_rn(q0, q1), h1 = __floats2bfloat162_rn(q2, q3);
+                const float2 f0 = __bfloat1622float2(h0), f1 = __bfloat1622float2(h1);
+                const __nv_bfloat162 l0 = __floats2bfloat162_rn(q0 - f0.x, q1 - f0.y), l1 = __floats2bfloat162_rn(q2 - f1.x, q3 - f1.y);
+                af[0] = *reinterpret_cast<const uint32_t*>(&h0);
+                af[2] = *reinterpret_cast<const uint32_t*>(&h1);
+                al[0] = *reinterpret_cast<const uint32_t*>(&l0);
+                al[2] = *reinterpret_cast<const uint32_t*>(&l1);
             }
         }
-    } else {
-        const int dc = tid % DC, sub = tid / DC;
-        float o[8][8];
 #pragma unroll
-        for (int h = 0; h < 8; ++h)
+        for (int w = 0; w < NW; ++w) {
 #pragma unroll
-            for (int i = 0; i < 8; ++i) o[h][i] = 0.f;
-        const T* vp = vbase + (size_t)k0 * stride + dc * 8;
-        constexpr int U = 4;
-        for (int key = sub; key < n; key += NSUB * U) {
-            uint4 vv[U];
-#pragma unroll
-            for (int u = 0; u < U; ++u) {
-                const int kk = key + u * NSUB;
-                if (kk < n) vv[u] = ld_cg_u4(vp + (size_t)kk * stride);
-            }
-#pragma unroll
-            for (int u = 0; u < U; ++u) {
-                const int kk = key + u * NSUB;
-                if (kk < n) {
-                    float vf[8];
-                    unpack8<T>(vv[u], vf);
-#pragma unroll
-                    for (int h = 0; h < 8; ++h) {
-                        if (h < mq) {
-                            const float p = s_logit[h * kAttnRowStride + kk];
-#pragma unroll
-                            for (int i = 0; i < 8; ++i) o[h][i] = fmaf(p, vf[i], o[h][i]);
-                        }
-                    }
-                }
+            for (int e = 0; e < 2; ++e) {            // element 2 w + e of the chunk = n-tile j
+                const uint32_t sel = e ? 0x7632u : 0x5410u;
+                const uint32_t b0 = __byte_perm(vw[0][w], vw[1][w], sel), b1 = __byte_perm(vw[2][w], vw[3][w], sel);
+                mma_attn<T>(o[2 * w + e], af, b0, b1);
+                if constexpr (!kHalf) mma_attn<T>(o[2 * w + e], al, b0, b1);
             }
         }
-        // reduce key subsets: inside the warp first (lanes with equal dc), then across warps via smem
+    }
+    __syncthreads();   // everyone is done reading probabilities; reuse s_logit as the reduction buffer
+    if (g < mq) {
+        const float sc = kHalf ? (1.f / 1024.f) : 1.f;
 #pragma unroll
-        for (int h = 0; h < 8; ++h)
-#pragma unroll
-            for (int i = 0; i < 8; ++i) {
-                float v = o[h][i];
-#pragma unroll
-                for (int off = DC; off < 32; off <<= 1) v += __shfl_xor_sync(0xffffffffu, v, off);
-                o[h][i] = v;
-            }
-        __syncthreads();   // everyone is done reading probabilities; reuse s_logit as the reduction buffer
-        if (lane < DC) {
-#pragma unroll
-            for (int h = 0; h < 8; ++h)
-                if (h < mq) {
-#pragma unroll
-                    for (int i = 0; i < 8; ++i) s_red[(warp * 8 + h) * D + lane * 8 + i] = o[h][i];
-                }
+        for (int j = 0; j < NJ; ++j) {
+            s_red[(warp * 8 + g) * D + NJ * (2 * t) + j] = o[j][0] * sc;
+            s_red[(warp * 8 + g) * D + NJ * (2 * t + 1) + j] = o[j][1] * sc;
         }
     }
     __syncthreads();
@@ -284,36 +219,6 @@ k_decode_attn(const T* __restrict__ q, const int32_t* __restrict__ buf_lens, T* 
 }
 
 
-// ---------------------------------------------------------------------------------------------------------
-// Latency-optimised variant for the small-batch / short-context regime (a B=1 decode step has 8 kv-heads of
-// work for 132 SMs): 512 threads, at most 256 keys per CTA, and EVERY global load of the CTA (q, its K tile,
-// its V rows) is issued before the first dependent instruction, so the whole CTA costs one memory round trip
-// instead of one per loop iteration.  Same math and split/combine contract as k_decode_attn.
-// ---------------------------------------------------------------------------------------------------------
-template <typename T, int D>
-__global__ void __launch_bounds__(kShortThreads)
-k_decode_attn_short(const T* __restrict__ q, const int32_t* __restrict__ buf_lens, T* const* __restrict__ k_addrs,
-                    T* const* __restrict__ v_addrs, const int8_t* __restrict__ mask, float scale,
-                    T* __restrict__ out, float* __restrict__ part_o, float* __restrict__ part_m,
-                    float* __restrict__ part_l, int len_q, int num_heads, int num_kv_heads, int m_query,
-                    int num_splits, int bshd, const uint8_t* __restrict__ pf_ptr, unsigned long long pf_bytes) {
-    extern __shared__ __align__(16) float s_dyn[];
-    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-    pdl_trigger();
-    // attention barely touches HBM at small batch: use the time to pull a later GEMM's weights into L2
-    if (pf_ptr) {
-        const int n_cta = gridDim.x * gridDim.y * gridDim.z;
-        const int cta = blockIdx.x + gridDim.x * (blockIdx.y + gridDim.y * blockIdx.z);
-        const int wpc = blockDim.x >> 5;
-        l2_prefetch_lines(pf_ptr, (size_t)pf_bytes, cta * wpc + warp, n_cta * wpc, lane);
-    }
-    pdl_wait();
-    attn_short_item<T, D>(q, buf_lens, k_addrs, v_addrs, mask, scale, out, part_o, part_m, part_l, len_q, num_heads,
-                          num_kv_heads, m_query, num_splits, bshd, (int)blockIdx.x, (int)blockIdx.y, (int)blockIdx.z,
-                          s_dyn);
-}
-
-
 // k_attn_combine (attn_combine.cuh): grid (B*len_q*num_heads), block D
 
 static int attn_num_splits(int B, int len_q, int num_kv_heads, int m_query, int max_len_buf) {
@@ -332,15 +237,6 @@ static int attn_num_splits(int B, int len_q, int num_kv_heads, int m_query, int 
 }  // namespace zl
 
 using namespace zl;
-
-// one-shot prefetch hint consumed by the next zl_decode_attention call on this thread (set by the decode driver)
-static thread_local const uint8_t* g_attn_pf_ptr = nullptr;
-static thread_local unsigned long long g_attn_pf_bytes = 0;
-extern "C" int zl_decode_attention_set_prefetch(const void* ptr, size_t bytes) {
-    g_attn_pf_ptr = static_cast<const uint8_t*>(ptr);
-    g_attn_pf_bytes = bytes;
-    return ZL_OK;
-}
 
 extern "C" size_t zl_decode_attention_workspace_bytes(int B, int len_q, int num_heads, int dim_head,
                                                       int max_len_buf) {
@@ -361,7 +257,7 @@ extern "C" int zl_decode_attention(const void* q, const int32_t* buf_lens, void*
     ZL_CHECK_SUPPORTED(dtype == ZL_F16 || dtype == ZL_BF16);
     const int m_query = num_heads / num_kv_heads;
     int splits = attn_num_splits(B, len_q, num_kv_heads, m_query, max_len_buf);
-    // latency regime: few CTAs of work -> 256-key CTAs that issue all their loads up front
+    // latency regime: few CTAs of work -> 256-key splits on the warp-per-32-keys kernel (one __syncthreads per CTA)
     const int hg0 = (m_query + 7) / 8;
     const int short_splits = cdiv(max_len_buf, kShortRange);
     const bool use_short = short_splits <= kAttnMaxSplits &&
@@ -380,39 +276,17 @@ extern "C" int zl_decode_attention(const void* q, const int32_t* buf_lens, void*
     }
     const int hgroups = (m_query + 7) / 8;
     dim3 grid(splits, num_kv_heads * hgroups, B * len_q), block(kAttnThreads);
-    // default for the latency regime: the warp-per-32-keys kernel (one __syncthreads per CTA); ZL_ATTN_OLD_SHORT=1 keeps the
-    // previous 512-thread short kernel for A/B measurements
-    static const bool old_short = getenv("ZL_ATTN_OLD_SHORT") != nullptr;
-    static const bool pv_fp32 = getenv("ZL_ATTN_PV_FP32") != nullptr;
-    const bool use_warp = use_short && !old_short;
 #define ZL_ATTN_LAUNCH(TT, DD)                                                                                  \
-    if (use_warp) {                                                                                             \
+    if (use_short) {                                                                                            \
         ZL_CHECK_CUDA(launch(k_decode_attn_warp<TT, DD>, grid, dim3(kWarpAttnWarps * 32),                       \
                              (size_t)warp_attn_smem_floats<DD>() * sizeof(float), stream, pdl != 0, (const TT*)q, \
                              buf_lens, (TT* const*)k_addrs, (TT* const*)v_addrs, mask, scale, (TT*)out, part_o, \
                              part_m, part_l, len_q, num_heads, num_kv_heads, m_query, splits, bshd));            \
-    } else if (use_short) {                                                                                     \
-        static bool attr_set = false;                                                                           \
-        if (!attr_set) {                                                                                        \
-            ZL_CHECK_CUDA(cudaFuncSetAttribute(k_decode_attn_short<TT, DD>,                                     \
-                                               cudaFuncAttributeMaxDynamicSharedMemorySize,                     \
-                                               short_smem_bytes<DD>()));                                        \
-            attr_set = true;                                                                                    \
-        }                                                                                                       \
-        ZL_CHECK_CUDA(launch(k_decode_attn_short<TT, DD>, grid, dim3(kShortThreads), short_smem_bytes<DD>(),    \
-                             stream, pdl != 0, (const TT*)q, buf_lens, (TT* const*)k_addrs,                     \
-                             (TT* const*)v_addrs, mask, scale, (TT*)out, part_o, part_m, part_l, len_q,         \
-                             num_heads, num_kv_heads, m_query, splits, bshd, g_attn_pf_ptr, g_attn_pf_bytes));                                  \
-    } else                                                                                                      \
-    if (pv_fp32) {                                                                                              \
-        ZL_CHECK_CUDA(launch(k_decode_attn<TT, DD, true>, grid, block, 0, stream, pdl != 0, (const TT*)q, buf_lens, \
+    } else {                                                                                                    \
+        ZL_CHECK_CUDA(launch(k_decode_attn<TT, DD>, grid, block, 0, stream, pdl != 0, (const TT*)q, buf_lens,   \
                              (TT* const*)k_addrs, (TT* const*)v_addrs, mask, scale, (TT*)out, part_o, part_m,   \
-                             part_l, len_q, num_heads, num_kv_heads, m_query, splits, bshd, g_attn_pf_ptr,      \
-                             g_attn_pf_bytes));                                                                 \
-    } else                                                                                                      \
-    ZL_CHECK_CUDA(launch(k_decode_attn<TT, DD, false>, grid, block, 0, stream, pdl != 0, (const TT*)q, buf_lens, \
-                         (TT* const*)k_addrs, (TT* const*)v_addrs, mask, scale, (TT*)out, part_o, part_m,       \
-                         part_l, len_q, num_heads, num_kv_heads, m_query, splits, bshd, g_attn_pf_ptr, g_attn_pf_bytes)); \
+                             part_l, len_q, num_heads, num_kv_heads, m_query, splits, bshd));                   \
+    }                                                                                                           \
     if (splits > 1)                                                                                             \
         ZL_CHECK_CUDA(launch(k_attn_combine<TT>, dim3((unsigned)vheads), dim3(DD), 0, stream, pdl != 0,         \
                              (const float*)part_o, (const float*)part_m, (const float*)part_l, (TT*)out, splits));
@@ -422,7 +296,5 @@ extern "C" int zl_decode_attention(const void* q, const int32_t* buf_lens, void*
         if (dim_head == 128) { ZL_ATTN_LAUNCH(__nv_bfloat16, 128) } else { ZL_ATTN_LAUNCH(__nv_bfloat16, 64) }
     }
 #undef ZL_ATTN_LAUNCH
-    g_attn_pf_ptr = nullptr;
-    g_attn_pf_bytes = 0;
     return ZL_OK;
 }

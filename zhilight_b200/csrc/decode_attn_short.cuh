@@ -1,6 +1,5 @@
-// Short-context decode attention work item (<= 256 keys of one kv-head group of one task), shared by the stand-alone
-// kernel k_decode_attn_short (decode_attn.cu) and the persistent whole-model decode kernel (llama_mega.cu).
-// 512 threads; every global load of the item is issued before the first dependent instruction.
+// Pieces shared by the decode attention kernels (decode_attn.cu, decode_attn_warp.cuh, decode_attn_kv8.cu, varlen_attn.cu):
+// the per-type tensor-core MMA, key-range rounding, and the key range of one latency-regime CTA.
 #pragma once
 #include "common.cuh"
 
@@ -20,190 +19,7 @@ __device__ __forceinline__ void mma_attn<__nv_bfloat16>(float (&d)[4], const uin
     mma_16816_bf16(d, a, b0, b1, d);
 }
 
-constexpr int kShortThreads = 512;
-constexpr int kShortWarps = 16;
+// keys per split in the latency regime (few CTAs of work), where zl_decode_attention runs the warp kernel
 constexpr int kShortRange = 256;
-constexpr int kShortRowStride = kShortRange + 4;
-
-template <int D>
-constexpr int short_smem_floats() { return 8 * kShortRowStride + kShortWarps * 8 * D + 16; }
-template <int D>
-constexpr int short_smem_bytes() { return short_smem_floats<D>() * (int)sizeof(float); }
-
-// s_dyn: short_smem_floats<D>() floats of shared memory owned by the calling CTA for the duration of the call.
-// The caller synchronises the CTA before s_dyn is reused.  split / head_group (= kv_head * hgroups + hg) / bq are
-// what blockIdx.x / .y / .z are in the stand-alone kernel.
-template <typename T, int D>
-__device__ __forceinline__ void attn_short_item(const T* __restrict__ q, const int32_t* __restrict__ buf_lens,
-                                                T* const* __restrict__ k_addrs, T* const* __restrict__ v_addrs,
-                                                const int8_t* __restrict__ mask, float scale, T* __restrict__ out,
-                                                float* __restrict__ part_o, float* __restrict__ part_m,
-                                                float* __restrict__ part_l, int len_q, int num_heads, int num_kv_heads,
-                                                int m_query, int num_splits, int bshd, int split, int head_group, int bq,
-                                                float* s_dyn) {
-    constexpr int NI = D / 32;
-    constexpr int DC = D / 8;                    // threads per V row
-    constexpr int NSUB = kShortThreads / DC;     // 32 (D=128) or 64 (D=64) key subsets
-    constexpr int VU = kShortRange / NSUB;       // V rows per thread: 8 or 4
-    float* s_logit = s_dyn;                                  // [8][kShortRowStride]
-    float* s_red = s_dyn + 8 * kShortRowStride;              // [16 warps][8 heads][D]
-    float* s_m = s_red + kShortWarps * 8 * D;                // [8]
-    float* s_l = s_m + 8;                                    // [8]
-
-    const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
-    const int g = lane >> 2, t = lane & 3;
-    const int hgroups = (m_query + 7) / 8;
-    const int hk = head_group / hgroups, hg = head_group % hgroups;
-    const int b = bq / len_q, qi = bq % len_q;
-    const int mq0 = hg * 8;
-    const int mq = min(8, m_query - mq0);
-    const int head0 = hk * m_query + mq0;
-
-    const int len_buf = buf_lens[b];
-    const int chunk = attn_round16((len_buf + num_splits - 1) / num_splits);   // host guarantees <= 256
-    const int k0 = split * chunk;
-    const int k1 = min(len_buf, k0 + chunk);
-    const int n = max(0, k1 - k0);
-
-    const size_t stride = bshd ? (size_t)num_kv_heads * D : (size_t)D;
-    const size_t base = bshd ? (size_t)hk * D : (size_t)hk * len_buf * D;
-    const T* kbase = k_addrs[b] + base;
-    const T* vbase = v_addrs[b] + base;
-    const int8_t* mrow = nullptr;
-    if (mask) {
-        size_t len_off = 0;
-        for (int j = 0; j < b; ++j) len_off += buf_lens[j];
-        mrow = mask + (size_t)len_q * len_off + (size_t)qi * len_buf;
-    }
-
-    // ---- issue every load of this CTA up front ----
-    uint4 qf[NI], ka[NI], kb[NI];
-    const int ntiles = (n + 15) >> 4;            // <= 16 == number of warps
-    const bool has_tile = warp < ntiles;
-    const int ka_i = k0 + warp * 16 + g, kb_i = ka_i + 8;
-#pragma unroll
-    for (int i = 0; i < NI; ++i)
-        qf[i] = (g < mq) ? ld_cg_u4(q + ((size_t)bq * num_heads + head0 + g) * D + i * 32 + t * 8) : make_uint4(0, 0, 0, 0);
-    if (has_tile) {
-        const T* pa = kbase + (size_t)min(ka_i, k1 - 1) * stride + t * 8;
-        const T* pb = kbase + (size_t)min(kb_i, k1 - 1) * stride + t * 8;
-#pragma unroll
-        for (int i = 0; i < NI; ++i) {
-            ka[i] = ld_cg_u4(pa + i * 32);
-            kb[i] = ld_cg_u4(pb + i * 32);
-        }
-    }
-    const int dc = tid % DC, sub = tid / DC;
-    uint4 vv[VU];
-    const T* vp = vbase + (size_t)k0 * stride + dc * 8;
-#pragma unroll
-    for (int u = 0; u < VU; ++u) {
-        const int kk = sub + u * NSUB;
-        if (kk < n) vv[u] = ld_cg_u4(vp + (size_t)kk * stride);
-    }
-
-    // ---- S = K.Q^T ----
-    if (has_tile) {
-        float acc[4] = {0.f, 0.f, 0.f, 0.f};
-#pragma unroll
-        for (int i = 0; i < NI; ++i) {
-            const uint32_t a0[4] = {ka[i].x, kb[i].x, ka[i].y, kb[i].y};
-            const uint32_t a1[4] = {ka[i].z, kb[i].z, ka[i].w, kb[i].w};
-            mma_attn<T>(acc, a0, qf[i].x, qf[i].y);
-            mma_attn<T>(acc, a1, qf[i].z, qf[i].w);
-        }
-        const bool va = ka_i < k1 && (!mrow || mrow[ka_i] != 0);
-        const bool vb = kb_i < k1 && (!mrow || mrow[kb_i] != 0);
-        const int la = warp * 16 + g;
-        const float ninf = -INFINITY;
-        if (2 * t < mq) {
-            s_logit[(2 * t) * kShortRowStride + la] = va ? acc[0] * scale : ninf;
-            s_logit[(2 * t) * kShortRowStride + la + 8] = vb ? acc[2] * scale : ninf;
-        }
-        if (2 * t + 1 < mq) {
-            s_logit[(2 * t + 1) * kShortRowStride + la] = va ? acc[1] * scale : ninf;
-            s_logit[(2 * t + 1) * kShortRowStride + la + 8] = vb ? acc[3] * scale : ninf;
-        }
-    }
-    __syncthreads();
-
-    // ---- masked softmax statistics, one warp per head ----
-    if (warp < mq) {
-        float* row = s_logit + warp * kShortRowStride;
-        float mx = -1e20f;
-        for (int i = lane; i < n; i += 32) mx = fmaxf(mx, row[i]);
-        mx = warp_max(mx);
-        float sum = 0.f;
-        for (int i = lane; i < n; i += 32) {
-            const float e = expf(row[i] - mx);
-            row[i] = e;
-            sum += e;
-        }
-        sum = warp_sum(sum) + 1e-20f;
-        if (lane == 0) {
-            s_m[warp] = mx;
-            s_l[warp] = sum;
-        }
-    }
-    __syncthreads();
-
-    // ---- O = P.V from the registers loaded at the top ----
-    float o[8][8];
-#pragma unroll
-    for (int h = 0; h < 8; ++h)
-#pragma unroll
-        for (int i = 0; i < 8; ++i) o[h][i] = 0.f;
-#pragma unroll
-    for (int u = 0; u < VU; ++u) {
-        const int kk = sub + u * NSUB;
-        if (kk < n) {
-            float vf[8];
-            unpack8<T>(vv[u], vf);
-#pragma unroll
-            for (int h = 0; h < 8; ++h) {
-                if (h < mq) {
-                    const float p = s_logit[h * kShortRowStride + kk];
-#pragma unroll
-                    for (int i = 0; i < 8; ++i) o[h][i] = fmaf(p, vf[i], o[h][i]);
-                }
-            }
-        }
-    }
-#pragma unroll
-    for (int h = 0; h < 8; ++h)
-#pragma unroll
-        for (int i = 0; i < 8; ++i) {
-            float v = o[h][i];
-#pragma unroll
-            for (int off = DC; off < 32; off <<= 1) v += __shfl_xor_sync(0xffffffffu, v, off);
-            o[h][i] = v;
-        }
-    if (lane < DC) {
-#pragma unroll
-        for (int h = 0; h < 8; ++h)
-            if (h < mq) {
-#pragma unroll
-                for (int i = 0; i < 8; ++i) s_red[(warp * 8 + h) * D + lane * 8 + i] = o[h][i];
-            }
-    }
-    __syncthreads();
-    for (int e = tid; e < mq * D; e += kShortThreads) {
-        const int h = e / D, d = e % D;
-        float v = 0.f;
-#pragma unroll
-        for (int w = 0; w < kShortWarps; ++w) v += s_red[(w * 8 + h) * D + d];
-        v = v / s_l[h];
-        const size_t vh = (size_t)bq * num_heads + head0 + h;
-        if (num_splits == 1) {
-            out[vh * D + d] = from_f32<T>(v);
-        } else {
-            part_o[(vh * num_splits + split) * D + d] = v;
-            if (d == 0) {
-                part_m[vh * num_splits + split] = s_m[h];
-                part_l[vh * num_splits + split] = s_l[h];
-            }
-        }
-    }
-}
 
 }  // namespace zl

@@ -7,8 +7,6 @@
 // B fragments makes every load a contiguous 16 bytes (see DESIGN.md section 4.2).
 #include "common.cuh"
 
-#include <cstdlib>
-
 extern unsigned long long* g_w4_trace;   // debug timeline buffer (zl_w4_set_trace), see w4a16_gemm_v3.cu
 
 namespace zl {
@@ -224,8 +222,6 @@ extern "C" int zl_dense_gemm_skinny(const void* x, int ldx, const void* w, const
     ZL_CHECK_SUPPORTED(K % 32 == 0);
     ZL_CHECK_ARG(ldx >= K && ldx % 8 == 0);
     ZL_CHECK_ARG((reinterpret_cast<uintptr_t>(x) & 15) == 0 && (reinterpret_cast<uintptr_t>(w) & 15) == 0);
-    static const bool no_pdl = getenv("ZL_DENSE_NO_PDL") != nullptr;   // experiment knob
-    if (no_pdl) pdl = 0;
     for (int m0 = 0; m0 < M; m0 += 32) {
         const int mc = (M - m0) < 32 ? (M - m0) : 32;
         const bool use_pdl = pdl != 0 && m0 == 0;

@@ -367,14 +367,8 @@ int to_k_major(zl_llama* m, const std::string& prefix, int K, int N, uint32_t* q
     return ZL_OK;
 }
 
-// ZL_W4_FORCE_HALF (A/B baseline): every W4 GEMM takes the fp16 mma.sync route.  Read once per process.
-bool force_half() {
-    static const bool v = getenv("ZL_W4_FORCE_HALF") != nullptr;
-    return v;
-}
-
 // The kernel that serves a W4 Linear at B rows: 3 exact-integer, 4 wgmma, 0 fp16 mma.sync.
-int route_of(const W4Lin& w, int B) { return w.packed_i && !force_half() ? zl_w4_int_layout_route(B, w.N, w.K) : 0; }
+int route_of(const W4Lin& w, int B) { return w.packed_i ? zl_w4_int_layout_route(B, w.N, w.K) : 0; }
 
 // The (N) fp16 bias of Linears fused along N: zeros, with each present `prefix.bias` at its row offset.  *out stays
 // empty when none has one.  Every staged bias is checked before the first copy.
@@ -466,7 +460,7 @@ int build_w4(zl_llama* m, const std::vector<std::string>& prefixes, const std::v
     // the ZLW4I layout serves the exact-integer kernel (M <= 16 when its staged activations fit) and the wgmma kernel
     // (any M, N % 128 == 0); the fp16 mma.sync layout is only materialised when some launch size has neither
     const int m_max = m->cfg.prefill_chunk > m->cfg.max_batch ? m->cfg.prefill_chunk : m->cfg.max_batch;
-    bool need_half = force_half();
+    bool need_half = false;
     for (int mm = 1; mm <= (m_max < 17 ? m_max : 17); ++mm)
         if (!zl_w4_int_layout_route(mm, N, K)) need_half = true;
     RCHECK(dmalloc(&out->packed_i, pbytes));
@@ -846,10 +840,10 @@ static size_t l2_whole_max() {
     return (size_t)v << 20;
 }
 
-// The launches of the decode chain, in order.  ZL_NO_PDL_MASK (experiments): bit 1 << stage launches that stage with a full
-// dependency instead of a programmatic one (1 qkv GEMM, 2 attention, 4 o GEMM, 8 gate_up GEMM, 16 down GEMM, 32 final
+// The launches of the decode chain, in order.  The stages whose bit (1 << stage) is set in the mask below launch with a
+// full dependency instead of a programmatic one (1 qkv GEMM, 2 attention, 4 o GEMM, 8 gate_up GEMM, 16 down GEMM, 32 final
 // norm, 64 lm_head, 128 argmax / sampler).
-// Single GPU, default 66 = lm_head + attention (a PDL-launched lm_head measured much slower, tools/gpu_tail.sh): on an
+// Single GPU, 66 = lm_head + attention (a PDL-launched lm_head measured much slower): on an
 // H100 80GB HBM3 at 400 W, Llama-3.1-8B batch-1 decode measured 425.8 tok/s (425.6-426.2 over 5 runs) against 413.2
 // (412.5-415.2) with the o GEMM also fully dependent (70), 420 with attention PDL-launched too (64), and 400-405 with
 // lm_head PDL-launched (2, 0)
@@ -858,12 +852,7 @@ static size_t l2_whole_max() {
 enum Stage { kQkv, kAttn, kO, kGateUp, kDown, kFinalNorm, kLmHead, kPick };
 
 static int stage_pdl(const zl_llama* m, Stage s) {
-    static int mask = -2;
-    if (mask == -2) {
-        const char* e = getenv("ZL_NO_PDL_MASK");
-        mask = e ? atoi(e) : -1;
-    }
-    const int npm = mask >= 0 ? mask : m->cfg.tp_size > 1 ? 68 : 66;
+    const int npm = m->cfg.tp_size > 1 ? 68 : 66;
     return (npm >> s & 1) ? 0 : m->cfg.use_pdl;
 }
 

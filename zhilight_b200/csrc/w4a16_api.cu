@@ -26,17 +26,10 @@ extern "C" int zl_prepare(void) {
     return prepare_sample();
 }
 
-// ZL_W4_NO_TC=1 (experiments): never route to the wgmma kernel
-static bool tc_disabled() {
-    static int v = -1;
-    if (v < 0) v = getenv("ZL_W4_NO_TC") ? 1 : 0;
-    return v != 0;
-}
-
 // which kernel serves (M, N, K) on the ZLW4I layout: 3 = exact-integer mma.sync, 4 = wgmma, 0 = neither
 static int int_layout_route(int M, int N, int K) {
     if (M <= 16 && w4_v3_fits(M, N, K)) return 3;
-    if (!tc_disabled() && w4_tc_supports(M < 256 ? M : 256, N, K)) return 4;
+    if (w4_tc_supports(M < 256 ? M : 256, N, K)) return 4;
     return 0;
 }
 

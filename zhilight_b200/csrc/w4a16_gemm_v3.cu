@@ -21,8 +21,6 @@
 #include "comm_dev.cuh"
 #include "kv8_quant.cuh"
 
-#include <cstdlib>
-
 namespace zl {
 
 __device__ __forceinline__ void imma_u8s8(int (&d)[4], const uint32_t (&a)[4], uint32_t b0, uint32_t b1) {
@@ -43,8 +41,8 @@ __device__ __forceinline__ void imma_u8u8(int (&d)[4], const uint32_t (&a)[4], u
 // reduction), while the integer decomposition of the activations is staged ONCE per CTA by all warps together:
 //   wide : SUBS=2 x 8 warps, 5-stage rings  (N/32 > #SMs: qkv, gate/up)  -- two tile pipelines per SM
 //   tall : SUBS=1 x 16 warps, 4-stage rings (N/32 <= #SMs: o_proj, down) -- k split 16 ways
-// RT = token rows kept in the split-k reduction buffers (even, >= mc): small batches shrink them to make room for
-// deeper rings -- the tile loop is latency-bound on ring depth (4 -> 5 stages is worth ~25 %).
+// RT = token rows kept in the split-k reduction buffers (>= mc; every launched variant keeps NT * 8).  The tile loop is
+// latency-bound on ring depth (4 -> 5 stages is worth ~25 %).
 __host__ __device__ constexpr int v3_smem_fixed(int NT, int WARPS, int SUBS, int STAGES, int RT) {
     return (WARPS * SUBS * STAGES * (kW4BlockBytes + 8) + SUBS * ((NT == 1) ? 2 : 1) * WARPS * RT * 32 * 4 +
             2 * WARPS * SUBS * NT * 8 * 4 + 2 * NT * 8 * 4 + 127) & ~127;
@@ -854,51 +852,19 @@ static cudaError_t v3_run(const W4Params& p, const V3Plan& pl, bool pdl, cudaStr
                   : launch_v3_t<NT, false, WARPS, SUBS, STAGES, RT, false>(p, pl, pdl, stream);
 }
 
-static int v3_max_stages() {
-    static int v = -1;
-    if (v < 0) {
-        // deeper rings only add HBM
-        // queueing, so the 6-stage variants stay opt-in
-        const char* e = getenv("ZL_W4_STAGES");
-        v = e ? atoi(e) : 4;
-    }
-    return v;
-}
-
-static bool v3_sub_major() {
-    static int v = -1;
-    if (v < 0) {
-        const char* e = getenv("ZL_W4_SUB_MAJOR");
-        v = e ? atoi(e) != 0 : 1;
-    }
-    return v != 0;
-}
-
-static bool v3_is_tall(int N, int G, int sm_count) {
-    static int force = -1;
-    if (force < 0) {
-        const char* e = getenv("ZL_W4_TALL");
-        force = e ? atoi(e) : 0;
-    }
-    if (force == 1) return G >= 32;
-    if (force == 2) return false;
-    return N / 32 <= sm_count && G >= 32;
-}
-
 // The one place that picks the v3 variant: launch_w4_v3 runs exactly this plan, and the L2 head of a successor launch
 // (w4_v3_l2_head) is computed from it.
 bool w4_v3_plan(int mc, int N, int K, int tp_mode, int sm_count, V3Plan* plan) {
     if (mc < 1 || N <= 0 || K <= 0 || N % 32 || K % kW4GroupK || sm_count < 1) return false;
     const int G = K / kW4GroupK;
-    const bool tall = v3_is_tall(N, G, sm_count);
-    static const bool no_one = getenv("ZL_W4_NO_ONE") != nullptr;
+    const bool tall = N / 32 <= sm_count && G >= 32;
     auto fits = [&](int nt, int warps, int subs, int stages, int rt) {
         const int smem = v3_smem_fixed(nt, warps, subs, stages, rt) + v3_stage_bytes(mc, K);
         if (G > 8 * warps * subs || smem > kV3Budget || mc > rt) return false;   // 8 = kMaxNg
         // sub-major tile order (two sub-CTAs): one CTA per SM up to one per tile, every SM busy
-        const int sub_major = subs > 1 && v3_sub_major();
+        const int sub_major = subs > 1;
         const int want = sub_major ? N / 32 : (N / 32 + subs - 1) / subs;
-        *plan = V3Plan{nt, warps, subs, stages, rt, nt == 1 && rt == nt * 8 && mc <= 4 && !no_one,
+        *plan = V3Plan{nt, warps, subs, stages, rt, nt == 1 && rt == nt * 8 && mc <= 4,
                        want < sm_count ? want : sm_count, smem, sub_major};
         return true;
     };
@@ -906,15 +872,6 @@ bool w4_v3_plan(int mc, int N, int K, int tp_mode, int sm_count, V3Plan* plan) {
         if (mc <= 8) return (tall && fits(1, 16, 1, 4, 8)) || fits(1, 8, 2, 4, 8);
         if (mc <= 16) return (tall && fits(2, 16, 1, 4, 16)) || fits(2, 8, 2, 4, 16);
         return false;
-    }
-    if (mc <= 2) {   // deepest ring that fits (reduction buffers shrunk to 2 token rows)
-        const int ms = v3_max_stages();
-        if (tall) {
-            if (ms >= 6 && fits(1, 16, 1, 6, 2)) return true;
-            if (ms >= 5 && fits(1, 16, 1, 5, 2)) return true;
-        } else {
-            if (ms >= 6 && fits(1, 8, 2, 6, 2)) return true;
-        }
     }
     if (mc <= 8) return (tall && fits(1, 16, 1, 4, 8)) || fits(1, 8, 2, 5, 8) || fits(1, 8, 2, 4, 8);
     if (mc <= 16) return (tall && fits(2, 16, 1, 4, 16)) || fits(2, 8, 2, 4, 16);
@@ -930,7 +887,6 @@ bool launch_w4_v3(const W4Params& p, bool pdl, cudaStream_t stream, cudaError_t*
         *err = v3_run<NT, W, SB, ST, RT>(p, pl, pdl, stream);                                                  \
         return true;                                                                                           \
     }
-    ZL_V3(1, 16, 1, 6, 2) ZL_V3(1, 16, 1, 5, 2) ZL_V3(1, 8, 2, 6, 2)
     ZL_V3(1, 16, 1, 4, 8) ZL_V3(1, 8, 2, 5, 8) ZL_V3(1, 8, 2, 4, 8)
     ZL_V3(2, 16, 1, 4, 16) ZL_V3(2, 8, 2, 4, 16)
 #undef ZL_V3
@@ -1031,12 +987,6 @@ cudaError_t prepare_w4_v3() {
     ZL_SET1(false, 8, 2, 5) ZL_SET1(true, 8, 2, 5) ZL_SET1(false, 8, 2, 4) ZL_SET1(true, 8, 2, 4)
     ZL_SET1(false, 16, 1, 4) ZL_SET1(true, 16, 1, 4)
 #undef ZL_SET1
-#define ZL_SET2(NORM, W, SB, ST)                                                                               \
-    e = v3_set_smem<1, NORM, W, SB, ST, 2>();                                                                  \
-    if (e != cudaSuccess) return e;
-    ZL_SET2(false, 16, 1, 6) ZL_SET2(true, 16, 1, 6) ZL_SET2(false, 16, 1, 5) ZL_SET2(true, 16, 1, 5)
-    ZL_SET2(false, 8, 2, 6) ZL_SET2(true, 8, 2, 6)
-#undef ZL_SET2
     ZL_SET(1, false, 8, 2, 5) ZL_SET(1, true, 8, 2, 5) ZL_SET(1, false, 8, 2, 4) ZL_SET(1, true, 8, 2, 4)
     ZL_SET(1, false, 16, 1, 4) ZL_SET(1, true, 16, 1, 4)
     ZL_SET(2, false, 8, 2, 4) ZL_SET(2, true, 8, 2, 4) ZL_SET(2, false, 16, 1, 4) ZL_SET(2, true, 16, 1, 4)

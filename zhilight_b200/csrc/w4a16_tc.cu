@@ -32,7 +32,6 @@
 #include "w4_params.h"
 #include "tc_common.cuh"
 
-#include <cstdlib>
 #include <map>
 #include <mutex>
 #include <tuple>
@@ -423,34 +422,23 @@ extern "C" int zl_w4_tc_schedule(int n_tiles, int G, int ctas, int cta, int* out
     return sch.n_segs;
 }
 
-// grid override: ZL_TC_CTAS in the environment, or zl_w4_tc_set_splits(n) = "at least n pieces per tile" (tests exercise
-// the partial-tile exchange on small shapes); 0 = automatic
-static int g_tc_splits = -2;
-static int tc_force_splits() {
-    if (g_tc_splits == -2) {
-        const char* e = getenv("ZL_TC_SPLITS");
-        g_tc_splits = e ? atoi(e) : 0;
-    }
-    return g_tc_splits;
-}
+// grid override: zl_w4_tc_set_splits(n) = "at least n pieces per tile" (tests exercise the partial-tile exchange on small
+// shapes); 0 = automatic
+static int g_tc_splits = 0;
 extern "C" int zl_w4_tc_set_splits(int splits) {
     g_tc_splits = splits < 0 ? 0 : splits;
     return ZL_OK;
 }
 
-// number of CTAs: every SM when each gets at least kMinUnits (tile, group) units, fewer for small GEMMs (every extra piece
+// number of CTAs: every SM when each gets at least min_units (tile, group) units, fewer for small GEMMs (every extra piece
 // of a tile is an fp32 round trip through L2 for its last arriver)
 static int tc_pick_ctas(int n_tiles, int G) {
-    static const int env_ctas = getenv("ZL_TC_CTAS") ? atoi(getenv("ZL_TC_CTAS")) : 0;
-    static const int min_units = getenv("ZL_TC_MIN_UNITS") ? atoi(getenv("ZL_TC_MIN_UNITS")) : 8;
+    constexpr int min_units = 8;
     const int sms = device_sm_count();
     const long long U = (long long)n_tiles * G;
     long long P = sms;
-    const int forced = tc_force_splits();
-    if (env_ctas > 0) {
-        P = env_ctas;
-    } else if (forced > 0) {
-        P = (long long)n_tiles * forced;
+    if (g_tc_splits > 0) {
+        P = (long long)n_tiles * g_tc_splits;
     } else if (U / P < min_units) {
         P = U / min_units;
         if (P < n_tiles) P = n_tiles;

@@ -19,8 +19,6 @@
 // every block the QMMA sum is folded into an fp32 sum times sx[kb, token] * sw[row / 128, kb].
 #include "common.cuh"
 
-#include <cstdlib>
-
 namespace zl {
 // wgmma W8A8 kernel (w8_tc.cu)
 bool w8_tc_supports(int N, int K);
@@ -440,8 +438,7 @@ static cudaError_t launch_w8(const uint8_t* xq, const float* sx, const uint8_t* 
 // wgmma kernel, skinny(m0, mc, pdl) on the mma.sync kernel (mc <= 32); only the first launch is PDL-launched.
 template <typename TcFn, typename SkinnyFn>
 static int w8_route(int M, int N, int K, int pdl, TcFn tc, SkinnyFn skinny) {
-    static const int tc_min_m = getenv("ZL_W8_TC_MIN_M") ? atoi(getenv("ZL_W8_TC_MIN_M")) : 33;
-    if (M >= tc_min_m && w8_tc_supports(N, K)) {
+    if (M > 32 && w8_tc_supports(N, K)) {
         static bool prepared[64] = {};   // zl_prepare() once per device: split-k workspace, opt-in shared memory
         int dev = 0;
         cudaGetDevice(&dev);

@@ -5,7 +5,7 @@
 // Replaces Int8Linear::forward = quant_calc_scale + cuBLASLt s32 GEMM (M padded to 32) + quant_scale_back
 // (reference src/nn/linear/linear.cpp:560-636, src/nn/quant/int8/quant_kernel.cu:231-306) and Fp8Linear::forward's
 // cuBLASLt fp8 GEMM (linear.cpp:1660-1695) for every M (decode and prefill chunks); the mma.sync kernel k_w8a8_skinny
-// (w8_linear.cu) stays as the fallback for K % 128 != 0 and as the A/B baseline (ZL_W8_NO_TC=1).
+// (w8_linear.cu) serves M <= 32 and K % 128 != 0 (w8_route).
 //
 // One CTA per SM, persistent over work items (128 weight rows x a k-slice); 9 warps:
 //   warps 0-7  consumers : two warpgroups, warpgroup r owns weight rows 64 r .. 64 r + 63 of the tile and all NTOK tokens:
@@ -17,7 +17,6 @@
 #include "common.cuh"
 #include "tc_common.cuh"
 
-#include <cstdlib>
 #include <type_traits>
 
 namespace zl {
@@ -259,8 +258,7 @@ static int w8_pick_splits(int n_tiles, int KS, int mc, size_t ws_bytes) {
 }
 
 bool w8_tc_supports(int N, int K) {
-    static const bool off = getenv("ZL_W8_NO_TC") != nullptr;
-    return !off && K % 128 == 0 && N >= 1 && (N + kTcRows - 1) / kTcRows <= kTcMaxTiles;
+    return K % 128 == 0 && N >= 1 && (N + kTcRows - 1) / kTcRows <= kTcMaxTiles;
 }
 
 template <typename T, bool FP8, int NTOK, bool BLK>

@@ -10,20 +10,10 @@
 // exact two-pass fp32 form inside the split (mask ? scale*s : -inf, max seeded -1e20, sum seeded 1e-20);
 // P.V runs on the tensor cores too, with fp32 accumulators.
 // Splits are merged with the reference's LSE rule (attention_kernel.cu:881-923).
-#include "common.cuh"
-#include "attn_combine.cuh"
-#include "decode_attn_short.cuh"
+#include "attn_common.cuh"
 #include "decode_attn_warp.cuh"
 
-#include <type_traits>
-
 namespace zl {
-
-constexpr int kAttnThreads = 128;
-constexpr int kAttnWarps = 4;
-constexpr int kAttnMaxRange = 1024;            // keys per CTA; logits live in shared memory
-constexpr int kAttnRowStride = kAttnMaxRange + 4;
-constexpr int kAttnMaxSplits = 64;
 
 template <typename T, int D>
 __global__ void __launch_bounds__(kAttnThreads)
@@ -38,42 +28,19 @@ k_decode_attn(const T* __restrict__ q, const int32_t* __restrict__ buf_lens, T* 
 
     const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
     const int g = lane >> 2, t = lane & 3;
-    const int hgroups = (m_query + 7) / 8;
-    const int split = blockIdx.x;
-    const int hk = blockIdx.y / hgroups, hg = blockIdx.y % hgroups;
-    const int bq = blockIdx.z, b = bq / len_q, qi = bq % len_q;
-    const int mq0 = hg * 8;
-    const int mq = min(8, m_query - mq0);
-    const int head0 = hk * m_query + mq0;
 
-    pdl_trigger();
-    pdl_wait();
-
-    const int len_buf = buf_lens[b];
-    const int chunk = attn_round16((len_buf + num_splits - 1) / num_splits);
-    const int k0 = split * chunk;
-    const int k1 = min(len_buf, k0 + chunk);
-    const int n = max(0, k1 - k0);
+    const DecodeAttnItem cta = decode_attn_prologue(buf_lens, len_q, m_query, num_splits);
+    const int mq = cta.mq, k0 = cta.k0, k1 = cta.k1, n = max(0, k1 - k0);
 
     const size_t stride = bshd ? (size_t)num_kv_heads * D : (size_t)D;
-    const size_t base = bshd ? (size_t)hk * D : (size_t)hk * len_buf * D;
-    const T* kbase = k_addrs[b] + base;
-    const T* vbase = v_addrs[b] + base;
-
-    const int8_t* mrow = nullptr;
-    if (mask) {
-        size_t len_off = 0;
-        for (int j = 0; j < b; ++j) len_off += buf_lens[j];
-        mrow = mask + (size_t)len_q * len_off + (size_t)qi * len_buf;
-    }
+    const size_t base = bshd ? (size_t)cta.hk * D : (size_t)cta.hk * cta.len_buf * D;
+    const T* kbase = k_addrs[cta.b] + base;
+    const T* vbase = v_addrs[cta.b] + base;
+    const int8_t* mrow = cta.mask_row(mask, buf_lens, len_q);
 
     // ---- phase 1: S = K.Q^T on tensor cores ----
     uint4 qf[NI];
-#pragma unroll
-    for (int i = 0; i < NI; ++i) {
-        qf[i] = (g < mq) ? ld_cg_u4(q + ((size_t)bq * num_heads + head0 + g) * D + i * 32 + t * 8)
-                         : make_uint4(0, 0, 0, 0);
-    }
+    decode_attn_load_q<D>(qf, q, cta, num_heads, g, t);
     const int ntiles = (n + 15) >> 4;
     for (int tile = warp; tile < ntiles; tile += kAttnWarps) {
         const int ka_i = k0 + tile * 16 + g, kb_i = ka_i + 8;
@@ -129,10 +96,9 @@ k_decode_attn(const T* __restrict__ q, const int32_t* __restrict__ buf_lens, T* 
     __syncthreads();
 
     // ---- phase 3: O = P.V on the tensor cores (mma.sync m16n8k16, fp32 accumulate) ----
-    // A = P [head (8 of 16 rows) x 16 keys]: fp16 models carry p * 2^10 in fp16 (11 significant bits, no subnormals); bf16
-    // models carry p as bf16 hi + lo (two MMAs), so that the product keeps ~16 bits of p.  B = V [16 keys x 8 columns]: a B
-    // register holds TWO KEYS of one column while V is key-major, so lane (g, t) loads D/8 contiguous elements (columns
-    // NJ g ..) of its four keys 2t, 2t+1, 2t+8, 2t+9 and interleaves row pairs with PRMT; n-tile j column c stands for column
+    // A = P [head (8 of 16 rows) x 16 keys], encoded by attn_pack_p.  B = V [16 keys x 8 columns]: a B register holds
+    // TWO KEYS of one column while V is key-major, so lane (g, t) loads D/8 contiguous elements (columns NJ g ..) of its
+    // four keys 2t, 2t+1, 2t+8, 2t+9 and interleaves row pairs with PRMT; n-tile j column c stands for column
     // d = NJ c + j of V (a permutation of the columns, undone when the accumulators are written out).
     constexpr int NJ = D / 8;                 // n-tiles = V columns per lane and key row
     constexpr int NW = NJ / 2;                // 32-bit words of a lane's column chunk (2 elements each)
@@ -164,19 +130,8 @@ k_decode_attn(const T* __restrict__ q, const int32_t* __restrict__ buf_lens, T* 
             const float2 p0 = *reinterpret_cast<const float2*>(pr), p1 = *reinterpret_cast<const float2*>(pr + 8);
             const float q0 = kb + 2 * t < n ? p0.x : 0.f, q1 = kb + 2 * t + 1 < n ? p0.y : 0.f;
             const float q2 = kb + 2 * t + 8 < n ? p1.x : 0.f, q3 = kb + 2 * t + 9 < n ? p1.y : 0.f;
-            if constexpr (kHalf) {
-                const __half2 h0 = __floats2half2_rn(q0 * 1024.f, q1 * 1024.f), h1 = __floats2half2_rn(q2 * 1024.f, q3 * 1024.f);
-                af[0] = *reinterpret_cast<const uint32_t*>(&h0);
-                af[2] = *reinterpret_cast<const uint32_t*>(&h1);
-            } else {
-                const __nv_bfloat162 h0 = __floats2bfloat162_rn(q0, q1), h1 = __floats2bfloat162_rn(q2, q3);
-                const float2 f0 = __bfloat1622float2(h0), f1 = __bfloat1622float2(h1);
-                const __nv_bfloat162 l0 = __floats2bfloat162_rn(q0 - f0.x, q1 - f0.y), l1 = __floats2bfloat162_rn(q2 - f1.x, q3 - f1.y);
-                af[0] = *reinterpret_cast<const uint32_t*>(&h0);
-                af[2] = *reinterpret_cast<const uint32_t*>(&h1);
-                al[0] = *reinterpret_cast<const uint32_t*>(&l0);
-                al[2] = *reinterpret_cast<const uint32_t*>(&l1);
-            }
+            attn_pack_p<T>(q0, q1, af[0], al[0]);
+            attn_pack_p<T>(q2, q3, af[2], al[2]);
         }
 #pragma unroll
         for (int w = 0; w < NW; ++w) {
@@ -199,39 +154,7 @@ k_decode_attn(const T* __restrict__ q, const int32_t* __restrict__ buf_lens, T* 
         }
     }
     __syncthreads();
-    for (int e = tid; e < mq * D; e += kAttnThreads) {
-        const int h = e / D, d = e % D;
-        float v = 0.f;
-#pragma unroll
-        for (int w = 0; w < kAttnWarps; ++w) v += s_red[(w * 8 + h) * D + d];
-        v = v / s_l[h];
-        const size_t vh = (size_t)bq * num_heads + head0 + h;
-        if (num_splits == 1) {
-            out[vh * D + d] = from_f32<T>(v);
-        } else {
-            part_o[(vh * num_splits + split) * D + d] = v;
-            if (d == 0) {
-                part_m[vh * num_splits + split] = s_m[h];
-                part_l[vh * num_splits + split] = s_l[h];
-            }
-        }
-    }
-}
-
-
-// k_attn_combine (attn_combine.cuh): grid (B*len_q*num_heads), block D
-
-static int attn_num_splits(int B, int len_q, int num_kv_heads, int m_query, int max_len_buf) {
-    const int hgroups = (m_query + 7) / 8;
-    const int base = B * len_q * num_kv_heads * hgroups;
-    const int min_splits = cdiv(max_len_buf, kAttnMaxRange);
-    const int want = cdiv(2 * device_sm_count(), base);
-    const int max_useful = cdiv(max_len_buf, 256) > 0 ? cdiv(max_len_buf, 256) : 1;   // >= 256 keys per split
-    int s = want < max_useful ? want : max_useful;
-    if (s > kAttnMaxSplits) s = kAttnMaxSplits;
-    if (s < min_splits) s = min_splits;
-    if (s < 1) s = 1;
-    return s;
+    decode_attn_reduce_store<T, D>(cta, s_red, s_m, s_l, num_heads, num_splits, out, part_o, part_m, part_l);
 }
 
 }  // namespace zl
@@ -243,7 +166,7 @@ extern "C" size_t zl_decode_attention_workspace_bytes(int B, int len_q, int num_
     if (B <= 0 || len_q <= 0 || num_heads <= 0 || dim_head <= 0) return 0;
     int splits = cdiv(max_len_buf > 0 ? max_len_buf : 1, kAttnMaxRange);
     if (splits < kAttnMaxSplits) splits = kAttnMaxSplits;
-    return (size_t)B * len_q * num_heads * splits * (dim_head + 2) * sizeof(float);
+    return attn_parts_bytes((size_t)B * len_q * num_heads, splits, dim_head);
 }
 
 extern "C" int zl_decode_attention(const void* q, const int32_t* buf_lens, void* const* k_addrs,
@@ -258,38 +181,27 @@ extern "C" int zl_decode_attention(const void* q, const int32_t* buf_lens, void*
     const int m_query = num_heads / num_kv_heads;
     int splits = attn_num_splits(B, len_q, num_kv_heads, m_query, max_len_buf);
     // latency regime: few CTAs of work -> 256-key splits on the warp-per-32-keys kernel (one __syncthreads per CTA)
-    const int hg0 = (m_query + 7) / 8;
+    const int hgroups = (m_query + 7) / 8;
     const int short_splits = cdiv(max_len_buf, kShortRange);
     const bool use_short = short_splits <= kAttnMaxSplits &&
-                           (long long)B * len_q * num_kv_heads * hg0 * short_splits <= 4 * device_sm_count();
+                           (long long)B * len_q * num_kv_heads * hgroups * short_splits <= 4 * device_sm_count();
     if (use_short) splits = short_splits;
     const size_t vheads = (size_t)B * len_q * num_heads;
-    float* part_o = nullptr;
-    float* part_m = nullptr;
-    float* part_l = nullptr;
-    if (splits > 1) {
-        const size_t need = vheads * splits * (dim_head + 2) * sizeof(float);
-        ZL_CHECK_ARG(workspace != nullptr && workspace_bytes >= need);
-        part_o = static_cast<float*>(workspace);
-        part_m = part_o + vheads * splits * dim_head;
-        part_l = part_m + vheads * splits;
-    }
-    const int hgroups = (m_query + 7) / 8;
+    if (splits > 1) ZL_CHECK_ARG(workspace != nullptr && workspace_bytes >= attn_parts_bytes(vheads, splits, dim_head));
+    const AttnParts part = attn_parts(workspace, vheads, splits, dim_head);
     dim3 grid(splits, num_kv_heads * hgroups, B * len_q), block(kAttnThreads);
 #define ZL_ATTN_LAUNCH(TT, DD)                                                                                  \
     if (use_short) {                                                                                            \
         ZL_CHECK_CUDA(launch(k_decode_attn_warp<TT, DD>, grid, dim3(kWarpAttnWarps * 32),                       \
                              (size_t)warp_attn_smem_floats<DD>() * sizeof(float), stream, pdl != 0, (const TT*)q, \
-                             buf_lens, (TT* const*)k_addrs, (TT* const*)v_addrs, mask, scale, (TT*)out, part_o, \
-                             part_m, part_l, len_q, num_heads, num_kv_heads, m_query, splits, bshd));            \
+                             buf_lens, (TT* const*)k_addrs, (TT* const*)v_addrs, mask, scale, (TT*)out, part.o, \
+                             part.m, part.l, len_q, num_heads, num_kv_heads, m_query, splits, bshd));            \
     } else {                                                                                                    \
         ZL_CHECK_CUDA(launch(k_decode_attn<TT, DD>, grid, block, 0, stream, pdl != 0, (const TT*)q, buf_lens,   \
-                             (TT* const*)k_addrs, (TT* const*)v_addrs, mask, scale, (TT*)out, part_o, part_m,   \
-                             part_l, len_q, num_heads, num_kv_heads, m_query, splits, bshd));                   \
+                             (TT* const*)k_addrs, (TT* const*)v_addrs, mask, scale, (TT*)out, part.o, part.m,   \
+                             part.l, len_q, num_heads, num_kv_heads, m_query, splits, bshd));                   \
     }                                                                                                           \
-    if (splits > 1)                                                                                             \
-        ZL_CHECK_CUDA(launch(k_attn_combine<TT>, dim3((unsigned)vheads), dim3(DD), 0, stream, pdl != 0,         \
-                             (const float*)part_o, (const float*)part_m, (const float*)part_l, (TT*)out, splits));
+    ZL_CHECK_CUDA(launch_attn_combine(part, vheads, DD, (TT*)out, splits, stream, pdl != 0));
     if (dtype == ZL_F16) {
         if (dim_head == 128) { ZL_ATTN_LAUNCH(__half, 128) } else { ZL_ATTN_LAUNCH(__half, 64) }
     } else {

@@ -9,21 +9,14 @@
 // scale buffers (len_buf, H_kv) fp32 = absmax / 127, one scale per (token, kv head).  q is fp16.
 //   logit[key] = scale * scale_k[key] * sum_d q[d] * (k[key, d] - 128)         (mask ? ... : -inf)
 //   out[d]     = sum_key softmax(logit)[key] * scale_v[key] * (v[key, d] - 128)
-// Same CTA decomposition as k_decode_attn (decode_attn.cu): one CTA per (kv split, kv head group, task x query), the whole
-// GQA group shares every cache byte; K bytes become exact fp16 integers (PRMT 0x64xx magic) and feed mma.sync with fp32
-// accumulation -- the reference multiplies and pair-adds in fp16 (quant_attention.cuh:60-70), so ours is the closer one
-// to the exact result.  Half the algorithmic bytes of the fp16 cache: 2 * H_kv * d * ctx + 8 * H_kv * ctx per task per layer.
-#include "common.cuh"
-#include "decode_attn_short.cuh"
+// Same CTA decomposition as k_decode_attn (decode_attn_prologue, attn_common.cuh): one CTA per (kv split, kv head
+// group, task x query), the whole GQA group shares every cache byte; K bytes become exact fp16 integers (PRMT 0x64xx
+// magic) and feed mma.sync with fp32 accumulation -- the reference multiplies and pair-adds in fp16
+// (quant_attention.cuh:60-70), so ours is the closer one to the exact result.  Half the algorithmic bytes of the fp16 cache: 2 * H_kv * d * ctx + 8 * H_kv * ctx per task per layer.
+#include "attn_common.cuh"
 #include "kv8_quant.cuh"
 
 namespace zl {
-
-constexpr int kA8Threads = 128;
-constexpr int kA8Warps = 4;
-constexpr int kA8MaxRange = 1024;
-constexpr int kA8RowStride = kA8MaxRange + 4;
-constexpr int kA8MaxSplits = 64;
 
 // 4 cache bytes -> 4 exact fp16 integers (u8 - 128): 0x64xx = 1024 + x, minus 1152
 __device__ __forceinline__ void u8x4_to_h2x2(uint32_t b, uint32_t& h01, uint32_t& h23) {
@@ -38,65 +31,37 @@ __device__ __forceinline__ float u8_to_f32(uint32_t word, int i) {
     const uint32_t sel = 0x7540u | (uint32_t)i;
     return __uint_as_float(__byte_perm(word, 0x4B000000u, sel)) - 8388736.f;
 }
-__device__ __forceinline__ uint2 ld_cg_b8(const void* p) {
-    uint2 r;
-    asm volatile("ld.global.cg.v2.u32 {%0,%1}, [%2];" : "=r"(r.x), "=r"(r.y) : "l"(p));
-    return r;
-}
 
 template <typename TO, int D>
-__global__ void __launch_bounds__(kA8Threads)
+__global__ void __launch_bounds__(kAttnThreads)
 k_decode_attn_kv8(const __half* __restrict__ q, const int32_t* __restrict__ buf_lens, uint8_t* const* __restrict__ k_addrs,
                   uint8_t* const* __restrict__ v_addrs, float* const* __restrict__ sk_addrs,
                   float* const* __restrict__ sv_addrs, const int8_t* __restrict__ mask, float scale, TO* __restrict__ out,
                   float* __restrict__ part_o, float* __restrict__ part_m, float* __restrict__ part_l, int len_q,
                   int num_heads, int num_kv_heads, int m_query, int num_splits) {
     constexpr int NI = D / 32;                 // 8-byte chunks per lane per key row
-    constexpr int DC = D / 8;                  // threads covering one V row (8 bytes each)
-    constexpr int NSUB = kA8Threads / DC;
-    __shared__ __align__(16) float s_logit[8 * kA8RowStride];
-    __shared__ float s_sv[kA8MaxRange];        // V scales of the split's keys
+    __shared__ __align__(16) float s_logit[8 * kAttnRowStride];
+    __shared__ float s_sv[kAttnMaxRange];      // V scales of the split's keys
     __shared__ float s_m[8], s_l[8], s_w[8];
 
     const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
     const int g = lane >> 2, t = lane & 3;
-    const int hgroups = (m_query + 7) / 8;
-    const int split = blockIdx.x;
-    const int hk = blockIdx.y / hgroups, hg = blockIdx.y % hgroups;
-    const int bq = blockIdx.z, b = bq / len_q, qi = bq % len_q;
-    const int mq0 = hg * 8;
-    const int mq = min(8, m_query - mq0);
-    const int head0 = hk * m_query + mq0;
 
-    pdl_trigger();
-    pdl_wait();
-
-    const int len_buf = buf_lens[b];
-    const int chunk = attn_round16((len_buf + num_splits - 1) / num_splits);
-    const int k0 = split * chunk;
-    const int k1 = min(len_buf, k0 + chunk);
-    const int n = max(0, k1 - k0);
+    const DecodeAttnItem cta = decode_attn_prologue(buf_lens, len_q, m_query, num_splits);
+    const int hk = cta.hk, mq = cta.mq, k0 = cta.k0, k1 = cta.k1, n = max(0, k1 - k0);
 
     const size_t stride = (size_t)num_kv_heads * D;          // BSHD, bytes
-    const uint8_t* kbase = k_addrs[b] + (size_t)hk * D;
-    const uint8_t* vbase = v_addrs[b] + (size_t)hk * D;
-    const float* skb = sk_addrs[b] + hk;                      // (len_buf, H_kv)
-    const float* svb = sv_addrs[b] + hk;
-
-    const int8_t* mrow = nullptr;
-    if (mask) {
-        size_t len_off = 0;
-        for (int j = 0; j < b; ++j) len_off += buf_lens[j];
-        mrow = mask + (size_t)len_q * len_off + (size_t)qi * len_buf;
-    }
+    const uint8_t* kbase = k_addrs[cta.b] + (size_t)hk * D;
+    const uint8_t* vbase = v_addrs[cta.b] + (size_t)hk * D;
+    const float* skb = sk_addrs[cta.b] + hk;                  // (len_buf, H_kv)
+    const float* svb = sv_addrs[cta.b] + hk;
+    const int8_t* mrow = cta.mask_row(mask, buf_lens, len_q);
 
     // ---- phase 1: S = K.Q^T on tensor cores (K bytes -> exact fp16 integers) ----
     uint4 qf[NI];
-#pragma unroll
-    for (int i = 0; i < NI; ++i)
-        qf[i] = (g < mq) ? ld_cg_u4(q + ((size_t)bq * num_heads + head0 + g) * D + i * 32 + t * 8) : make_uint4(0, 0, 0, 0);
+    decode_attn_load_q<D>(qf, q, cta, num_heads, g, t);
     const int ntiles = (n + 15) >> 4;
-    for (int tile = warp; tile < ntiles; tile += kA8Warps) {
+    for (int tile = warp; tile < ntiles; tile += kAttnWarps) {
         const int ka_i = k0 + tile * 16 + g, kb_i = ka_i + 8;
         const int ra = min(ka_i, k1 - 1), rb = min(kb_i, k1 - 1);
         const uint8_t* pa = kbase + (size_t)ra * stride + t * 8;
@@ -104,8 +69,8 @@ k_decode_attn_kv8(const __half* __restrict__ q, const int32_t* __restrict__ buf_
         uint2 ka[NI], kb[NI];
 #pragma unroll
         for (int i = 0; i < NI; ++i) {
-            ka[i] = ld_cg_b8(pa + i * 32);
-            kb[i] = ld_cg_b8(pb + i * 32);
+            ka[i] = ld_cg_u2(pa + i * 32);
+            kb[i] = ld_cg_u2(pb + i * 32);
         }
         const float sa = __ldcg(skb + (size_t)ra * num_kv_heads), sb = __ldcg(skb + (size_t)rb * num_kv_heads);
         if (t == 0) {   // the V scales ride along with the K loads, so that phase 2 reads them from shared memory
@@ -130,20 +95,20 @@ k_decode_attn_kv8(const __half* __restrict__ q, const int32_t* __restrict__ buf_
         const int la = tile * 16 + g;
         const float ninf = -INFINITY;
         if (2 * t < mq) {
-            s_logit[(2 * t) * kA8RowStride + la] = va ? acc[0] * sa * scale : ninf;
-            s_logit[(2 * t) * kA8RowStride + la + 8] = vb ? acc[2] * sb * scale : ninf;
+            s_logit[(2 * t) * kAttnRowStride + la] = va ? acc[0] * sa * scale : ninf;
+            s_logit[(2 * t) * kAttnRowStride + la + 8] = vb ? acc[2] * sb * scale : ninf;
         }
         if (2 * t + 1 < mq) {
-            s_logit[(2 * t + 1) * kA8RowStride + la] = va ? acc[1] * sa * scale : ninf;
-            s_logit[(2 * t + 1) * kA8RowStride + la + 8] = vb ? acc[3] * sb * scale : ninf;
+            s_logit[(2 * t + 1) * kAttnRowStride + la] = va ? acc[1] * sa * scale : ninf;
+            s_logit[(2 * t + 1) * kAttnRowStride + la + 8] = vb ? acc[3] * sb * scale : ninf;
         }
     }
     __syncthreads();
 
     // ---- phase 2: masked softmax statistics per head; the V scale is folded into the stored weights w = e * scale_v,
     // and s_w keeps the split's largest weight per head (floored at 1e-30 so that 1024 / s_w stays finite) ----
-    for (int h = warp; h < mq; h += kA8Warps) {
-        float* row = s_logit + h * kA8RowStride;
+    for (int h = warp; h < mq; h += kAttnWarps) {
+        float* row = s_logit + h * kAttnRowStride;
         float mx = -1e20f;
         for (int i = lane; i < n; i += 32) mx = fmaxf(mx, row[i]);
         mx = warp_max(mx);
@@ -179,7 +144,7 @@ k_decode_attn_kv8(const __half* __restrict__ q, const int32_t* __restrict__ buf_
     for (int j = 0; j < NJ; ++j) o[j][0] = o[j][1] = o[j][2] = o[j][3] = 0.f;
     const __half2 voff = __float2half2_rn(1152.f);   // 1024 (magic) + 128 (zero point of the cache)
     const float wenc = g < mq ? 1024.f / s_w[g] : 0.f;
-    for (int tile = warp; tile < ntiles; tile += kA8Warps) {
+    for (int tile = warp; tile < ntiles; tile += kAttnWarps) {
         const int kb = tile * 16;                    // first key of the tile, relative to k0
         uint32_t vw[4][NW];
 #pragma unroll
@@ -193,14 +158,14 @@ k_decode_attn_kv8(const __half* __restrict__ q, const int32_t* __restrict__ buf_
                     const uint4 v = ld_cg_u4(src);
                     vw[r][0] = v.x, vw[r][1] = v.y, vw[r][2] = v.z, vw[r][3] = v.w;
                 } else {
-                    const uint2 v = ld_cg_b8(src);
+                    const uint2 v = ld_cg_u2(src);
                     vw[r][0] = v.x, vw[r][1] = v.y;
                 }
             }
         }
         uint32_t af[4] = {0u, 0u, 0u, 0u};
         if (g < mq) {
-            const float* pr = s_logit + g * kA8RowStride + kb + 2 * t;
+            const float* pr = s_logit + g * kAttnRowStride + kb + 2 * t;
             const float2 p0 = *reinterpret_cast<const float2*>(pr), p1 = *reinterpret_cast<const float2*>(pr + 8);
             const bool in0 = kb + 2 * t < n, in1 = kb + 2 * t + 1 < n, in2 = kb + 2 * t + 8 < n, in3 = kb + 2 * t + 9 < n;
             const __half2 h0 = __floats2half2_rn(in0 ? p0.x * wenc : 0.f, in1 ? p0.y * wenc : 0.f);
@@ -235,41 +200,7 @@ k_decode_attn_kv8(const __half* __restrict__ q, const int32_t* __restrict__ buf_
         }
     }
     __syncthreads();
-    for (int e = tid; e < mq * D; e += kA8Threads) {
-        const int h = e / D, d = e % D;
-        float v = 0.f;
-#pragma unroll
-        for (int w = 0; w < kA8Warps; ++w) v += s_red[(w * 8 + h) * D + d];
-        v = v / s_l[h];
-        const size_t vh = (size_t)bq * num_heads + head0 + h;
-        if (num_splits == 1) {
-            out[vh * D + d] = from_f32<TO>(v);
-        } else {
-            part_o[(vh * num_splits + split) * D + d] = v;
-            if (d == 0) {
-                part_m[vh * num_splits + split] = s_m[h];
-                part_l[vh * num_splits + split] = s_l[h];
-            }
-        }
-    }
-}
-
-// grid (B*len_q*num_heads), block D: LSE combine of the splits (attention_kernel.cu:881-923)
-template <typename TO>
-__global__ void k_attn_combine_kv8(const float* __restrict__ part_o, const float* __restrict__ part_m,
-                                   const float* __restrict__ part_l, TO* __restrict__ out, int num_splits) {
-    const int vh = blockIdx.x, D = blockDim.x, d = threadIdx.x;
-    pdl_trigger();
-    pdl_wait();
-    const float* pm = part_m + (size_t)vh * num_splits;
-    const float* pl = part_l + (size_t)vh * num_splits;
-    float gm = -1e20f;
-    for (int i = 0; i < num_splits; ++i) gm = fmaxf(gm, pm[i]);
-    float gs = 0.f;
-    for (int i = 0; i < num_splits; ++i) gs += pl[i] * expf(pm[i] - gm);
-    float res = 0.f;
-    for (int i = 0; i < num_splits; ++i) res += part_o[((size_t)vh * num_splits + i) * D + d] * (pl[i] / gs * expf(pm[i] - gm));
-    out[(size_t)vh * D + d] = from_f32<TO>(res);
+    decode_attn_reduce_store<TO, D>(cta, s_red, s_m, s_l, num_heads, num_splits, out, part_o, part_m, part_l);
 }
 
 // quant_calc_scale(x, 127, 128) of one (token, kv head) row + scatter into the task's cache at placement (BSHD):
@@ -361,34 +292,18 @@ extern "C" int zl_decode_attention_kv8(const void* q, const int32_t* buf_lens, v
     ZL_CHECK_SUPPORTED(dim_head == 128 || dim_head == 64);     // the reference: 128 only (attention_kernel.cu:1314)
     ZL_CHECK_SUPPORTED(out_dtype == ZL_F16 || out_dtype == ZL_BF16);
     const int m_query = num_heads / num_kv_heads;
-    const int hgroups = (m_query + 7) / 8;
-    const int base = B * len_q * num_kv_heads * hgroups;
-    int splits = cdiv(2 * device_sm_count(), base);
-    const int max_useful = cdiv(max_len_buf, 256);
-    if (splits > max_useful) splits = max_useful;
-    if (splits > kA8MaxSplits) splits = kA8MaxSplits;
-    const int min_splits = cdiv(max_len_buf, kA8MaxRange);
-    if (splits < min_splits) splits = min_splits;
-    if (splits < 1) splits = 1;
-    ZL_CHECK_SUPPORTED(splits <= kA8MaxSplits);
+    const int splits = attn_num_splits(B, len_q, num_kv_heads, m_query, max_len_buf);
+    ZL_CHECK_SUPPORTED(splits <= kAttnMaxSplits);
     const size_t vheads = (size_t)B * len_q * num_heads;
-    float *part_o = nullptr, *part_m = nullptr, *part_l = nullptr;
-    if (splits > 1) {
-        const size_t need = vheads * splits * (dim_head + 2) * sizeof(float);
-        ZL_CHECK_ARG(workspace != nullptr && workspace_bytes >= need);
-        part_o = static_cast<float*>(workspace);
-        part_m = part_o + vheads * splits * dim_head;
-        part_l = part_m + vheads * splits;
-    }
-    dim3 grid(splits, num_kv_heads * hgroups, B * len_q), block(kA8Threads);
+    if (splits > 1) ZL_CHECK_ARG(workspace != nullptr && workspace_bytes >= attn_parts_bytes(vheads, splits, dim_head));
+    const AttnParts part = attn_parts(workspace, vheads, splits, dim_head);
+    dim3 grid(splits, num_kv_heads * ((m_query + 7) / 8), B * len_q), block(kAttnThreads);
 #define ZL_A8_LAUNCH(TO, DD)                                                                                         \
     ZL_CHECK_CUDA(launch(k_decode_attn_kv8<TO, DD>, grid, block, 0, stream, pdl != 0, (const __half*)q, buf_lens,    \
                          (uint8_t* const*)k_addrs, (uint8_t* const*)v_addrs, (float* const*)scale_k_addrs,           \
-                         (float* const*)scale_v_addrs, mask, scale, (TO*)out, part_o, part_m, part_l, len_q,         \
+                         (float* const*)scale_v_addrs, mask, scale, (TO*)out, part.o, part.m, part.l, len_q,         \
                          num_heads, num_kv_heads, m_query, splits));                                                 \
-    if (splits > 1)                                                                                                  \
-        ZL_CHECK_CUDA(launch(k_attn_combine_kv8<TO>, dim3((unsigned)vheads), dim3(DD), 0, stream, pdl != 0,          \
-                             (const float*)part_o, (const float*)part_m, (const float*)part_l, (TO*)out, splits));
+    ZL_CHECK_CUDA(launch_attn_combine(part, vheads, DD, (TO*)out, splits, stream, pdl != 0));
     if (out_dtype == ZL_F16) {
         if (dim_head == 128) { ZL_A8_LAUNCH(__half, 128) } else { ZL_A8_LAUNCH(__half, 64) }
     } else {

@@ -8,8 +8,7 @@
 // fp32 exp, sum seeded with 1e-20, o = sum p.v in fp32; the per-warp partial results are merged with the reference's
 // own split rule (KERNEL_mqa_combine), which is exact up to fp32 rounding.
 #pragma once
-#include "common.cuh"
-#include "decode_attn_short.cuh"
+#include "attn_common.cuh"
 
 namespace zl {
 
@@ -36,35 +35,17 @@ k_decode_attn_warp(const T* __restrict__ q, const int32_t* __restrict__ buf_lens
     float* s_o = s_p + 32 * 8;                           // [head 8][D]
     float* s_ml = s_o + 8 * D;                           // m[8], l[8]
 
-    const int hgroups = (m_query + 7) / 8;
-    const int split = blockIdx.x;
-    const int hk = blockIdx.y / hgroups, hg = blockIdx.y % hgroups;
-    const int bq = blockIdx.z, b = bq / len_q, qi = bq % len_q;
-    const int mq0 = hg * 8;
-    const int mq = min(8, m_query - mq0);
-    const int head0 = hk * m_query + mq0;
-
-    pdl_trigger();
-    pdl_wait();
-
-    const int len_buf = buf_lens[b];
-    const int chunk = attn_round16((len_buf + num_splits - 1) / num_splits);   // host guarantees <= kWarpAttnRange
-    const int c0 = split * chunk;
-    const int c1 = min(len_buf, c0 + chunk);
-    const int k0 = c0 + warp * 32;                 // this warp's keys [k0, k1)
-    const int k1 = min(c1, k0 + 32);
+    const DecodeAttnItem cta = decode_attn_prologue(buf_lens, len_q, m_query, num_splits);   // <= kWarpAttnRange keys
+    const int mq = cta.mq;
+    const int k0 = cta.k0 + warp * 32;               // this warp's keys [k0, k1)
+    const int k1 = min(cta.k1, k0 + 32);
     const int n = max(0, k1 - k0);
 
     const size_t stride = bshd ? (size_t)num_kv_heads * D : (size_t)D;
-    const size_t base = bshd ? (size_t)hk * D : (size_t)hk * len_buf * D;
-    const T* kbase = k_addrs[b] + base;
-    const T* vbase = v_addrs[b] + base;
-    const int8_t* mrow = nullptr;
-    if (mask) {
-        size_t len_off = 0;
-        for (int j = 0; j < b; ++j) len_off += buf_lens[j];
-        mrow = mask + (size_t)len_q * len_off + (size_t)qi * len_buf;
-    }
+    const size_t base = bshd ? (size_t)cta.hk * D : (size_t)cta.hk * cta.len_buf * D;
+    const T* kbase = k_addrs[cta.b] + base;
+    const T* vbase = v_addrs[cta.b] + base;
+    const int8_t* mrow = cta.mask_row(mask, buf_lens, len_q);
 
     float m_w[2] = {-1e20f, -1e20f}, l_w[2] = {0.f, 0.f};   // heads 2t, 2t+1 of this lane
     float o[8][8];
@@ -76,9 +57,7 @@ k_decode_attn_warp(const T* __restrict__ q, const int32_t* __restrict__ buf_lens
     if (n > 0) {
         // ---- every load of the warp up front ----
         uint4 qf[NI], ka[2][NI], kb[2][NI];
-#pragma unroll
-        for (int i = 0; i < NI; ++i)
-            qf[i] = (g < mq) ? ld_cg_u4(q + ((size_t)bq * num_heads + head0 + g) * D + i * 32 + t * 8) : make_uint4(0, 0, 0, 0);
+        decode_attn_load_q<D>(qf, q, cta, num_heads, g, t);
 #pragma unroll
         for (int tl = 0; tl < 2; ++tl) {
             const T* pa = kbase + (size_t)min(k0 + tl * 16 + g, k1 - 1) * stride + t * 8;
@@ -205,17 +184,7 @@ k_decode_attn_warp(const T* __restrict__ q, const int32_t* __restrict__ buf_lens
             gl += s_dyn[w * WS + 32 * 8 + 8 * D + 8 + h] * f;
             acc += s_dyn[w * WS + 32 * 8 + h * D + d] * f;
         }
-        const float v = acc / gl;
-        const size_t vh = (size_t)bq * num_heads + head0 + h;
-        if (num_splits == 1) {
-            out[vh * D + d] = from_f32<T>(v);
-        } else {
-            part_o[(vh * num_splits + split) * D + d] = v;
-            if (d == 0) {
-                part_m[vh * num_splits + split] = gm;
-                part_l[vh * num_splits + split] = gl;
-            }
-        }
+        decode_attn_store<T, D>(cta, h, d, acc / gl, gm, gl, num_heads, num_splits, out, part_o, part_m, part_l);
     }
 }
 

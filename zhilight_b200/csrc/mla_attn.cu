@@ -20,11 +20,8 @@
 // host sync.  Keys past the split's end are zero-filled, never read, so stale or NaN cache rows cannot reach P.V.
 // P is carried in 16 bits: fp16 models as p * 2^10 in fp16 (11 significant bits), bf16 models as bf16 (8 bits; a
 // hi + lo pair would double the P.V MMAs that bound H = 128).  Key splits are merged by k_attn_combine in a fixed order.
-#include "common.cuh"
-#include "attn_combine.cuh"
+#include "attn_common.cuh"
 #include "tc_common.cuh"
-
-#include <type_traits>
 
 namespace zl {
 
@@ -55,10 +52,6 @@ __device__ __forceinline__ uint64_t mla_desc(uint32_t saddr, uint32_t lbo) {
     d |= (uint64_t)(1024 >> 4) << 32;
     d |= (uint64_t)1 << 62;
     return d;
-}
-
-__device__ __forceinline__ void mla_cp16(uint32_t dst, const void* src, int src_bytes) {
-    asm volatile("cp.async.cg.shared.global [%0], [%1], 16, %2;" ::"r"(dst), "l"(src), "r"(src_bytes) : "memory");
 }
 
 #define MLA_ACC8(C, i) C(d[i]), C(d[i + 1]), C(d[i + 2]), C(d[i + 3]), C(d[i + 4]), C(d[i + 5]), C(d[i + 6]), C(d[i + 7])
@@ -103,27 +96,6 @@ __device__ __forceinline__ void mla_wg_pv(float (&d)[128], const uint32_t (&a)[4
 #undef MLA_D32
 #undef MLA_ACC8
 
-__device__ __forceinline__ float mla_quad_max(float v) {
-    v = fmaxf(v, __shfl_xor_sync(0xffffffffu, v, 1));
-    return fmaxf(v, __shfl_xor_sync(0xffffffffu, v, 2));
-}
-__device__ __forceinline__ float mla_quad_sum(float v) {
-    v += __shfl_xor_sync(0xffffffffu, v, 1);
-    return v + __shfl_xor_sync(0xffffffffu, v, 2);
-}
-
-// the P.V A operand of probabilities (x, y) (lower key first): fp16 p * 2^10, or bf16 p
-template <typename T>
-__device__ __forceinline__ uint32_t mla_pack_p(float x, float y) {
-    if constexpr (std::is_same<T, __half>::value) {
-        const __half2 h = __floats2half2_rn(x * 1024.f, y * 1024.f);
-        return *reinterpret_cast<const uint32_t*>(&h);
-    } else {
-        const __nv_bfloat162 h = __floats2bfloat162_rn(x, y);
-        return *reinterpret_cast<const uint32_t*>(&h);
-    }
-}
-
 // grid (num_splits, row tiles, B), block kMlaThreads, dynamic shared memory kMlaSmem
 template <typename T>
 __global__ void __launch_bounds__(kMlaThreads, 1)
@@ -153,9 +125,7 @@ k_mla_decode_attn(const T* __restrict__ q, const int32_t* __restrict__ buf_lens,
     // this thread's accumulator rows: 16 warp + g and + 8 of the tile
     int r_row[2];
     const int8_t* mrow[2] = {nullptr, nullptr};
-    size_t len_off = 0;
-    if (mask)
-        for (int j = 0; j < b; ++j) len_off += buf_lens[j];
+    const size_t len_off = mask ? attn_keys_before(buf_lens, b) : 0;
 #pragma unroll
     for (int i = 0; i < 2; ++i) {
         r_row[i] = warp * 16 + g + 8 * i;
@@ -171,9 +141,9 @@ k_mla_decode_attn(const T* __restrict__ q, const int32_t* __restrict__ buf_lens,
         for (int i = tid; i < kMlaKeys * kMlaChunks; i += kMlaThreads) {
             const int r = i / kMlaChunks, c = i % kMlaChunks;
             const bool ok = kb + r < k1;
-            mla_cp16(dst + mla_off(r, c), kvbase + (ok ? (size_t)(kb + r) * kMlaD + c * 8 : 0), ok ? 16 : 0);
+            cp_async16(dst + mla_off(r, c), kvbase + (ok ? (size_t)(kb + r) * kMlaD + c * 8 : 0), ok ? 16 : 0);
         }
-        asm volatile("cp.async.commit_group;" ::: "memory");
+        cp_async_commit();
     };
 
     float o[128];
@@ -185,16 +155,16 @@ k_mla_decode_attn(const T* __restrict__ q, const int32_t* __restrict__ buf_lens,
         for (int i = tid; i < kMlaRows * kMlaChunks; i += kMlaThreads) {
             const int r = i / kMlaChunks, c = i % kMlaChunks;
             const bool ok = r < nrows;
-            mla_cp16(sq + mla_off(r, c), qbase + (ok ? (size_t)r * kMlaD + c * 8 : 0), ok ? 16 : 0);
+            cp_async16(sq + mla_off(r, c), qbase + (ok ? (size_t)r * kMlaD + c * 8 : 0), ok ? 16 : 0);
         }
         load_stage(0);
     }
     for (int it = 0; it < ntiles; ++it) {
         if (it + 1 < ntiles) {
             load_stage(it + 1);
-            asm volatile("cp.async.wait_group 1;" ::: "memory");
+            cp_async_wait<1>();
         } else {
-            asm volatile("cp.async.wait_group 0;" ::: "memory");
+            cp_async_wait<0>();
         }
         // cp.async wrote through the generic proxy; wgmma reads through the async proxy
         asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
@@ -230,7 +200,7 @@ k_mla_decode_attn(const T* __restrict__ q, const int32_t* __restrict__ buf_lens,
         float alpha[2];
 #pragma unroll
         for (int i = 0; i < 2; ++i) {
-            const float mn = fmaxf(m_r[i], mla_quad_max(mx[i]));
+            const float mn = fmaxf(m_r[i], quad_max(mx[i]));
             alpha[i] = expf(m_r[i] - mn);
             m_r[i] = mn;
         }
@@ -247,11 +217,11 @@ k_mla_decode_attn(const T* __restrict__ q, const int32_t* __restrict__ buf_lens,
         for (int j = 0; j < 128; ++j) o[j] *= alpha[(j >> 1) & 1];
 
         // ---- O += P.V: k-step kk covers keys 16 kk .. 16 kk + 15; this warpgroup's columns start at block 4 wg ----
-        uint32_t a[4][4];
+        uint32_t a[4][4], lo;   // lo is unused: P.V runs on the hi word alone
 #pragma unroll
         for (int kk = 0; kk < 4; ++kk)
 #pragma unroll
-            for (int r = 0; r < 4; ++r) a[kk][r] = mla_pack_p<T>(s[8 * kk + 2 * r], s[8 * kk + 2 * r + 1]);
+            for (int r = 0; r < 4; ++r) attn_pack_p<T>(s[8 * kk + 2 * r], s[8 * kk + 2 * r + 1], a[kk][r], lo);
         wg_fence();
 #pragma unroll
         for (int kk = 0; kk < 4; ++kk) mla_wg_pv<!kHalf>(o, a[kk], mla_desc(kt + wg * 4 * kMlaBlk + kk * 2048, kMlaBlk));
@@ -263,7 +233,7 @@ k_mla_decode_attn(const T* __restrict__ q, const int32_t* __restrict__ buf_lens,
     const float sc = kHalf ? (1.f / 1024.f) : 1.f;
 #pragma unroll
     for (int i = 0; i < 2; ++i) {
-        const float l = mla_quad_sum(l_r[i]) + 1e-20f;
+        const float l = quad_sum(l_r[i]) + 1e-20f;
         if (r_row[i] >= nrows) continue;
         const size_t vh = (size_t)b * task_rows + row0 + r_row[i];
         const int col0 = wg * 256 + 2 * t;
@@ -313,7 +283,7 @@ using namespace zl;
 extern "C" size_t zl_mla_decode_attention_workspace_bytes(int B, int len_q, int num_heads, int max_len_buf) {
     if (B <= 0 || len_q <= 0 || num_heads <= 0 || max_len_buf <= 0) return 0;
     const int s = mla_max_splits(max_len_buf);
-    return s > 1 ? (size_t)B * len_q * num_heads * s * (kMlaDv + 2) * sizeof(float) : 0;
+    return s > 1 ? attn_parts_bytes((size_t)B * len_q * num_heads, s, kMlaDv) : 0;
 }
 
 extern "C" int zl_mla_decode_attention(const void* q, const int32_t* buf_lens, void* const* kv_addrs, const int8_t* mask,
@@ -328,28 +298,16 @@ extern "C" int zl_mla_decode_attention(const void* q, const int32_t* buf_lens, v
     const int row_tiles = cdiv(len_q * num_heads, kMlaRows);
     const int splits = mla_num_splits(B, row_tiles, max_len_buf);
     const size_t vheads = (size_t)B * len_q * num_heads;
-    float *part_o = nullptr, *part_m = nullptr, *part_l = nullptr;
-    if (splits > 1) {
-        part_o = static_cast<float*>(workspace);
-        part_m = part_o + vheads * splits * kMlaDv;
-        part_l = part_m + vheads * splits;
-    }
+    const AttnParts part = attn_parts(workspace, vheads, splits, kMlaDv);
     const dim3 grid(splits, row_tiles, B);
     cudaStream_t st = (cudaStream_t)stream;
 #define ZL_MLA_LAUNCH(TT)                                                                                              \
     {                                                                                                                  \
-        static bool attr_set = false;                                                                                  \
-        if (!attr_set) {                                                                                               \
-            ZL_CHECK_CUDA(cudaFuncSetAttribute(k_mla_decode_attn<TT>, cudaFuncAttributeMaxDynamicSharedMemorySize,     \
-                                               kMlaSmem));                                                             \
-            attr_set = true;                                                                                           \
-        }                                                                                                              \
+        ZL_CHECK_CUDA(attn_smem_opt_in<k_mla_decode_attn<TT>>(kMlaSmem));                                             \
         ZL_CHECK_CUDA(launch(k_mla_decode_attn<TT>, grid, dim3(kMlaThreads), (size_t)kMlaSmem, st, pdl != 0,           \
-                             (const TT*)q, buf_lens, (TT* const*)kv_addrs, mask, scale, (TT*)out, part_o, part_m,     \
-                             part_l, len_q, num_heads, splits));                                                       \
-        if (splits > 1)                                                                                                \
-            ZL_CHECK_CUDA(launch(k_attn_combine<TT>, dim3((unsigned)vheads), dim3(kMlaDv), 0, st, pdl != 0,           \
-                                 (const float*)part_o, (const float*)part_m, (const float*)part_l, (TT*)out, splits)); \
+                             (const TT*)q, buf_lens, (TT* const*)kv_addrs, mask, scale, (TT*)out, part.o, part.m,     \
+                             part.l, len_q, num_heads, splits));                                                       \
+        ZL_CHECK_CUDA(launch_attn_combine(part, vheads, kMlaDv, (TT*)out, splits, st, pdl != 0));                     \
     }
     if (dtype == ZL_F16) ZL_MLA_LAUNCH(__half) else ZL_MLA_LAUNCH(__nv_bfloat16)
 #undef ZL_MLA_LAUNCH

@@ -12,18 +12,14 @@
 // byte staged in shared memory feeds the whole GQA group and every query row of the tile.  K/V tiles of 64 keys are
 // double-buffered with cp.async (keys at or past the tile's last position + 1 are zero-filled, never read); S = Q.K^T and
 // O += P.V run on mma.sync m16n8k16 with fp32 accumulate; softmax is online in fp32 (max seeded -1e20, the reference's
-// 1e-20 added to the sum), and the P.V operand is encoded as in k_decode_attn (fp16: p * 2^10 in fp16; bf16: hi + lo).
+// 1e-20 added to the sum), and the P.V operand is encoded by attn_pack_p (fp16: p * 2^10 in fp16; bf16: hi + lo).
 // Key tiles past the tile's last position are never visited, and only tiles that reach past its first position are
 // masked per element.
 //
 // Batch invariance: split s always covers keys [512 s, 512 (s + 1)), whatever the launch holds.  A row's splits, and so
 // its output bits, depend only on its q, its task's cache and its position.  A split holding none of a row's keys writes
 // the empty partial (max -1e20, sum 1e-20, o = 0), which k_attn_combine weighs by exactly 0.
-#include "common.cuh"
-#include "attn_combine.cuh"
-#include "decode_attn_short.cuh"
-
-#include <type_traits>
+#include "attn_common.cuh"
 
 namespace zl {
 
@@ -46,14 +42,6 @@ __device__ __forceinline__ int va_off(int r, int c) {
     return r * D + ((c ^ (r & 7)) << 3);
 }
 
-__device__ __forceinline__ void cp_async16(uint32_t dst, const void* src, int src_bytes) {
-    asm volatile("cp.async.cg.shared.global [%0], [%1], 16, %2;" ::"r"(dst), "l"(src), "r"(src_bytes) : "memory");
-}
-__device__ __forceinline__ void cp_async_commit() { asm volatile("cp.async.commit_group;" ::: "memory"); }
-template <int N>
-__device__ __forceinline__ void cp_async_wait() {
-    asm volatile("cp.async.wait_group %0;" ::"n"(N) : "memory");
-}
 __device__ __forceinline__ void ldsm_x4(uint32_t addr, uint32_t& r0, uint32_t& r1, uint32_t& r2, uint32_t& r3) {
     asm volatile("ldmatrix.sync.aligned.m8n8.x4.shared.b16 {%0,%1,%2,%3}, [%4];"
                  : "=r"(r0), "=r"(r1), "=r"(r2), "=r"(r3)
@@ -64,31 +52,6 @@ __device__ __forceinline__ void ldsm_x4_t(uint32_t addr, uint32_t& r0, uint32_t&
                  : "=r"(r0), "=r"(r1), "=r"(r2), "=r"(r3)
                  : "r"(addr));
 }
-__device__ __forceinline__ float quad_max(float v) {
-    v = fmaxf(v, __shfl_xor_sync(0xffffffffu, v, 1));
-    return fmaxf(v, __shfl_xor_sync(0xffffffffu, v, 2));
-}
-__device__ __forceinline__ float quad_sum(float v) {
-    v += __shfl_xor_sync(0xffffffffu, v, 1);
-    return v + __shfl_xor_sync(0xffffffffu, v, 2);
-}
-
-// the P.V A operand of probabilities (x, y) (lower key first): fp16 p * 2^10, or bf16 hi and lo
-template <typename T>
-__device__ __forceinline__ void va_pack_p(float x, float y, uint32_t& hi, uint32_t& lo) {
-    if constexpr (std::is_same<T, __half>::value) {
-        const __half2 h = __floats2half2_rn(x * 1024.f, y * 1024.f);
-        hi = *reinterpret_cast<const uint32_t*>(&h);
-        lo = 0u;
-    } else {
-        const __nv_bfloat162 h = __floats2bfloat162_rn(x, y);
-        const float2 f = __bfloat1622float2(h);
-        const __nv_bfloat162 l = __floats2bfloat162_rn(x - f.x, y - f.y);
-        hi = *reinterpret_cast<const uint32_t*>(&h);
-        lo = *reinterpret_cast<const uint32_t*>(&l);
-    }
-}
-
 template <typename T, int D>
 __global__ void __launch_bounds__(kVaThreads)
 k_varlen_attn(const T* __restrict__ q, const int4* __restrict__ seg, int nseg, T* const* __restrict__ k_addrs,
@@ -249,10 +212,10 @@ k_varlen_attn(const T* __restrict__ q, const int4* __restrict__ seg, int nseg, T
 #pragma unroll
             for (int kk = 0; kk < kVaKeyTile / 16; ++kk) {
                 uint32_t af[4], al[4];
-                va_pack_p<T>(s[2 * kk][0], s[2 * kk][1], af[0], al[0]);
-                va_pack_p<T>(s[2 * kk][2], s[2 * kk][3], af[1], al[1]);
-                va_pack_p<T>(s[2 * kk + 1][0], s[2 * kk + 1][1], af[2], al[2]);
-                va_pack_p<T>(s[2 * kk + 1][2], s[2 * kk + 1][3], af[3], al[3]);
+                attn_pack_p<T>(s[2 * kk][0], s[2 * kk][1], af[0], al[0]);
+                attn_pack_p<T>(s[2 * kk][2], s[2 * kk][3], af[1], al[1]);
+                attn_pack_p<T>(s[2 * kk + 1][0], s[2 * kk + 1][1], af[2], al[2]);
+                attn_pack_p<T>(s[2 * kk + 1][2], s[2 * kk + 1][3], af[3], al[3]);
 #pragma unroll
                 for (int jp = 0; jp < DC / 2; ++jp) {
                     const int r = 16 * kk + (mat & 1) * 8 + mr, c = 2 * jp + (mat >> 1);
@@ -311,7 +274,7 @@ using namespace zl;
 extern "C" size_t zl_varlen_attention_workspace_bytes(int rows, int nseg, int num_heads, int dim_head, int max_keys) {
     if (rows <= 0 || nseg <= 0 || nseg > rows || num_heads <= 0 || dim_head <= 0 || max_keys <= 0) return 0;
     const int splits = cdiv(max_keys, kVaSplitKeys);
-    return splits > 1 ? (size_t)rows * num_heads * splits * (dim_head + 2) * sizeof(float) : 0;
+    return splits > 1 ? attn_parts_bytes((size_t)rows * num_heads, splits, dim_head) : 0;
 }
 
 extern "C" int zl_varlen_attention(const void* q, const int32_t* seg, int nseg, int rows, void* const* k_addrs,
@@ -326,33 +289,20 @@ extern "C" int zl_varlen_attention(const void* q, const int32_t* seg, int nseg, 
     ZL_CHECK_ARG(reinterpret_cast<uintptr_t>(seg) % 16 == 0);
     const int splits = cdiv(max_keys, kVaSplitKeys);
     ZL_CHECK_SUPPORTED(splits <= 65535);
-    float *part_o = nullptr, *part_m = nullptr, *part_l = nullptr;
     const size_t vheads = (size_t)rows * num_heads;
-    if (splits > 1) {
-        ZL_CHECK_ARG(ws != nullptr && ws_bytes >= zl_varlen_attention_workspace_bytes(rows, nseg, num_heads, dim_head,
-                                                                                       max_keys));
-        part_o = static_cast<float*>(ws);
-        part_m = part_o + vheads * splits * dim_head;
-        part_l = part_m + vheads * splits;
-    }
+    if (splits > 1) ZL_CHECK_ARG(ws != nullptr && ws_bytes >= attn_parts_bytes(vheads, splits, dim_head));
+    const AttnParts part = attn_parts(ws, vheads, splits, dim_head);
     const int m_query = num_heads / num_kv_heads;
     const int gh = va_group_heads(m_query), qt = va_tile_rows(gh);
     const dim3 grid(cdiv(rows, qt) + nseg, num_kv_heads * cdiv(m_query, gh), splits);
     cudaStream_t st = (cudaStream_t)stream;
 #define ZL_VA_LAUNCH(TT, DD)                                                                                          \
     {                                                                                                                 \
-        static bool attr_set = false;                                                                                 \
-        if (!attr_set) {                                                                                              \
-            ZL_CHECK_CUDA(cudaFuncSetAttribute(k_varlen_attn<TT, DD>, cudaFuncAttributeMaxDynamicSharedMemorySize,    \
-                                               va_smem_bytes<DD>()));                                                 \
-            attr_set = true;                                                                                          \
-        }                                                                                                             \
+        ZL_CHECK_CUDA((attn_smem_opt_in<k_varlen_attn<TT, DD>>(va_smem_bytes<DD>())));                                \
         ZL_CHECK_CUDA(launch(k_varlen_attn<TT, DD>, grid, dim3(kVaThreads), (size_t)va_smem_bytes<DD>(), st, pdl != 0, \
                              (const TT*)q, (const int4*)seg, nseg, (TT* const*)k_addrs, (TT* const*)v_addrs, scale,    \
-                             (TT*)out, part_o, part_m, part_l, num_heads, num_kv_heads, m_query, gh, qt, splits));    \
-        if (splits > 1)                                                                                               \
-            ZL_CHECK_CUDA(launch(k_attn_combine<TT>, dim3((unsigned)vheads), dim3(DD), 0, st, pdl != 0,               \
-                                 (const float*)part_o, (const float*)part_m, (const float*)part_l, (TT*)out, splits)); \
+                             (TT*)out, part.o, part.m, part.l, num_heads, num_kv_heads, m_query, gh, qt, splits));    \
+        ZL_CHECK_CUDA(launch_attn_combine(part, vheads, DD, (TT*)out, splits, st, pdl != 0));                         \
     }
     if (dtype == ZL_F16) {
         if (dim_head == 128) ZL_VA_LAUNCH(__half, 128) else ZL_VA_LAUNCH(__half, 64)

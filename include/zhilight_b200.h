@@ -545,6 +545,32 @@ int zl_llama_stats(zl_llama_t* m, int B, double* weight_bytes, int* kernels_per_
  * Returns total milliseconds, the number of GEMM launches and their algorithmic bytes. */
 int zl_llama_bench_gemms(zl_llama_t* m, int B, int iters, float* ms, int* launches, double* bytes);
 
+/* Prompt prefix cache (enable_prompt_caching of the reference: PrefixCache, src/generator/prefix_cache.hpp:35-117, created
+ * at src/generator/batch_generator.cpp:626-645, matched at :1033-1045 and :1120, filled after a prompt's prefill at
+ * :1213-1224).  The model owns a device pool of num_blocks blocks of block_tokens KV rows each, for every layer, K and V:
+ * pool [layer][K|V][block][block_tokens][H_kv][d] in the cache's element type, and with kv_int8 the fp32 scales
+ * [layer][K|V][block][block_tokens][H_kv] beside it, so that codes and scales always move together.  Which blocks hold
+ * which tokens is the caller's policy (zhilight_b200/prefix_cache.py keys a block by every block before it).
+ * Call after zl_llama_finalize; zl_llama_destroy frees the pool.  block_tokens: 16, 32, 64, 128 or 256, else
+ * ZL_ERR_INVALID_ARG; a second call: ZL_ERR_STATE; max_seq * (bytes of one cached row) not a multiple of 16:
+ * ZL_ERR_UNSUPPORTED.  A model without a pool allocates nothing for it and runs the same kernels per step. */
+int zl_llama_kv_pool_create(zl_llama_t* m, int num_blocks, int block_tokens);
+/* Copy n blocks of task `task` into the pool (save: task block task_blocks[i] -> pool block pool_blocks[i]) or out of it
+ * (load: pool block pool_blocks[i] -> task block task_blocks[i]).  Task block j is rows [j bt, (j + 1) bt) of the task's
+ * buffers.  One kernel launch (k_kv_block_copy) for every layer, K, V and, with kv_int8, the scales.  HOST arrays, staged
+ * before the call returns; stream-ordered after every step already enqueued, no device sync.  Loading writes KV rows
+ * only: the positions stay with the caller (zl_llama_prefill with pos0 = the loaded length, or a joined segment).
+ * Every check runs before anything is enqueued: no pool -> ZL_ERR_STATE; task out of range, a block out of range or past
+ * max_seq ((j + 1) bt > max_seq), or a destination block named twice -> ZL_ERR_INVALID_ARG. */
+int zl_llama_kv_blocks_save(zl_llama_t* m, int task, const int32_t* task_blocks, const int32_t* pool_blocks, int n);
+int zl_llama_kv_blocks_load(zl_llama_t* m, int task, const int32_t* task_blocks, const int32_t* pool_blocks, int n);
+/* Bandwidth probe of the block copy: one warm-up pass, then `iters` passes of the same save (load = 0) or load between
+ * CUDA events on the driver's stream, as the k_kv_block_copy launch or (per_range_memcpy != 0) as one cudaMemcpyAsync per
+ * (block, layer, tensor) range.  Returns the milliseconds of the timed passes and the bytes one pass reads plus writes.
+ * Rewrites the destination blocks; the same checks as zl_llama_kv_blocks_save / load. */
+int zl_llama_kv_blocks_bench(zl_llama_t* m, int task, const int32_t* task_blocks, const int32_t* pool_blocks, int n,
+                             int load, int per_range_memcpy, int iters, float* ms, double* bytes);
+
 #ifdef __cplusplus
 }
 #endif

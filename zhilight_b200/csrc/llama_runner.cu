@@ -10,6 +10,7 @@
 #include "w4_layout.cuh"
 #include "comm_dev.cuh"
 #include "w4_params.h"
+#include "kv_pool.cuh"
 
 #include <cstdlib>
 #include <cstring>
@@ -151,6 +152,18 @@ struct zl_llama {
     // between launches (every qkv GEMM of the model runs in stream order on the compute stream)
     dev_ptr<__half> kv8_rows;
     dev_ptr<uint32_t> kv8_cnt;
+    // prompt prefix cache (zl_llama_kv_pool_create): the device block pool [layer][K|V][block][bt][H_kv][d] (+ fp32 scales
+    // [layer][K|V][block][bt][H_kv] at kv_int8), the task buffers of every layer as a device table (4 per layer: k, v,
+    // scale k, scale v), and the block lists of zl_llama_kv_blocks_save / load staged like zl_llama_set_state's: one pinned
+    // host slot and one device slot per event, never rewritten while the copy that reads it is still queued
+    dev_ptr<> pool, pool_scales;
+    dev_ptr<void*> pool_tab;
+    int pool_blocks = 0, pool_bt = 0, pool_cap = 0;   // pool_cap: block pairs one slot holds
+    host_ptr<int32_t> pool_h;                         // [kStageSlots][2 * pool_cap]
+    dev_ptr<int32_t> pool_d;
+    cudaEvent_t pool_ev[kStageSlots] = {};
+    bool pool_used[kStageSlots] = {};
+    int pool_next = 0;
 };
 
 namespace {
@@ -1485,6 +1498,8 @@ extern "C" void zl_llama_destroy(zl_llama_t* m) {
             if (e) cudaEventDestroy(e);
     for (cudaEvent_t e : m->ring_ev)
         if (e) cudaEventDestroy(e);
+    for (cudaEvent_t e : m->pool_ev)
+        if (e) cudaEventDestroy(e);
     if (m->reduce_stream) cudaStreamDestroy(m->reduce_stream);
     cudaStreamDestroy(m->stream);
     delete m;   // the members free their device and pinned buffers
@@ -1941,4 +1956,181 @@ extern "C" int zl_llama_stats(zl_llama_t* m, int B, double* weight_bytes, int* k
     if (weight_bytes) *weight_bytes = m->weight_bytes;
     if (kernels_per_step) *kernels_per_step = m->kernels_per_step;
     return ZL_OK;
+}
+
+// ------------------------------------------------------------------------------------------------------------------
+// Prompt prefix cache: the block pool and the block copies (PrefixCache, src/generator/prefix_cache.hpp:35-117).  Which
+// blocks to save and load is the caller's policy (zhilight_b200/prefix_cache.py); this owns the memory and the copies.
+// ------------------------------------------------------------------------------------------------------------------
+extern "C" int zl_llama_kv_pool_create(zl_llama_t* m, int num_blocks, int block_tokens) {
+    ZL_CHECK_ARG(m && num_blocks > 0);
+    ZL_CHECK_ARG(block_tokens == 16 || block_tokens == 32 || block_tokens == 64 || block_tokens == 128 ||
+                 block_tokens == 256);
+    if (!m->finalized) return fail_state(__LINE__, "zl_llama_kv_pool_create needs a finalized model");
+    if (m->pool) return fail_state(__LINE__, "the KV block pool already exists");
+    const auto& c = m->cfg;
+    const int L = c.num_layers;
+    const int row_bytes = m->hkv * c.dim_head * (c.kv_int8 ? 1 : 2);
+    const int srow_bytes = c.kv_int8 ? m->hkv * 4 : 0;
+    if (!kv_block_copy_aligned(block_tokens, c.max_seq, row_bytes, srow_bytes))
+        return fail_state(__LINE__, "KV block copies need max_seq * (bytes of one cached row) to be a multiple of 16",
+                          ZL_ERR_UNSUPPORTED);
+    const size_t blk = (size_t)block_tokens * row_bytes, sblk = (size_t)block_tokens * srow_bytes;
+    const int cap = num_blocks > c.max_seq / block_tokens ? num_blocks : c.max_seq / block_tokens;
+    dev_ptr<> pool, scales;
+    dev_ptr<void*> tab;
+    dev_ptr<int32_t> dslots;
+    RCHECK(dmalloc(&pool, (size_t)L * 2 * num_blocks * blk));
+    if (c.kv_int8) RCHECK(dmalloc(&scales, (size_t)L * 2 * num_blocks * sblk));
+    std::vector<void*> h_tab((size_t)4 * L, nullptr);
+    for (int l = 0; l < L; ++l) {
+        const Layer& Ly = m->layers[l];
+        h_tab[4 * l] = Ly.kbuf.get();
+        h_tab[4 * l + 1] = Ly.vbuf.get();
+        h_tab[4 * l + 2] = Ly.skbuf.get();
+        h_tab[4 * l + 3] = Ly.svbuf.get();
+    }
+    RCHECK(dmalloc(&tab, sizeof(void*) * 4 * L));
+    ZL_CHECK_CUDA(cudaMemcpyAsync(tab.get(), h_tab.data(), sizeof(void*) * 4 * L, cudaMemcpyHostToDevice, m->stream));
+    RCHECK(dmalloc(&dslots, sizeof(int32_t) * zl_llama::kStageSlots * 2 * cap));
+    int32_t* hs = nullptr;
+    ZL_CHECK_CUDA(cudaMallocHost((void**)&hs, sizeof(int32_t) * zl_llama::kStageSlots * 2 * cap));
+    host_ptr<int32_t> hslots(hs);
+    for (int i = 0; i < zl_llama::kStageSlots; ++i)
+        if (!m->pool_ev[i]) ZL_CHECK_CUDA(cudaEventCreateWithFlags(&m->pool_ev[i], cudaEventDisableTiming));
+    ZL_CHECK_CUDA(cudaStreamSynchronize(m->stream));   // h_tab is pageable and goes out of scope
+    m->pool = std::move(pool);
+    m->pool_scales = std::move(scales);
+    m->pool_tab = std::move(tab);
+    m->pool_d = std::move(dslots);
+    m->pool_h = std::move(hslots);
+    m->pool_blocks = num_blocks;
+    m->pool_bt = block_tokens;
+    m->pool_cap = cap;
+    return ZL_OK;
+}
+
+namespace {
+
+// every check of a save / load before anything is enqueued
+int check_kv_blocks(zl_llama* m, int task, const int32_t* task_blocks, const int32_t* pool_blocks, int n, bool to_pool) {
+    ZL_CHECK_ARG(m && task_blocks && pool_blocks && n > 0);
+    if (!m->finalized || !m->pool) return fail_state(__LINE__, "no KV block pool (zl_llama_kv_pool_create)");
+    const auto& c = m->cfg;
+    ZL_CHECK_ARG(task >= 0 && task < c.max_batch && n <= m->pool_cap);
+    const int task_max = c.max_seq / m->pool_bt;   // (j + 1) * bt <= max_seq
+    std::vector<char> seen(to_pool ? m->pool_blocks : task_max, 0);
+    for (int i = 0; i < n; ++i) {
+        ZL_CHECK_ARG(task_blocks[i] >= 0 && task_blocks[i] < task_max);
+        ZL_CHECK_ARG(pool_blocks[i] >= 0 && pool_blocks[i] < m->pool_blocks);
+        const int dst = to_pool ? pool_blocks[i] : task_blocks[i];
+        ZL_CHECK_ARG(!seen[dst]);   // no destination twice
+        seen[dst] = 1;
+    }
+    return ZL_OK;
+}
+
+KvBlockCopyArgs kv_copy_args(zl_llama* m, int task, const int32_t* d_pairs, int n, bool to_pool) {
+    const auto& c = m->cfg;
+    KvBlockCopyArgs a{};
+    a.task_bases = m->pool_tab.get();
+    a.pool = static_cast<char*>(m->pool.get());
+    a.pool_scales = static_cast<char*>(m->pool_scales.get());
+    a.pairs = d_pairs;
+    a.n = n;
+    a.layers = c.num_layers;
+    a.num_blocks = m->pool_blocks;
+    a.bt = m->pool_bt;
+    a.task = task;
+    a.task_rows = c.max_seq;
+    a.row_bytes = m->hkv * c.dim_head * (c.kv_int8 ? 1 : 2);
+    a.srow_bytes = c.kv_int8 ? m->hkv * 4 : 0;
+    a.to_pool = to_pool ? 1 : 0;
+    return a;
+}
+
+// stage the block lists in the next ring slot (waiting for the copy that last read it) -> its device copy
+int stage_kv_blocks(zl_llama* m, const int32_t* task_blocks, const int32_t* pool_blocks, int n, const int32_t** d_pairs,
+                    int* slot_out) {
+    const int slot = m->pool_next;
+    m->pool_next = (slot + 1) % zl_llama::kStageSlots;
+    if (m->pool_used[slot]) ZL_CHECK_CUDA(cudaEventSynchronize(m->pool_ev[slot]));
+    int32_t* hs = m->pool_h.get() + (size_t)slot * 2 * m->pool_cap;
+    int32_t* ds = m->pool_d.get() + (size_t)slot * 2 * m->pool_cap;
+    std::memcpy(hs, task_blocks, sizeof(int32_t) * n);
+    std::memcpy(hs + n, pool_blocks, sizeof(int32_t) * n);
+    ZL_CHECK_CUDA(cudaMemcpyAsync(ds, hs, sizeof(int32_t) * 2 * n, cudaMemcpyHostToDevice, m->stream));
+    *d_pairs = ds;
+    *slot_out = slot;
+    return ZL_OK;
+}
+
+int kv_blocks(zl_llama* m, int task, const int32_t* task_blocks, const int32_t* pool_blocks, int n, bool to_pool) {
+    RCHECK(check_kv_blocks(m, task, task_blocks, pool_blocks, n, to_pool));
+    const int32_t* d_pairs = nullptr;
+    int slot = 0;
+    RCHECK(stage_kv_blocks(m, task_blocks, pool_blocks, n, &d_pairs, &slot));
+    RCHECK(kv_block_copy(kv_copy_args(m, task, d_pairs, n, to_pool), m->stream));
+    ZL_CHECK_CUDA(cudaEventRecord(m->pool_ev[slot], m->stream));   // after the kernel that reads the device slot
+    m->pool_used[slot] = true;
+    return ZL_OK;
+}
+
+}  // namespace
+
+extern "C" int zl_llama_kv_blocks_save(zl_llama_t* m, int task, const int32_t* task_blocks, const int32_t* pool_blocks,
+                                       int n) {
+    return kv_blocks(m, task, task_blocks, pool_blocks, n, true);
+}
+
+extern "C" int zl_llama_kv_blocks_load(zl_llama_t* m, int task, const int32_t* task_blocks, const int32_t* pool_blocks,
+                                       int n) {
+    return kv_blocks(m, task, task_blocks, pool_blocks, n, false);
+}
+
+extern "C" int zl_llama_kv_blocks_bench(zl_llama_t* m, int task, const int32_t* task_blocks, const int32_t* pool_blocks,
+                                        int n, int load, int per_range_memcpy, int iters, float* ms, double* bytes) {
+    ZL_CHECK_ARG(iters > 0 && ms);
+    const bool to_pool = !load;
+    RCHECK(check_kv_blocks(m, task, task_blocks, pool_blocks, n, to_pool));
+    const auto& c = m->cfg;
+    const KvBlockCopyArgs a0 = kv_copy_args(m, task, nullptr, 0, to_pool);
+    const size_t blk = (size_t)a0.bt * a0.row_bytes, sblk = (size_t)a0.bt * a0.srow_bytes;
+    const int32_t* d_pairs = nullptr;
+    int slot = 0;
+    RCHECK(stage_kv_blocks(m, task_blocks, pool_blocks, n, &d_pairs, &slot));
+    const KvBlockCopyArgs a = kv_copy_args(m, task, d_pairs, n, to_pool);
+    auto one_pass = [&]() -> int {
+        if (!per_range_memcpy) return kv_block_copy(a, m->stream);
+        for (int i = 0; i < n; ++i)
+            for (int l = 0; l < c.num_layers; ++l) {
+                const Layer& Ly = m->layers[l];
+                void* tbuf[4] = {Ly.kbuf.get(), Ly.vbuf.get(), Ly.skbuf.get(), Ly.svbuf.get()};
+                for (int t = 0; t < (sblk ? 4 : 2); ++t) {
+                    const bool sc = t >= 2;
+                    const size_t rb = sc ? a.srow_bytes : a.row_bytes, bb = sc ? sblk : blk;
+                    char* tp = static_cast<char*>(tbuf[t]) + ((size_t)task * c.max_seq + (size_t)task_blocks[i] * a.bt) * rb;
+                    char* pp = (sc ? a.pool_scales : a.pool) + ((size_t)(l * 2 + (t & 1)) * a.num_blocks + pool_blocks[i]) * bb;
+                    ZL_CHECK_CUDA(cudaMemcpyAsync(to_pool ? pp : tp, to_pool ? tp : pp, bb, cudaMemcpyDeviceToDevice,
+                                                  m->stream));
+                }
+            }
+        return ZL_OK;
+    };
+    cudaEvent_t e0, e1;
+    ZL_CHECK_CUDA(cudaEventCreate(&e0));
+    ZL_CHECK_CUDA(cudaEventCreate(&e1));
+    int rc = one_pass();   // warm-up
+    if (rc == ZL_OK) rc = cudaEventRecord(e0, m->stream) == cudaSuccess ? ZL_OK : ZL_ERR_CUDA;
+    for (int it = 0; it < iters && rc == ZL_OK; ++it) rc = one_pass();
+    if (rc == ZL_OK) rc = cudaEventRecord(e1, m->stream) == cudaSuccess ? ZL_OK : ZL_ERR_CUDA;
+    if (rc == ZL_OK) rc = cudaEventRecord(m->pool_ev[slot], m->stream) == cudaSuccess ? ZL_OK : ZL_ERR_CUDA;
+    m->pool_used[slot] = true;
+    if (rc == ZL_OK) rc = cudaEventSynchronize(e1) == cudaSuccess ? ZL_OK : ZL_ERR_CUDA;
+    if (rc == ZL_OK) rc = cudaEventElapsedTime(ms, e0, e1) == cudaSuccess ? ZL_OK : ZL_ERR_CUDA;
+    cudaEventDestroy(e0);
+    cudaEventDestroy(e1);
+    if (rc == ZL_ERR_CUDA) zl_set_last_error(__FILE__, __LINE__, "CUDA event failed in zl_llama_kv_blocks_bench");
+    if (bytes) *bytes = 2.0 * n * c.num_layers * 2 * (double)(blk + sblk);   // read + write
+    return rc;
 }

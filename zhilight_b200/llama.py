@@ -10,6 +10,7 @@ import ctypes
 import numpy as np
 
 from . import _lib
+from .prefix_cache import PrefixCache
 
 MODEL_PRESETS = {
     # SURVEY.md section 8: shapes of the BASELINE.json configs
@@ -157,6 +158,59 @@ class LlamaDecoder:
             nxt.ctypes.data_as(ctypes.c_void_p),
             logits.ctypes.data_as(ctypes.c_void_p) if want_logits and n_emit else None))
         return (nxt, logits) if want_logits else nxt
+
+    def enable_prefix_cache(self, num_blocks, block_tokens=128):
+        """Prompt prefix caching: a device pool of num_blocks blocks of block_tokens (16 .. 256) KV rows of every layer
+        (zl_llama_kv_pool_create) and the host policy that fills it (prefix_cache.PrefixCache).  Call after the weights
+        are loaded; once per model."""
+        _lib.check(self.lib.zl_llama_kv_pool_create(self.h, int(num_blocks), int(block_tokens)))
+        self.prefix_cache = PrefixCache(num_blocks, block_tokens)
+
+    def _kv_blocks(self, fn, task, task_blocks, pool_blocks):
+        tb = np.ascontiguousarray(task_blocks, dtype=np.int32).reshape(-1)
+        pb = np.ascontiguousarray(pool_blocks, dtype=np.int32).reshape(-1)
+        if tb.size != pb.size:
+            raise ValueError("task_blocks and pool_blocks differ in length (%d, %d)" % (tb.size, pb.size))
+        if tb.size:
+            _lib.check(fn(self.h, int(task), tb.ctypes.data_as(ctypes.c_void_p), pb.ctypes.data_as(ctypes.c_void_p),
+                          tb.size))
+
+    def kv_save_blocks(self, task, task_blocks, pool_blocks):
+        """Copy the task's blocks task_blocks[i] (rows [j bt, (j + 1) bt)) into pool blocks pool_blocks[i], every layer;
+        stream-ordered after the steps already issued (zl_llama_kv_blocks_save)."""
+        self._kv_blocks(self.lib.zl_llama_kv_blocks_save, task, task_blocks, pool_blocks)
+
+    def kv_load_blocks(self, task, task_blocks, pool_blocks):
+        """Copy pool blocks pool_blocks[i] into the task's blocks task_blocks[i] (zl_llama_kv_blocks_load).  Writes KV rows
+        only: continue with prefill(task, rest, pos0=loaded length) or a step_joined segment at that position."""
+        self._kv_blocks(self.lib.zl_llama_kv_blocks_load, task, task_blocks, pool_blocks)
+
+    def prefill_cached(self, task, tokens, want_logits=False):
+        """prefill() through the prefix cache: load the longest cached prefix of `tokens` into the task, prefill the
+        rest at pos0 = its length, then cache the prompt's new blocks.  Returns (next token, cached length
+        [, logits]).  A cached row holds the bits of the prefill that wrote it, so the logits can differ in their last
+        bits from a cold prefill that split the prompt into different chunks."""
+        pc = getattr(self, "prefix_cache", None)
+        if pc is None:
+            raise RuntimeError("prefill_cached needs enable_prefix_cache() first")
+        t = np.ascontiguousarray(tokens, dtype=np.int32).reshape(-1)
+        hit = pc.match(t)
+        self.kv_load_blocks(task, range(len(hit)), hit)
+        m = len(hit) * pc.block_tokens
+        out = self.prefill(task, t[m:], pos0=m, want_logits=want_logits)
+        save = pc.insert(t)
+        self.kv_save_blocks(task, [j for j, _ in save], [b for _, b in save])
+        return (out[0], m, out[1]) if want_logits else (out, m)
+
+    def bench_kv_blocks(self, task, task_blocks, pool_blocks, load=True, per_range_memcpy=False, iters=20):
+        """-> (ms per pass, bytes one pass reads plus writes) of `iters` timed block copies (zl_llama_kv_blocks_bench)."""
+        tb = np.ascontiguousarray(task_blocks, dtype=np.int32)
+        pb = np.ascontiguousarray(pool_blocks, dtype=np.int32)
+        ms, by = ctypes.c_float(), ctypes.c_double()
+        _lib.check(self.lib.zl_llama_kv_blocks_bench(
+            self.h, int(task), tb.ctypes.data_as(ctypes.c_void_p), pb.ctypes.data_as(ctypes.c_void_p), tb.size,
+            int(bool(load)), int(bool(per_range_memcpy)), int(iters), ctypes.byref(ms), ctypes.byref(by)))
+        return ms.value / iters, by.value
 
     def set_sampling(self, task, temperature=0.0, top_p=1.0, top_k=0, repetition_penalty=1.0, presence_penalty=0.0,
                      seed=0):

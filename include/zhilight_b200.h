@@ -402,6 +402,19 @@ size_t zl_sample_workspace_bytes(int T, int V);
 int zl_sample(const float* logits, int T, int V, const zl_sample_params_t* params, const int32_t* row_task,
               const int32_t* counter, uint32_t* history, int history_words, int32_t* out, void* ws, size_t ws_bytes,
               int pdl, zl_stream_t stream);
+/* Beam-search selection (beam_utility::log_softmax_bias, generator/beam_util.cu:20-130, then topk_all.get_top_k over each
+ * task's flattened (beam x vocab) scores, generator/batch_generator.cpp:1770-1778), without writing an (R, V) tensor.
+ * logits (R, V) fp32 and cum (R) fp32 on the device; groups (G, 2) {row0, width} a HOST array whose groups tile rows
+ * [0, R) in order.  For each group g the K largest s = cum[r] + logits[r, v] - lse_r over its rows r and every v, with
+ * lse_r = max_r + log(1e-20 + sum_v exp(logits[r, v] - max_r)) in fp32, sorted by score descending and ties by the flat
+ * index (r - row0) * V + v ascending: parent[g, k] = r - row0, token[g, k] = v, score[g, k] = s (device (G, K) arrays).
+ * A row with cum = -inf is dead: its logits are never read (they may hold NaN).  Only finite scores are candidates; a group
+ * with fewer than K gets parent = token = -1 and score = -inf in the rest.  1 <= K <= 32 and 1 <= width <= 16, else
+ * ZL_ERR_INVALID_ARG; V > 262144: ZL_ERR_UNSUPPORTED; every check runs before anything is enqueued.  Two launches, after
+ * a copy of the groups into the workspace (ws_bytes >= zl_beam_topk_workspace_bytes(R, V, K)). */
+size_t zl_beam_topk_workspace_bytes(int R, int V, int K);
+int zl_beam_topk(const float* logits, int R, int V, const float* cum, const int32_t* groups, int G, int K,
+                 int32_t* parent, int32_t* token, float* score, void* ws, size_t ws_bytes, int pdl, zl_stream_t stream);
 /* synthetic-checkpoint generators (bench / tests): counter-based hash RNG, reproducible per seed. */
 int zl_fill_random_u32(uint32_t* p, size_t n, uint64_t seed, zl_stream_t stream);
 int zl_fill_const_u32(uint32_t* p, size_t n, uint32_t value, zl_stream_t stream);
@@ -570,6 +583,22 @@ int zl_llama_kv_blocks_load(zl_llama_t* m, int task, const int32_t* task_blocks,
  * Rewrites the destination blocks; the same checks as zl_llama_kv_blocks_save / load. */
 int zl_llama_kv_blocks_bench(zl_llama_t* m, int task, const int32_t* task_blocks, const int32_t* pool_blocks, int n,
                              int load, int per_range_memcpy, int iters, float* ms, double* bytes);
+
+/* Beam search (SearcherImplV1::pick_top_k, src/generator/batch_generator.cpp:1762-1852).  Each beam owns a task slot; the
+ * policy that picks beams and slots is the caller's (zhilight_b200/beam_search.py).
+ * One beam step: the decode step over tasks 0 .. B-1 (tokens / positions HOST (B) as zl_llama_decode), with the pick
+ * replaced by zl_beam_topk on the step's logits -- same CUDA graph, one per (B, G, K, length bucket), no argmax.  groups
+ * (G, 2), cum (B) HOST; parent / token / score (G, K) HOST outputs as zl_beam_topk's; logits_host NULL or (B, vocab).
+ * Synchronous.  Bad groups, K, cum (NaN or +inf), tokens or positions: ZL_ERR_INVALID_ARG; vocab > 262144 or tp_size > 1:
+ * ZL_ERR_UNSUPPORTED; a task of the batch that samples or has penalties (zl_llama_set_sampling): ZL_ERR_STATE. */
+int zl_llama_beam_step(zl_llama_t* m, const int32_t* tokens, const int32_t* positions, int B, const int32_t* groups, int G,
+                       const float* cum, int K, int32_t* parent, int32_t* token, float* score, float* logits_host);
+/* Beam forks: one launch copies rows [row0, row1) of task src into task dst for every range ranges_host[i] = {src task,
+ * dst task, row0, row1} (HOST (n, 4)), every layer, K and V, and with kv_int8 the fp32 scales.  Staged before the call
+ * returns; stream-ordered after the steps already issued, no device sync.  Every check runs before anything is enqueued:
+ * a task out of range, rows outside [0, max_seq) or an empty range, a destination named twice, or a task that is both a
+ * source and a destination: ZL_ERR_INVALID_ARG. */
+int zl_llama_kv_copy_rows(zl_llama_t* m, const int32_t* ranges_host, int n);
 
 #ifdef __cplusplus
 }

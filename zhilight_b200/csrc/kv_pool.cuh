@@ -25,4 +25,15 @@ struct KvBlockCopyArgs {
 bool kv_block_copy_aligned(int bt, int task_rows, int row_bytes, int srow_bytes);
 int kv_block_copy(const KvBlockCopyArgs& a, cudaStream_t stream);
 
+// One launch copies n row ranges between tasks, every layer, K and V (and their fp32 scales with an int8 cache): range i
+// = ranges[4 i ..] {src task, dst task, row0, row1} moves rows [row0, row1) of the src task's (max_seq, H_kv, d) buffers
+// to the same rows of the dst task's.  No task may be both a source and a destination, and no destination may repeat.
+struct KvRowCopyArgs {
+    void* const* task_bases;   // device table, 4 per layer as in KvBlockCopyArgs
+    const int32_t* ranges;     // device (n, 4)
+    int n, layers, task_rows, max_rows;   // max_rows: the longest range
+    int row_bytes, srow_bytes;            // row_bytes % 16 == 0; srow_bytes 0 (no scales) or a multiple of 4
+};
+int kv_row_copy(const KvRowCopyArgs& a, cudaStream_t stream);
+
 }  // namespace zl

@@ -11,6 +11,7 @@
 #include "comm_dev.cuh"
 #include "w4_params.h"
 #include "kv_pool.cuh"
+#include "beam.cuh"
 
 #include <cstdlib>
 #include <cstring>
@@ -164,6 +165,17 @@ struct zl_llama {
     cudaEvent_t pool_ev[kStageSlots] = {};
     bool pool_used[kStageSlots] = {};
     int pool_next = 0;
+    // beam search, allocated by the first zl_llama_beam_step / zl_llama_kv_copy_rows: the selection's inputs and outputs
+    // (cum (max_batch) f32 | groups (2 max_batch) | parent, token, score (max_batch x 32) each), its workspace, their
+    // pinned host mirror (the beam step is synchronous), and the row-copy ranges staged like the block lists
+    dev_ptr<> beam_d, beam_ws;
+    host_ptr<int32_t> beam_h;
+    dev_ptr<void*> rows_tab;                          // the task buffers of every layer, 4 per layer as pool_tab
+    host_ptr<int32_t> rows_h;                         // [kStageSlots][4 * max_batch]
+    dev_ptr<int32_t> rows_d;
+    cudaEvent_t rows_ev[kStageSlots] = {};
+    bool rows_used[kStageSlots] = {};
+    int rows_next = 0;
 };
 
 namespace {
@@ -1227,7 +1239,18 @@ int prefill_layers_dual(zl_llama* m, const Segments& pf) {
     return ZL_OK;
 }
 
-int enqueue_step(zl_llama* m, int n_tasks, int len_bucket, const Segments* pf = nullptr, bool sampler = false) {
+// The pick of a beam step (zl_llama_beam_step): zl_beam_topk's launches over the step's logits, device arguments
+struct BeamPick {
+    const float* cum = nullptr;
+    const int32_t* groups = nullptr;
+    int G = 0, K = 0;
+    int32_t *parent = nullptr, *token = nullptr;
+    float* score = nullptr;
+    void* ws = nullptr;
+};
+
+int enqueue_step(zl_llama* m, int n_tasks, int len_bucket, const Segments* pf = nullptr, bool sampler = false,
+                 const BeamPick* beam = nullptr) {
     const auto& c = m->cfg;
     const int B = pf ? pf->n : n_tasks;   // rows (tokens) of every activation matrix in this launch sequence
     const int D = c.dim_model, d = c.dim_head, dt = c.dtype, pdl = c.use_pdl;
@@ -1360,7 +1383,11 @@ int enqueue_step(zl_llama* m, int n_tasks, int len_bucket, const Segments* pf = 
     // vocab-parallel lm_head (embedding.cu:353-392): each rank owns vshard rows
     RCHECK(zl_dense_gemm_skinny(head_x, D, m->lm_head, nullptr, m->logits.get(), HB, m->vshard, D, dt, ZL_F32,
                                 stage_pdl(m, kLmHead), st));
-    if (sampler) {
+    if (beam) {
+        // decode rows only, single rank, no sampling (zl_llama_beam_step checks)
+        RCHECK(beam_topk_launch(m->logits.get(), HB, m->vshard, beam->cum, beam->groups, beam->G, beam->K, beam->parent,
+                                beam->token, beam->score, beam->ws, stage_pdl(m, kPick), st));
+    } else if (sampler) {
         // one row per task at decode (row b = task b, counter = its input position); prefill: the task's last prompt
         // position; joined: each emitting segment's task and last position.  set_sampling keeps this off under tensor
         // parallelism.
@@ -1395,17 +1422,19 @@ bool sampler_on(const zl_llama* m, int first, int n) {
     return false;
 }
 
-int run_step(zl_llama* m, int B) {
+int run_step(zl_llama* m, int B, const BeamPick* beam = nullptr) {
     const int bucket = len_bucket_of(m, m->cur_max_len);
     const bool sampler = sampler_on(m, 0, B);
-    if (!m->cfg.use_graph) return enqueue_step(m, B, bucket, nullptr, sampler);
-    // parameter changes need no re-capture (they live on the device), only switching the sampler on or off does
-    const long long key = ((long long)B << 33) | ((long long)sampler << 32) | (unsigned)bucket;
+    if (!m->cfg.use_graph) return enqueue_step(m, B, bucket, nullptr, sampler, beam);
+    // parameter changes need no re-capture (they live on the device), only switching the sampler on or off does.  A beam
+    // step (bit 62) bakes its group count (bits 44-54) and K (bits 55-60) into its launches; B < 2048 at a beam step.
+    long long key = ((long long)B << 33) | ((long long)sampler << 32) | (unsigned)bucket;
+    if (beam) key |= (1LL << 62) | ((long long)beam->K << 55) | ((long long)beam->G << 44);
     auto it = m->graphs.find(key);
     if (it == m->graphs.end()) {
         cudaGraph_t graph = nullptr;
         ZL_CHECK_CUDA(cudaStreamBeginCapture(m->stream, cudaStreamCaptureModeThreadLocal));
-        int rc = enqueue_step(m, B, bucket, nullptr, sampler);
+        int rc = enqueue_step(m, B, bucket, nullptr, sampler, beam);
         cudaError_t ce = cudaStreamEndCapture(m->stream, &graph);
         if (rc != ZL_OK) {
             if (graph) cudaGraphDestroy(graph);
@@ -1499,6 +1528,8 @@ extern "C" void zl_llama_destroy(zl_llama_t* m) {
     for (cudaEvent_t e : m->ring_ev)
         if (e) cudaEventDestroy(e);
     for (cudaEvent_t e : m->pool_ev)
+        if (e) cudaEventDestroy(e);
+    for (cudaEvent_t e : m->rows_ev)
         if (e) cudaEventDestroy(e);
     if (m->reduce_stream) cudaStreamDestroy(m->reduce_stream);
     cudaStreamDestroy(m->stream);
@@ -2133,4 +2164,155 @@ extern "C" int zl_llama_kv_blocks_bench(zl_llama_t* m, int task, const int32_t* 
     if (rc == ZL_ERR_CUDA) zl_set_last_error(__FILE__, __LINE__, "CUDA event failed in zl_llama_kv_blocks_bench");
     if (bytes) *bytes = 2.0 * n * c.num_layers * 2 * (double)(blk + sblk);   // read + write
     return rc;
+}
+
+// ------------------------------------------------------------------------------------------------------------------
+// Beam search (SearcherImplV1 with beam_size > 1, src/generator/batch_generator.cpp:1762-1852): the decode step with the
+// pick replaced by zl_beam_topk, and beam forks as KV row copies between task slots.  The policy -- which candidates live,
+// finish or stop a group, and which slot each beam takes -- is the caller's (zhilight_b200/beam_search.py).
+// ------------------------------------------------------------------------------------------------------------------
+namespace {
+
+constexpr int kBeamK = 32;   // zl_beam_topk's largest K
+
+int ensure_beam(zl_llama* m) {
+    if (m->beam_d) return ZL_OK;
+    const int MB = m->cfg.max_batch;
+    size_t ws = 0;   // the workspace of the largest R <= max_batch
+    for (int r = 1; r <= MB; ++r) {
+        const size_t b = zl_beam_topk_workspace_bytes(r, m->vshard, kBeamK);
+        if (b > ws) ws = b;
+    }
+    const size_t words = (size_t)MB * (3 + 3 * kBeamK);
+    dev_ptr<> d, w;
+    RCHECK(dmalloc(&d, words * 4));
+    RCHECK(dmalloc(&w, ws));
+    int32_t* h = nullptr;
+    ZL_CHECK_CUDA(cudaMallocHost((void**)&h, words * 4));
+    m->beam_h.reset(h);
+    m->beam_d = std::move(d);
+    m->beam_ws = std::move(w);
+    return ZL_OK;
+}
+
+int ensure_row_copies(zl_llama* m) {
+    if (m->rows_tab) return ZL_OK;
+    const int L = m->cfg.num_layers, MB = m->cfg.max_batch;
+    std::vector<void*> h_tab((size_t)4 * L, nullptr);
+    for (int l = 0; l < L; ++l) {
+        const Layer& Ly = m->layers[l];
+        h_tab[4 * l] = Ly.kbuf.get();
+        h_tab[4 * l + 1] = Ly.vbuf.get();
+        h_tab[4 * l + 2] = Ly.skbuf.get();
+        h_tab[4 * l + 3] = Ly.svbuf.get();
+    }
+    dev_ptr<void*> tab;
+    dev_ptr<int32_t> dslots;
+    RCHECK(dmalloc(&tab, sizeof(void*) * 4 * L));
+    RCHECK(dmalloc(&dslots, sizeof(int32_t) * zl_llama::kStageSlots * 4 * MB));
+    int32_t* hs = nullptr;
+    ZL_CHECK_CUDA(cudaMallocHost((void**)&hs, sizeof(int32_t) * zl_llama::kStageSlots * 4 * MB));
+    host_ptr<int32_t> hslots(hs);
+    for (int i = 0; i < zl_llama::kStageSlots; ++i)
+        if (!m->rows_ev[i]) ZL_CHECK_CUDA(cudaEventCreateWithFlags(&m->rows_ev[i], cudaEventDisableTiming));
+    ZL_CHECK_CUDA(cudaMemcpyAsync(tab.get(), h_tab.data(), sizeof(void*) * 4 * L, cudaMemcpyHostToDevice, m->stream));
+    ZL_CHECK_CUDA(cudaStreamSynchronize(m->stream));   // h_tab is pageable and goes out of scope
+    m->rows_tab = std::move(tab);
+    m->rows_d = std::move(dslots);
+    m->rows_h = std::move(hslots);
+    return ZL_OK;
+}
+
+}  // namespace
+
+extern "C" int zl_llama_beam_step(zl_llama_t* m, const int32_t* tokens, const int32_t* positions, int B,
+                                  const int32_t* groups, int G, const float* cum, int K, int32_t* parent, int32_t* token,
+                                  float* score, float* logits_host) {
+    ZL_CHECK_ARG(m && tokens && positions && groups && cum && parent && token && score);
+    ZL_CHECK_ARG(B > 0 && B <= m->cfg.max_batch);
+    RCHECK(beam_topk_check(B, m->vshard, groups, G, K));
+    for (int i = 0; i < B; ++i) ZL_CHECK_ARG(cum[i] < INFINITY);   // -inf: a dead row; NaN and +inf are refused
+    if (m->cfg.tp_size > 1)
+        return fail_state(__LINE__, "beam steps need the whole vocabulary on one rank (tp_size 1)", ZL_ERR_UNSUPPORTED);
+    ZL_CHECK_SUPPORTED(B < 2048);   // the graph key holds B and G in 11 bits
+    if (!m->finalized) return fail_state(__LINE__, "model not finalized");
+    if (sampler_on(m, 0, B)) return fail_state(__LINE__, "a task of the beam step samples or has penalties");
+    RCHECK(ensure_beam(m));
+    const int MB = m->cfg.max_batch;
+    int32_t* d = static_cast<int32_t*>(m->beam_d.get());
+    int32_t* h = m->beam_h.get();
+    // layout (max_batch words each, the outputs 32 x max_batch): cum | groups (2) | parent | token | score
+    BeamPick bp;
+    bp.cum = reinterpret_cast<const float*>(d);
+    bp.groups = d + MB;
+    bp.G = G;
+    bp.K = K;
+    bp.parent = d + 3 * MB;
+    bp.token = bp.parent + kBeamK * MB;
+    bp.score = reinterpret_cast<float*>(bp.token + kBeamK * MB);
+    bp.ws = m->beam_ws.get();
+    RCHECK(zl_llama_set_state(m, tokens, positions, B));   // checks tokens and positions before its copies
+    std::memcpy(h, cum, sizeof(float) * B);
+    std::memcpy(h + MB, groups, sizeof(int32_t) * 2 * G);
+    cudaStream_t st = m->stream;
+    ZL_CHECK_CUDA(cudaMemcpyAsync(d, h, sizeof(float) * B, cudaMemcpyHostToDevice, st));
+    ZL_CHECK_CUDA(cudaMemcpyAsync(d + MB, h + MB, sizeof(int32_t) * 2 * G, cudaMemcpyHostToDevice, st));
+    RCHECK(run_step(m, B, &bp));
+    const size_t n = (size_t)G * K;
+    int32_t* hp = h + 3 * MB;
+    int32_t* ht = hp + kBeamK * MB;
+    int32_t* hs = ht + kBeamK * MB;
+    ZL_CHECK_CUDA(cudaMemcpyAsync(hp, bp.parent, n * 4, cudaMemcpyDeviceToHost, st));
+    ZL_CHECK_CUDA(cudaMemcpyAsync(ht, bp.token, n * 4, cudaMemcpyDeviceToHost, st));
+    ZL_CHECK_CUDA(cudaMemcpyAsync(hs, bp.score, n * 4, cudaMemcpyDeviceToHost, st));
+    if (logits_host)
+        ZL_CHECK_CUDA(cudaMemcpyAsync(logits_host, m->logits.get(), (size_t)B * m->vshard * 4, cudaMemcpyDeviceToHost, st));
+    ZL_CHECK_CUDA(cudaStreamSynchronize(st));   // also frees the pinned staging for the next call
+    std::memcpy(parent, hp, n * 4);
+    std::memcpy(token, ht, n * 4);
+    std::memcpy(score, hs, n * 4);
+    return ZL_OK;
+}
+
+extern "C" int zl_llama_kv_copy_rows(zl_llama_t* m, const int32_t* ranges_host, int n) {
+    ZL_CHECK_ARG(m && ranges_host && n > 0);
+    const auto& c = m->cfg;
+    ZL_CHECK_ARG(n <= c.max_batch);
+    // every check before anything is enqueued
+    std::vector<char> role(c.max_batch, 0);   // 1 source, 2 destination
+    int max_rows = 0;
+    for (int i = 0; i < n; ++i) {
+        const int32_t* r4 = ranges_host + 4 * i;
+        ZL_CHECK_ARG(r4[0] >= 0 && r4[0] < c.max_batch && r4[1] >= 0 && r4[1] < c.max_batch && r4[0] != r4[1]);
+        ZL_CHECK_ARG(r4[2] >= 0 && r4[2] < r4[3] && r4[3] <= c.max_seq);
+        ZL_CHECK_ARG(role[r4[0]] != 2 && role[r4[1]] == 0);   // no destination twice, no task both source and destination
+        role[r4[0]] = 1;
+        role[r4[1]] = 2;
+        if (r4[3] - r4[2] > max_rows) max_rows = r4[3] - r4[2];
+    }
+    if (!m->finalized) return fail_state(__LINE__, "model not finalized");
+    const int row_bytes = m->hkv * c.dim_head * (c.kv_int8 ? 1 : 2);
+    if (row_bytes % 16 != 0)
+        return fail_state(__LINE__, "KV row copies need 16-byte cached rows (H_kv * dim_head)", ZL_ERR_UNSUPPORTED);
+    RCHECK(ensure_row_copies(m));
+    const int slot = m->rows_next;
+    m->rows_next = (slot + 1) % zl_llama::kStageSlots;
+    if (m->rows_used[slot]) ZL_CHECK_CUDA(cudaEventSynchronize(m->rows_ev[slot]));   // its previous copy has executed
+    int32_t* hs = m->rows_h.get() + (size_t)slot * 4 * c.max_batch;
+    int32_t* ds = m->rows_d.get() + (size_t)slot * 4 * c.max_batch;
+    std::memcpy(hs, ranges_host, sizeof(int32_t) * 4 * n);
+    ZL_CHECK_CUDA(cudaMemcpyAsync(ds, hs, sizeof(int32_t) * 4 * n, cudaMemcpyHostToDevice, m->stream));
+    KvRowCopyArgs a{};
+    a.task_bases = m->rows_tab.get();
+    a.ranges = ds;
+    a.n = n;
+    a.layers = c.num_layers;
+    a.task_rows = c.max_seq;
+    a.max_rows = max_rows;
+    a.row_bytes = row_bytes;
+    a.srow_bytes = c.kv_int8 ? m->hkv * 4 : 0;
+    RCHECK(kv_row_copy(a, m->stream));
+    ZL_CHECK_CUDA(cudaEventRecord(m->rows_ev[slot], m->stream));   // after the kernel that reads the device slot
+    m->rows_used[slot] = true;
+    return ZL_OK;
 }

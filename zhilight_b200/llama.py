@@ -10,6 +10,7 @@ import ctypes
 import numpy as np
 
 from . import _lib
+from . import beam_search as _beam
 from .prefix_cache import PrefixCache
 
 MODEL_PRESETS = {
@@ -211,6 +212,47 @@ class LlamaDecoder:
             self.h, int(task), tb.ctypes.data_as(ctypes.c_void_p), pb.ctypes.data_as(ctypes.c_void_p), tb.size,
             int(bool(load)), int(bool(per_range_memcpy)), int(iters), ctypes.byref(ms), ctypes.byref(by)))
         return ms.value / iters, by.value
+
+    def beam_step(self, tokens, positions, groups, cum, k, want_logits=False):
+        """One beam step (zl_llama_beam_step): the decode step over tasks 0 .. B-1 with zl_beam_topk as its pick.
+        groups (G, 2) {row0, width} tile the rows; cum (B) the rows' cumulative log-probabilities (-inf: dead row).
+        Returns (parent, token, score), each (G, k) [, logits (B, V)]."""
+        t = np.ascontiguousarray(tokens, dtype=np.int32)
+        p = np.ascontiguousarray(positions, dtype=np.int32)
+        g = np.ascontiguousarray(groups, dtype=np.int32).reshape(-1, 2)
+        c = np.ascontiguousarray(cum, dtype=np.float32)
+        if c.size != t.size or p.size != t.size:
+            raise ValueError("tokens, positions and cum differ in length (%d, %d, %d)" % (t.size, p.size, c.size))
+        n, k = g.shape[0], int(k)
+        parent = np.empty((n, max(k, 0)), np.int32)
+        token = np.empty_like(parent)
+        score = np.empty((n, max(k, 0)), np.float32)
+        logits = np.empty((t.size, self.vocab_shard), dtype=np.float32) if want_logits else None
+        ptr = lambda a: a.ctypes.data_as(ctypes.c_void_p)
+        _lib.check(self.lib.zl_llama_beam_step(self.h, ptr(t), ptr(p), t.size, ptr(g), n, ptr(c), k, ptr(parent),
+                                               ptr(token), ptr(score), ptr(logits) if want_logits else None))
+        return (parent, token, score, logits) if want_logits else (parent, token, score)
+
+    def kv_copy_rows(self, ranges):
+        """Copy KV rows between tasks, every layer (zl_llama_kv_copy_rows): ranges (n, 4) {src task, dst task, row0, row1};
+        stream-ordered after the steps already issued."""
+        r = np.ascontiguousarray(ranges, dtype=np.int32).reshape(-1, 4)
+        if r.shape[0]:
+            _lib.check(self.lib.zl_llama_kv_copy_rows(self.h, r.ctypes.data_as(ctypes.c_void_p), r.shape[0]))
+
+    def beam_search(self, prompts, beam_width, max_new_tokens, eos_id, num_results=1, trace=None):
+        """Beam search (beam_search.beam_search) over prompts, prompt g in tasks [g W, (g + 1) W): needs
+        max_batch >= len(prompts) * beam_width and, for prompts longer than one token, prefill_chunk > 0.  Returns per
+        prompt up to num_results (tokens, score, cum_logprob) best first; score = cum_logprob / len(tokens + EOS)."""
+        need = len(prompts) * int(beam_width)
+        if need > self.max_batch:
+            raise ValueError("beam search over %d prompts of width %d needs max_batch >= %d (have %d)"
+                             % (len(prompts), beam_width, need, self.max_batch))
+        if self.cfg.prefill_chunk <= 0 and any(len(p) > 1 for p in prompts):
+            raise ValueError("beam search over prompts longer than one token needs prefill_chunk > 0")
+        return _beam.beam_search(
+            lambda t, p, g, c, k: self.beam_step(t, p, g, c, k), self.kv_copy_rows,
+            lambda s, toks: self.prefill(s, toks), prompts, beam_width, max_new_tokens, eos_id, num_results, trace)
 
     def set_sampling(self, task, temperature=0.0, top_p=1.0, top_k=0, repetition_penalty=1.0, presence_penalty=0.0,
                      seed=0):

@@ -548,3 +548,20 @@ def sample(logits, params, row_task=None, counter=None, history=None, pdl=False)
     _lib.call("zl_sample", _p(logits), t, v, _p(dparams), _p(row_task), _p(counter), _p(history), hw, _p(out), None, 0,
               int(pdl), _stream())
     return out
+
+
+def beam_topk(logits, cum, groups, k, pdl=False):
+    """zl_beam_topk: logits (R, V) fp32 and cum (R) fp32 CUDA tensors, groups (G, 2) {row0, width} host ints.
+    -> (parent, token, score), each (G, k) on the device."""
+    import numpy as np
+    r, v = logits.shape
+    g = np.ascontiguousarray(groups, dtype=np.int32).reshape(-1, 2)
+    n = g.shape[0]
+    parent = torch.empty((n, k), dtype=torch.int32, device=logits.device)
+    token = torch.empty_like(parent)
+    score = torch.empty((n, k), dtype=torch.float32, device=logits.device)
+    nb = _lib.load().zl_beam_topk_workspace_bytes(r, v, k)
+    ws = torch.empty(max(nb, 16), dtype=torch.uint8, device=logits.device)
+    _lib.call("zl_beam_topk", _p(logits), r, v, _p(cum), g.ctypes.data_as(ctypes.c_void_p), n, k, _p(parent), _p(token),
+              _p(score), _p(ws), nb, int(pdl), _stream())
+    return parent, token, score

@@ -402,6 +402,32 @@ size_t zl_sample_workspace_bytes(int T, int V);
 int zl_sample(const float* logits, int T, int V, const zl_sample_params_t* params, const int32_t* row_task,
               const int32_t* counter, uint32_t* history, int history_words, int32_t* out, void* ws, size_t ws_bytes,
               int pdl, zl_stream_t stream);
+/* Logits processors on top of zl_sample: the n-gram repetition penalty (calc_repetition_ngram +
+ * apply_beam_repetition_penalty, generator/beam_util.cu:318-375, chosen at batch_generator.cpp:1662-1705) and logit_bias
+ * (SearcherImplV1::add_logit_bias, batch_generator.cpp:1709-1728).  For a row of task t, on a copy of its fp32 logits:
+ *   1. penalties.  ngram_penalty[t] > 1: with r the task's sequence most recent first and lev[j] the reference's
+ *      ngrams[j] of r (KMP next[] over r, then ngrams[i - L] = max(ngrams[i - L], L) with L = next[i] + 1), every token
+ *      occurring in r gets f = max over its occurrences j of powf(ngram_penalty, lev[j] + 1) * repetition_penalty and
+ *      l = l < 0 ? l * f : l / f; presence_penalty is ignored (the reference's n-gram path passes no presence values).
+ *      Otherwise (ngram_penalty NULL or <= 1) zl_sample's bitmap rule, unchanged;
+ *   2. l += bias for each (token, bias) entry of the task, in fp32 (the reference adds it in the logits dtype);
+ *   3. the pick: steps 2-5 of zl_sample's contract on the processed row.
+ * The rule is chosen per task, so a row's token depends only on its logits, its task's parameters, bias list and
+ * sequence, and its counter; never on the batch (the reference decides the n-gram path per batch).
+ * ngram_penalty (tasks) fp32 or NULL (no n-gram launch); seq (tasks, seq_stride) int32 generated tokens, oldest first, with
+ * seq_len (tasks): the pick is appended there (dropped once seq_len == seq_stride), as zl_sample records it into history;
+ * rows naming one task must not pass a sequence.  bias_tokens / bias_values (tasks, bias_stride) with bias_count (tasks),
+ * or NULL: distinct tokens per task (a repeated token is added once per entry; ids outside [0, V) are ignored).
+ * ws: zl_sample_processed_workspace_bytes(T, seq_stride) bytes when ngram_penalty is given (k_ngram_levels writes each
+ * row's distinct tokens and levels there), else may be NULL.  Launches: k_sample, plus k_ngram_levels (one CTA per row;
+ * rows whose task has ngram_penalty <= 1 exit at once) when ngram_penalty is given. */
+#define ZL_MAX_LOGIT_BIAS 1024
+size_t zl_sample_processed_workspace_bytes(int T, int seq_stride);
+int zl_sample_processed(const float* logits, int T, int V, const zl_sample_params_t* params, const int32_t* row_task,
+                        const int32_t* counter, uint32_t* history, int history_words, const float* ngram_penalty,
+                        int32_t* seq, int32_t* seq_len, int seq_stride, const int32_t* bias_tokens,
+                        const float* bias_values, const int32_t* bias_count, int bias_stride, int32_t* out, void* ws,
+                        size_t ws_bytes, int pdl, zl_stream_t stream);
 /* Beam-search selection (beam_utility::log_softmax_bias, generator/beam_util.cu:20-130, then topk_all.get_top_k over each
  * task's flattened (beam x vocab) scores, generator/batch_generator.cpp:1770-1778), without writing an (R, V) tensor.
  * logits (R, V) fp32 and cum (R) fp32 on the device; groups (G, 2) {row0, width} a HOST array whose groups tile rows
@@ -538,12 +564,22 @@ int zl_llama_prefill(zl_llama_t* m, int task, const int32_t* tokens_host, int n,
 int zl_llama_step_joined(zl_llama_t* m, const int32_t* tokens_host, const int32_t* seg_host, int nseg, int32_t* next_host,
                          float* logits_host);
 /* Per-task sampling (zl_sample's contract) for the picks of zl_llama_decode / step_device / prefill.  Copies *p (HOST
- * pointer) to the device and clears the task's history; p == NULL returns the task to plain greedy.  Invalid values:
+ * pointer) to the device and clears the task's history and generated-token sequence; p == NULL returns the task to plain greedy.  Invalid values:
  * ZL_ERR_INVALID_ARG; anything but plain greedy under tp_size > 1: ZL_ERR_UNSUPPORTED (vocabulary shards would need a
  * global top-k / top-p threshold).  The decode step runs zl_sample instead of zl_argmax while a task in the batch
  * samples or has penalties (counter = the input token's position; prefill: pos0 + n - 1), so a task draws the same
  * tokens with host or device-resident stepping, with or without the graph.  The logits stay the raw lm_head output. */
 int zl_llama_set_sampling(zl_llama_t* m, int task, const zl_sample_params_t* p);
+/* Per-task logits processors (zl_sample_processed's contract) for the picks of zl_llama_decode / step_device / prefill /
+ * step_joined.  Stream-ordered after the steps already enqueued; the HOST arrays are staged before the call returns.
+ * ngram_penalty finite and > 0 (<= 1: off, batch_generator.cpp:1664); n_bias in [0, ZL_MAX_LOGIT_BIAS] distinct tokens in
+ * [0, vocab) with finite or -inf values (NaN and +inf are refused): ZL_ERR_INVALID_ARG otherwise.  n_bias = 0 with
+ * ngram_penalty <= 1 returns the task to plain behaviour.  Anything on under tp_size > 1: ZL_ERR_UNSUPPORTED.  Every
+ * check runs before anything is enqueued.  A task with processors makes its batch's pick run the sampler, as a penalty
+ * does.  The n-gram rule reads the task's generated-token sequence: the picks of the sampler route since
+ * zl_llama_set_sampling last cleared it, up to max_seq tokens (later picks are not recorded). */
+int zl_llama_set_logits_processors(zl_llama_t* m, int task, float ngram_penalty, const int32_t* bias_tokens_host,
+                                   const float* bias_values_host, int n_bias);
 /* Copy rows row0 .. row0 + n of task `task`'s layer-`layer` KV cache to the host (the reference's dump_task_buf,
  * rag_buffer_context.h:199-233).  Synchronous.  Plain cache: k_host / v_host get (n, H_kv, d) activation-dtype values and
  * sk_host / sv_host must be NULL.  kv_int8: k_host / v_host get (n, H_kv, d) uint8 codes and sk_host / sv_host (n, H_kv)
@@ -590,7 +626,8 @@ int zl_llama_kv_blocks_bench(zl_llama_t* m, int task, const int32_t* task_blocks
  * replaced by zl_beam_topk on the step's logits -- same CUDA graph, one per (B, G, K, length bucket), no argmax.  groups
  * (G, 2), cum (B) HOST; parent / token / score (G, K) HOST outputs as zl_beam_topk's; logits_host NULL or (B, vocab).
  * Synchronous.  Bad groups, K, cum (NaN or +inf), tokens or positions: ZL_ERR_INVALID_ARG; vocab > 262144 or tp_size > 1:
- * ZL_ERR_UNSUPPORTED; a task of the batch that samples or has penalties (zl_llama_set_sampling): ZL_ERR_STATE. */
+ * ZL_ERR_UNSUPPORTED; a task of the batch that samples or has penalties (zl_llama_set_sampling) or logits processors
+ * (zl_llama_set_logits_processors): ZL_ERR_STATE. */
 int zl_llama_beam_step(zl_llama_t* m, const int32_t* tokens, const int32_t* positions, int B, const int32_t* groups, int G,
                        const float* cum, int K, int32_t* parent, int32_t* token, float* score, float* logits_host);
 /* Beam forks: one launch copies rows [row0, row1) of task src into task dst for every range ranges_host[i] = {src task,

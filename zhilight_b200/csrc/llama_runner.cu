@@ -13,6 +13,7 @@
 #include "kv_pool.cuh"
 #include "beam.cuh"
 
+#include <algorithm>
 #include <cstdlib>
 #include <cstring>
 #include <map>
@@ -142,7 +143,18 @@ struct zl_llama {
     dev_ptr<zl_sample_params_t> d_sparams;   // (max_batch)
     dev_ptr<uint32_t> d_hist;                // (max_batch, hwords)
     int hwords = 0;
-    std::vector<char> samp_on;
+    std::vector<char> samp_on;               // pen_on[t] || proc_on[t]
+    std::vector<char> pen_on;                // set by zl_llama_set_sampling: samples or has penalties
+    // logits processors (zl_llama_set_logits_processors): per-task n-gram penalty and bias lists, and every task's
+    // generated-token sequence (appended by the sampler where it sets the history bit, cleared with it); the n-gram
+    // workspace (k_ngram_levels' tables, max_batch rows) is allocated by the first task that turns the n-gram rule on
+    dev_ptr<float> d_ngram;                  // (max_batch)
+    dev_ptr<int32_t> d_seq, d_seq_len;       // (max_batch, max_seq), (max_batch)
+    dev_ptr<int32_t> d_bias_tok, d_bias_cnt; // (max_batch, ZL_MAX_LOGIT_BIAS), (max_batch)
+    dev_ptr<float> d_bias_val;               // (max_batch, ZL_MAX_LOGIT_BIAS)
+    dev_ptr<> ngram_ws;
+    size_t ngram_ws_bytes = 0;
+    std::vector<char> proc_on, ngram_on;
     // int8 KV cache: the rotated fp16 K / V rows of the launch sequence are staged in kv_stage (k: tok_cap x Hkv x d, then
     // v) and quantised into the cache from there.  A qkv GEMM with the RoPE / KV-append epilogue appends into the staging
     // rows as into the cache of one task: stage_addrs = {k rows, v rows}, token -> task map d_zeros, placement d_rowidx.
@@ -828,6 +840,18 @@ int alloc_runtime(zl_llama* m) {
         ZL_CHECK_CUDA(cudaStreamSynchronize(m->stream));   // `init` is pageable and goes out of scope
     }
     m->samp_on.assign(B, 0);
+    m->pen_on.assign(B, 0);
+    m->proc_on.assign(B, 0);
+    m->ngram_on.assign(B, 0);
+    RCHECK(dmalloc(&m->d_ngram, (size_t)B * 4));
+    RCHECK(dmalloc(&m->d_seq, (size_t)B * c.max_seq * 4));
+    RCHECK(dmalloc(&m->d_seq_len, (size_t)B * 4));
+    RCHECK(dmalloc(&m->d_bias_tok, (size_t)B * ZL_MAX_LOGIT_BIAS * 4));
+    RCHECK(dmalloc(&m->d_bias_val, (size_t)B * ZL_MAX_LOGIT_BIAS * 4));
+    RCHECK(dmalloc(&m->d_bias_cnt, (size_t)B * 4));
+    ZL_CHECK_CUDA(cudaMemsetAsync(m->d_ngram.get(), 0, (size_t)B * 4, m->stream));   // 0.0f: off
+    ZL_CHECK_CUDA(cudaMemsetAsync(m->d_seq_len.get(), 0, (size_t)B * 4, m->stream));
+    ZL_CHECK_CUDA(cudaMemsetAsync(m->d_bias_cnt.get(), 0, (size_t)B * 4, m->stream));
     int32_t *stage = nullptr, *ring = nullptr;
     ZL_CHECK_CUDA(cudaMallocHost((void**)&stage, sizeof(int32_t) * (4 * B + 4 + T)));
     m->h_stage.reset(stage);
@@ -1250,7 +1274,7 @@ struct BeamPick {
 };
 
 int enqueue_step(zl_llama* m, int n_tasks, int len_bucket, const Segments* pf = nullptr, bool sampler = false,
-                 const BeamPick* beam = nullptr) {
+                 const BeamPick* beam = nullptr, bool ngram = false) {
     const auto& c = m->cfg;
     const int B = pf ? pf->n : n_tasks;   // rows (tokens) of every activation matrix in this launch sequence
     const int D = c.dim_model, d = c.dim_head, dt = c.dtype, pdl = c.use_pdl;
@@ -1393,8 +1417,12 @@ int enqueue_step(zl_llama* m, int n_tasks, int len_bucket, const Segments* pf = 
         // parallelism.
         const int32_t* row_task = joined ? j_task : pf ? m->d_iota.get() + pf->task : m->d_iota.get();
         const int32_t* counter = joined ? j_pos : pf ? m->d_pf_pos.get() + (pf->n - 1) : m->d_pos.get();
-        RCHECK(zl_sample(m->logits.get(), HB, m->vshard, m->d_sparams.get(), row_task, counter, m->d_hist.get(), m->hwords,
-                         m->d_next.get(), nullptr, 0, stage_pdl(m, kPick), st));
+        // k_ngram_levels runs only when a task of the step has the n-gram rule on (`ngram`, a bit of the graph key)
+        RCHECK(zl_sample_processed(m->logits.get(), HB, m->vshard, m->d_sparams.get(), row_task, counter, m->d_hist.get(),
+                                   m->hwords, ngram ? m->d_ngram.get() : nullptr, m->d_seq.get(), m->d_seq_len.get(),
+                                   c.max_seq, m->d_bias_tok.get(), m->d_bias_val.get(), m->d_bias_cnt.get(),
+                                   ZL_MAX_LOGIT_BIAS, m->d_next.get(), ngram ? m->ngram_ws.get() : nullptr,
+                                   m->ngram_ws_bytes, stage_pdl(m, kPick), st));
     } else if (!tp) {
         RCHECK(zl_argmax(m->logits.get(), m->d_next.get(), HB, m->vshard, m->argmax_ws.get(), zl_argmax_workspace_bytes(HB),
                          stage_pdl(m, kPick), st));
@@ -1422,19 +1450,26 @@ bool sampler_on(const zl_llama* m, int first, int n) {
     return false;
 }
 
+bool ngram_on(const zl_llama* m, int first, int n) {
+    for (int t = first; t < first + n; ++t)
+        if (m->ngram_on[t]) return true;
+    return false;
+}
+
 int run_step(zl_llama* m, int B, const BeamPick* beam = nullptr) {
     const int bucket = len_bucket_of(m, m->cur_max_len);
-    const bool sampler = sampler_on(m, 0, B);
-    if (!m->cfg.use_graph) return enqueue_step(m, B, bucket, nullptr, sampler, beam);
-    // parameter changes need no re-capture (they live on the device), only switching the sampler on or off does.  A beam
-    // step (bit 62) bakes its group count (bits 44-54) and K (bits 55-60) into its launches; B < 2048 at a beam step.
-    long long key = ((long long)B << 33) | ((long long)sampler << 32) | (unsigned)bucket;
+    const bool sampler = sampler_on(m, 0, B), ngram = ngram_on(m, 0, B);
+    if (!m->cfg.use_graph) return enqueue_step(m, B, bucket, nullptr, sampler, beam, ngram);
+    // parameter changes need no re-capture (they live on the device), only switching the sampler (bit 32) or the n-gram
+    // launch (bit 31; buckets stay below 2^31) on or off does.  A beam step (bit 62) bakes its group count (bits 44-54)
+    // and K (bits 55-60) into its launches; B < 2048 at a beam step.
+    long long key = ((long long)B << 33) | ((long long)sampler << 32) | ((long long)ngram << 31) | (unsigned)bucket;
     if (beam) key |= (1LL << 62) | ((long long)beam->K << 55) | ((long long)beam->G << 44);
     auto it = m->graphs.find(key);
     if (it == m->graphs.end()) {
         cudaGraph_t graph = nullptr;
         ZL_CHECK_CUDA(cudaStreamBeginCapture(m->stream, cudaStreamCaptureModeThreadLocal));
-        int rc = enqueue_step(m, B, bucket, nullptr, sampler, beam);
+        int rc = enqueue_step(m, B, bucket, nullptr, sampler, beam, ngram);
         cudaError_t ce = cudaStreamEndCapture(m->stream, &graph);
         if (rc != ZL_OK) {
             if (graph) cudaGraphDestroy(graph);
@@ -1844,7 +1879,7 @@ extern "C" int zl_llama_prefill(zl_llama_t* m, int task, const int32_t* tokens_h
         pc.pos0 = pos0 + c0;
         pc.n = cn;
         pc.last = c0 + cn == n;
-        RCHECK(enqueue_step(m, 1, 0, &pc, sampler_on(m, task, 1)));
+        RCHECK(enqueue_step(m, 1, 0, &pc, sampler_on(m, task, 1), nullptr, ngram_on(m, task, 1)));
     }
     ZL_CHECK_CUDA(cudaMemcpyAsync(m->h_stage.get() + 3 * m->cfg.max_batch, m->d_next.get(), 4, cudaMemcpyDeviceToHost, m->stream));
     if (logits_host)
@@ -1895,7 +1930,7 @@ extern "C" int zl_llama_step_joined(zl_llama_t* m, const int32_t* tokens_host, c
     sg.joined = true;
     sg.n = rows;
     sg.nseg = nseg;
-    bool sampler = false;
+    bool sampler = false, ngram = false;
     for (int s = 0, row0 = 0; s < nseg; ++s) {
         const int task = seg_host[4 * s], pos0 = seg_host[4 * s + 1], n = seg_host[4 * s + 2];
         for (int i = 0; i < n; ++i) {
@@ -1913,6 +1948,7 @@ extern "C" int zl_llama_step_joined(zl_llama_t* m, const int32_t* tokens_host, c
             h_epos[sg.n_emit] = pos0 + n - 1;
             ++sg.n_emit;
             sampler |= m->samp_on[task] != 0;
+            ngram |= m->ngram_on[task] != 0;
         }
         if (pos0 + n > sg.max_keys) sg.max_keys = pos0 + n;
         row0 += n;
@@ -1922,7 +1958,7 @@ extern "C" int zl_llama_step_joined(zl_llama_t* m, const int32_t* tokens_host, c
     ZL_CHECK_CUDA(cudaMemcpyAsync(m->d_pf_pos.get(), h_pos, (size_t)rows * 4, cudaMemcpyHostToDevice, st));
     ZL_CHECK_CUDA(cudaMemcpyAsync(m->d_tb.get(), h_tb, (size_t)rows * 4, cudaMemcpyHostToDevice, st));
     ZL_CHECK_CUDA(cudaMemcpyAsync(m->d_join.get(), h_seg, (size_t)7 * MB * 4, cudaMemcpyHostToDevice, st));
-    RCHECK(enqueue_step(m, 0, 0, &sg, sampler));
+    RCHECK(enqueue_step(m, 0, 0, &sg, sampler, nullptr, ngram));
     int32_t* h_next = m->h_stage.get() + 3 * MB;
     if (sg.n_emit) {
         ZL_CHECK_CUDA(cudaMemcpyAsync(h_next, m->d_next.get(), (size_t)sg.n_emit * 4, cudaMemcpyDeviceToHost, st));
@@ -1950,7 +1986,45 @@ extern "C" int zl_llama_set_sampling(zl_llama_t* m, int task, const zl_sample_pa
     // stream-ordered after every step already enqueued; the pageable source is staged before the call returns
     ZL_CHECK_CUDA(cudaMemcpyAsync(m->d_sparams.get() + task, &q, sizeof(q), cudaMemcpyHostToDevice, m->stream));
     ZL_CHECK_CUDA(cudaMemsetAsync(m->d_hist.get() + (size_t)task * m->hwords, 0, (size_t)m->hwords * 4, m->stream));
-    m->samp_on[task] = on ? 1 : 0;
+    ZL_CHECK_CUDA(cudaMemsetAsync(m->d_seq_len.get() + task, 0, 4, m->stream));
+    m->pen_on[task] = on ? 1 : 0;
+    m->samp_on[task] = m->pen_on[task] || m->proc_on[task];
+    return ZL_OK;
+}
+
+extern "C" int zl_llama_set_logits_processors(zl_llama_t* m, int task, float ngram_penalty, const int32_t* bias_tokens_host,
+                                              const float* bias_values_host, int n_bias) {
+    ZL_CHECK_ARG(m && task >= 0 && task < m->cfg.max_batch);
+    ZL_CHECK_ARG(ngram_penalty > 0.f && ngram_penalty < INFINITY);
+    ZL_CHECK_ARG(n_bias >= 0 && n_bias <= ZL_MAX_LOGIT_BIAS);
+    ZL_CHECK_ARG(n_bias == 0 || (bias_tokens_host && bias_values_host));
+    std::vector<int32_t> sorted(bias_tokens_host, bias_tokens_host + n_bias);
+    for (int i = 0; i < n_bias; ++i) {
+        ZL_CHECK_ARG(bias_tokens_host[i] >= 0 && bias_tokens_host[i] < m->cfg.vocab_size);
+        ZL_CHECK_ARG(bias_values_host[i] < INFINITY);   // finite or -inf: NaN and +inf fail
+    }
+    std::sort(sorted.begin(), sorted.end());
+    ZL_CHECK_ARG(std::adjacent_find(sorted.begin(), sorted.end()) == sorted.end());
+    const bool ngram = ngram_penalty > 1.f, on = ngram || n_bias > 0;
+    ZL_CHECK_SUPPORTED(!on || m->cfg.tp_size == 1);
+    if (!m->finalized) return fail_state(__LINE__, "model not finalized");
+    if (ngram && !m->ngram_ws) {
+        m->ngram_ws_bytes = zl_sample_processed_workspace_bytes(m->cfg.max_batch, m->cfg.max_seq);
+        RCHECK(dmalloc(&m->ngram_ws, m->ngram_ws_bytes));
+    }
+    // stream-ordered after every step already enqueued; pageable sources are staged before the copies return
+    cudaStream_t st = m->stream;
+    ZL_CHECK_CUDA(cudaMemcpyAsync(m->d_ngram.get() + task, &ngram_penalty, 4, cudaMemcpyHostToDevice, st));
+    if (n_bias > 0) {
+        ZL_CHECK_CUDA(cudaMemcpyAsync(m->d_bias_tok.get() + (size_t)task * ZL_MAX_LOGIT_BIAS, bias_tokens_host,
+                                      (size_t)n_bias * 4, cudaMemcpyHostToDevice, st));
+        ZL_CHECK_CUDA(cudaMemcpyAsync(m->d_bias_val.get() + (size_t)task * ZL_MAX_LOGIT_BIAS, bias_values_host,
+                                      (size_t)n_bias * 4, cudaMemcpyHostToDevice, st));
+    }
+    ZL_CHECK_CUDA(cudaMemcpyAsync(m->d_bias_cnt.get() + task, &n_bias, 4, cudaMemcpyHostToDevice, st));
+    m->proc_on[task] = on ? 1 : 0;
+    m->ngram_on[task] = ngram ? 1 : 0;
+    m->samp_on[task] = m->pen_on[task] || m->proc_on[task];
     return ZL_OK;
 }
 
@@ -2236,7 +2310,7 @@ extern "C" int zl_llama_beam_step(zl_llama_t* m, const int32_t* tokens, const in
         return fail_state(__LINE__, "beam steps need the whole vocabulary on one rank (tp_size 1)", ZL_ERR_UNSUPPORTED);
     ZL_CHECK_SUPPORTED(B < 2048);   // the graph key holds B and G in 11 bits
     if (!m->finalized) return fail_state(__LINE__, "model not finalized");
-    if (sampler_on(m, 0, B)) return fail_state(__LINE__, "a task of the beam step samples or has penalties");
+    if (sampler_on(m, 0, B)) return fail_state(__LINE__, "a task of the beam step samples, has penalties or has logits processors");
     RCHECK(ensure_beam(m));
     const int MB = m->cfg.max_batch;
     int32_t* d = static_cast<int32_t*>(m->beam_d.get());

@@ -14,6 +14,11 @@
 // Masses are fixed point: w = round(exp(x - max x) * 2^44) as uint64, so sums are exact integers and do not depend on
 // the summation order (a launch is reproducible bit for bit, whatever the atomics' order).  A token whose weight is below
 // ~2^-45 of the maximum gets mass 0 and is never picked (probability < 3e-14 under the exact contract).
+//
+// Logits processors (zl_sample_processed): the n-gram repetition penalty (calc_repetition_ngram +
+// apply_beam_repetition_penalty, src/generator/beam_util.cu:318-375) and logit_bias (SearcherImplV1::add_logit_bias,
+// batch_generator.cpp:1709-1728).  k_ngram_levels gives each distinct token of a task's generated sequence its largest
+// n-gram level, in a per-row hash table; k_sample then stages a processed copy of its slice in shared memory.
 #include "common.cuh"
 
 #include <cooperative_groups.h>
@@ -196,10 +201,107 @@ __device__ SelResult cluster_select(SampleShared& s, cg::cluster_group& cl, cons
     return r;
 }
 
+// The processors' device arguments (zl_sample_processed); all NULL for zl_sample.
+struct SampleProc {
+    const float* ngram;       // (tasks) or NULL: no n-gram rule
+    int32_t* seq;             // (tasks, seq_stride) generated tokens, oldest first, or NULL
+    int32_t* seq_len;         // (tasks)
+    int seq_stride;
+    const int32_t* bias_tok;  // (tasks, bias_stride) or NULL
+    const float* bias_val;
+    const int32_t* bias_cnt;  // (tasks)
+    int bias_stride;
+    int2* table;              // k_ngram_levels' output: per row, table_stride {token, level} slots
+    int table_stride;
+};
+
+constexpr int kNgramThreads = 1024;
+constexpr int kNgramSmem = 12032;   // sequence elements staged in shared memory; the rest is read from global memory
+
+// hash table slots for n distinct tokens at most: a power of two >= 2n, so an insert always finds a free slot
+__host__ __device__ inline int ngram_table_size(int n) {
+    int h = 2;
+    while (h < 2 * n) h <<= 1;
+    return h;
+}
+
+// Fibonacci hashing: the top log2(h) bits of tok * 2^32 / phi (h is a power of two >= 2)
+__device__ __forceinline__ int ngram_slot(int tok, int h) {
+    return (int)(((uint32_t)tok * 2654435761u) >> (32 - (__ffs(h) - 1)));
+}
+
+// open addressing: the slot of `tok` keeps the largest level inserted for it
+__device__ void ngram_insert(int2* tab, int h, int tok, int lev) {
+    if (tok < 0) return;   // -1 marks an empty slot; a negative id never matches a vocabulary slice
+    for (int i = ngram_slot(tok, h);; i = (i + 1) & (h - 1)) {
+        const int prev = atomicCAS(&tab[i].x, -1, tok);
+        if (prev == -1 || prev == tok) {
+            if (lev > 0) atomicMax(&tab[i].y, lev);
+            return;
+        }
+    }
+}
+
+// One CTA per row whose task has ngram > 1.  r = the task's sequence, most recent first (r[k] = seq[n-1-k]).  The
+// reference's levels (KMP next[] over r, then ngrams[i - L] = max(ngrams[i - L], L) with L = next[i] + 1) equal, with
+// z the Z-function of r and R(s) = max(0, max over s' < s of s' + z[s'] - 1):
+//   lev[s-1] = z[s] where z[s] > 0 and s + z[s] - 1 > R(s), and 0 everywhere else.
+// One thread per start s extends z[s] by direct comparison (work = sum of z: ~n / alphabet on text, n^2 / 2 for one
+// repeated token); a block max-scan over tiles of 1024 starts carries R.  Writes, for every distinct token of r, its
+// largest level into the row's table of ngram_table_size(n) slots.
+__global__ void __launch_bounds__(kNgramThreads) k_ngram_levels(int T, const int32_t* __restrict__ row_task, SampleProc pr) {
+    __shared__ int rs[kNgramSmem];
+    __shared__ int wmax[kNgramThreads / 32];
+    __shared__ int carry;
+    const int row = blockIdx.x, tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+    pdl_trigger();
+    pdl_wait();
+    if (row >= T) return;
+    const int task = row_task ? row_task[row] : row;
+    if (!(pr.ngram[task] > 1.f)) return;
+    const int n = min(max(pr.seq_len[task], 0), pr.seq_stride);
+    const int32_t* sq = pr.seq + (size_t)task * pr.seq_stride;
+    int2* tab = pr.table + (size_t)row * pr.table_stride;
+    const int h = ngram_table_size(n);
+    for (int k = tid; k < min(n, kNgramSmem); k += kNgramThreads) rs[k] = sq[n - 1 - k];
+    for (int i = tid; i < h; i += kNgramThreads) tab[i] = make_int2(-1, 0);
+    if (tid == 0) carry = 0;
+    __syncthreads();
+    auto at = [&](int k) { return k < kNgramSmem ? rs[k] : sq[n - 1 - k]; };
+    for (int base = 1; base < n; base += kNgramThreads) {
+        const int s = base + tid;
+        int z = 0;
+        if (s < n)
+            while (s + z < n && at(s + z) == at(z)) ++z;
+        const int e = s < n ? s + z - 1 : 0;
+        int inc = e;   // inclusive max-scan within the warp
+#pragma unroll
+        for (int o = 1; o < 32; o <<= 1) {
+            const int v = __shfl_up_sync(0xffffffffu, inc, o);
+            if (lane >= o) inc = max(inc, v);
+        }
+        const int exc = __shfl_up_sync(0xffffffffu, inc, 1);
+        if (lane == 31) wmax[warp] = inc;
+        __syncthreads();
+        int R = carry;
+        for (int w = 0; w < warp; ++w) R = max(R, wmax[w]);
+        if (lane > 0) R = max(R, exc);
+        if (s < n) ngram_insert(tab, h, at(s - 1), (z > 0 && e > R) ? z : 0);
+        __syncthreads();   // every thread has read carry and wmax
+        if (tid == 0) {
+            int c = carry;
+            for (int w = 0; w < kNgramThreads / 32; ++w) c = max(c, wmax[w]);
+            carry = c;
+        }
+        __syncthreads();
+    }
+    if (tid == 0 && n > 0) ngram_insert(tab, h, at(n - 1), 0);   // the oldest token has level 0
+}
+
 __global__ void __cluster_dims__(kSampleCluster, 1, 1) __launch_bounds__(kSampleThreads, 1)
     k_sample(const float* __restrict__ logits, int T, int V, int S, const zl_sample_params_t* __restrict__ params,
              const int32_t* __restrict__ row_task, const int32_t* __restrict__ counter, uint32_t* __restrict__ history,
-             int hwords, int32_t* __restrict__ out) {
+             int hwords, int32_t* __restrict__ out, SampleProc pr) {
     extern __shared__ float xs[];
     __shared__ SampleShared s;
     cg::cluster_group cl = cg::this_cluster();
@@ -216,14 +318,52 @@ __global__ void __cluster_dims__(kSampleCluster, 1, 1) __launch_bounds__(kSample
     const int lo = rank * S;
     const int n = max(0, min(V, lo + S) - lo);
     const float* src = logits + (size_t)row * V + lo;
+    const int nbias = pr.bias_tok ? min(pr.bias_cnt[task], pr.bias_stride) : 0;
+    const float ngram = pr.ngram ? pr.ngram[task] : 1.f;
+    const bool proc = nbias > 0 || ngram > 1.f;
+    if (proc) {
+        // this thread's first bias entry, loaded before the slice so that its latency overlaps the slice's
+        const int32_t* bt = pr.bias_tok + (size_t)task * pr.bias_stride;
+        const float* bv = pr.bias_val + (size_t)task * pr.bias_stride;
+        const int g0 = tid < nbias ? bt[tid] : -1;
+        const float b0 = tid < nbias ? bv[tid] : 0.f;
+        // the processed slice in shared memory: penalties (the n-gram rule replaces the bitmap rule), then the bias
+        for (int i = tid; i < n; i += kSampleThreads) {
+            float l = src[i];
+            const int g = lo + i;
+            if (!(ngram > 1.f) && pen && ((hist[g >> 5] >> (g & 31)) & 1u))
+                l = p.presence_penalty != 0.f ? l - p.presence_penalty
+                                              : (l < 0.f ? l * p.repetition_penalty : l / p.repetition_penalty);
+            xs[i] = l;
+        }
+        __syncthreads();
+        if (ngram > 1.f) {   // each table slot names a distinct token: no two threads touch one element
+            const int2* tab = pr.table + (size_t)row * pr.table_stride;
+            const int h = ngram_table_size(min(max(pr.seq_len[task], 0), pr.seq_stride));
+            for (int i = tid; i < h; i += kSampleThreads) {
+                const int2 e = tab[i];
+                if (e.x < lo || e.x >= lo + n) continue;
+                const float f = powf(ngram, (float)(e.y + 1)) * p.repetition_penalty;   // beam_util.cu:345, :368
+                const float l = xs[e.x - lo];
+                xs[e.x - lo] = l < 0.f ? l * f : l / f;
+            }
+            __syncthreads();
+        }
+        if (g0 >= lo && g0 < lo + n) xs[g0 - lo] += b0;   // distinct tokens (zl_llama_set_logits_processors checks)
+        for (int j = tid + kSampleThreads; j < nbias; j += kSampleThreads) {
+            const int g = bt[j];
+            if (g >= lo && g < lo + n) xs[g - lo] += bv[j];
+        }
+        __syncthreads();
+    }
 
     // pass 1: penalties, the greedy pick of the penalised row (zl_argmax's rule: max, ties -> lowest index), max of x
     float best = -INFINITY, xmax = -INFINITY;
     int bi = 0x7fffffff;
     for (int i = tid; i < n; i += kSampleThreads) {
-        float l = src[i];
+        float l = proc ? xs[i] : src[i];
         const int g = lo + i;
-        if (pen && ((hist[g >> 5] >> (g & 31)) & 1u)) {   // beam_util.cu:212-219
+        if (!proc && pen && ((hist[g >> 5] >> (g & 31)) & 1u)) {   // beam_util.cu:212-219
             if (p.presence_penalty != 0.f)
                 l = l - p.presence_penalty;
             else
@@ -397,6 +537,13 @@ __global__ void __cluster_dims__(kSampleCluster, 1, 1) __launch_bounds__(kSample
     if (owner && tid == 0) {
         out[row] = tok;
         if (hist) atomicOr(&hist[tok >> 5], 1u << (tok & 31));
+        if (pr.seq) {   // appends past the capacity are dropped
+            const int len = pr.seq_len[task];
+            if (len >= 0 && len < pr.seq_stride) {
+                pr.seq[(size_t)task * pr.seq_stride + len] = tok;
+                pr.seq_len[task] = len + 1;
+            }
+        }
     }
     cl.sync();   // no CTA leaves while another may still read its shared memory
 }
@@ -437,19 +584,55 @@ int prepare_sample() {
     return ZL_OK;
 }
 
+// the one launcher behind zl_sample and zl_sample_processed
+static int sample_launch(const float* logits, int T, int V, const zl_sample_params_t* params, const int32_t* row_task,
+                  const int32_t* counter, uint32_t* history, int history_words, const SampleProc& pr, int32_t* out,
+                  int pdl, cudaStream_t stream) {
+    ZL_CHECK_ARG(logits && params && out && T > 0 && V > 0);
+    ZL_CHECK_SUPPORTED(V <= kSampleMaxVocab);
+    ZL_CHECK_ARG(!history || history_words >= cdiv(V, 32));
+    const int rc = prepare_sample();
+    if (rc != ZL_OK) return rc;
+    if (pr.ngram)
+        ZL_CHECK_CUDA(launch(k_ngram_levels, dim3(T), dim3(kNgramThreads), 0, stream, pdl != 0, T, row_task, pr));
+    const int S = cdiv(V, kSampleCluster);
+    const int ty = T < 65535 ? T : 65535;   // rows: blockIdx.z * gridDim.y + blockIdx.y
+    ZL_CHECK_CUDA(launch(k_sample, dim3(kSampleCluster, ty, cdiv(T, ty)), dim3(kSampleThreads), (size_t)S * sizeof(float),
+                         stream, pdl != 0, logits, T, V, S, params, row_task, counter, history, history_words, out, pr));
+    return ZL_OK;
+}
+
 extern "C" int zl_sample(const float* logits, int T, int V, const zl_sample_params_t* params, const int32_t* row_task,
                          const int32_t* counter, uint32_t* history, int history_words, int32_t* out, void* ws,
                          size_t ws_bytes, int pdl, zl_stream_t stream) {
     (void)ws;
-    ZL_CHECK_ARG(logits && params && out && T > 0 && V > 0);
-    ZL_CHECK_SUPPORTED(V <= kSampleMaxVocab);
-    ZL_CHECK_ARG(!history || history_words >= cdiv(V, 32));
     ZL_CHECK_ARG(ws_bytes >= zl_sample_workspace_bytes(T, V));
-    const int rc = prepare_sample();
-    if (rc != ZL_OK) return rc;
-    const int S = cdiv(V, kSampleCluster);
-    const int ty = T < 65535 ? T : 65535;   // rows: blockIdx.z * gridDim.y + blockIdx.y
-    ZL_CHECK_CUDA(launch(k_sample, dim3(kSampleCluster, ty, cdiv(T, ty)), dim3(kSampleThreads), (size_t)S * sizeof(float),
-                         stream, pdl != 0, logits, T, V, S, params, row_task, counter, history, history_words, out));
-    return ZL_OK;
+    return sample_launch(logits, T, V, params, row_task, counter, history, history_words, SampleProc{}, out, pdl, stream);
+}
+
+extern "C" size_t zl_sample_processed_workspace_bytes(int T, int seq_stride) {
+    if (T <= 0 || seq_stride <= 0) return 0;
+    return (size_t)T * ngram_table_size(seq_stride) * sizeof(int2);
+}
+
+extern "C" int zl_sample_processed(const float* logits, int T, int V, const zl_sample_params_t* params,
+                                   const int32_t* row_task, const int32_t* counter, uint32_t* history, int history_words,
+                                   const float* ngram_penalty, int32_t* seq, int32_t* seq_len, int seq_stride,
+                                   const int32_t* bias_tokens, const float* bias_values, const int32_t* bias_count,
+                                   int bias_stride, int32_t* out, void* ws, size_t ws_bytes, int pdl, zl_stream_t stream) {
+    ZL_CHECK_ARG(!seq || (seq_len && seq_stride > 0));
+    ZL_CHECK_ARG(!ngram_penalty || (seq && ws && ws_bytes >= zl_sample_processed_workspace_bytes(T, seq_stride)));
+    ZL_CHECK_ARG(!bias_tokens || (bias_values && bias_count && bias_stride > 0));
+    SampleProc pr{};
+    pr.ngram = ngram_penalty;
+    pr.seq = seq;
+    pr.seq_len = seq_len;
+    pr.seq_stride = seq_stride;
+    pr.bias_tok = bias_tokens;
+    pr.bias_val = bias_values;
+    pr.bias_cnt = bias_count;
+    pr.bias_stride = bias_stride;
+    pr.table = static_cast<int2*>(ws);
+    pr.table_stride = seq_stride > 0 ? ngram_table_size(seq_stride) : 0;
+    return sample_launch(logits, T, V, params, row_task, counter, history, history_words, pr, out, pdl, stream);
 }

@@ -32,6 +32,33 @@ MODEL_PRESETS = {
                  vocab_size=512, eps=1e-5, rope_theta=10000.0, rope_llama3=None),
 }
 
+MAX_LOGIT_BIAS = 1024   # ZL_MAX_LOGIT_BIAS
+
+
+def logit_bias_arrays(logit_bias, vocab_size):
+    """{token: bias} (keys may be ints or decimal strings, as in the OpenAI protocol) -> (int32 tokens, fp32 values).
+    Raises ValueError for a repeated token, an id outside [0, vocab_size), a NaN or +inf bias, or more than
+    MAX_LOGIT_BIAS entries; -inf bans a token."""
+    items = list((logit_bias or {}).items())
+    if len(items) > MAX_LOGIT_BIAS:
+        raise ValueError("logit_bias has %d entries, at most %d are served" % (len(items), MAX_LOGIT_BIAS))
+    toks = np.array([int(k) for k, _ in items], dtype=np.int64)
+    vals = np.array([float(v) for _, v in items], dtype=np.float32)
+    if np.unique(toks).size != toks.size:
+        raise ValueError("logit_bias names a token twice")
+    if toks.size and (toks.min() < 0 or toks.max() >= vocab_size):
+        raise ValueError("logit_bias token outside [0, %d)" % vocab_size)
+    if np.isnan(vals).any() or (vals == np.inf).any():
+        raise ValueError("logit_bias values must be finite or -inf")
+    return toks.astype(np.int32), vals
+
+
+def check_ngram_penalty(ngram_penalty):
+    """ngram_penalty must be finite and > 0; <= 1 turns the n-gram rule off (batch_generator.cpp:1664)."""
+    if not (np.isfinite(ngram_penalty) and ngram_penalty > 0):
+        raise ValueError("ngram_penalty must be finite and > 0, got %r" % (ngram_penalty,))
+
+
 QUANT_NONE, QUANT_AUTO_INT8, QUANT_GPTQ, QUANT_AWQ, QUANT_FP8, QUANT_FP8_BLOCK = 0, 2, 5, 6, 7, 10   # model_config.hpp:132-144
 
 
@@ -255,11 +282,22 @@ class LlamaDecoder:
             lambda s, toks: self.prefill(s, toks), prompts, beam_width, max_new_tokens, eos_id, num_results, trace)
 
     def set_sampling(self, task, temperature=0.0, top_p=1.0, top_k=0, repetition_penalty=1.0, presence_penalty=0.0,
-                     seed=0):
-        """Per-task sampling for the following steps (zl_llama_set_sampling); clears the task's penalty history.
+                     seed=0, ngram_penalty=1.0, logit_bias=None):
+        """Per-task sampling and logits processors for the following steps (zl_llama_set_sampling, then
+        zl_llama_set_logits_processors); clears the task's penalty history and generated-token sequence.  Both are set on
+        every call, so a reused task slot never keeps an earlier request's bias.  logit_bias: {token: bias} or None.
+        As GeneratorArg (zhilight/dynamic_batch.py:110-111), ngram_penalty is 1 when presence_penalty != 0.
         The defaults are plain greedy."""
+        check_ngram_penalty(ngram_penalty)
+        ngram = 1.0 if presence_penalty else float(ngram_penalty)
+        toks, vals = logit_bias_arrays(logit_bias, self.cfg.vocab_size)
+        if self.cfg.tp_size > 1 and (ngram > 1 or toks.size):
+            # refused here so that neither the sampling nor the processors change
+            raise _lib.ZLError(-2, "logits processors are not served under tensor parallelism")
         p = _lib.sample_params(temperature, top_p, top_k, repetition_penalty, presence_penalty, seed)
         _lib.check(self.lib.zl_llama_set_sampling(self.h, int(task), ctypes.byref(p)))
+        _lib.check(self.lib.zl_llama_set_logits_processors(self.h, int(task), ngram, toks.ctypes.data_as(ctypes.c_void_p),
+                                                           vals.ctypes.data_as(ctypes.c_void_p), toks.size))
 
     def read_kv(self, layer, task, row0, n):
         """Rows row0 .. row0 + n of a task's layer-`layer` KV cache (zl_llama_read_kv), each (n, H_kv, d).

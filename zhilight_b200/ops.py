@@ -550,6 +550,27 @@ def sample(logits, params, row_task=None, counter=None, history=None, pdl=False)
     return out
 
 
+def sample_processed(logits, params, seq, seq_len, ngram_penalty=None, bias_tokens=None, bias_values=None,
+                     bias_count=None, row_task=None, counter=None, history=None, pdl=False):
+    """zl_sample_processed: ops.sample with the n-gram penalty and logit bias.  seq (tasks, stride) int32 generated
+    tokens, oldest first, and seq_len (tasks) int32, both updated in place with the pick; ngram_penalty (tasks) fp32 or
+    None (no n-gram launch); bias_tokens / bias_values (tasks, stride) int32 / fp32 with bias_count (tasks) int32, or
+    None.  params, row_task, counter and history as ops.sample, with one task per row of seq."""
+    t, v = logits.shape
+    n_tasks, stride = seq.shape
+    arr = sample_params_array(params, n_tasks)
+    dparams = torch.frombuffer(bytearray(bytes(arr)), dtype=torch.uint8).to(logits.device)
+    out = torch.empty(t, dtype=torch.int32, device=logits.device)
+    hw = history.shape[1] if history is not None else 0
+    nb = _lib.load().zl_sample_processed_workspace_bytes(t, stride) if ngram_penalty is not None else 0
+    ws = torch.empty(max(nb, 16), dtype=torch.uint8, device=logits.device) if nb else None
+    bstride = bias_tokens.shape[1] if bias_tokens is not None else 0
+    _lib.call("zl_sample_processed", _p(logits), t, v, _p(dparams), _p(row_task), _p(counter), _p(history), hw,
+              _p(ngram_penalty), _p(seq), _p(seq_len), stride, _p(bias_tokens), _p(bias_values), _p(bias_count), bstride,
+              _p(out), _p(ws), nb, int(pdl), _stream())
+    return out
+
+
 def beam_topk(logits, cum, groups, k, pdl=False):
     """zl_beam_topk: logits (R, V) fp32 and cum (R) fp32 CUDA tensors, groups (G, 2) {row0, width} host ints.
     -> (parent, token, score), each (G, k) on the device."""

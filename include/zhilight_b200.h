@@ -637,6 +637,37 @@ int zl_llama_beam_step(zl_llama_t* m, const int32_t* tokens, const int32_t* posi
  * source and a destination: ZL_ERR_INVALID_ARG. */
 int zl_llama_kv_copy_rows(zl_llama_t* m, const int32_t* ranges_host, int n);
 
+/* Generate until stop on the device (the reference stops a task at eos_id or max_length,
+ * src/generator/batch_generator.cpp:1744-1753, 1812-1817).  Each step of zl_llama_generate is the step of
+ * zl_llama_step_device -- forward, pick (greedy, or the task's sampling and processors), feedback -- over tasks 0 .. B-1.
+ * A running task emits its pick, then stops: 1 when the pick is one of its stop ids, 2 when it has emitted max_new_tokens
+ * tokens since its last zl_llama_set_stop, 3 when its next position would reach max_seq.  The emitted token is kept, a
+ * stop id included.  A finished task emits nothing until zl_llama_set_stop re-arms it; its row still runs through the
+ * forward (the batch shape is baked into the graph) but leaves its KV rows up to its last fed position, its sampler
+ * history and its generated-token sequence as they were, and its (token, position) state stays (the emitted token, the
+ * position it would be fed).  A task that stopped at position max_seq - 1 re-runs that position while it sits out
+ * (there is no later row to write): the same inputs give its last KV row the same values, bit for bit while the batch
+ * size and weight format do not couple rows.  Its state position is max_seq, so zl_llama_step_device refuses the batch
+ * until zl_llama_set_state moves it.  A task without a stop rule has no stop ids and no budget.
+ * Per-task stop rule for zl_llama_generate: up to ZL_MAX_STOP_IDS distinct ids in [0, vocab); max_new_tokens >= 1, or 0
+ * for no budget.  Re-arms a finished task and resets its emitted count.  Stream-ordered; host arrays staged before return.
+ * Bad task or ids, a repeated id, n_stop > ZL_MAX_STOP_IDS or max_new_tokens < 0: ZL_ERR_INVALID_ARG; tp_size > 1:
+ * ZL_ERR_UNSUPPORTED; a model not finalized: ZL_ERR_STATE. */
+#define ZL_MAX_STOP_IDS 8
+int zl_llama_set_stop(zl_llama_t* m, int task, const int32_t* stop_ids_host, int n_stop, int max_new_tokens);
+/* Up to max_steps (1 .. max_seq) device-resident decode steps of rows 0..B-1, stopping early when all have finished.
+ * tokens_host (max_steps, B) step-major: emitted tokens (-1 where a row emitted nothing); n_out_host (B) tokens emitted
+ * per task; finish_host (B) 0 running / 1 stop id / 2 max_new_tokens / 3 max_seq; *steps_host steps run.  Synchronous.
+ * Starts from the device-resident state (zl_llama_set_state, or earlier steps) and leaves it there, so calls with a small
+ * max_steps stream a generation.  The steps run as a CUDA graph per (B, sampling, n-gram launch, attention length
+ * bucket): a head kernel and a while-loop conditional node whose body is the decode step plus the stop rules; a call
+ * crosses buckets with one graph launch per bucket, without a host sync in between, and syncs once at the end.  A call
+ * whose tasks have all finished runs 0 steps and enqueues nothing.  Bad B, max_steps or output pointers:
+ * ZL_ERR_INVALID_ARG; tp_size > 1 or use_graph == 0: ZL_ERR_UNSUPPORTED; a model not finalized: ZL_ERR_STATE.  Every
+ * check runs before anything is enqueued. */
+int zl_llama_generate(zl_llama_t* m, int B, int max_steps, int32_t* tokens_host, int32_t* n_out_host,
+                      int32_t* finish_host, int* steps_host);
+
 #ifdef __cplusplus
 }
 #endif

@@ -12,6 +12,7 @@
 #include "w4_params.h"
 #include "kv_pool.cuh"
 #include "beam.cuh"
+#include "sample.cuh"
 
 #include <algorithm>
 #include <cstdlib>
@@ -188,6 +189,14 @@ struct zl_llama {
     cudaEvent_t rows_ev[kStageSlots] = {};
     bool rows_used[kStageSlots] = {};
     int rows_next = 0;
+    // generation loop (zl_llama_generate): the per-task stop rules and progress, the loop's control words and the ring of
+    // emitted tokens on the device (gen_state lays them out in d_gen), their pinned host mirror, a host mirror of the
+    // finish reasons, and one loop graph per (B, sampler, n-gram launch, length bucket), apart from `graphs`
+    dev_ptr<int32_t> d_gen;
+    host_ptr<int32_t> h_gen;                          // ring rows (max_seq x max_batch) | finish | positions | control
+    std::vector<char> gen_fin;
+    std::map<long long, cudaGraphExec_t> gen_graphs;
+    const int32_t* pick_frozen = nullptr;   // set while a loop body is captured: the sampler records no pick of a finished task
 };
 
 namespace {
@@ -737,6 +746,54 @@ int finalize_globals(zl_llama* m) {
     return ZL_OK;
 }
 
+// zl_llama_generate's device state, views of d_gen: per task its stop rule, emitted count, finish reason and the
+// last-position bookkeeping; the loop's control words; the ring of emitted tokens
+struct GenState {
+    int32_t* stop;      // (max_batch, ZL_MAX_STOP_IDS)
+    int32_t* n_stop;    // (max_batch) each from here to edge
+    int32_t* budget;    // max_new_tokens, 0: none
+    int32_t* emitted;   // tokens emitted since the task's last zl_llama_set_stop
+    int32_t* fin;       // 0 running, 1 stop id, 2 max_new_tokens, 3 max_seq
+    int32_t* ftok;      // a task that filled its KV buffer: the token it fed at max_seq - 1 ...
+    int32_t* stok;      // ... and the token it emitted there
+    int32_t* edge;      // 1 while such a task re-feeds max_seq - 1 inside a launch
+    int32_t* ctl;       // {steps run in this call, steps left in this launch}
+    int32_t* ring;      // (max_seq, max_batch): row s = the tokens emitted at step s of the call, -1 where none
+    int max_batch, max_seq;
+};
+constexpr int kGenTaskWords = ZL_MAX_STOP_IDS + 7;   // words per task: stop ids and the seven (max_batch) arrays
+constexpr int kGenCtlWords = 4;
+
+GenState gen_state(zl_llama* m) {
+    const int MB = m->cfg.max_batch;
+    GenState g;
+    int32_t* p = m->d_gen.get();
+    g.stop = p;
+    p += (size_t)MB * ZL_MAX_STOP_IDS;
+    for (int32_t** a : {&g.n_stop, &g.budget, &g.emitted, &g.fin, &g.ftok, &g.stok, &g.edge}) {
+        *a = p;
+        p += MB;
+    }
+    g.ctl = p;
+    g.ring = p + kGenCtlWords;
+    g.max_batch = MB;
+    g.max_seq = m->cfg.max_seq;
+    return g;
+}
+
+// every task starts without a stop rule and running
+int alloc_generate(zl_llama* m) {
+    const auto& c = m->cfg;
+    const size_t task_words = (size_t)c.max_batch * kGenTaskWords, ring = (size_t)c.max_seq * c.max_batch;
+    RCHECK(dmalloc(&m->d_gen, (task_words + kGenCtlWords + ring) * 4));
+    ZL_CHECK_CUDA(cudaMemsetAsync(m->d_gen.get(), 0, (task_words + kGenCtlWords) * 4, m->stream));
+    int32_t* h = nullptr;
+    ZL_CHECK_CUDA(cudaMallocHost((void**)&h, (ring + 2 * (size_t)c.max_batch + kGenCtlWords) * 4));
+    m->h_gen.reset(h);
+    m->gen_fin.assign(c.max_batch, 0);
+    return ZL_OK;
+}
+
 int alloc_runtime(zl_llama* m) {
     const auto& c = m->cfg;
     const int B = c.max_batch, D = c.dim_model, d = c.dim_head;
@@ -852,6 +909,7 @@ int alloc_runtime(zl_llama* m) {
     ZL_CHECK_CUDA(cudaMemsetAsync(m->d_ngram.get(), 0, (size_t)B * 4, m->stream));   // 0.0f: off
     ZL_CHECK_CUDA(cudaMemsetAsync(m->d_seq_len.get(), 0, (size_t)B * 4, m->stream));
     ZL_CHECK_CUDA(cudaMemsetAsync(m->d_bias_cnt.get(), 0, (size_t)B * 4, m->stream));
+    RCHECK(alloc_generate(m));
     int32_t *stage = nullptr, *ring = nullptr;
     ZL_CHECK_CUDA(cudaMallocHost((void**)&stage, sizeof(int32_t) * (4 * B + 4 + T)));
     m->h_stage.reset(stage);
@@ -1418,11 +1476,11 @@ int enqueue_step(zl_llama* m, int n_tasks, int len_bucket, const Segments* pf = 
         const int32_t* row_task = joined ? j_task : pf ? m->d_iota.get() + pf->task : m->d_iota.get();
         const int32_t* counter = joined ? j_pos : pf ? m->d_pf_pos.get() + (pf->n - 1) : m->d_pos.get();
         // k_ngram_levels runs only when a task of the step has the n-gram rule on (`ngram`, a bit of the graph key)
-        RCHECK(zl_sample_processed(m->logits.get(), HB, m->vshard, m->d_sparams.get(), row_task, counter, m->d_hist.get(),
-                                   m->hwords, ngram ? m->d_ngram.get() : nullptr, m->d_seq.get(), m->d_seq_len.get(),
-                                   c.max_seq, m->d_bias_tok.get(), m->d_bias_val.get(), m->d_bias_cnt.get(),
-                                   ZL_MAX_LOGIT_BIAS, m->d_next.get(), ngram ? m->ngram_ws.get() : nullptr,
-                                   m->ngram_ws_bytes, stage_pdl(m, kPick), st));
+        RCHECK(sample_processed_launch(m->logits.get(), HB, m->vshard, m->d_sparams.get(), row_task, counter,
+                                       m->d_hist.get(), m->hwords, ngram ? m->d_ngram.get() : nullptr, m->d_seq.get(),
+                                       m->d_seq_len.get(), c.max_seq, m->d_bias_tok.get(), m->d_bias_val.get(),
+                                       m->d_bias_cnt.get(), ZL_MAX_LOGIT_BIAS, m->pick_frozen, m->d_next.get(),
+                                       ngram ? m->ngram_ws.get() : nullptr, m->ngram_ws_bytes, stage_pdl(m, kPick), st));
     } else if (!tp) {
         RCHECK(zl_argmax(m->logits.get(), m->d_next.get(), HB, m->vshard, m->argmax_ws.get(), zl_argmax_workspace_bytes(HB),
                          stage_pdl(m, kPick), st));
@@ -1557,6 +1615,7 @@ extern "C" void zl_llama_destroy(zl_llama_t* m) {
     cudaStreamSynchronize(m->stream);
     if (m->reduce_stream) cudaStreamSynchronize(m->reduce_stream);
     for (auto& g : m->graphs) cudaGraphExecDestroy(g.second);
+    for (auto& g : m->gen_graphs) cudaGraphExecDestroy(g.second);
     for (int h = 0; h < 2; ++h)
         for (cudaEvent_t e : {m->ev_o[h], m->ev_r1[h], m->ev_dn[h], m->ev_r2[h]})
             if (e) cudaEventDestroy(e);
@@ -2388,5 +2447,267 @@ extern "C" int zl_llama_kv_copy_rows(zl_llama_t* m, const int32_t* ranges_host, 
     RCHECK(kv_row_copy(a, m->stream));
     ZL_CHECK_CUDA(cudaEventRecord(m->rows_ev[slot], m->stream));   // after the kernel that reads the device slot
     m->rows_used[slot] = true;
+    return ZL_OK;
+}
+
+// ------------------------------------------------------------------------------------------------------------------
+// Generate until stop (the reference's stop rules, src/generator/batch_generator.cpp:1744-1753, 1812-1817): decode steps
+// in a CUDA-graph while loop that applies each task's stop ids, token budget and the end of its KV buffer on the device.
+// Graph: k_gen_head -> while (live tasks and steps left) { the decode step; k_gen_advance } -> k_gen_tail.
+// ------------------------------------------------------------------------------------------------------------------
+namespace {
+
+constexpr int kGenThreads = 256;
+
+struct StopRule {
+    int32_t ids[ZL_MAX_STOP_IDS];
+    int32_t n, budget;
+};
+
+// zl_llama_set_stop: the task's rule, emitted count 0, running
+__global__ void k_gen_arm(GenState g, int task, StopRule r) {
+    for (int j = 0; j < ZL_MAX_STOP_IDS; ++j) g.stop[task * ZL_MAX_STOP_IDS + j] = r.ids[j];
+    g.n_stop[task] = r.n;
+    g.budget[task] = r.budget;
+    g.emitted[task] = 0;
+    g.fin[task] = 0;
+}
+
+// before each graph launch of a call: the step counter (first launch) and the steps this launch may run
+__global__ void k_gen_begin(GenState g, int first, int steps) {
+    if (first) g.ctl[0] = 0;
+    g.ctl[1] = steps;
+}
+
+__device__ int gen_block_sum(int v) {
+    __shared__ int part[kGenThreads / 32];
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
+    if ((threadIdx.x & 31) == 0) part[threadIdx.x >> 5] = v;
+    __syncthreads();
+    int s = 0;
+    if (threadIdx.x == 0)
+        for (int w = 0; w < kGenThreads / 32; ++w) s += part[w];
+    return s;   // thread 0
+}
+
+// A task whose state position is max_seq (it stopped at max_seq - 1) cannot be fed there: while the launch runs it
+// re-feeds its last (token, position), which rewrites that KV row with what it already holds.  A task re-armed in that
+// state finishes at once (reason 3) without emitting.  Then the loop's first condition: running tasks and steps left.
+__global__ void __launch_bounds__(kGenThreads) k_gen_head(GenState g, int32_t* __restrict__ tokens,
+                                                          int32_t* __restrict__ pos, int B, cudaGraphConditionalHandle h) {
+    int live = 0;
+    for (int i = threadIdx.x; i < B; i += kGenThreads) {
+        if (pos[i] >= g.max_seq) {
+            g.stok[i] = tokens[i];
+            tokens[i] = g.ftok[i];
+            pos[i] = g.max_seq - 1;
+            g.edge[i] = 1;
+            if (g.fin[i] == 0) g.fin[i] = 3;
+        }
+        live += g.fin[i] == 0;
+    }
+    live = gen_block_sum(live);
+    if (threadIdx.x == 0) cudaGraphSetConditional(h, live > 0 && g.ctl[1] > 0);
+}
+
+// In place of k_advance: each running task emits its pick into ring row `step`, applies its stop rules and is fed its
+// pick at the next position; a finished task's row emits -1 and keeps its state.  Sets the loop condition.
+__global__ void __launch_bounds__(kGenThreads) k_gen_advance(GenState g, int32_t* __restrict__ tokens,
+                                                             int32_t* __restrict__ pos, const int32_t* __restrict__ next,
+                                                             int B, cudaGraphConditionalHandle h) {
+    const int step = g.ctl[0];
+    int live = 0;
+    for (int i = threadIdx.x; i < B; i += kGenThreads) {
+        int out = -1;
+        if (g.fin[i] == 0) {
+            const int tok = next[i];
+            out = tok;
+            const int e = g.emitted[i] + 1;
+            g.emitted[i] = e;
+            const int p1 = pos[i] + 1;
+            int reason = 0;
+            for (int j = 0; j < g.n_stop[i]; ++j)
+                if (g.stop[i * ZL_MAX_STOP_IDS + j] == tok) reason = 1;
+            if (!reason && g.budget[i] > 0 && e >= g.budget[i]) reason = 2;
+            if (!reason && p1 >= g.max_seq) reason = 3;
+            if (p1 < g.max_seq) {
+                tokens[i] = tok;
+                pos[i] = p1;
+            } else {   // the buffer is full: the state (tok, max_seq) is restored by k_gen_tail
+                g.ftok[i] = tokens[i];
+                g.stok[i] = tok;
+                g.edge[i] = 1;
+            }
+            g.fin[i] = reason;
+            live += reason == 0;
+        }
+        g.ring[(size_t)step * g.max_batch + i] = out;
+    }
+    live = gen_block_sum(live);
+    if (threadIdx.x == 0) {
+        const int left = g.ctl[1] - 1;
+        g.ctl[0] = step + 1;
+        g.ctl[1] = left;
+        cudaGraphSetConditional(h, live > 0 && left > 0);
+    }
+}
+
+// after the loop: the tasks that re-fed max_seq - 1 get back their state (emitted token, max_seq)
+__global__ void k_gen_tail(GenState g, int32_t* __restrict__ tokens, int32_t* __restrict__ pos, int B) {
+    for (int i = threadIdx.x; i < B; i += blockDim.x)
+        if (g.edge[i]) {
+            tokens[i] = g.stok[i];
+            pos[i] = g.max_seq;
+            g.edge[i] = 0;
+        }
+}
+
+// The loop graph of (B, sampler, n-gram launch, bucket).  The body keeps the step's programmatic dependent launches.
+int build_gen_graph(zl_llama* m, int B, bool sampler, bool ngram, int bucket, cudaGraphExec_t* out) {
+    GenState gs = gen_state(m);
+    int32_t* tokens = m->d_tokens.get();
+    int32_t* pos = m->d_pos.get();
+    const int32_t* next = m->d_next.get();
+    cudaGraph_t g = nullptr;
+    ZL_CHECK_CUDA(cudaGraphCreate(&g, 0));
+    std::unique_ptr<CUgraph_st, cudaError_t (*)(cudaGraph_t)> own(g, cudaGraphDestroy);
+    cudaGraphConditionalHandle h;
+    ZL_CHECK_CUDA(cudaGraphConditionalHandleCreate(&h, g, 0, 0));
+    cudaKernelNodeParams kp = {};
+    void* head_args[] = {&gs, &tokens, &pos, &B, &h};
+    kp.func = (void*)k_gen_head;
+    kp.gridDim = dim3(1);
+    kp.blockDim = dim3(kGenThreads);
+    kp.kernelParams = head_args;
+    cudaGraphNode_t head = nullptr, loop = nullptr, tail = nullptr;
+    ZL_CHECK_CUDA(cudaGraphAddKernelNode(&head, g, nullptr, 0, &kp));
+    cudaGraphNodeParams cp = {};
+    cp.type = cudaGraphNodeTypeConditional;
+    cp.conditional.handle = h;
+    cp.conditional.type = cudaGraphCondTypeWhile;
+    cp.conditional.size = 1;
+    ZL_CHECK_CUDA(cudaGraphAddNode(&loop, g, &head, 1, &cp));
+    cudaGraph_t body = cp.conditional.phGraph_out[0];
+    // the body: the unchanged decode step, then k_gen_advance in k_advance's place
+    ZL_CHECK_CUDA(cudaStreamBeginCaptureToGraph(m->stream, body, nullptr, nullptr, 0, cudaStreamCaptureModeThreadLocal));
+    m->pick_frozen = gs.fin;
+    int rc = enqueue_step(m, B, bucket, nullptr, sampler, nullptr, ngram);
+    m->pick_frozen = nullptr;
+    if (rc == ZL_OK) {
+        k_gen_advance<<<1, kGenThreads, 0, m->stream>>>(gs, tokens, pos, next, B, h);
+        if (cudaGetLastError() != cudaSuccess) rc = fail_state(__LINE__, "k_gen_advance launch failed", ZL_ERR_CUDA);
+    }
+    const cudaError_t ce = cudaStreamEndCapture(m->stream, &body);
+    if (rc != ZL_OK) return rc;
+    ZL_CHECK_CUDA(ce);
+    void* tail_args[] = {&gs, &tokens, &pos, &B};
+    kp.func = (void*)k_gen_tail;
+    kp.kernelParams = tail_args;
+    ZL_CHECK_CUDA(cudaGraphAddKernelNode(&tail, g, &loop, 1, &kp));
+    ZL_CHECK_CUDA(cudaGraphInstantiate(out, g, 0));
+    return ZL_OK;
+}
+
+int gen_graph(zl_llama* m, int B, bool sampler, bool ngram, int bucket, cudaGraphExec_t* out) {
+    const long long key = ((long long)B << 33) | ((long long)sampler << 32) | ((long long)ngram << 31) | (unsigned)bucket;
+    auto it = m->gen_graphs.find(key);
+    if (it != m->gen_graphs.end()) {
+        *out = it->second;
+        return ZL_OK;
+    }
+    cudaGraphExec_t exec = nullptr;
+    RCHECK(build_gen_graph(m, B, sampler, ngram, bucket, &exec));
+    m->gen_graphs.emplace(key, exec);
+    *out = exec;
+    return ZL_OK;
+}
+
+}  // namespace
+
+extern "C" int zl_llama_set_stop(zl_llama_t* m, int task, const int32_t* stop_ids_host, int n_stop, int max_new_tokens) {
+    ZL_CHECK_ARG(m && task >= 0 && task < m->cfg.max_batch);
+    ZL_CHECK_ARG(n_stop >= 0 && n_stop <= ZL_MAX_STOP_IDS && (n_stop == 0 || stop_ids_host));
+    ZL_CHECK_ARG(max_new_tokens >= 0);
+    StopRule r{};
+    for (int j = 0; j < n_stop; ++j) {
+        ZL_CHECK_ARG(stop_ids_host[j] >= 0 && stop_ids_host[j] < m->cfg.vocab_size);
+        for (int k = 0; k < j; ++k) ZL_CHECK_ARG(stop_ids_host[k] != stop_ids_host[j]);
+        r.ids[j] = stop_ids_host[j];
+    }
+    r.n = n_stop;
+    r.budget = max_new_tokens;
+    if (m->cfg.tp_size > 1) return fail_state(__LINE__, "zl_llama_set_stop: tensor parallelism is not served", ZL_ERR_UNSUPPORTED);
+    if (!m->finalized) return fail_state(__LINE__, "model not finalized");
+    // stream-ordered after every step already enqueued; the rule travels as a kernel argument
+    k_gen_arm<<<1, 1, 0, m->stream>>>(gen_state(m), task, r);
+    ZL_CHECK_LAUNCH();
+    m->gen_fin[task] = 0;
+    return ZL_OK;
+}
+
+extern "C" int zl_llama_generate(zl_llama_t* m, int B, int max_steps, int32_t* tokens_host, int32_t* n_out_host,
+                                 int32_t* finish_host, int* steps_host) {
+    ZL_CHECK_ARG(m && tokens_host && n_out_host && finish_host && steps_host);
+    const auto& c = m->cfg;
+    ZL_CHECK_ARG(B > 0 && B <= c.max_batch && max_steps >= 1 && max_steps <= c.max_seq);
+    if (c.tp_size > 1) return fail_state(__LINE__, "zl_llama_generate: tensor parallelism is not served", ZL_ERR_UNSUPPORTED);
+    if (!c.use_graph) return fail_state(__LINE__, "zl_llama_generate runs as a CUDA graph (use_graph = 0)", ZL_ERR_UNSUPPORTED);
+    if (!m->finalized) return fail_state(__LINE__, "model not finalized");
+    const int MB = c.max_batch;
+    bool all_done = true;
+    for (int i = 0; i < B; ++i) all_done = all_done && m->gen_fin[i] != 0;
+    if (all_done) {
+        for (size_t k = 0; k < (size_t)max_steps * B; ++k) tokens_host[k] = -1;
+        for (int i = 0; i < B; ++i) {
+            n_out_host[i] = 0;
+            finish_host[i] = m->gen_fin[i];
+        }
+        *steps_host = 0;
+        return ZL_OK;
+    }
+    const bool sampler = sampler_on(m, 0, B), ngram = ngram_on(m, 0, B);
+    const GenState gs = gen_state(m);
+    // attention lengths at step s are at most min(L0 + s, max_seq): one launch per length bucket crossed
+    const int L0 = m->cur_max_len;
+    for (int s = 0; s < max_steps;) {
+        const int len = std::min(L0 + s, c.max_seq);
+        const int bucket = len_bucket_of(m, len);
+        int n = max_steps - s;
+        if (bucket < c.max_seq) n = std::min(n, bucket - (L0 + s) + 1);
+        cudaGraphExec_t exec = nullptr;
+        RCHECK(gen_graph(m, B, sampler, ngram, bucket, &exec));
+        k_gen_begin<<<1, 1, 0, m->stream>>>(gs, s == 0, n);
+        ZL_CHECK_LAUNCH();
+        ZL_CHECK_CUDA(cudaGraphLaunch(exec, m->stream));
+        s += n;
+    }
+    // one sync: ring rows | finish reasons | positions | control
+    int32_t* h_ring = m->h_gen.get();
+    int32_t* h_fin = h_ring + (size_t)c.max_seq * MB;
+    int32_t* h_pos = h_fin + MB;
+    int32_t* h_ctl = h_pos + MB;
+    cudaStream_t st = m->stream;
+    ZL_CHECK_CUDA(cudaMemcpyAsync(h_ring, gs.ring, (size_t)max_steps * MB * 4, cudaMemcpyDeviceToHost, st));
+    ZL_CHECK_CUDA(cudaMemcpyAsync(h_fin, gs.fin, (size_t)B * 4, cudaMemcpyDeviceToHost, st));
+    ZL_CHECK_CUDA(cudaMemcpyAsync(h_pos, m->d_pos.get(), (size_t)B * 4, cudaMemcpyDeviceToHost, st));
+    ZL_CHECK_CUDA(cudaMemcpyAsync(h_ctl, gs.ctl, kGenCtlWords * 4, cudaMemcpyDeviceToHost, st));
+    ZL_CHECK_CUDA(cudaStreamSynchronize(st));
+    const int steps = h_ctl[0];
+    for (int i = 0; i < B; ++i) n_out_host[i] = 0;
+    for (int s = 0; s < max_steps; ++s)
+        for (int i = 0; i < B; ++i) {
+            const int32_t t = s < steps ? h_ring[(size_t)s * MB + i] : -1;
+            tokens_host[(size_t)s * B + i] = t;
+            n_out_host[i] += t >= 0;
+        }
+    int mx = m->cur_max_len;
+    for (int i = 0; i < B; ++i) {
+        finish_host[i] = h_fin[i];
+        m->gen_fin[i] = (char)h_fin[i];
+        mx = std::max(mx, h_pos[i] + 1);
+    }
+    m->cur_max_len = mx;
+    *steps_host = steps;
     return ZL_OK;
 }

@@ -20,6 +20,7 @@
 // batch_generator.cpp:1709-1728).  k_ngram_levels gives each distinct token of a task's generated sequence its largest
 // n-gram level, in a per-row hash table; k_sample then stages a processed copy of its slice in shared memory.
 #include "common.cuh"
+#include "sample.cuh"
 
 #include <cooperative_groups.h>
 
@@ -213,6 +214,7 @@ struct SampleProc {
     int bias_stride;
     int2* table;              // k_ngram_levels' output: per row, table_stride {token, level} slots
     int table_stride;
+    const int32_t* frozen;    // (tasks) or NULL: a row whose task has frozen[task] != 0 records its pick nowhere
 };
 
 constexpr int kNgramThreads = 1024;
@@ -536,8 +538,9 @@ __global__ void __cluster_dims__(kSampleCluster, 1, 1) __launch_bounds__(kSample
     }
     if (owner && tid == 0) {
         out[row] = tok;
-        if (hist) atomicOr(&hist[tok >> 5], 1u << (tok & 31));
-        if (pr.seq) {   // appends past the capacity are dropped
+        const bool record = !pr.frozen || pr.frozen[task] == 0;
+        if (hist && record) atomicOr(&hist[tok >> 5], 1u << (tok & 31));
+        if (pr.seq && record) {   // appends past the capacity are dropped
             const int len = pr.seq_len[task];
             if (len >= 0 && len < pr.seq_stride) {
                 pr.seq[(size_t)task * pr.seq_stride + len] = tok;
@@ -615,11 +618,12 @@ extern "C" size_t zl_sample_processed_workspace_bytes(int T, int seq_stride) {
     return (size_t)T * ngram_table_size(seq_stride) * sizeof(int2);
 }
 
-extern "C" int zl_sample_processed(const float* logits, int T, int V, const zl_sample_params_t* params,
-                                   const int32_t* row_task, const int32_t* counter, uint32_t* history, int history_words,
-                                   const float* ngram_penalty, int32_t* seq, int32_t* seq_len, int seq_stride,
-                                   const int32_t* bias_tokens, const float* bias_values, const int32_t* bias_count,
-                                   int bias_stride, int32_t* out, void* ws, size_t ws_bytes, int pdl, zl_stream_t stream) {
+int zl::sample_processed_launch(const float* logits, int T, int V, const zl_sample_params_t* params,
+                                const int32_t* row_task, const int32_t* counter, uint32_t* history, int history_words,
+                                const float* ngram_penalty, int32_t* seq, int32_t* seq_len, int seq_stride,
+                                const int32_t* bias_tokens, const float* bias_values, const int32_t* bias_count,
+                                int bias_stride, const int32_t* frozen, int32_t* out, void* ws, size_t ws_bytes, int pdl,
+                                cudaStream_t stream) {
     ZL_CHECK_ARG(!seq || (seq_len && seq_stride > 0));
     ZL_CHECK_ARG(!ngram_penalty || (seq && ws && ws_bytes >= zl_sample_processed_workspace_bytes(T, seq_stride)));
     ZL_CHECK_ARG(!bias_tokens || (bias_values && bias_count && bias_stride > 0));
@@ -634,5 +638,16 @@ extern "C" int zl_sample_processed(const float* logits, int T, int V, const zl_s
     pr.bias_stride = bias_stride;
     pr.table = static_cast<int2*>(ws);
     pr.table_stride = seq_stride > 0 ? ngram_table_size(seq_stride) : 0;
+    pr.frozen = frozen;
     return sample_launch(logits, T, V, params, row_task, counter, history, history_words, pr, out, pdl, stream);
+}
+
+extern "C" int zl_sample_processed(const float* logits, int T, int V, const zl_sample_params_t* params,
+                                   const int32_t* row_task, const int32_t* counter, uint32_t* history, int history_words,
+                                   const float* ngram_penalty, int32_t* seq, int32_t* seq_len, int seq_stride,
+                                   const int32_t* bias_tokens, const float* bias_values, const int32_t* bias_count,
+                                   int bias_stride, int32_t* out, void* ws, size_t ws_bytes, int pdl, zl_stream_t stream) {
+    return sample_processed_launch(logits, T, V, params, row_task, counter, history, history_words, ngram_penalty, seq,
+                                   seq_len, seq_stride, bias_tokens, bias_values, bias_count, bias_stride, nullptr, out,
+                                   ws, ws_bytes, pdl, static_cast<cudaStream_t>(stream));
 }

@@ -59,6 +59,24 @@ def check_ngram_penalty(ngram_penalty):
         raise ValueError("ngram_penalty must be finite and > 0, got %r" % (ngram_penalty,))
 
 
+MAX_STOP_IDS = 8   # ZL_MAX_STOP_IDS
+
+
+def stop_rule(stop_ids, max_new_tokens, vocab_size):
+    """Check a stop rule for zl_llama_set_stop -> (int32 stop ids, max_new_tokens).  Raises ValueError for more than
+    MAX_STOP_IDS ids, a repeated id, an id outside [0, vocab_size), or max_new_tokens < 0 (0: no budget)."""
+    ids = np.asarray(list(stop_ids), dtype=np.int64).reshape(-1)
+    if ids.size > MAX_STOP_IDS:
+        raise ValueError("%d stop ids, at most %d are served" % (ids.size, MAX_STOP_IDS))
+    if np.unique(ids).size != ids.size:
+        raise ValueError("a stop id is named twice")
+    if ids.size and (ids.min() < 0 or ids.max() >= vocab_size):
+        raise ValueError("stop id outside [0, %d)" % vocab_size)
+    if int(max_new_tokens) != max_new_tokens or max_new_tokens < 0:
+        raise ValueError("max_new_tokens must be an integer >= 0 (0: no budget), got %r" % (max_new_tokens,))
+    return ids.astype(np.int32), int(max_new_tokens)
+
+
 QUANT_NONE, QUANT_AUTO_INT8, QUANT_GPTQ, QUANT_AWQ, QUANT_FP8, QUANT_FP8_BLOCK = 0, 2, 5, 6, 7, 10   # model_config.hpp:132-144
 
 
@@ -336,6 +354,29 @@ class LlamaDecoder:
 
     def step_device(self, b):
         _lib.check(self.lib.zl_llama_step_device(self.h, b))
+
+    def set_stop(self, task, stop_ids=(), max_new_tokens=0):
+        """The stop rule of `task` for generate(): it finishes when it emits one of stop_ids (at most MAX_STOP_IDS
+        distinct ids, e.g. the EOS ids) or after max_new_tokens emitted tokens (0: no budget), and always when its KV
+        buffer is full.  Re-arms a finished task and restarts its count (zl_llama_set_stop)."""
+        ids, budget = stop_rule(stop_ids, max_new_tokens, self.cfg.vocab_size)
+        _lib.check(self.lib.zl_llama_set_stop(self.h, int(task), ids.ctypes.data_as(ctypes.c_void_p), ids.size, budget))
+
+    def generate(self, b, max_steps):
+        """Up to max_steps device-resident decode steps of tasks 0 .. b-1 from their (token, position) state
+        (set_state, or earlier steps), ending early once every task has finished (zl_llama_generate).  Returns
+        (list of b int32 arrays: the tokens each task emitted, stop ids included; finish reasons (b,) int32: 0 running,
+        1 stop id, 2 max_new_tokens, 3 KV buffer full; steps run).  Call again to continue: the state stays on the
+        device."""
+        b, max_steps = int(b), int(max_steps)
+        toks = np.empty((max(max_steps, 0), max(b, 0)), np.int32)
+        n_out = np.empty(max(b, 0), np.int32)
+        fin = np.empty(max(b, 0), np.int32)
+        steps = ctypes.c_int()
+        p = lambda a: a.ctypes.data_as(ctypes.c_void_p)
+        _lib.check(self.lib.zl_llama_generate(self.h, b, max_steps, p(toks), p(n_out), p(fin), ctypes.byref(steps)))
+        out = [toks[:steps.value, i][toks[:steps.value, i] >= 0].copy() for i in range(b)]
+        return out, fin, steps.value
 
     def sync(self):
         _lib.check(self.lib.zl_llama_sync(self.h))

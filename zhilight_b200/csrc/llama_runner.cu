@@ -15,15 +15,24 @@
 #include "sample.cuh"
 
 #include <algorithm>
+#include <array>
 #include <cstdlib>
 #include <cstring>
+#include <functional>
 #include <map>
 #include <memory>
+#include <numeric>
 #include <utility>
 #include <string>
 #include <vector>
 
 extern unsigned long long* g_w4_trace;   // debug timeline buffer (zl_w4_set_trace)
+
+#define RCHECK(expr)                \
+    do {                            \
+        int _rc = (expr);           \
+        if (_rc != ZL_OK) return _rc; \
+    } while (0)
 
 namespace {
 
@@ -78,6 +87,65 @@ struct Layer {
     dev_ptr<void*> sv_addrs;
 };
 
+// Staging slots for host -> device copies: a pinned copy reads its host slot when it EXECUTES, and a kernel reads its device
+// slot when it runs, so a caller that runs ahead of the GPU must not rewrite a slot whose reader is still queued.  kSlots
+// slots of `words` int32 each, on the host and (when allocated) on the device, one event each.
+struct StageRing {
+    static constexpr int kSlots = 8;
+    host_ptr<int32_t> h;
+    dev_ptr<int32_t> d;
+    size_t words = 0;
+    cudaEvent_t ev[kSlots] = {};
+    bool used[kSlots] = {};
+    int next = 0, cur = 0;   // cur: the slot acquire() returned last
+
+    StageRing() = default;
+    StageRing(const StageRing&) = delete;
+    StageRing& operator=(const StageRing&) = delete;
+    ~StageRing() {
+        for (cudaEvent_t e : ev)
+            if (e) cudaEventDestroy(e);
+    }
+    int alloc(size_t slot_words, bool device);
+    // the next slot's host (and device) words, once the reader it was last released to has executed
+    int acquire(int32_t** hs, int32_t** ds = nullptr);
+    // call after the copy or kernel that reads the acquired slot has been enqueued on st
+    int release(cudaStream_t st);
+};
+
+// Instantiated graphs by key, destroyed with the cache.  get() returns the graph of `key`, or instantiates and keeps the
+// graph build(&graph) makes (the cache owns that graph, also when build fails) and stores its node count in *nodes.
+struct GraphCache {
+    std::map<long long, cudaGraphExec_t> execs;
+
+    GraphCache() = default;
+    GraphCache(const GraphCache&) = delete;
+    GraphCache& operator=(const GraphCache&) = delete;
+    ~GraphCache() {
+        for (auto& g : execs) cudaGraphExecDestroy(g.second);
+    }
+    template <typename Build>
+    int get(long long key, Build&& build, cudaGraphExec_t* out, int* nodes = nullptr) {
+        auto it = execs.find(key);
+        if (it == execs.end()) {
+            cudaGraph_t graph = nullptr;
+            const int rc = build(&graph);
+            std::unique_ptr<CUgraph_st, cudaError_t (*)(cudaGraph_t)> own(graph, cudaGraphDestroy);
+            RCHECK(rc);
+            cudaGraphExec_t exec = nullptr;
+            ZL_CHECK_CUDA(cudaGraphInstantiate(&exec, graph, 0));
+            if (nodes) {
+                size_t n_nodes = 0;
+                cudaGraphGetNodes(graph, nullptr, &n_nodes);
+                *nodes = (int)n_nodes;
+            }
+            it = execs.emplace(key, exec).first;
+        }
+        *out = it->second;
+        return ZL_OK;
+    }
+};
+
 }  // namespace
 
 struct zl_llama {
@@ -102,24 +170,18 @@ struct zl_llama {
     size_t attn_ws_bytes = 0;
     dev_ptr<> argmax_ws;
     host_ptr<int32_t> h_stage;   // tokens | pos | lens | next
-    // zl_llama_set_state staging: pinned H2D copies read the host buffer when they EXECUTE, so a set_state -> step_device
-    // loop that runs ahead of the GPU must not rewrite a slot whose copy is still queued: ring of slots, one event each
-    static constexpr int kStageSlots = 8;
-    host_ptr<int32_t> h_ring;    // [kStageSlots][2 * max_batch]
-    cudaEvent_t ring_ev[kStageSlots] = {};
-    bool ring_used[kStageSlots] = {};
-    int ring_next = 0;
+    // zl_llama_set_state staging: a set_state -> step_device loop that runs ahead of the GPU must not rewrite a slot whose
+    // copies are still queued.  Host slots of 2 * max_batch words.
+    StageRing state_ring;
     // prefill keeps its own (token, position) arrays: the decode-state arrays d_tokens / d_pos of tasks 0..B-1 survive a
     // prefill that happens between two zl_llama_step_device calls (continuous batching)
     dev_ptr<int32_t> d_pf_tokens, d_pf_pos;
-    const int32_t* cur_pos = nullptr;      // positions of the launch sequence being enqueued (d_pos or d_pf_pos)
-    const int32_t* cur_tokens = nullptr;
     zl_comm_t* comm = nullptr;            // TP exchange (set by zl_llama_set_comm when tp_size > 1)
     int vshard = 0;                       // vocabulary rows of lm_head held by this rank
     dev_ptr<> cand;                       // [B] {float value, int index} local argmax candidates
     dev_ptr<> cand_all;                   // [tp][B] gathered candidates
-    std::map<long long, cudaGraphExec_t> graphs;   // key = B * 2^32 + attention length bucket
-    int cur_max_len = 0;                            // host-side upper bound of buf_lens (positions + 1)
+    GraphCache graphs;                    // decode-step graphs, by graph_key (+ the beam bits)
+    int cur_max_len = 0;                  // host-side upper bound of buf_lens (positions + 1)
     double weight_bytes = 0;
     int kernels_per_step = 0;
     // chunked prefill (cfg.prefill_chunk > 0): activation buffers hold tok_cap = max(max_batch, chunk) tokens
@@ -131,8 +193,7 @@ struct zl_llama {
     dev_ptr<> xq;              // W8A8: quantised activations of the Linear being run (tok_cap x max K bytes)
     dev_ptr<float> xs;         //       their scales (tok_cap; fp8 block: (max K/128, round_up(tok_cap, 4)))
     dev_ptr<int32_t> d_tb;     // token -> task map of the chunk being prefilled
-    const int32_t* cur_tb = nullptr;   // token -> task map of the launch sequence being enqueued (d_iota at decode)
-    dev_ptr<int8_t> d_mask;    // (chunk, max_seq) causal mask of the chunk
+    dev_ptr<int8_t> d_mask;   // (chunk, max_seq) causal mask of the chunk
     // joined steps (zl_llama_step_joined): segments {task, row0, pos0, n} for zl_varlen_attention, then per emitting
     // segment its last row | its task | that row's position (max_batch each); h_join stages them with the tokens,
     // positions and token -> task map of the rows (tok_cap each) for the copies into d_pf_tokens / d_pf_pos / d_tb
@@ -166,54 +227,65 @@ struct zl_llama {
     // between launches (every qkv GEMM of the model runs in stream order on the compute stream)
     dev_ptr<__half> kv8_rows;
     dev_ptr<uint32_t> kv8_cnt;
+    // the task buffers of every layer as a device table (4 per layer: kv_bases), built by the first block pool or row copy
+    dev_ptr<void*> kv_tab;
     // prompt prefix cache (zl_llama_kv_pool_create): the device block pool [layer][K|V][block][bt][H_kv][d] (+ fp32 scales
-    // [layer][K|V][block][bt][H_kv] at kv_int8), the task buffers of every layer as a device table (4 per layer: k, v,
-    // scale k, scale v), and the block lists of zl_llama_kv_blocks_save / load staged like zl_llama_set_state's: one pinned
-    // host slot and one device slot per event, never rewritten while the copy that reads it is still queued
+    // [layer][K|V][block][bt][H_kv] at kv_int8), and the block lists of zl_llama_kv_blocks_save / load, staged on the host
+    // and the device in slots of 2 * pool_cap words
     dev_ptr<> pool, pool_scales;
-    dev_ptr<void*> pool_tab;
     int pool_blocks = 0, pool_bt = 0, pool_cap = 0;   // pool_cap: block pairs one slot holds
-    host_ptr<int32_t> pool_h;                         // [kStageSlots][2 * pool_cap]
-    dev_ptr<int32_t> pool_d;
-    cudaEvent_t pool_ev[kStageSlots] = {};
-    bool pool_used[kStageSlots] = {};
-    int pool_next = 0;
+    StageRing pool_ring;
     // beam search, allocated by the first zl_llama_beam_step / zl_llama_kv_copy_rows: the selection's inputs and outputs
     // (cum (max_batch) f32 | groups (2 max_batch) | parent, token, score (max_batch x 32) each), its workspace, their
-    // pinned host mirror (the beam step is synchronous), and the row-copy ranges staged like the block lists
+    // pinned host mirror (the beam step is synchronous), and the row-copy ranges staged like the block lists, in slots of
+    // 4 * max_batch words
     dev_ptr<> beam_d, beam_ws;
     host_ptr<int32_t> beam_h;
-    dev_ptr<void*> rows_tab;                          // the task buffers of every layer, 4 per layer as pool_tab
-    host_ptr<int32_t> rows_h;                         // [kStageSlots][4 * max_batch]
-    dev_ptr<int32_t> rows_d;
-    cudaEvent_t rows_ev[kStageSlots] = {};
-    bool rows_used[kStageSlots] = {};
-    int rows_next = 0;
+    StageRing rows_ring;
     // generation loop (zl_llama_generate): the per-task stop rules and progress, the loop's control words and the ring of
     // emitted tokens on the device (gen_state lays them out in d_gen), their pinned host mirror, a host mirror of the
     // finish reasons, and one loop graph per (B, sampler, n-gram launch, length bucket), apart from `graphs`
     dev_ptr<int32_t> d_gen;
     host_ptr<int32_t> h_gen;                          // ring rows (max_seq x max_batch) | finish | positions | control
     std::vector<char> gen_fin;
-    std::map<long long, cudaGraphExec_t> gen_graphs;
-    const int32_t* pick_frozen = nullptr;   // set while a loop body is captured: the sampler records no pick of a finished task
+    GraphCache gen_graphs;
 };
 
 namespace {
 
 using namespace zl;
 
-#define RCHECK(expr)                \
-    do {                            \
-        int _rc = (expr);           \
-        if (_rc != ZL_OK) return _rc; \
-    } while (0)
-
 template <typename T>
 int dmalloc(dev_ptr<T>* p, size_t bytes) {
     void* raw = nullptr;
     ZL_CHECK_CUDA(cudaMalloc(&raw, bytes ? bytes : 16));
     p->reset(static_cast<T*>(raw));
+    return ZL_OK;
+}
+
+int StageRing::alloc(size_t slot_words, bool device) {
+    if (device) RCHECK(dmalloc(&d, sizeof(int32_t) * kSlots * slot_words));
+    int32_t* p = nullptr;
+    ZL_CHECK_CUDA(cudaMallocHost((void**)&p, sizeof(int32_t) * kSlots * slot_words));
+    h.reset(p);
+    for (cudaEvent_t& e : ev)
+        if (!e) ZL_CHECK_CUDA(cudaEventCreateWithFlags(&e, cudaEventDisableTiming));
+    words = slot_words;
+    return ZL_OK;
+}
+
+int StageRing::acquire(int32_t** hs, int32_t** ds) {
+    cur = next;
+    next = (cur + 1) % kSlots;
+    if (used[cur]) ZL_CHECK_CUDA(cudaEventSynchronize(ev[cur]));   // its previous reader has executed
+    *hs = h.get() + (size_t)cur * words;
+    if (ds) *ds = d.get() + (size_t)cur * words;
+    return ZL_OK;
+}
+
+int StageRing::release(cudaStream_t st) {
+    ZL_CHECK_CUDA(cudaEventRecord(ev[cur], st));
+    used[cur] = true;
     return ZL_OK;
 }
 
@@ -314,6 +386,12 @@ const Staged* find(const zl_llama* m, const std::string& name) {
 }
 
 void drop(zl_llama* m, const std::string& name) { m->staged.erase(name); }
+
+// drop prefix + suffix for every prefix and suffix
+void drop_parts(zl_llama* m, const std::vector<std::string>& prefixes, std::initializer_list<const char*> suffixes) {
+    for (const auto& p : prefixes)
+        for (const char* s : suffixes) drop(m, p + s);
+}
 
 int fail_state(int line, const std::string& msg, int code = ZL_ERR_STATE) {
     zl_set_last_error(__FILE__, line, msg.c_str());
@@ -446,8 +524,7 @@ int build_bias(zl_llama* m, const std::vector<std::string>& prefixes, const std:
 // keep_perm = false: the weight rows are sequentialised but the GEMM runs without k_perm (its producer wrote x permuted).
 int build_w4(zl_llama* m, const std::vector<std::string>& prefixes, const std::vector<int>& ns, int K, bool swiglu,
              W4Lin* out, bool qkv_rope = false, const std::vector<int32_t>* out_rows = nullptr, bool keep_perm = true) {
-    int N = 0;
-    for (int n : ns) N += n;
+    const int N = std::accumulate(ns.begin(), ns.end(), 0);
     const int G = K / m->cfg.group_size;
     // act-order: Linears fused along N share their input, so they must share its permutation.  Real checkpoints give
     // q / k / v (and gate / up) the same g_idx: their GPTQ Hessian is that of the same input.
@@ -528,41 +605,48 @@ int build_w4(zl_llama* m, const std::vector<std::string>& prefixes, const std::v
         }
     }
     ZL_CHECK_CUDA(cudaStreamSynchronize(m->stream));
-    for (auto& p : prefixes) {
-        drop(m, p + ".qweight");
-        drop(m, p + ".qzeros");
-        drop(m, p + ".scales");
-        drop(m, p + ".g_idx");
-        drop(m, p + ".bias");
-    }
+    drop_parts(m, prefixes, {".qweight", ".qzeros", ".scales", ".g_idx", ".bias"});
     out->N = N;
     out->K = K;
     m->weight_bytes += (double)pbytes;
     return ZL_OK;
 }
 
-int build_dense(zl_llama* m, const std::vector<std::string>& prefixes, const std::vector<int>& ns, int K,
-                DenseLin* out) {
-    int N = 0;
-    for (int n : ns) N += n;
-    RCHECK(dmalloc(&out->w, (size_t)N * K * 2));
+// The part loop of a Linear fused along N from Linears that share its input.  Part i's `prefixes[i].weight` must be
+// (ns[i], K) of `elem`-byte elements and, with a PartScale, `prefixes[i] + scale->suffix` must be f32 and pass scale->ok
+// (when given); then the weight is copied into `fused` at the part's row offset and scale->copy enqueues what the part's
+// scale needs.  A missing or ill-shaped part is reported as "missing/ill-shaped <what> <prefix>".
+struct PartScale {
+    const char* suffix;
+    std::function<bool(size_t i, const Staged& s)> ok;
+    std::function<int(size_t i, int off, const Staged& s)> copy;
+};
+
+int fuse_parts(zl_llama* m, const std::vector<std::string>& prefixes, const std::vector<int>& ns, int K, int elem,
+               void* fused, const std::string& what, const PartScale* scale = nullptr) {
     int off = 0;
     for (size_t i = 0; i < prefixes.size(); ++i) {
         const Staged* w = find(m, prefixes[i] + ".weight");
-        if (!w || w->rows != ns[i] || w->cols != K || w->elem != 2) {
-            zl_set_last_error(__FILE__, __LINE__, ("missing/ill-shaped dense weight " + prefixes[i]).c_str());
-            return ZL_ERR_STATE;
-        }
-        ZL_CHECK_CUDA(cudaMemcpyAsync((char*)out->w.get() + (size_t)off * K * 2, w->ptr.get(), (size_t)ns[i] * K * 2,
+        const Staged* s = scale ? find(m, prefixes[i] + scale->suffix) : nullptr;
+        if (!w || w->rows != ns[i] || w->cols != K || w->elem != elem ||
+            (scale && (!s || s->elem != 4 || (scale->ok && !scale->ok(i, *s)))))
+            return fail_state(__LINE__, "missing/ill-shaped " + what + " " + prefixes[i]);
+        ZL_CHECK_CUDA(cudaMemcpyAsync((char*)fused + (size_t)off * K * elem, w->ptr.get(), (size_t)ns[i] * K * elem,
                                       cudaMemcpyDeviceToDevice, m->stream));
+        if (scale) RCHECK(scale->copy(i, off, *s));
         off += ns[i];
     }
+    return ZL_OK;
+}
+
+int build_dense(zl_llama* m, const std::vector<std::string>& prefixes, const std::vector<int>& ns, int K,
+                DenseLin* out) {
+    const int N = std::accumulate(ns.begin(), ns.end(), 0);
+    RCHECK(dmalloc(&out->w, (size_t)N * K * 2));
+    RCHECK(fuse_parts(m, prefixes, ns, K, 2, out->w.get(), "dense weight"));
     RCHECK(build_bias(m, prefixes, ns, &out->bias));
     ZL_CHECK_CUDA(cudaStreamSynchronize(m->stream));
-    for (auto& p : prefixes) {
-        drop(m, p + ".weight");
-        drop(m, p + ".bias");
-    }
+    drop_parts(m, prefixes, {".weight", ".bias"});
     out->N = N;
     out->K = K;
     m->weight_bytes += (double)N * K * 2;
@@ -594,32 +678,20 @@ int dense_to_int8(zl_llama* m, DenseLin* d) {
 // quant_type 7 (Fp8Linear, linear.cpp:1612-1695): e4m3 weights + one f32 weight_scale per Linear.  Projections that
 // share an input are fused along N with their scalar scales expanded to one scale per output row.
 int build_fp8(zl_llama* m, const std::vector<std::string>& prefixes, const std::vector<int>& ns, int K, DenseLin* out) {
-    int N = 0;
-    for (int n : ns) N += n;
+    const int N = std::accumulate(ns.begin(), ns.end(), 0);
     RCHECK(dmalloc(&out->w8, (size_t)N * K));
     RCHECK(dmalloc(&out->w_scale, (size_t)N * 4));
-    int off = 0;
-    for (size_t i = 0; i < prefixes.size(); ++i) {
-        const Staged* w = find(m, prefixes[i] + ".weight");
-        const Staged* ws = find(m, prefixes[i] + ".weight_scale");
-        if (!w || w->rows != ns[i] || w->cols != K || w->elem != 1 || !ws || ws->elem != 4) {
-            zl_set_last_error(__FILE__, __LINE__, ("missing/ill-shaped fp8 weight or weight_scale " + prefixes[i]).c_str());
-            return ZL_ERR_STATE;
-        }
-        ZL_CHECK_CUDA(cudaMemcpyAsync((char*)out->w8.get() + (size_t)off * K, w->ptr.get(), (size_t)ns[i] * K,
-                                      cudaMemcpyDeviceToDevice, m->stream));
-        k_fill_from_scalar<<<cdiv(ns[i], 256), 256, 0, m->stream>>>(static_cast<float*>(out->w_scale.get()) + off, ns[i],
-                                                                     static_cast<const float*>(ws->ptr.get()));
-        ZL_CHECK_LAUNCH();
-        off += ns[i];
-    }
+    float* w_scale = static_cast<float*>(out->w_scale.get());
+    const PartScale expand{".weight_scale", nullptr, [&](size_t i, int off, const Staged& ws) -> int {
+                               k_fill_from_scalar<<<cdiv(ns[i], 256), 256, 0, m->stream>>>(
+                                   w_scale + off, ns[i], static_cast<const float*>(ws.ptr.get()));
+                               ZL_CHECK_LAUNCH();
+                               return ZL_OK;
+                           }};
+    RCHECK(fuse_parts(m, prefixes, ns, K, 1, out->w8.get(), "fp8 weight or weight_scale", &expand));
     RCHECK(build_bias(m, prefixes, ns, &out->bias));
     ZL_CHECK_CUDA(cudaStreamSynchronize(m->stream));
-    for (auto& p : prefixes) {
-        drop(m, p + ".weight");
-        drop(m, p + ".weight_scale");
-        drop(m, p + ".bias");
-    }
+    drop_parts(m, prefixes, {".weight", ".weight_scale", ".bias"});
     out->N = N;
     out->K = K;
     out->w8_kind = ZL_W8_FP8_ROWS;
@@ -632,8 +704,7 @@ int build_fp8(zl_llama* m, const std::vector<std::string>& prefixes, const std::
 // which needs every part's N to be a multiple of 128.  Fp8Block has no bias (set_has_bias throws).
 int build_fp8_block(zl_llama* m, const std::vector<std::string>& prefixes, const std::vector<int>& ns, int K,
                     DenseLin* out) {
-    int N = 0;
-    for (int n : ns) N += n;
+    const int N = std::accumulate(ns.begin(), ns.end(), 0);
     if (K % 128 != 0 || (prefixes.size() > 1 && N % 128 != 0))
         return fail_state(__LINE__, "fp8 block weights need K % 128 == 0 and every fused part's N % 128 == 0",
                           ZL_ERR_UNSUPPORTED);
@@ -648,28 +719,18 @@ int build_fp8_block(zl_llama* m, const std::vector<std::string>& prefixes, const
     const int KB = K / 128, NB = (N + 127) / 128;
     RCHECK(dmalloc(&out->w8, (size_t)N * K));
     RCHECK(dmalloc(&out->w_scale, (size_t)NB * KB * 4));
-    int off = 0;
-    for (size_t i = 0; i < prefixes.size(); ++i) {
-        const Staged* w = find(m, prefixes[i] + ".weight");
-        const Staged* ws = find(m, prefixes[i] + ".weight_scale_inv");
-        const int nb = (ns[i] + 127) / 128;
-        if (!w || w->rows != ns[i] || w->cols != K || w->elem != 1 || !ws || ws->elem != 4 || ws->rows != nb ||
-            ws->cols != KB) {
-            zl_set_last_error(__FILE__, __LINE__,
-                              ("missing/ill-shaped fp8 block weight or weight_scale_inv " + prefixes[i]).c_str());
-            return ZL_ERR_STATE;
-        }
-        ZL_CHECK_CUDA(cudaMemcpyAsync((char*)out->w8.get() + (size_t)off * K, w->ptr.get(), (size_t)ns[i] * K,
-                                      cudaMemcpyDeviceToDevice, m->stream));
-        ZL_CHECK_CUDA(cudaMemcpyAsync((char*)out->w_scale.get() + (size_t)(off / 128) * KB * 4, ws->ptr.get(),
-                                      (size_t)nb * KB * 4, cudaMemcpyDeviceToDevice, m->stream));
-        off += ns[i];
-    }
+    char* w_scale = static_cast<char*>(out->w_scale.get());
+    const PartScale scale_rows{".weight_scale_inv",
+                               [&](size_t i, const Staged& ws) { return ws.rows == (ns[i] + 127) / 128 && ws.cols == KB; },
+                               [&](size_t, int off, const Staged& ws) -> int {
+                                   ZL_CHECK_CUDA(cudaMemcpyAsync(w_scale + (size_t)(off / 128) * KB * 4, ws.ptr.get(),
+                                                                 (size_t)ws.rows * KB * 4, cudaMemcpyDeviceToDevice,
+                                                                 m->stream));
+                                   return ZL_OK;
+                               }};
+    RCHECK(fuse_parts(m, prefixes, ns, K, 1, out->w8.get(), "fp8 block weight or weight_scale_inv", &scale_rows));
     ZL_CHECK_CUDA(cudaStreamSynchronize(m->stream));
-    for (auto& p : prefixes) {
-        drop(m, p + ".weight");
-        drop(m, p + ".weight_scale_inv");
-    }
+    drop_parts(m, prefixes, {".weight", ".weight_scale_inv"});
     out->N = N;
     out->K = K;
     out->w8_kind = kW8Block;
@@ -679,10 +740,8 @@ int build_fp8_block(zl_llama* m, const std::vector<std::string>& prefixes, const
 
 int take_vector(zl_llama* m, const std::string& name, int n, dev_ptr<>* out) {
     auto it = m->staged.find(name);
-    if (it == m->staged.end() || (size_t)it->second.rows * it->second.cols != (size_t)n || it->second.elem != 2) {
-        zl_set_last_error(__FILE__, __LINE__, ("missing/ill-shaped tensor " + name).c_str());
-        return ZL_ERR_STATE;
-    }
+    if (it == m->staged.end() || (size_t)it->second.rows * it->second.cols != (size_t)n || it->second.elem != 2)
+        return fail_state(__LINE__, "missing/ill-shaped tensor " + name);
     *out = std::move(it->second.ptr);
     m->staged.erase(it);
     m->weight_bytes += (double)n * 2;
@@ -696,36 +755,43 @@ int finalize_layer(zl_llama* m, int l) {
     const int D = c.dim_model, d = c.dim_head;
     RCHECK(take_vector(m, p + "ln_attn.weight", D, &L.ln_attn));
     RCHECK(take_vector(m, p + "ln_ff.weight", D, &L.ln_ff));
-    const std::vector<std::string> qkv = {p + "attn.project_q", p + "attn.project_k", p + "attn.project_v"};
-    const std::vector<int> qkv_n = {m->hq * d, m->hkv * d, m->hkv * d};
-    const std::vector<std::string> gu = {p + "ff.w_in", p + "ff.w_gated"};
-    const std::vector<int> gu_n = {m->ff, m->ff};
+    // the layer's Linears in build order, each fused along N from parts that share its input
+    struct Lin {
+        std::vector<std::string> prefixes;
+        std::vector<int> ns;
+        int K;
+        W4Lin* q;
+        DenseLin* d;
+    };
+    const Lin lins[] = {
+        {{p + "attn.project_q", p + "attn.project_k", p + "attn.project_v"}, {m->hq * d, m->hkv * d, m->hkv * d}, D,
+         &L.q_qkv, &L.d_qkv},
+        {{p + "attn.attn_out"}, {D}, m->hq * d, &L.q_o, &L.d_o},
+        {{p + "ff.w_in", p + "ff.w_gated"}, {m->ff, m->ff}, D, &L.q_gu, &L.d_gu},
+        {{p + "ff.w_out"}, {D}, m->ff, &L.q_down, &L.d_down},
+    };
+    const Lin &qkv = lins[0], &gu = lins[2], &down = lins[3];
     if (c.quant_type == 5 || c.quant_type == 6) {
         // act-order w_out: its permutation orders the gate / up rows, so down runs without one.  A bad w_out g_idx is
         // reported by its own build_w4 below, after the errors of the Linears built before it.
         std::vector<int32_t> down_perm;
-        if (g_idx_perm(m, p + "ff.w_out", m->ff, &down_perm) != ZL_OK) down_perm.clear();
-        RCHECK(build_w4(m, qkv, qkv_n, D, false, &L.q_qkv, c.fuse >= 2));
-        RCHECK(build_w4(m, {p + "attn.attn_out"}, {D}, m->hq * d, false, &L.q_o));
-        RCHECK(build_w4(m, gu, gu_n, D, true, &L.q_gu, false, &down_perm));
-        RCHECK(build_w4(m, {p + "ff.w_out"}, {D}, m->ff, false, &L.q_down, false, nullptr, false));
-    } else if (c.quant_type == 7) {
-        RCHECK(build_fp8(m, qkv, qkv_n, D, &L.d_qkv));
-        RCHECK(build_fp8(m, {p + "attn.attn_out"}, {D}, m->hq * d, &L.d_o));
-        RCHECK(build_fp8(m, gu, gu_n, D, &L.d_gu));
-        RCHECK(build_fp8(m, {p + "ff.w_out"}, {D}, m->ff, &L.d_down));
-    } else if (c.quant_type == 10) {
-        RCHECK(build_fp8_block(m, qkv, qkv_n, D, &L.d_qkv));
-        RCHECK(build_fp8_block(m, {p + "attn.attn_out"}, {D}, m->hq * d, &L.d_o));
-        RCHECK(build_fp8_block(m, gu, gu_n, D, &L.d_gu));
-        RCHECK(build_fp8_block(m, {p + "ff.w_out"}, {D}, m->ff, &L.d_down));
+        if (g_idx_perm(m, down.prefixes[0], m->ff, &down_perm) != ZL_OK) down_perm.clear();
+        for (const Lin& f : lins) {
+            const bool swiglu = &f == &gu;
+            RCHECK(build_w4(m, f.prefixes, f.ns, f.K, swiglu, f.q, &f == &qkv && c.fuse >= 2,
+                            swiglu ? &down_perm : nullptr, &f != &down));
+        }
     } else {
-        RCHECK(build_dense(m, qkv, qkv_n, D, &L.d_qkv));
-        RCHECK(build_dense(m, {p + "attn.attn_out"}, {D}, m->hq * d, &L.d_o));
-        RCHECK(build_dense(m, gu, gu_n, D, &L.d_gu));
-        RCHECK(build_dense(m, {p + "ff.w_out"}, {D}, m->ff, &L.d_down));
+        for (const Lin& f : lins) {
+            if (c.quant_type == 7)
+                RCHECK(build_fp8(m, f.prefixes, f.ns, f.K, f.d));
+            else if (c.quant_type == 10)
+                RCHECK(build_fp8_block(m, f.prefixes, f.ns, f.K, f.d));
+            else
+                RCHECK(build_dense(m, f.prefixes, f.ns, f.K, f.d));
+        }
         if (c.quant_type == 2)
-            for (DenseLin* dl : {&L.d_qkv, &L.d_o, &L.d_gu, &L.d_down}) RCHECK(dense_to_int8(m, dl));
+            for (const Lin& f : lins) RCHECK(dense_to_int8(m, f.d));
     }
     return ZL_OK;
 }
@@ -910,13 +976,10 @@ int alloc_runtime(zl_llama* m) {
     ZL_CHECK_CUDA(cudaMemsetAsync(m->d_seq_len.get(), 0, (size_t)B * 4, m->stream));
     ZL_CHECK_CUDA(cudaMemsetAsync(m->d_bias_cnt.get(), 0, (size_t)B * 4, m->stream));
     RCHECK(alloc_generate(m));
-    int32_t *stage = nullptr, *ring = nullptr;
+    int32_t* stage = nullptr;
     ZL_CHECK_CUDA(cudaMallocHost((void**)&stage, sizeof(int32_t) * (4 * B + 4 + T)));
     m->h_stage.reset(stage);
-    ZL_CHECK_CUDA(cudaMallocHost((void**)&ring, sizeof(int32_t) * zl_llama::kStageSlots * 2 * B));
-    m->h_ring.reset(ring);
-    for (int i = 0; i < zl_llama::kStageSlots; ++i)
-        ZL_CHECK_CUDA(cudaEventCreateWithFlags(&m->ring_ev[i], cudaEventDisableTiming));
+    RCHECK(m->state_ring.alloc((size_t)2 * B, false));
     ZL_CHECK_CUDA(cudaStreamSynchronize(m->stream));
     return ZL_OK;
 }
@@ -991,6 +1054,11 @@ struct Chain {
         kAllReduce,     // tensor parallel: o / down partial sums -> one-shot all-reduce fused with the residual add
     };
     int row0 = 0, n = 0;       // rows of the activation matrices this sequence covers
+    // of the whole launch sequence (index them from row0): its token -> task map (d_iota at decode), positions (d_pos or
+    // d_pf_pos) and tokens
+    const int32_t* tb = nullptr;
+    const int32_t* pos = nullptr;
+    const int32_t* tokens = nullptr;
     Sink sink = kAddResidual;
     bool no_pdl = false;       // full dependencies and no L2 head: the next launch is not the chain successor (dual stream)
     bool gemm_only = false;    // launch only what the GEMMs of this fuse level comprise: no stand-alone RMSNorm (fuse 0)
@@ -1030,10 +1098,7 @@ int w4_gemm(zl_llama* m, int l, Stage s, const Chain& ch, const W4Lin& w, const 
     const int route = route_of(w, ch.n);
     a.packed = route ? w.packed_i.get() : w.packed.get();
     a.variant = route ? 1 : 0;
-    if (!a.packed) {
-        zl_set_last_error(__FILE__, __LINE__, "no packed weight variant for this batch size");
-        return ZL_ERR_STATE;
-    }
+    if (!a.packed) return fail_state(__LINE__, "no packed weight variant for this batch size");
     const int pdl = ch.no_pdl ? 0 : c.use_pdl;
     if (ln_w && (c.fuse == 0 || route == 4 || (w.k_perm && route != 3))) {
         // the RMSNorm runs as its own kernel (reference order, block.cpp:125,131) into the matching rows of xn: at fuse 0,
@@ -1080,7 +1145,7 @@ int kv8_append(zl_llama* m, int l, const Chain& ch, int pdl) {
     const size_t row = (size_t)m->hkv * c.dim_head;
     const __half* ks = static_cast<const __half*>(m->kv_stage.get()) + ch.row0 * row;
     const __half* vs = static_cast<const __half*>(m->kv_stage.get()) + ((size_t)m->tok_cap + ch.row0) * row;
-    return zl_kv_int8_quant_append(ks, vs, m->cur_tb + ch.row0, m->cur_pos + ch.row0, L.k_addrs.get(), L.v_addrs.get(),
+    return zl_kv_int8_quant_append(ks, vs, ch.tb + ch.row0, ch.pos + ch.row0, L.k_addrs.get(), L.v_addrs.get(),
                                    L.sk_addrs.get(), L.sv_addrs.get(), ch.n, m->hkv, c.dim_head, c.dtype, pdl, m->stream);
 }
 
@@ -1110,8 +1175,8 @@ int qkv_gemm(zl_llama* m, int l, Chain& ch) {
     const float* cos = m->cosb.get() + (size_t)ch.row0 * d;
     const float* sin = m->sinb.get() + (size_t)ch.row0 * d;
     void* q = rows(m->q.get(), ch.row0, m->hq * d);
-    const int32_t* tb = m->cur_tb + ch.row0;
-    const int32_t* pos = m->cur_pos + ch.row0;
+    const int32_t* tb = ch.tb + ch.row0;
+    const int32_t* pos = ch.pos + ch.row0;
     // int8 cache at fuse >= 2 on the exact-integer route (M <= 16): the epilogue quantises K / V into the cache.  The wgmma
     // and fp16 routes, and act-order qkv, append fp16 rows to the staging rows and kv8_append quantises them.
     const bool fused_kv8 = c.kv_int8 && c.fuse >= 2 && !L.q_qkv.k_perm && route_of(L.q_qkv, ch.n) == 3;
@@ -1270,7 +1335,8 @@ static bool prefill_dual_enabled(const zl_llama* m, int n) {
     return force == 1 || (force == 2 && c.tp_size > 1);
 }
 
-int prefill_layers_dual(zl_llama* m, const Segments& pf) {
+// ch: the chunk's launch sequence, whose token -> task map, positions and tokens the halves share
+int prefill_layers_dual(zl_llama* m, const Segments& pf, const Chain& ch) {
     const auto& c = m->cfg;
     RCHECK(ensure_dual_resources(m));
     const int D = c.dim_model, d = c.dim_head, dt = c.dtype;
@@ -1282,6 +1348,9 @@ int prefill_layers_dual(zl_llama* m, const Segments& pf) {
     for (int h = 0; h < 2; ++h) {
         half[h].row0 = h ? n0 : 0;
         half[h].n = h ? pf.n - n0 : n0;
+        half[h].tb = ch.tb;
+        half[h].pos = ch.pos;
+        half[h].tokens = ch.tokens;
         half[h].sink = Chain::kPartial;
         half[h].no_pdl = true;
         half[h].h = m->h.get();
@@ -1331,8 +1400,41 @@ struct BeamPick {
     void* ws = nullptr;
 };
 
-int enqueue_step(zl_llama* m, int n_tasks, int len_bucket, const Segments* pf = nullptr, bool sampler = false,
-                 const BeamPick* beam = nullptr, bool ngram = false) {
+// How a launch sequence picks its tokens: zl_argmax (or the tensor-parallel candidate exchange), the sampler -- with the
+// n-gram launch when `ngram` -- or a beam step's top-k.  frozen (a loop graph's finish reasons): the sampler records no
+// pick of a finished task.
+struct Pick {
+    bool sampler = false, ngram = false;
+    const BeamPick* beam = nullptr;
+    const int32_t* frozen = nullptr;
+
+    // task t samples (or has penalties or logits processors), and has the n-gram rule on
+    void add(const zl_llama* m, int t) {
+        sampler |= m->samp_on[t] != 0;
+        ngram |= m->ngram_on[t] != 0;
+    }
+};
+
+// the pick of tasks first .. first + n - 1
+Pick pick_of(const zl_llama* m, int first, int n) {
+    Pick pk;
+    for (int t = first; t < first + n; ++t) pk.add(m, t);
+    return pk;
+}
+
+// The final RMSNorm of rows row0 .. row0 + n - 1 of the residual stream h into xn.  W4: the down epilogue already added
+// the residual; dense: the last down's output (pend) is added here.
+int final_norm(zl_llama* m, void* h, int row0, int n, int pdl) {
+    const auto& c = m->cfg;
+    const int D = c.dim_model;
+    void* hr = rows(h, row0, D);
+    if (c.quant_type == 5 || c.quant_type == 6)
+        return zl_rmsnorm(hr, m->ln_f.get(), m->xn.get(), n, D, c.eps, 1.f, c.dtype, pdl, m->stream);
+    return zl_add_rmsnorm(hr, rows(m->pend.get(), row0, D), m->ln_f.get(), hr, m->xn.get(), n, D, c.eps, 1.f, 0, c.dtype,
+                          pdl, m->stream);
+}
+
+int enqueue_step(zl_llama* m, int n_tasks, int len_bucket, const Segments* pf, const Pick& pk) {
     const auto& c = m->cfg;
     const int B = pf ? pf->n : n_tasks;   // rows (tokens) of every activation matrix in this launch sequence
     const int D = c.dim_model, d = c.dim_head, dt = c.dtype, pdl = c.use_pdl;
@@ -1340,10 +1442,7 @@ int enqueue_step(zl_llama* m, int n_tasks, int len_bucket, const Segments* pf = 
     const bool w4 = c.quant_type == 5 || c.quant_type == 6;
     const bool tp = c.tp_size > 1;
     const bool joined = pf && pf->joined;
-    if (tp && !m->comm) {
-        zl_set_last_error(__FILE__, __LINE__, "tp_size > 1 but zl_llama_set_comm was not called");
-        return ZL_ERR_STATE;
-    }
+    if (tp && !m->comm) return fail_state(__LINE__, "tp_size > 1 but zl_llama_set_comm was not called");
     // joined steps: d_join = segments (nseg x 4) | emitting rows | their tasks | their positions (max_batch each)
     const int32_t* j_seg = joined ? m->d_join.get() : nullptr;
     const int32_t* j_rows = joined ? j_seg + 4 * c.max_batch : nullptr;
@@ -1359,15 +1458,15 @@ int enqueue_step(zl_llama* m, int n_tasks, int len_bucket, const Segments* pf = 
         ZL_CHECK_CUDA(launch(k_lens_from_pos, dim3(cdiv(B, 64)), dim3(64), 0, st, false, (const int32_t*)m->d_pos.get(),
                              m->d_lens.get(), B, g_w4_trace));
     }
-    m->cur_tb = pf ? m->d_tb.get() : m->d_iota.get();
-    m->cur_pos = pf ? m->d_pf_pos.get() : m->d_pos.get();
-    m->cur_tokens = pf ? m->d_pf_tokens.get() : m->d_tokens.get();
-    RCHECK(zl_rope_cos_sin(m->cur_pos, m->cosb.get(), m->sinb.get(), B, d, c.rope_theta, c.rope_llama3_factor,
-                           c.rope_low_freq_factor, c.rope_high_freq_factor, c.rope_orig_ctx, 1, st));
-    RCHECK(zl_embedding(m->cur_tokens, m->emb.get(), m->h.get(), B, D, c.vocab_size, dt, 0, st));
-    const bool dual = pf && !joined && prefill_dual_enabled(m, pf->n);
-    if (dual) RCHECK(prefill_layers_dual(m, *pf));
     Chain ch;
+    ch.tb = pf ? m->d_tb.get() : m->d_iota.get();
+    ch.pos = pf ? m->d_pf_pos.get() : m->d_pos.get();
+    ch.tokens = pf ? m->d_pf_tokens.get() : m->d_tokens.get();
+    RCHECK(zl_rope_cos_sin(ch.pos, m->cosb.get(), m->sinb.get(), B, d, c.rope_theta, c.rope_llama3_factor,
+                           c.rope_low_freq_factor, c.rope_high_freq_factor, c.rope_orig_ctx, 1, st));
+    RCHECK(zl_embedding(ch.tokens, m->emb.get(), m->h.get(), B, D, c.vocab_size, dt, 0, st));
+    const bool dual = pf && !joined && prefill_dual_enabled(m, pf->n);
+    if (dual) RCHECK(prefill_layers_dual(m, *pf, ch));
     ch.n = B;
     ch.sink = tp ? Chain::kAllReduce : Chain::kAddResidual;
     ch.h = m->h.get();
@@ -1395,7 +1494,7 @@ int enqueue_step(zl_llama* m, int n_tasks, int len_bucket, const Segments* pf = 
             if (c.kv_int8) {
                 RCHECK(kv8_rope_append(m, l, ch, m->qkv.get(), m->q.get(), pdl));
             } else {
-                RCHECK(zl_qkv_rope_append(m->cosb.get(), m->sinb.get(), m->qkv.get(), m->q.get(), m->cur_tb, m->cur_pos,
+                RCHECK(zl_qkv_rope_append(m->cosb.get(), m->sinb.get(), m->qkv.get(), m->q.get(), ch.tb, ch.pos,
                                           L.k_addrs.get(), L.v_addrs.get(), B, m->hq, m->hkv, d, 1, 1, m->d_lens.get(), dt,
                                           pdl, st));
             }
@@ -1436,11 +1535,7 @@ int enqueue_step(zl_llama* m, int n_tasks, int len_bucket, const Segments* pf = 
         if (pf->n_emit == 0) return ZL_OK;
         // the final norm is row-wise: norm every row, then gather the emitting segments' last rows into rows
         // 0 .. n_emit - 1 of pend (free after the norm), so that only they reach lm_head
-        if (w4)
-            RCHECK(zl_rmsnorm(m->h.get(), m->ln_f.get(), m->xn.get(), B, D, c.eps, 1.f, dt, pdl, st));
-        else
-            RCHECK(zl_add_rmsnorm(m->h.get(), m->pend.get(), m->ln_f.get(), m->h.get(), m->xn.get(), B, D, c.eps, 1.f, 0,
-                                  dt, pdl, st));
+        RCHECK(final_norm(m, m->h.get(), 0, B, pdl));
         k_gather_rows<<<pf->n_emit, 256, 0, st>>>(static_cast<const uint16_t*>(m->xn.get()), j_rows,
                                                  static_cast<uint16_t*>(m->pend.get()), D);
         ZL_CHECK_LAUNCH();
@@ -1448,39 +1543,31 @@ int enqueue_step(zl_llama* m, int n_tasks, int len_bucket, const Segments* pf = 
     } else if (pf) {
         if (!pf->last) return ZL_OK;
         // only the last prompt position feeds the head: move it to row 0 semantics by pointing at its row
-        void* hl = rows(m->h.get(), pf->n - 1, D);
-        if (w4) {
-            RCHECK(zl_rmsnorm(hl, m->ln_f.get(), m->xn.get(), 1, D, c.eps, 1.f, dt, pdl, st));
-        } else {
-            RCHECK(zl_add_rmsnorm(hl, rows(m->pend.get(), pf->n - 1, D), m->ln_f.get(), hl, m->xn.get(), 1, D, c.eps, 1.f,
-                                  0, dt, pdl, st));
-        }
-    } else if (w4) {
-        RCHECK(zl_rmsnorm(ch.h, m->ln_f.get(), m->xn.get(), B, D, c.eps, 1.f, dt, stage_pdl(m, kFinalNorm), st));
+        RCHECK(final_norm(m, m->h.get(), pf->n - 1, 1, pdl));
     } else {
-        RCHECK(zl_add_rmsnorm(m->h.get(), m->pend.get(), m->ln_f.get(), m->h.get(), m->xn.get(), B, D, c.eps, 1.f, 0, dt,
-                              stage_pdl(m, kFinalNorm), st));
+        // ch.h: the stream the last exchange left the residual in (h2 after a fused tensor-parallel exchange)
+        RCHECK(final_norm(m, ch.h, 0, B, stage_pdl(m, kFinalNorm)));
     }
     const int HB = joined ? pf->n_emit : pf ? 1 : B;   // rows that reach lm_head
     // vocab-parallel lm_head (embedding.cu:353-392): each rank owns vshard rows
     RCHECK(zl_dense_gemm_skinny(head_x, D, m->lm_head, nullptr, m->logits.get(), HB, m->vshard, D, dt, ZL_F32,
                                 stage_pdl(m, kLmHead), st));
-    if (beam) {
+    if (const BeamPick* beam = pk.beam) {
         // decode rows only, single rank, no sampling (zl_llama_beam_step checks)
         RCHECK(beam_topk_launch(m->logits.get(), HB, m->vshard, beam->cum, beam->groups, beam->G, beam->K, beam->parent,
                                 beam->token, beam->score, beam->ws, stage_pdl(m, kPick), st));
-    } else if (sampler) {
+    } else if (pk.sampler) {
         // one row per task at decode (row b = task b, counter = its input position); prefill: the task's last prompt
         // position; joined: each emitting segment's task and last position.  set_sampling keeps this off under tensor
         // parallelism.
         const int32_t* row_task = joined ? j_task : pf ? m->d_iota.get() + pf->task : m->d_iota.get();
         const int32_t* counter = joined ? j_pos : pf ? m->d_pf_pos.get() + (pf->n - 1) : m->d_pos.get();
-        // k_ngram_levels runs only when a task of the step has the n-gram rule on (`ngram`, a bit of the graph key)
+        // k_ngram_levels runs only when a task of the step has the n-gram rule on (`pk.ngram`, a bit of the graph key)
         RCHECK(sample_processed_launch(m->logits.get(), HB, m->vshard, m->d_sparams.get(), row_task, counter,
-                                       m->d_hist.get(), m->hwords, ngram ? m->d_ngram.get() : nullptr, m->d_seq.get(),
+                                       m->d_hist.get(), m->hwords, pk.ngram ? m->d_ngram.get() : nullptr, m->d_seq.get(),
                                        m->d_seq_len.get(), c.max_seq, m->d_bias_tok.get(), m->d_bias_val.get(),
-                                       m->d_bias_cnt.get(), ZL_MAX_LOGIT_BIAS, m->pick_frozen, m->d_next.get(),
-                                       ngram ? m->ngram_ws.get() : nullptr, m->ngram_ws_bytes, stage_pdl(m, kPick), st));
+                                       m->d_bias_cnt.get(), ZL_MAX_LOGIT_BIAS, pk.frozen, m->d_next.get(),
+                                       pk.ngram ? m->ngram_ws.get() : nullptr, m->ngram_ws_bytes, stage_pdl(m, kPick), st));
     } else if (!tp) {
         RCHECK(zl_argmax(m->logits.get(), m->d_next.get(), HB, m->vshard, m->argmax_ws.get(), zl_argmax_workspace_bytes(HB),
                          stage_pdl(m, kPick), st));
@@ -1502,47 +1589,48 @@ int len_bucket_of(const zl_llama* m, int max_len) {
     return b < m->cfg.max_seq ? b : (m->cfg.max_seq > 256 ? m->cfg.max_seq : 256);
 }
 
-bool sampler_on(const zl_llama* m, int first, int n) {
-    for (int t = first; t < first + n; ++t)
-        if (m->samp_on[t]) return true;
-    return false;
-}
-
-bool ngram_on(const zl_llama* m, int first, int n) {
-    for (int t = first; t < first + n; ++t)
-        if (m->ngram_on[t]) return true;
-    return false;
+// The key bits the step and loop graphs share: B (bits 33 ..), the sampler (bit 32), the n-gram launch (bit 31) and the
+// length bucket (below 2^31).  Parameter changes need no re-capture (they live on the device), only switching the sampler
+// or the n-gram launch on or off does.
+long long graph_key(int B, const Pick& pk, int bucket) {
+    return ((long long)B << 33) | ((long long)pk.sampler << 32) | ((long long)pk.ngram << 31) | (unsigned)bucket;
 }
 
 int run_step(zl_llama* m, int B, const BeamPick* beam = nullptr) {
     const int bucket = len_bucket_of(m, m->cur_max_len);
-    const bool sampler = sampler_on(m, 0, B), ngram = ngram_on(m, 0, B);
-    if (!m->cfg.use_graph) return enqueue_step(m, B, bucket, nullptr, sampler, beam, ngram);
-    // parameter changes need no re-capture (they live on the device), only switching the sampler (bit 32) or the n-gram
-    // launch (bit 31; buckets stay below 2^31) on or off does.  A beam step (bit 62) bakes its group count (bits 44-54)
-    // and K (bits 55-60) into its launches; B < 2048 at a beam step.
-    long long key = ((long long)B << 33) | ((long long)sampler << 32) | ((long long)ngram << 31) | (unsigned)bucket;
+    Pick pk = pick_of(m, 0, B);
+    pk.beam = beam;
+    if (!m->cfg.use_graph) return enqueue_step(m, B, bucket, nullptr, pk);
+    // a beam step (bit 62) bakes its group count (bits 44-54) and K (bits 55-60) into its launches; B < 2048 at a beam step
+    long long key = graph_key(B, pk, bucket);
     if (beam) key |= (1LL << 62) | ((long long)beam->K << 55) | ((long long)beam->G << 44);
-    auto it = m->graphs.find(key);
-    if (it == m->graphs.end()) {
-        cudaGraph_t graph = nullptr;
+    auto capture = [&](cudaGraph_t* graph) -> int {
         ZL_CHECK_CUDA(cudaStreamBeginCapture(m->stream, cudaStreamCaptureModeThreadLocal));
-        int rc = enqueue_step(m, B, bucket, nullptr, sampler, beam, ngram);
-        cudaError_t ce = cudaStreamEndCapture(m->stream, &graph);
-        if (rc != ZL_OK) {
-            if (graph) cudaGraphDestroy(graph);
-            return rc;
-        }
+        const int rc = enqueue_step(m, B, bucket, nullptr, pk);
+        const cudaError_t ce = cudaStreamEndCapture(m->stream, graph);
+        RCHECK(rc);
         ZL_CHECK_CUDA(ce);
-        cudaGraphExec_t exec = nullptr;
-        ZL_CHECK_CUDA(cudaGraphInstantiate(&exec, graph, 0));
-        size_t n_nodes = 0;
-        cudaGraphGetNodes(graph, nullptr, &n_nodes);
-        m->kernels_per_step = (int)n_nodes;
-        cudaGraphDestroy(graph);
-        it = m->graphs.emplace(key, exec).first;
+        return ZL_OK;
+    };
+    cudaGraphExec_t exec = nullptr;
+    RCHECK(m->graphs.get(key, capture, &exec, &m->kernels_per_step));
+    ZL_CHECK_CUDA(cudaGraphLaunch(exec, m->stream));
+    return ZL_OK;
+}
+
+// The pick readback: the n picks in d_next and, when logits_host is given, their n logits rows, once everything enqueued
+// has executed.  *picks: the picks in the pinned staging words.
+int read_picks(zl_llama* m, int n, float* logits_host, const int32_t** picks) {
+    int32_t* h = m->h_stage.get() + 3 * m->cfg.max_batch;
+    cudaStream_t st = m->stream;
+    if (n > 0) {
+        ZL_CHECK_CUDA(cudaMemcpyAsync(h, m->d_next.get(), (size_t)n * 4, cudaMemcpyDeviceToHost, st));
+        if (logits_host)   // (n, vocab/tp) of this rank's shard
+            ZL_CHECK_CUDA(cudaMemcpyAsync(logits_host, m->logits.get(), (size_t)n * m->vshard * 4, cudaMemcpyDeviceToHost,
+                                          st));
     }
-    ZL_CHECK_CUDA(cudaGraphLaunch(it->second, m->stream));
+    ZL_CHECK_CUDA(cudaStreamSynchronize(st));
+    *picks = h;
     return ZL_OK;
 }
 
@@ -1614,29 +1702,18 @@ extern "C" void zl_llama_destroy(zl_llama_t* m) {
     if (!m) return;
     cudaStreamSynchronize(m->stream);
     if (m->reduce_stream) cudaStreamSynchronize(m->reduce_stream);
-    for (auto& g : m->graphs) cudaGraphExecDestroy(g.second);
-    for (auto& g : m->gen_graphs) cudaGraphExecDestroy(g.second);
     for (int h = 0; h < 2; ++h)
         for (cudaEvent_t e : {m->ev_o[h], m->ev_r1[h], m->ev_dn[h], m->ev_r2[h]})
             if (e) cudaEventDestroy(e);
-    for (cudaEvent_t e : m->ring_ev)
-        if (e) cudaEventDestroy(e);
-    for (cudaEvent_t e : m->pool_ev)
-        if (e) cudaEventDestroy(e);
-    for (cudaEvent_t e : m->rows_ev)
-        if (e) cudaEventDestroy(e);
     if (m->reduce_stream) cudaStreamDestroy(m->reduce_stream);
     cudaStreamDestroy(m->stream);
-    delete m;   // the members free their device and pinned buffers
+    delete m;   // the members free their device and pinned buffers, graphs and staging events
 }
 
 extern "C" int zl_llama_load_tensor(zl_llama_t* m, const char* name, const void* data_host, int rows, int cols,
                                     int elem_bytes) {
     ZL_CHECK_ARG(m && name && data_host && rows > 0 && cols > 0 && elem_bytes > 0);
-    if (m->finalized) {
-        zl_set_last_error(__FILE__, __LINE__, "model already finalized");
-        return ZL_ERR_STATE;
-    }
+    if (m->finalized) return fail_state(__LINE__, "model already finalized");
     Staged s;
     s.rows = rows;
     s.cols = cols;
@@ -1740,10 +1817,7 @@ int stage_random_linear(zl_llama* m, const std::string& prefix, int K, int N, ui
 
 extern "C" int zl_llama_init_synthetic(zl_llama_t* m, uint64_t seed) {
     ZL_CHECK_ARG(m);
-    if (m->finalized) {
-        zl_set_last_error(__FILE__, __LINE__, "model already finalized");
-        return ZL_ERR_STATE;
-    }
+    if (m->finalized) return fail_state(__LINE__, "model already finalized");
     const auto& c = m->cfg;
     const int D = c.dim_model, d = c.dim_head;
     for (int l = 0; l < c.num_layers; ++l) {
@@ -1773,14 +1847,9 @@ extern "C" int zl_llama_init_synthetic(zl_llama_t* m, uint64_t seed) {
 extern "C" int zl_llama_set_state(zl_llama_t* m, const int32_t* tokens_host, const int32_t* positions_host,
                                   int B) {
     ZL_CHECK_ARG(m && tokens_host && positions_host && B > 0 && B <= m->cfg.max_batch);
-    if (!m->finalized) {
-        zl_set_last_error(__FILE__, __LINE__, "model not finalized");
-        return ZL_ERR_STATE;
-    }
-    const int slot = m->ring_next;
-    m->ring_next = (slot + 1) % zl_llama::kStageSlots;
-    if (m->ring_used[slot]) ZL_CHECK_CUDA(cudaEventSynchronize(m->ring_ev[slot]));   // its previous copies have executed
-    int32_t* hs = m->h_ring.get() + (size_t)slot * 2 * m->cfg.max_batch;
+    if (!m->finalized) return fail_state(__LINE__, "model not finalized");
+    int32_t* hs = nullptr;
+    RCHECK(m->state_ring.acquire(&hs));
     int mx = 0;
     for (int i = 0; i < B; ++i) {
         ZL_CHECK_ARG(positions_host[i] >= 0 && positions_host[i] < m->cfg.max_seq);
@@ -1792,17 +1861,12 @@ extern "C" int zl_llama_set_state(zl_llama_t* m, const int32_t* tokens_host, con
     m->cur_max_len = mx;
     ZL_CHECK_CUDA(cudaMemcpyAsync(m->d_tokens.get(), hs, B * 4, cudaMemcpyHostToDevice, m->stream));
     ZL_CHECK_CUDA(cudaMemcpyAsync(m->d_pos.get(), hs + B, B * 4, cudaMemcpyHostToDevice, m->stream));
-    ZL_CHECK_CUDA(cudaEventRecord(m->ring_ev[slot], m->stream));
-    m->ring_used[slot] = true;
-    return ZL_OK;
+    return m->state_ring.release(m->stream);
 }
 
 extern "C" int zl_llama_step_device(zl_llama_t* m, int B) {
     ZL_CHECK_ARG(m && B > 0 && B <= m->cfg.max_batch);
-    if (m->cur_max_len >= m->cfg.max_seq) {
-        zl_set_last_error(__FILE__, __LINE__, "KV buffers full (max_seq reached)");
-        return ZL_ERR_STATE;
-    }
+    if (m->cur_max_len >= m->cfg.max_seq) return fail_state(__LINE__, "KV buffers full (max_seq reached)");
     RCHECK(run_step(m, B));
     k_advance<<<cdiv(B, 64), 64, 0, m->stream>>>(m->d_tokens.get(), m->d_pos.get(), m->d_next.get(), B, g_w4_trace);
     ZL_CHECK_LAUNCH();
@@ -1815,12 +1879,9 @@ extern "C" int zl_llama_decode(zl_llama_t* m, const int32_t* tokens_host, const 
     ZL_CHECK_ARG(next_tokens_host != nullptr);
     RCHECK(zl_llama_set_state(m, tokens_host, positions_host, B));
     RCHECK(run_step(m, B));
-    ZL_CHECK_CUDA(cudaMemcpyAsync(m->h_stage.get() + 3 * B, m->d_next.get(), B * 4, cudaMemcpyDeviceToHost, m->stream));
-    if (logits_host)   // (B, vocab/tp) of this rank's shard
-        ZL_CHECK_CUDA(cudaMemcpyAsync(logits_host, m->logits.get(), (size_t)B * m->vshard * 4, cudaMemcpyDeviceToHost,
-                                      m->stream));
-    ZL_CHECK_CUDA(cudaStreamSynchronize(m->stream));
-    for (int i = 0; i < B; ++i) next_tokens_host[i] = m->h_stage.get()[3 * B + i];
+    const int32_t* picks = nullptr;
+    RCHECK(read_picks(m, B, logits_host, &picks));
+    for (int i = 0; i < B; ++i) next_tokens_host[i] = picks[i];
     return ZL_OK;
 }
 
@@ -1856,8 +1917,8 @@ extern "C" int zl_llama_bench_gemms(zl_llama_t* m, int B, int iters, float* ms, 
     ch.n = B;
     ch.gemm_only = true;
     ch.h = m->h.get();
-    m->cur_tb = m->d_iota.get();
-    m->cur_pos = m->d_pos.get();
+    ch.tb = m->d_iota.get();
+    ch.pos = m->d_pos.get();
     cudaEvent_t e0, e1;
     ZL_CHECK_CUDA(cudaEventCreate(&e0));
     ZL_CHECK_CUDA(cudaEventCreate(&e1));
@@ -1916,14 +1977,8 @@ extern "C" int zl_llama_prefill(zl_llama_t* m, int task, const int32_t* tokens_h
     ZL_CHECK_ARG(m && m->finalized && tokens_host && next_token_host && n > 0 && pos0 >= 0);
     ZL_CHECK_ARG(task >= 0 && task < m->cfg.max_batch);
     const int chunk = m->cfg.prefill_chunk;
-    if (chunk <= 0) {
-        zl_set_last_error(__FILE__, __LINE__, "zl_llama_prefill needs cfg.prefill_chunk > 0");
-        return ZL_ERR_STATE;
-    }
-    if (pos0 + n > m->cfg.max_seq) {
-        zl_set_last_error(__FILE__, __LINE__, "prompt does not fit the KV buffers (max_seq)");
-        return ZL_ERR_STATE;
-    }
+    if (chunk <= 0) return fail_state(__LINE__, "zl_llama_prefill needs cfg.prefill_chunk > 0");
+    if (pos0 + n > m->cfg.max_seq) return fail_state(__LINE__, "prompt does not fit the KV buffers (max_seq)");
     int32_t* h_tok = m->h_stage.get() + 4 * m->cfg.max_batch + 4;   // pinned staging for one chunk of token ids
     for (int c0 = 0; c0 < n; c0 += chunk) {
         const int cn = (n - c0) < chunk ? (n - c0) : chunk;
@@ -1938,13 +1993,11 @@ extern "C" int zl_llama_prefill(zl_llama_t* m, int task, const int32_t* tokens_h
         pc.pos0 = pos0 + c0;
         pc.n = cn;
         pc.last = c0 + cn == n;
-        RCHECK(enqueue_step(m, 1, 0, &pc, sampler_on(m, task, 1), nullptr, ngram_on(m, task, 1)));
+        RCHECK(enqueue_step(m, 1, 0, &pc, pick_of(m, task, 1)));
     }
-    ZL_CHECK_CUDA(cudaMemcpyAsync(m->h_stage.get() + 3 * m->cfg.max_batch, m->d_next.get(), 4, cudaMemcpyDeviceToHost, m->stream));
-    if (logits_host)
-        ZL_CHECK_CUDA(cudaMemcpyAsync(logits_host, m->logits.get(), (size_t)m->vshard * 4, cudaMemcpyDeviceToHost, m->stream));
-    ZL_CHECK_CUDA(cudaStreamSynchronize(m->stream));
-    *next_token_host = m->h_stage.get()[3 * m->cfg.max_batch];
+    const int32_t* picks = nullptr;
+    RCHECK(read_picks(m, 1, logits_host, &picks));
+    *next_token_host = picks[0];
     if (pos0 + n > m->cur_max_len) m->cur_max_len = pos0 + n;
     return ZL_OK;
 }
@@ -1953,10 +2006,7 @@ extern "C" int zl_llama_step_joined(zl_llama_t* m, const int32_t* tokens_host, c
                                     int32_t* next_host, float* logits_host) {
     ZL_CHECK_ARG(m && tokens_host && seg_host && next_host && nseg > 0);
     const auto& c = m->cfg;
-    if (c.prefill_chunk <= 0) {
-        zl_set_last_error(__FILE__, __LINE__, "zl_llama_step_joined needs cfg.prefill_chunk > 0");
-        return ZL_ERR_STATE;
-    }
+    if (c.prefill_chunk <= 0) return fail_state(__LINE__, "zl_llama_step_joined needs cfg.prefill_chunk > 0");
     // zl_varlen_attention reads the activation-dtype cache of one rank
     if (c.kv_int8 || c.tp_size > 1)
         return fail_state(__LINE__, "joined steps are not available with an int8 KV cache or tensor parallelism",
@@ -1989,7 +2039,7 @@ extern "C" int zl_llama_step_joined(zl_llama_t* m, const int32_t* tokens_host, c
     sg.joined = true;
     sg.n = rows;
     sg.nseg = nseg;
-    bool sampler = false, ngram = false;
+    Pick pk;   // of the emitting tasks
     for (int s = 0, row0 = 0; s < nseg; ++s) {
         const int task = seg_host[4 * s], pos0 = seg_host[4 * s + 1], n = seg_host[4 * s + 2];
         for (int i = 0; i < n; ++i) {
@@ -2006,8 +2056,7 @@ extern "C" int zl_llama_step_joined(zl_llama_t* m, const int32_t* tokens_host, c
             h_etask[sg.n_emit] = task;
             h_epos[sg.n_emit] = pos0 + n - 1;
             ++sg.n_emit;
-            sampler |= m->samp_on[task] != 0;
-            ngram |= m->ngram_on[task] != 0;
+            pk.add(m, task);
         }
         if (pos0 + n > sg.max_keys) sg.max_keys = pos0 + n;
         row0 += n;
@@ -2017,16 +2066,10 @@ extern "C" int zl_llama_step_joined(zl_llama_t* m, const int32_t* tokens_host, c
     ZL_CHECK_CUDA(cudaMemcpyAsync(m->d_pf_pos.get(), h_pos, (size_t)rows * 4, cudaMemcpyHostToDevice, st));
     ZL_CHECK_CUDA(cudaMemcpyAsync(m->d_tb.get(), h_tb, (size_t)rows * 4, cudaMemcpyHostToDevice, st));
     ZL_CHECK_CUDA(cudaMemcpyAsync(m->d_join.get(), h_seg, (size_t)7 * MB * 4, cudaMemcpyHostToDevice, st));
-    RCHECK(enqueue_step(m, 0, 0, &sg, sampler, nullptr, ngram));
-    int32_t* h_next = m->h_stage.get() + 3 * MB;
-    if (sg.n_emit) {
-        ZL_CHECK_CUDA(cudaMemcpyAsync(h_next, m->d_next.get(), (size_t)sg.n_emit * 4, cudaMemcpyDeviceToHost, st));
-        if (logits_host)
-            ZL_CHECK_CUDA(cudaMemcpyAsync(logits_host, m->logits.get(), (size_t)sg.n_emit * m->vshard * 4,
-                                          cudaMemcpyDeviceToHost, st));
-    }
-    ZL_CHECK_CUDA(cudaStreamSynchronize(st));   // also frees the pinned staging for the next call
-    for (int s = 0, e = 0; s < nseg; ++s) next_host[s] = seg_host[4 * s + 3] ? h_next[e++] : -1;
+    RCHECK(enqueue_step(m, 0, 0, &sg, pk));
+    const int32_t* picks = nullptr;
+    RCHECK(read_picks(m, sg.n_emit, logits_host, &picks));   // also frees the pinned staging for the next call
+    for (int s = 0, e = 0; s < nseg; ++s) next_host[s] = seg_host[4 * s + 3] ? picks[e++] : -1;
     if (sg.max_keys > m->cur_max_len) m->cur_max_len = sg.max_keys;
     return ZL_OK;
 }
@@ -2037,10 +2080,7 @@ extern "C" int zl_llama_set_sampling(zl_llama_t* m, int task, const zl_sample_pa
     const bool on = p && ((p->temperature > 0.f && p->top_k != 1) || p->repetition_penalty != 1.f ||
                           p->presence_penalty != 0.f);
     ZL_CHECK_SUPPORTED(!on || m->cfg.tp_size == 1);
-    if (!m->finalized) {
-        zl_set_last_error(__FILE__, __LINE__, "model not finalized");
-        return ZL_ERR_STATE;
-    }
+    if (!m->finalized) return fail_state(__LINE__, "model not finalized");
     const zl_sample_params_t q = p ? *p : zl_sample_params_t{0.f, 1.f, 1.f, 0.f, 0, 0};
     // stream-ordered after every step already enqueued; the pageable source is staged before the call returns
     ZL_CHECK_CUDA(cudaMemcpyAsync(m->d_sparams.get() + task, &q, sizeof(q), cudaMemcpyHostToDevice, m->stream));
@@ -2126,6 +2166,28 @@ extern "C" int zl_llama_stats(zl_llama_t* m, int B, double* weight_bytes, int* k
 // Prompt prefix cache: the block pool and the block copies (PrefixCache, src/generator/prefix_cache.hpp:35-117).  Which
 // blocks to save and load is the caller's policy (zhilight_b200/prefix_cache.py); this owns the memory and the copies.
 // ------------------------------------------------------------------------------------------------------------------
+namespace {
+
+// layer L's task buffers: k, v, scale k, scale v (the scales are null without an int8 cache)
+std::array<void*, 4> kv_bases(const Layer& L) { return {L.kbuf.get(), L.vbuf.get(), L.skbuf.get(), L.svbuf.get()}; }
+
+// kv_tab, built by the first block pool or row copy
+int ensure_kv_tab(zl_llama* m) {
+    if (m->kv_tab) return ZL_OK;
+    std::vector<void*> h_tab;
+    for (const Layer& L : m->layers)
+        for (void* p : kv_bases(L)) h_tab.push_back(p);
+    dev_ptr<void*> tab;
+    RCHECK(dmalloc(&tab, sizeof(void*) * h_tab.size()));
+    ZL_CHECK_CUDA(cudaMemcpyAsync(tab.get(), h_tab.data(), sizeof(void*) * h_tab.size(), cudaMemcpyHostToDevice,
+                                  m->stream));
+    ZL_CHECK_CUDA(cudaStreamSynchronize(m->stream));   // h_tab is pageable and goes out of scope
+    m->kv_tab = std::move(tab);
+    return ZL_OK;
+}
+
+}  // namespace
+
 extern "C" int zl_llama_kv_pool_create(zl_llama_t* m, int num_blocks, int block_tokens) {
     ZL_CHECK_ARG(m && num_blocks > 0);
     ZL_CHECK_ARG(block_tokens == 16 || block_tokens == 32 || block_tokens == 64 || block_tokens == 128 ||
@@ -2142,32 +2204,12 @@ extern "C" int zl_llama_kv_pool_create(zl_llama_t* m, int num_blocks, int block_
     const size_t blk = (size_t)block_tokens * row_bytes, sblk = (size_t)block_tokens * srow_bytes;
     const int cap = num_blocks > c.max_seq / block_tokens ? num_blocks : c.max_seq / block_tokens;
     dev_ptr<> pool, scales;
-    dev_ptr<void*> tab;
-    dev_ptr<int32_t> dslots;
     RCHECK(dmalloc(&pool, (size_t)L * 2 * num_blocks * blk));
     if (c.kv_int8) RCHECK(dmalloc(&scales, (size_t)L * 2 * num_blocks * sblk));
-    std::vector<void*> h_tab((size_t)4 * L, nullptr);
-    for (int l = 0; l < L; ++l) {
-        const Layer& Ly = m->layers[l];
-        h_tab[4 * l] = Ly.kbuf.get();
-        h_tab[4 * l + 1] = Ly.vbuf.get();
-        h_tab[4 * l + 2] = Ly.skbuf.get();
-        h_tab[4 * l + 3] = Ly.svbuf.get();
-    }
-    RCHECK(dmalloc(&tab, sizeof(void*) * 4 * L));
-    ZL_CHECK_CUDA(cudaMemcpyAsync(tab.get(), h_tab.data(), sizeof(void*) * 4 * L, cudaMemcpyHostToDevice, m->stream));
-    RCHECK(dmalloc(&dslots, sizeof(int32_t) * zl_llama::kStageSlots * 2 * cap));
-    int32_t* hs = nullptr;
-    ZL_CHECK_CUDA(cudaMallocHost((void**)&hs, sizeof(int32_t) * zl_llama::kStageSlots * 2 * cap));
-    host_ptr<int32_t> hslots(hs);
-    for (int i = 0; i < zl_llama::kStageSlots; ++i)
-        if (!m->pool_ev[i]) ZL_CHECK_CUDA(cudaEventCreateWithFlags(&m->pool_ev[i], cudaEventDisableTiming));
-    ZL_CHECK_CUDA(cudaStreamSynchronize(m->stream));   // h_tab is pageable and goes out of scope
+    RCHECK(ensure_kv_tab(m));
+    RCHECK(m->pool_ring.alloc((size_t)2 * cap, true));
     m->pool = std::move(pool);
     m->pool_scales = std::move(scales);
-    m->pool_tab = std::move(tab);
-    m->pool_d = std::move(dslots);
-    m->pool_h = std::move(hslots);
     m->pool_blocks = num_blocks;
     m->pool_bt = block_tokens;
     m->pool_cap = cap;
@@ -2197,7 +2239,7 @@ int check_kv_blocks(zl_llama* m, int task, const int32_t* task_blocks, const int
 KvBlockCopyArgs kv_copy_args(zl_llama* m, int task, const int32_t* d_pairs, int n, bool to_pool) {
     const auto& c = m->cfg;
     KvBlockCopyArgs a{};
-    a.task_bases = m->pool_tab.get();
+    a.task_bases = m->kv_tab.get();
     a.pool = static_cast<char*>(m->pool.get());
     a.pool_scales = static_cast<char*>(m->pool_scales.get());
     a.pairs = d_pairs;
@@ -2213,31 +2255,23 @@ KvBlockCopyArgs kv_copy_args(zl_llama* m, int task, const int32_t* d_pairs, int 
     return a;
 }
 
-// stage the block lists in the next ring slot (waiting for the copy that last read it) -> its device copy
-int stage_kv_blocks(zl_llama* m, const int32_t* task_blocks, const int32_t* pool_blocks, int n, const int32_t** d_pairs,
-                    int* slot_out) {
-    const int slot = m->pool_next;
-    m->pool_next = (slot + 1) % zl_llama::kStageSlots;
-    if (m->pool_used[slot]) ZL_CHECK_CUDA(cudaEventSynchronize(m->pool_ev[slot]));
-    int32_t* hs = m->pool_h.get() + (size_t)slot * 2 * m->pool_cap;
-    int32_t* ds = m->pool_d.get() + (size_t)slot * 2 * m->pool_cap;
+// stage the block lists in the next pool_ring slot -> its device copy; release the slot after the kernel that reads it
+int stage_kv_blocks(zl_llama* m, const int32_t* task_blocks, const int32_t* pool_blocks, int n, const int32_t** d_pairs) {
+    int32_t *hs = nullptr, *ds = nullptr;
+    RCHECK(m->pool_ring.acquire(&hs, &ds));
     std::memcpy(hs, task_blocks, sizeof(int32_t) * n);
     std::memcpy(hs + n, pool_blocks, sizeof(int32_t) * n);
     ZL_CHECK_CUDA(cudaMemcpyAsync(ds, hs, sizeof(int32_t) * 2 * n, cudaMemcpyHostToDevice, m->stream));
     *d_pairs = ds;
-    *slot_out = slot;
     return ZL_OK;
 }
 
 int kv_blocks(zl_llama* m, int task, const int32_t* task_blocks, const int32_t* pool_blocks, int n, bool to_pool) {
     RCHECK(check_kv_blocks(m, task, task_blocks, pool_blocks, n, to_pool));
     const int32_t* d_pairs = nullptr;
-    int slot = 0;
-    RCHECK(stage_kv_blocks(m, task_blocks, pool_blocks, n, &d_pairs, &slot));
+    RCHECK(stage_kv_blocks(m, task_blocks, pool_blocks, n, &d_pairs));
     RCHECK(kv_block_copy(kv_copy_args(m, task, d_pairs, n, to_pool), m->stream));
-    ZL_CHECK_CUDA(cudaEventRecord(m->pool_ev[slot], m->stream));   // after the kernel that reads the device slot
-    m->pool_used[slot] = true;
-    return ZL_OK;
+    return m->pool_ring.release(m->stream);
 }
 
 }  // namespace
@@ -2261,15 +2295,13 @@ extern "C" int zl_llama_kv_blocks_bench(zl_llama_t* m, int task, const int32_t* 
     const KvBlockCopyArgs a0 = kv_copy_args(m, task, nullptr, 0, to_pool);
     const size_t blk = (size_t)a0.bt * a0.row_bytes, sblk = (size_t)a0.bt * a0.srow_bytes;
     const int32_t* d_pairs = nullptr;
-    int slot = 0;
-    RCHECK(stage_kv_blocks(m, task_blocks, pool_blocks, n, &d_pairs, &slot));
+    RCHECK(stage_kv_blocks(m, task_blocks, pool_blocks, n, &d_pairs));
     const KvBlockCopyArgs a = kv_copy_args(m, task, d_pairs, n, to_pool);
     auto one_pass = [&]() -> int {
         if (!per_range_memcpy) return kv_block_copy(a, m->stream);
         for (int i = 0; i < n; ++i)
             for (int l = 0; l < c.num_layers; ++l) {
-                const Layer& Ly = m->layers[l];
-                void* tbuf[4] = {Ly.kbuf.get(), Ly.vbuf.get(), Ly.skbuf.get(), Ly.svbuf.get()};
+                const auto tbuf = kv_bases(m->layers[l]);
                 for (int t = 0; t < (sblk ? 4 : 2); ++t) {
                     const bool sc = t >= 2;
                     const size_t rb = sc ? a.srow_bytes : a.row_bytes, bb = sc ? sblk : blk;
@@ -2288,8 +2320,7 @@ extern "C" int zl_llama_kv_blocks_bench(zl_llama_t* m, int task, const int32_t* 
     if (rc == ZL_OK) rc = cudaEventRecord(e0, m->stream) == cudaSuccess ? ZL_OK : ZL_ERR_CUDA;
     for (int it = 0; it < iters && rc == ZL_OK; ++it) rc = one_pass();
     if (rc == ZL_OK) rc = cudaEventRecord(e1, m->stream) == cudaSuccess ? ZL_OK : ZL_ERR_CUDA;
-    if (rc == ZL_OK) rc = cudaEventRecord(m->pool_ev[slot], m->stream) == cudaSuccess ? ZL_OK : ZL_ERR_CUDA;
-    m->pool_used[slot] = true;
+    if (rc == ZL_OK) rc = m->pool_ring.release(m->stream);   // after the last pass that reads the device slot
     if (rc == ZL_OK) rc = cudaEventSynchronize(e1) == cudaSuccess ? ZL_OK : ZL_ERR_CUDA;
     if (rc == ZL_OK) rc = cudaEventElapsedTime(ms, e0, e1) == cudaSuccess ? ZL_OK : ZL_ERR_CUDA;
     cudaEventDestroy(e0);
@@ -2328,34 +2359,6 @@ int ensure_beam(zl_llama* m) {
     return ZL_OK;
 }
 
-int ensure_row_copies(zl_llama* m) {
-    if (m->rows_tab) return ZL_OK;
-    const int L = m->cfg.num_layers, MB = m->cfg.max_batch;
-    std::vector<void*> h_tab((size_t)4 * L, nullptr);
-    for (int l = 0; l < L; ++l) {
-        const Layer& Ly = m->layers[l];
-        h_tab[4 * l] = Ly.kbuf.get();
-        h_tab[4 * l + 1] = Ly.vbuf.get();
-        h_tab[4 * l + 2] = Ly.skbuf.get();
-        h_tab[4 * l + 3] = Ly.svbuf.get();
-    }
-    dev_ptr<void*> tab;
-    dev_ptr<int32_t> dslots;
-    RCHECK(dmalloc(&tab, sizeof(void*) * 4 * L));
-    RCHECK(dmalloc(&dslots, sizeof(int32_t) * zl_llama::kStageSlots * 4 * MB));
-    int32_t* hs = nullptr;
-    ZL_CHECK_CUDA(cudaMallocHost((void**)&hs, sizeof(int32_t) * zl_llama::kStageSlots * 4 * MB));
-    host_ptr<int32_t> hslots(hs);
-    for (int i = 0; i < zl_llama::kStageSlots; ++i)
-        if (!m->rows_ev[i]) ZL_CHECK_CUDA(cudaEventCreateWithFlags(&m->rows_ev[i], cudaEventDisableTiming));
-    ZL_CHECK_CUDA(cudaMemcpyAsync(tab.get(), h_tab.data(), sizeof(void*) * 4 * L, cudaMemcpyHostToDevice, m->stream));
-    ZL_CHECK_CUDA(cudaStreamSynchronize(m->stream));   // h_tab is pageable and goes out of scope
-    m->rows_tab = std::move(tab);
-    m->rows_d = std::move(dslots);
-    m->rows_h = std::move(hslots);
-    return ZL_OK;
-}
-
 }  // namespace
 
 extern "C" int zl_llama_beam_step(zl_llama_t* m, const int32_t* tokens, const int32_t* positions, int B,
@@ -2369,7 +2372,8 @@ extern "C" int zl_llama_beam_step(zl_llama_t* m, const int32_t* tokens, const in
         return fail_state(__LINE__, "beam steps need the whole vocabulary on one rank (tp_size 1)", ZL_ERR_UNSUPPORTED);
     ZL_CHECK_SUPPORTED(B < 2048);   // the graph key holds B and G in 11 bits
     if (!m->finalized) return fail_state(__LINE__, "model not finalized");
-    if (sampler_on(m, 0, B)) return fail_state(__LINE__, "a task of the beam step samples, has penalties or has logits processors");
+    if (pick_of(m, 0, B).sampler)
+        return fail_state(__LINE__, "a task of the beam step samples, has penalties or has logits processors");
     RCHECK(ensure_beam(m));
     const int MB = m->cfg.max_batch;
     int32_t* d = static_cast<int32_t*>(m->beam_d.get());
@@ -2427,16 +2431,14 @@ extern "C" int zl_llama_kv_copy_rows(zl_llama_t* m, const int32_t* ranges_host, 
     const int row_bytes = m->hkv * c.dim_head * (c.kv_int8 ? 1 : 2);
     if (row_bytes % 16 != 0)
         return fail_state(__LINE__, "KV row copies need 16-byte cached rows (H_kv * dim_head)", ZL_ERR_UNSUPPORTED);
-    RCHECK(ensure_row_copies(m));
-    const int slot = m->rows_next;
-    m->rows_next = (slot + 1) % zl_llama::kStageSlots;
-    if (m->rows_used[slot]) ZL_CHECK_CUDA(cudaEventSynchronize(m->rows_ev[slot]));   // its previous copy has executed
-    int32_t* hs = m->rows_h.get() + (size_t)slot * 4 * c.max_batch;
-    int32_t* ds = m->rows_d.get() + (size_t)slot * 4 * c.max_batch;
+    RCHECK(ensure_kv_tab(m));
+    if (!m->rows_ring.h) RCHECK(m->rows_ring.alloc((size_t)4 * c.max_batch, true));
+    int32_t *hs = nullptr, *ds = nullptr;
+    RCHECK(m->rows_ring.acquire(&hs, &ds));
     std::memcpy(hs, ranges_host, sizeof(int32_t) * 4 * n);
     ZL_CHECK_CUDA(cudaMemcpyAsync(ds, hs, sizeof(int32_t) * 4 * n, cudaMemcpyHostToDevice, m->stream));
     KvRowCopyArgs a{};
-    a.task_bases = m->rows_tab.get();
+    a.task_bases = m->kv_tab.get();
     a.ranges = ds;
     a.n = n;
     a.layers = c.num_layers;
@@ -2445,9 +2447,7 @@ extern "C" int zl_llama_kv_copy_rows(zl_llama_t* m, const int32_t* ranges_host, 
     a.row_bytes = row_bytes;
     a.srow_bytes = c.kv_int8 ? m->hkv * 4 : 0;
     RCHECK(kv_row_copy(a, m->stream));
-    ZL_CHECK_CUDA(cudaEventRecord(m->rows_ev[slot], m->stream));   // after the kernel that reads the device slot
-    m->rows_used[slot] = true;
-    return ZL_OK;
+    return m->rows_ring.release(m->stream);
 }
 
 // ------------------------------------------------------------------------------------------------------------------
@@ -2563,15 +2563,15 @@ __global__ void k_gen_tail(GenState g, int32_t* __restrict__ tokens, int32_t* __
         }
 }
 
-// The loop graph of (B, sampler, n-gram launch, bucket).  The body keeps the step's programmatic dependent launches.
-int build_gen_graph(zl_llama* m, int B, bool sampler, bool ngram, int bucket, cudaGraphExec_t* out) {
+// The loop graph of (B, pick, bucket) into *out, which the caller owns also when this fails.  The body keeps the step's
+// programmatic dependent launches.
+int build_gen_graph(zl_llama* m, int B, const Pick& pk, int bucket, cudaGraph_t* out) {
     GenState gs = gen_state(m);
     int32_t* tokens = m->d_tokens.get();
     int32_t* pos = m->d_pos.get();
     const int32_t* next = m->d_next.get();
-    cudaGraph_t g = nullptr;
-    ZL_CHECK_CUDA(cudaGraphCreate(&g, 0));
-    std::unique_ptr<CUgraph_st, cudaError_t (*)(cudaGraph_t)> own(g, cudaGraphDestroy);
+    ZL_CHECK_CUDA(cudaGraphCreate(out, 0));
+    cudaGraph_t g = *out;
     cudaGraphConditionalHandle h;
     ZL_CHECK_CUDA(cudaGraphConditionalHandleCreate(&h, g, 0, 0));
     cudaKernelNodeParams kp = {};
@@ -2591,9 +2591,9 @@ int build_gen_graph(zl_llama* m, int B, bool sampler, bool ngram, int bucket, cu
     cudaGraph_t body = cp.conditional.phGraph_out[0];
     // the body: the unchanged decode step, then k_gen_advance in k_advance's place
     ZL_CHECK_CUDA(cudaStreamBeginCaptureToGraph(m->stream, body, nullptr, nullptr, 0, cudaStreamCaptureModeThreadLocal));
-    m->pick_frozen = gs.fin;
-    int rc = enqueue_step(m, B, bucket, nullptr, sampler, nullptr, ngram);
-    m->pick_frozen = nullptr;
+    Pick body_pick = pk;
+    body_pick.frozen = gs.fin;   // the sampler records no pick of a finished task
+    int rc = enqueue_step(m, B, bucket, nullptr, body_pick);
     if (rc == ZL_OK) {
         k_gen_advance<<<1, kGenThreads, 0, m->stream>>>(gs, tokens, pos, next, B, h);
         if (cudaGetLastError() != cudaSuccess) rc = fail_state(__LINE__, "k_gen_advance launch failed", ZL_ERR_CUDA);
@@ -2605,21 +2605,6 @@ int build_gen_graph(zl_llama* m, int B, bool sampler, bool ngram, int bucket, cu
     kp.func = (void*)k_gen_tail;
     kp.kernelParams = tail_args;
     ZL_CHECK_CUDA(cudaGraphAddKernelNode(&tail, g, &loop, 1, &kp));
-    ZL_CHECK_CUDA(cudaGraphInstantiate(out, g, 0));
-    return ZL_OK;
-}
-
-int gen_graph(zl_llama* m, int B, bool sampler, bool ngram, int bucket, cudaGraphExec_t* out) {
-    const long long key = ((long long)B << 33) | ((long long)sampler << 32) | ((long long)ngram << 31) | (unsigned)bucket;
-    auto it = m->gen_graphs.find(key);
-    if (it != m->gen_graphs.end()) {
-        *out = it->second;
-        return ZL_OK;
-    }
-    cudaGraphExec_t exec = nullptr;
-    RCHECK(build_gen_graph(m, B, sampler, ngram, bucket, &exec));
-    m->gen_graphs.emplace(key, exec);
-    *out = exec;
     return ZL_OK;
 }
 
@@ -2666,7 +2651,7 @@ extern "C" int zl_llama_generate(zl_llama_t* m, int B, int max_steps, int32_t* t
         *steps_host = 0;
         return ZL_OK;
     }
-    const bool sampler = sampler_on(m, 0, B), ngram = ngram_on(m, 0, B);
+    const Pick pk = pick_of(m, 0, B);
     const GenState gs = gen_state(m);
     // attention lengths at step s are at most min(L0 + s, max_seq): one launch per length bucket crossed
     const int L0 = m->cur_max_len;
@@ -2676,7 +2661,9 @@ extern "C" int zl_llama_generate(zl_llama_t* m, int B, int max_steps, int32_t* t
         int n = max_steps - s;
         if (bucket < c.max_seq) n = std::min(n, bucket - (L0 + s) + 1);
         cudaGraphExec_t exec = nullptr;
-        RCHECK(gen_graph(m, B, sampler, ngram, bucket, &exec));
+        RCHECK(m->gen_graphs.get(
+            graph_key(B, pk, bucket),
+            [&](cudaGraph_t* g) { return build_gen_graph(m, B, pk, bucket, g); }, &exec));
         k_gen_begin<<<1, 1, 0, m->stream>>>(gs, s == 0, n);
         ZL_CHECK_LAUNCH();
         ZL_CHECK_CUDA(cudaGraphLaunch(exec, m->stream));

@@ -53,30 +53,36 @@ struct Staged {
     int rows = 0, cols = 0, elem = 0;
 };
 
-struct W4Lin {
-    dev_ptr<> packed;     // ZLW4  (fp16 HMMA kernels) -- only kept when some batch size needs it
+// The weight format of a Linear.  lin_format: that of every Linear of a model, by quant_type -- W4A16 GPTQ / AWQ (5, 6;
+// 8 is served as 5), dense (0), or W8A8 with int8 rows (2), fp8 rows (7) or fp8 128x128 blocks (10).
+enum LinFormat { kW4, kDense, kInt8, kFp8Rows, kFp8Block };
+LinFormat lin_format(const zl_llama_config_t& c) {
+    switch (c.quant_type) {
+        case 5: case 6: return kW4;
+        case 2: return kInt8;
+        case 7: return kFp8Rows;
+        case 10: return kFp8Block;
+        default: return kDense;
+    }
+}
+
+struct Lin {
+    LinFormat fmt = kDense;
+    int N = 0, K = 0;
+    dev_ptr<> bias;
+    dev_ptr<> packed;     // W4: ZLW4  (fp16 HMMA kernels) -- only kept when some batch size needs it
     dev_ptr<> packed_i;   // ZLW4I (exact-integer IMMA kernel, small M)
-    dev_ptr<> bias;
-    int N = 0, K = 0;
     dev_ptr<int32_t> k_perm;   // act-order: the GEMM reads x[:, k_perm] (K int32); empty: sequential g_idx
-};
-struct DenseLin {
+    // dense and W8A8: the (N, K) weight, in the activation dtype or as 8-bit codes
     dev_ptr<> w;
-    dev_ptr<> bias;
-    int N = 0, K = 0;
-    // W8A8 (quant_type 2 / 7 / 10): 8-bit weights (N, K) + scales; w is released
-    dev_ptr<> w8;
     dev_ptr<> w_scale;   // int8: (N) in the activation dtype (linear.cpp:541); fp8: (N) f32 rows;
                          // fp8 block: (N/128, K/128) f32 weight_scale_inv
-    int w8_kind = -1;    // ZL_W8_INT8, ZL_W8_FP8_ROWS or kW8Block
 };
-constexpr int kW8Block = 10;   // QuantType 10 (Fp8Block): served by zl_fp8_block_gemm, not a zl_w8a8_gemm kind
 
 struct Layer {
     dev_ptr<> ln_attn;
     dev_ptr<> ln_ff;
-    W4Lin q_qkv, q_o, q_gu, q_down;
-    DenseLin d_qkv, d_o, d_gu, d_down;
+    Lin qkv, o, gu, down;
     dev_ptr<> kbuf;   // (max_batch, max_seq, Hkv, d): activation dtype, or uint8 codes at kv_int8
     dev_ptr<> vbuf;
     dev_ptr<void*> k_addrs;   // (max_batch)
@@ -492,7 +498,7 @@ int to_k_major(zl_llama* m, const std::string& prefix, int K, int N, uint32_t* q
 }
 
 // The kernel that serves a W4 Linear at B rows: 3 exact-integer, 4 wgmma, 0 fp16 mma.sync.
-int route_of(const W4Lin& w, int B) { return w.packed_i ? zl_w4_int_layout_route(B, w.N, w.K) : 0; }
+int route_of(const Lin& w, int B) { return w.packed_i ? zl_w4_int_layout_route(B, w.N, w.K) : 0; }
 
 // The (N) fp16 bias of Linears fused along N: zeros, with each present `prefix.bias` at its row offset.  *out stays
 // empty when none has one.  Every staged bias is checked before the first copy.
@@ -523,7 +529,7 @@ int build_bias(zl_llama* m, const std::vector<std::string>& prefixes, const std:
 // out_rows (swiglu only, act-order w_out): w_out's permutation, folded into the gate / up row order.
 // keep_perm = false: the weight rows are sequentialised but the GEMM runs without k_perm (its producer wrote x permuted).
 int build_w4(zl_llama* m, const std::vector<std::string>& prefixes, const std::vector<int>& ns, int K, bool swiglu,
-             W4Lin* out, bool qkv_rope = false, const std::vector<int32_t>* out_rows = nullptr, bool keep_perm = true) {
+             Lin* out, bool qkv_rope = false, const std::vector<int32_t>* out_rows = nullptr, bool keep_perm = true) {
     const int N = std::accumulate(ns.begin(), ns.end(), 0);
     const int G = K / m->cfg.group_size;
     // act-order: Linears fused along N share their input, so they must share its permutation.  Real checkpoints give
@@ -606,6 +612,7 @@ int build_w4(zl_llama* m, const std::vector<std::string>& prefixes, const std::v
     }
     ZL_CHECK_CUDA(cudaStreamSynchronize(m->stream));
     drop_parts(m, prefixes, {".qweight", ".qzeros", ".scales", ".g_idx", ".bias"});
+    out->fmt = kW4;
     out->N = N;
     out->K = K;
     m->weight_bytes += (double)pbytes;
@@ -639,14 +646,14 @@ int fuse_parts(zl_llama* m, const std::vector<std::string>& prefixes, const std:
     return ZL_OK;
 }
 
-int build_dense(zl_llama* m, const std::vector<std::string>& prefixes, const std::vector<int>& ns, int K,
-                DenseLin* out) {
+int build_dense(zl_llama* m, const std::vector<std::string>& prefixes, const std::vector<int>& ns, int K, Lin* out) {
     const int N = std::accumulate(ns.begin(), ns.end(), 0);
     RCHECK(dmalloc(&out->w, (size_t)N * K * 2));
     RCHECK(fuse_parts(m, prefixes, ns, K, 2, out->w.get(), "dense weight"));
     RCHECK(build_bias(m, prefixes, ns, &out->bias));
     ZL_CHECK_CUDA(cudaStreamSynchronize(m->stream));
     drop_parts(m, prefixes, {".weight", ".bias"});
+    out->fmt = kDense;
     out->N = N;
     out->K = K;
     m->weight_bytes += (double)N * K * 2;
@@ -655,13 +662,14 @@ int build_dense(zl_llama* m, const std::vector<std::string>& prefixes, const std
 
 // quant_type 2 (AutoInt8, linear.cpp:521-550): the fp weight is quantised per output row at load with the same kernel
 // as the activations; the scale is kept in the activation dtype (functions::typecast, linear.cpp:541).
-int dense_to_int8(zl_llama* m, DenseLin* d) {
+int dense_to_int8(zl_llama* m, Lin* d) {
     const auto& c = m->cfg;
+    dev_ptr<> w8;
     dev_ptr<float> sf;
-    RCHECK(dmalloc(&d->w8, (size_t)d->N * d->K));
+    RCHECK(dmalloc(&w8, (size_t)d->N * d->K));
     RCHECK(dmalloc(&sf, (size_t)d->N * 4));
     RCHECK(dmalloc(&d->w_scale, (size_t)d->N * 2));
-    RCHECK(zl_int8_quant_per_token(d->w.get(), d->K, d->w8.get(), sf.get(), d->N, d->K, c.dtype, 0, m->stream));
+    RCHECK(zl_int8_quant_per_token(d->w.get(), d->K, w8.get(), sf.get(), d->N, d->K, c.dtype, 0, m->stream));
     if (c.dtype == ZL_F16)
         k_f32_to_t<__half><<<cdiv(d->N, 256), 256, 0, m->stream>>>(sf.get(), static_cast<__half*>(d->w_scale.get()), d->N);
     else
@@ -669,17 +677,17 @@ int dense_to_int8(zl_llama* m, DenseLin* d) {
             sf.get(), static_cast<__nv_bfloat16*>(d->w_scale.get()), d->N);
     ZL_CHECK_LAUNCH();
     ZL_CHECK_CUDA(cudaStreamSynchronize(m->stream));
-    d->w.reset();
-    d->w8_kind = ZL_W8_INT8;
+    d->w = std::move(w8);
+    d->fmt = kInt8;
     m->weight_bytes += (double)d->N * d->K + (double)d->N * 2 - (double)d->N * d->K * 2;
     return ZL_OK;
 }
 
 // quant_type 7 (Fp8Linear, linear.cpp:1612-1695): e4m3 weights + one f32 weight_scale per Linear.  Projections that
 // share an input are fused along N with their scalar scales expanded to one scale per output row.
-int build_fp8(zl_llama* m, const std::vector<std::string>& prefixes, const std::vector<int>& ns, int K, DenseLin* out) {
+int build_fp8(zl_llama* m, const std::vector<std::string>& prefixes, const std::vector<int>& ns, int K, Lin* out) {
     const int N = std::accumulate(ns.begin(), ns.end(), 0);
-    RCHECK(dmalloc(&out->w8, (size_t)N * K));
+    RCHECK(dmalloc(&out->w, (size_t)N * K));
     RCHECK(dmalloc(&out->w_scale, (size_t)N * 4));
     float* w_scale = static_cast<float*>(out->w_scale.get());
     const PartScale expand{".weight_scale", nullptr, [&](size_t i, int off, const Staged& ws) -> int {
@@ -688,13 +696,13 @@ int build_fp8(zl_llama* m, const std::vector<std::string>& prefixes, const std::
                                ZL_CHECK_LAUNCH();
                                return ZL_OK;
                            }};
-    RCHECK(fuse_parts(m, prefixes, ns, K, 1, out->w8.get(), "fp8 weight or weight_scale", &expand));
+    RCHECK(fuse_parts(m, prefixes, ns, K, 1, out->w.get(), "fp8 weight or weight_scale", &expand));
     RCHECK(build_bias(m, prefixes, ns, &out->bias));
     ZL_CHECK_CUDA(cudaStreamSynchronize(m->stream));
     drop_parts(m, prefixes, {".weight", ".weight_scale", ".bias"});
     out->N = N;
     out->K = K;
-    out->w8_kind = ZL_W8_FP8_ROWS;
+    out->fmt = kFp8Rows;
     m->weight_bytes += (double)N * K + (double)N * 4;
     return ZL_OK;
 }
@@ -703,7 +711,7 @@ int build_fp8(zl_llama* m, const std::vector<std::string>& prefixes, const std::
 // Projections that share an input are fused along N by concatenating both their weight rows and their scale rows,
 // which needs every part's N to be a multiple of 128.  Fp8Block has no bias (set_has_bias throws).
 int build_fp8_block(zl_llama* m, const std::vector<std::string>& prefixes, const std::vector<int>& ns, int K,
-                    DenseLin* out) {
+                    Lin* out) {
     const int N = std::accumulate(ns.begin(), ns.end(), 0);
     if (K % 128 != 0 || (prefixes.size() > 1 && N % 128 != 0))
         return fail_state(__LINE__, "fp8 block weights need K % 128 == 0 and every fused part's N % 128 == 0",
@@ -717,7 +725,7 @@ int build_fp8_block(zl_llama* m, const std::vector<std::string>& prefixes, const
                               ZL_ERR_UNSUPPORTED);
     }
     const int KB = K / 128, NB = (N + 127) / 128;
-    RCHECK(dmalloc(&out->w8, (size_t)N * K));
+    RCHECK(dmalloc(&out->w, (size_t)N * K));
     RCHECK(dmalloc(&out->w_scale, (size_t)NB * KB * 4));
     char* w_scale = static_cast<char*>(out->w_scale.get());
     const PartScale scale_rows{".weight_scale_inv",
@@ -728,12 +736,12 @@ int build_fp8_block(zl_llama* m, const std::vector<std::string>& prefixes, const
                                                                  m->stream));
                                    return ZL_OK;
                                }};
-    RCHECK(fuse_parts(m, prefixes, ns, K, 1, out->w8.get(), "fp8 block weight or weight_scale_inv", &scale_rows));
+    RCHECK(fuse_parts(m, prefixes, ns, K, 1, out->w.get(), "fp8 block weight or weight_scale_inv", &scale_rows));
     ZL_CHECK_CUDA(cudaStreamSynchronize(m->stream));
     drop_parts(m, prefixes, {".weight", ".weight_scale_inv"});
     out->N = N;
     out->K = K;
-    out->w8_kind = kW8Block;
+    out->fmt = kFp8Block;
     m->weight_bytes += (double)N * K + (double)NB * KB * 4;
     return ZL_OK;
 }
@@ -756,42 +764,42 @@ int finalize_layer(zl_llama* m, int l) {
     RCHECK(take_vector(m, p + "ln_attn.weight", D, &L.ln_attn));
     RCHECK(take_vector(m, p + "ln_ff.weight", D, &L.ln_ff));
     // the layer's Linears in build order, each fused along N from parts that share its input
-    struct Lin {
+    struct Spec {
         std::vector<std::string> prefixes;
         std::vector<int> ns;
         int K;
-        W4Lin* q;
-        DenseLin* d;
+        Lin* out;
     };
-    const Lin lins[] = {
+    const Spec lins[] = {
         {{p + "attn.project_q", p + "attn.project_k", p + "attn.project_v"}, {m->hq * d, m->hkv * d, m->hkv * d}, D,
-         &L.q_qkv, &L.d_qkv},
-        {{p + "attn.attn_out"}, {D}, m->hq * d, &L.q_o, &L.d_o},
-        {{p + "ff.w_in", p + "ff.w_gated"}, {m->ff, m->ff}, D, &L.q_gu, &L.d_gu},
-        {{p + "ff.w_out"}, {D}, m->ff, &L.q_down, &L.d_down},
+         &L.qkv},
+        {{p + "attn.attn_out"}, {D}, m->hq * d, &L.o},
+        {{p + "ff.w_in", p + "ff.w_gated"}, {m->ff, m->ff}, D, &L.gu},
+        {{p + "ff.w_out"}, {D}, m->ff, &L.down},
     };
-    const Lin &qkv = lins[0], &gu = lins[2], &down = lins[3];
-    if (c.quant_type == 5 || c.quant_type == 6) {
+    const Spec &qkv = lins[0], &gu = lins[2], &down = lins[3];
+    const LinFormat fmt = lin_format(c);
+    if (fmt == kW4) {
         // act-order w_out: its permutation orders the gate / up rows, so down runs without one.  A bad w_out g_idx is
         // reported by its own build_w4 below, after the errors of the Linears built before it.
         std::vector<int32_t> down_perm;
         if (g_idx_perm(m, down.prefixes[0], m->ff, &down_perm) != ZL_OK) down_perm.clear();
-        for (const Lin& f : lins) {
+        for (const Spec& f : lins) {
             const bool swiglu = &f == &gu;
-            RCHECK(build_w4(m, f.prefixes, f.ns, f.K, swiglu, f.q, &f == &qkv && c.fuse >= 2,
+            RCHECK(build_w4(m, f.prefixes, f.ns, f.K, swiglu, f.out, &f == &qkv && c.fuse >= 2,
                             swiglu ? &down_perm : nullptr, &f != &down));
         }
     } else {
-        for (const Lin& f : lins) {
-            if (c.quant_type == 7)
-                RCHECK(build_fp8(m, f.prefixes, f.ns, f.K, f.d));
-            else if (c.quant_type == 10)
-                RCHECK(build_fp8_block(m, f.prefixes, f.ns, f.K, f.d));
+        for (const Spec& f : lins) {
+            if (fmt == kFp8Rows)
+                RCHECK(build_fp8(m, f.prefixes, f.ns, f.K, f.out));
+            else if (fmt == kFp8Block)
+                RCHECK(build_fp8_block(m, f.prefixes, f.ns, f.K, f.out));
             else
-                RCHECK(build_dense(m, f.prefixes, f.ns, f.K, f.d));
+                RCHECK(build_dense(m, f.prefixes, f.ns, f.K, f.out));
         }
-        if (c.quant_type == 2)
-            for (const Lin& f : lins) RCHECK(dense_to_int8(m, f.d));
+        if (fmt == kInt8)
+            for (const Spec& f : lins) RCHECK(dense_to_int8(m, f.out));
     }
     return ZL_OK;
 }
@@ -911,7 +919,7 @@ int alloc_runtime(zl_llama* m) {
     RCHECK(dmalloc(&m->gu, (size_t)T * 2 * m->ff * 2));
     RCHECK(dmalloc(&m->act, (size_t)T * m->ff * 2));
     bool act_order = false;
-    for (const auto& L : m->layers) act_order |= L.q_qkv.k_perm || L.q_o.k_perm || L.q_gu.k_perm;
+    for (const auto& L : m->layers) act_order |= L.qkv.k_perm || L.o.k_perm || L.gu.k_perm;
     if (act_order) RCHECK(dmalloc(&m->xperm, (size_t)T * (D > m->hq * d ? D : m->hq * d) * 2));
     RCHECK(dmalloc(&m->logits, (size_t)B * c.vocab_size * 4));
     RCHECK(dmalloc(&m->cand, (size_t)((B * 8 + 15) / 16) * 16));
@@ -921,12 +929,13 @@ int alloc_runtime(zl_llama* m) {
     RCHECK(dmalloc(&m->d_tokens, B * 4));
     RCHECK(dmalloc(&m->d_pos, B * 4));
     RCHECK(dmalloc(&m->d_lens, B * 4));
-    if (c.quant_type == 2 || c.quant_type == 7 || c.quant_type == 10) {
+    const LinFormat fmt = lin_format(c);
+    if (fmt != kW4 && fmt != kDense) {   // W8A8
         int kmax = D > m->ff ? D : m->ff;
         kmax = kmax > m->hq * d ? kmax : m->hq * d;
         RCHECK(dmalloc(&m->xq, (size_t)T * kmax));
         // fp8 block: one scale per (token, 128 columns), column-major with leading dimension round_up(tokens, 4)
-        RCHECK(dmalloc(&m->xs, c.quant_type == 10 ? (size_t)(kmax / 128 + 1) * ((T + 3) / 4 * 4) * 4 : (size_t)T * 4));
+        RCHECK(dmalloc(&m->xs, fmt == kFp8Block ? (size_t)(kmax / 128 + 1) * ((T + 3) / 4 * 4) * 4 : (size_t)T * 4));
     }
     if (c.prefill_chunk > 0) {
         RCHECK(dmalloc(&m->d_tb, T * 4));
@@ -1029,15 +1038,15 @@ static int stage_pdl(const zl_llama* m, Stage s) {
 // the successor of W4 GEMM stage s of layer l in the decode chain -- qkv -> o -> gate_up -> down -> next layer's qkv -- and
 // its tensor-parallel mode given this GEMM's (the fused exchange alternates push / reduce-in; the last layer's down keeps
 // the stand-alone all-reduce).  The lm_head boundary is left out.
-static const W4Lin* w4_successor(zl_llama* m, int l, Stage s, int tp_mode, int* succ_tp) {
+static const Lin* w4_successor(zl_llama* m, int l, Stage s, int tp_mode, int* succ_tp) {
     Layer& L = m->layers[l];
     const bool last = l + 1 >= m->cfg.num_layers;
     *succ_tp = 0;
     switch (s) {
-        case kQkv: *succ_tp = tp_mode ? 2 : 0; return &L.q_o;
-        case kO: *succ_tp = tp_mode ? 1 : 0; return &L.q_gu;
-        case kGateUp: *succ_tp = tp_mode && !last ? 2 : 0; return &L.q_down;
-        case kDown: *succ_tp = tp_mode ? 1 : 0; return last ? nullptr : &m->layers[l + 1].q_qkv;
+        case kQkv: *succ_tp = tp_mode ? 2 : 0; return &L.o;
+        case kO: *succ_tp = tp_mode ? 1 : 0; return &L.gu;
+        case kGateUp: *succ_tp = tp_mode && !last ? 2 : 0; return &L.down;
+        case kDown: *succ_tp = tp_mode ? 1 : 0; return last ? nullptr : &m->layers[l + 1].qkv;
         default: return nullptr;
     }
 }
@@ -1048,6 +1057,7 @@ void* rows(const void* base, int row, int width) { return (char*)base + (size_t)
 // One launch sequence of the layer GEMMs -- a decode step, one half of a dual-stream prefill chunk, or
 // zl_llama_bench_gemms -- and the residual stream it updates.
 struct Chain {
+    // where a W4 o / down GEMM's output goes (dense and W8A8 ones write pend, all-reduced in place at kAllReduce)
     enum Sink {
         kAddResidual,   // o / down add their output to the residual stream in the epilogue
         kPartial,       // o / down write partial sums to pend; the caller reduces them (dual-stream prefill)
@@ -1062,7 +1072,7 @@ struct Chain {
     Sink sink = kAddResidual;
     bool no_pdl = false;       // full dependencies and no L2 head: the next launch is not the chain successor (dual stream)
     bool gemm_only = false;    // launch only what the GEMMs of this fuse level comprise: no stand-alone RMSNorm (fuse 0)
-                               // or RoPE / KV append (fuse < 2)
+                               // or RoPE / KV append (fuse < 2); dense and W8A8: the GEMM and its activation quant
     void* h = nullptr;         // current residual stream
     // Fused tensor-parallel exchange (decode-sized W4 steps): the row-parallel GEMMs (o, down but the last layer's) push
     // their fp16 partial tiles into every rank's inbox from the epilogue; the next GEMM (gate_up, next layer's qkv)
@@ -1093,7 +1103,7 @@ struct Chain {
 // One W4 GEMM of stage s of layer l.  The caller sets a's activation, output, epilogue, RoPE and exchange fields; this adds
 // the weights, the RMSNorm ln_w (fused into the GEMM or as its own kernel), the act-order gather, the PDL flag and the L2
 // head of the successor.
-int w4_gemm(zl_llama* m, int l, Stage s, const Chain& ch, const W4Lin& w, const void* ln_w, zl_w4_fused_args_t a) {
+int w4_gemm(zl_llama* m, int l, Stage s, const Chain& ch, const Lin& w, const void* ln_w, zl_w4_fused_args_t a) {
     const auto& c = m->cfg;
     const int route = route_of(w, ch.n);
     a.packed = route ? w.packed_i.get() : w.packed.get();
@@ -1120,7 +1130,7 @@ int w4_gemm(zl_llama* m, int l, Stage s, const Chain& ch, const W4Lin& w, const 
     W4L2Head l2;
     if (!ch.no_pdl && route == 3 && (l2_head_depth() > 0 || l2_whole_max() > 0)) {
         int succ_tp = 0;
-        const W4Lin* nx = w4_successor(m, l, s, a.tp_mode, &succ_tp);
+        const Lin* nx = w4_successor(m, l, s, a.tp_mode, &succ_tp);
         if (nx && route_of(*nx, ch.n) == 3)
             w4_v3_l2_head(nx->packed_i.get(), ch.n, nx->N, nx->K, succ_tp, device_sm_count(), l2_head_depth(),
                           l2_whole_max(), &l2);
@@ -1162,9 +1172,43 @@ int kv8_rope_append(zl_llama* m, int l, const Chain& ch, const void* qkv, void* 
     return kv8_append(m, l, ch, pdl);
 }
 
-// qkv: RMSNorm + GEMM; at fuse >= 2 the epilogue splits q / k / v, applies RoPE and appends K / V, otherwise
-// zl_qkv_rope_append does.  int8 KV cache: the epilogue appends to the staging rows instead (fuse >= 2) or
-// zl_rope_qk_cache writes them (fuse < 2), and kv8_append quantises them into the cache.
+// One dense or W8A8 Linear: dense (NormalLinear), or W8A8 = activation quant + fused 8-bit GEMM (Int8Linear::forward /
+// Fp8Linear::forward in two launches instead of three)
+int dense_or_w8(zl_llama* m, const void* x, const Lin& L, void* y, int B, int pdl) {
+    const auto& c = m->cfg;
+    cudaStream_t st = m->stream;
+    if (L.fmt == kDense) return zl_dense_gemm_skinny(x, L.K, L.w.get(), L.bias.get(), y, B, L.N, L.K, c.dtype, c.dtype, pdl, st);
+    if (L.fmt == kInt8) {
+        RCHECK(zl_int8_quant_per_token(x, L.K, m->xq.get(), m->xs.get(), B, L.K, c.dtype, pdl, st));
+        return zl_w8a8_gemm(m->xq.get(), m->xs.get(), L.w.get(), L.w_scale.get(), c.dtype, L.bias.get(), y, B, L.N, L.K,
+                            ZL_W8_INT8, c.dtype, pdl, st);
+    }
+    if (L.fmt == kFp8Block) {   // Fp8Block::forward: per_token_cast_to_fp8 + the block-scaled GEMM
+        const int ld = (B + 3) / 4 * 4;
+        RCHECK(zl_fp8_quant_per_token_group(x, L.K, m->xq.get(), m->xs.get(), ld, B, L.K, c.dtype, pdl, st));
+        return zl_fp8_block_gemm(m->xq.get(), m->xs.get(), ld, L.w.get(), static_cast<const float*>(L.w_scale.get()), y,
+                                 B, L.N, L.K, c.dtype, pdl, st);
+    }
+    RCHECK(zl_fp8_quant_per_tensor(x, m->xq.get(), m->xs.get(), (size_t)B * L.K, c.dtype, pdl, st));
+    return zl_w8a8_gemm(m->xq.get(), m->xs.get(), L.w.get(), L.w_scale.get(), ZL_F32, L.bias.get(), y, B, L.N, L.K,
+                        ZL_W8_FP8_ROWS, c.dtype, pdl, st);
+}
+
+// Dense and W8A8: the RMSNorm ln of ch's rows of the residual stream into xn, after adding pend_in to them (the previous
+// row-parallel Linear's output, or nullptr: block.cpp:139-141 + 131), then the Linear w from xn into y
+int dense_norm_gemm(zl_llama* m, const Chain& ch, const void* pend_in, const void* ln, const Lin& w, void* y) {
+    const auto& c = m->cfg;
+    const int pdl = ch.no_pdl ? 0 : c.use_pdl;
+    void* h = rows(ch.h, ch.row0, c.dim_model);
+    void* xn = rows(m->xn.get(), ch.row0, c.dim_model);
+    if (!ch.gemm_only)
+        RCHECK(zl_add_rmsnorm(h, pend_in, ln, h, xn, ch.n, c.dim_model, c.eps, 1.f, 0, c.dtype, pdl, m->stream));
+    return dense_or_w8(m, xn, w, y, ch.n, pdl);
+}
+
+// qkv: RMSNorm + GEMM; at fuse >= 2 a W4 GEMM's epilogue splits q / k / v, applies RoPE and appends K / V, otherwise
+// zl_qkv_rope_append does from the GEMM's output rows a.y.  int8 KV cache: the epilogue appends to the staging rows
+// instead (fuse >= 2) or zl_rope_qk_cache writes them (fuse < 2), and kv8_append quantises them into the cache.
 int qkv_gemm(zl_llama* m, int l, Chain& ch) {
     const auto& c = m->cfg;
     const Layer& L = m->layers[l];
@@ -1177,10 +1221,11 @@ int qkv_gemm(zl_llama* m, int l, Chain& ch) {
     void* q = rows(m->q.get(), ch.row0, m->hq * d);
     const int32_t* tb = ch.tb + ch.row0;
     const int32_t* pos = ch.pos + ch.row0;
+    const bool epi = L.qkv.fmt == kW4 && c.fuse >= 2;
     // int8 cache at fuse >= 2 on the exact-integer route (M <= 16): the epilogue quantises K / V into the cache.  The wgmma
     // and fp16 routes, and act-order qkv, append fp16 rows to the staging rows and kv8_append quantises them.
-    const bool fused_kv8 = c.kv_int8 && c.fuse >= 2 && !L.q_qkv.k_perm && route_of(L.q_qkv, ch.n) == 3;
-    if (c.fuse >= 2) {
+    const bool fused_kv8 = c.kv_int8 && epi && !L.qkv.k_perm && route_of(L.qkv, ch.n) == 3;
+    if (epi) {
         a.epilogue = ZL_EPI_QKV_ROPE;
         a.cos = cos;
         a.sin = sin;
@@ -1207,13 +1252,17 @@ int qkv_gemm(zl_llama* m, int l, Chain& ch) {
     } else {
         a.y = rows(m->qkv.get(), ch.row0, hqkv);
     }
-    ch.reduce_in(&a);
-    RCHECK(w4_gemm(m, l, kQkv, ch, L.q_qkv, L.ln_attn.get(), a));
-    if (ch.gemm_only) return ZL_OK;
     const int pdl = ch.no_pdl ? 0 : c.use_pdl;
-    if (fused_kv8) return ZL_OK;
-    if (c.kv_int8) return c.fuse >= 2 ? kv8_append(m, l, ch, pdl) : kv8_rope_append(m, l, ch, a.y, q, pdl);
-    if (c.fuse >= 2) return ZL_OK;
+    if (L.qkv.fmt == kW4) {
+        ch.reduce_in(&a);
+        RCHECK(w4_gemm(m, l, kQkv, ch, L.qkv, L.ln_attn.get(), a));
+    } else {
+        RCHECK(dense_norm_gemm(m, ch, l == 0 ? nullptr : rows(m->pend.get(), ch.row0, c.dim_model), L.ln_attn.get(), L.qkv,
+                               a.y));
+    }
+    if (ch.gemm_only || fused_kv8) return ZL_OK;
+    if (c.kv_int8) return epi ? kv8_append(m, l, ch, pdl) : kv8_rope_append(m, l, ch, a.y, q, pdl);
+    if (epi) return ZL_OK;
     return zl_qkv_rope_append(cos, sin, a.y, q, tb, pos, L.k_addrs.get(), L.v_addrs.get(), ch.n, m->hq, m->hkv, d, 1, 1,
                               m->d_lens.get(), c.dtype, pdl, m->stream);
 }
@@ -1235,64 +1284,53 @@ int attention(zl_llama* m, int l, const void* q, int task0, const int8_t* mask, 
                                c.dtype, pdl, st);
 }
 
-// gate_up: RMSNorm + GEMM + SwiGLU epilogue into act
+// gate_up: RMSNorm + GEMM + SwiGLU into act: in the W4 GEMM's epilogue, or zl_gate_mul after a dense or W8A8 GEMM
 int gate_up_gemm(zl_llama* m, int l, Chain& ch) {
     const auto& c = m->cfg;
+    const Layer& L = m->layers[l];
     zl_w4_fused_args_t a = {};
     a.x = rows(ch.h, ch.row0, c.dim_model);
     a.ldx = c.dim_model;
     a.y = rows(m->act.get(), ch.row0, m->ff);
     a.epilogue = ZL_EPI_SWIGLU;
+    if (L.gu.fmt != kW4) {
+        void* gu = rows(m->gu.get(), ch.row0, 2 * m->ff);
+        RCHECK(dense_norm_gemm(m, ch, rows(m->pend.get(), ch.row0, c.dim_model), L.ln_ff.get(), L.gu, gu));
+        if (ch.gemm_only) return ZL_OK;
+        return zl_gate_mul(gu, 2 * m->ff, (char*)gu + (size_t)m->ff * 2, 2 * m->ff, a.y, m->ff, ch.n, m->ff, 0, c.dtype,
+                           m->stream);
+    }
     ch.reduce_in(&a);
-    return w4_gemm(m, l, kGateUp, ch, m->layers[l].q_gu, m->layers[l].ln_ff.get(), a);
+    return w4_gemm(m, l, kGateUp, ch, L.gu, L.ln_ff.get(), a);
 }
 
-// o (input ao) and down (input act): row-parallel under tensor parallelism, their output goes to ch.sink
+// o (input ao) and down (input act): row-parallel under tensor parallelism.  W4: the output goes to ch.sink.  Dense and
+// W8A8: it goes to pend, all-reduced in place under tensor parallelism, and the next norm adds it to the residual stream.
 int row_parallel_gemm(zl_llama* m, int l, Stage s, Chain& ch) {
     const auto& c = m->cfg;
-    const W4Lin& w = s == kO ? m->layers[l].q_o : m->layers[l].q_down;
+    const Lin& w = s == kO ? m->layers[l].o : m->layers[l].down;
+    const bool w4 = w.fmt == kW4;
     zl_w4_fused_args_t a = {};
     a.x = rows(s == kO ? m->ao.get() : m->act.get(), ch.row0, w.K);
     a.ldx = w.K;
     // the last layer's down keeps the stand-alone all-reduce: the final norm is not a GEMM
-    const bool push = ch.fused && (s == kO || l + 1 < c.num_layers);
+    const bool push = w4 && ch.fused && (s == kO || l + 1 < c.num_layers);
     if (push) {
         ch.push(&a);
-    } else if (ch.sink == Chain::kAddResidual) {
+    } else if (w4 && ch.sink == Chain::kAddResidual) {
         a.residual = a.y = rows(ch.h, ch.row0, c.dim_model);
         a.epilogue = ZL_EPI_RESIDUAL;
     } else {
         a.y = rows(m->pend.get(), ch.row0, c.dim_model);
     }
-    RCHECK(w4_gemm(m, l, s, ch, w, nullptr, a));
-    if (push || ch.sink != Chain::kAllReduce) return ZL_OK;
-    return zl_allreduce_one_shot(m->comm, a.y, ch.h, ch.h, (size_t)ch.n * c.dim_model, c.dtype, c.tp_int8,
-                                 ch.no_pdl ? 0 : c.use_pdl, m->stream);
+    const int pdl = ch.no_pdl ? 0 : c.use_pdl;
+    RCHECK(w4 ? w4_gemm(m, l, s, ch, w, nullptr, a) : dense_or_w8(m, a.x, w, a.y, ch.n, pdl));
+    if (push || ch.gemm_only || ch.sink != Chain::kAllReduce) return ZL_OK;
+    return zl_allreduce_one_shot(m->comm, a.y, w4 ? ch.h : nullptr, w4 ? ch.h : a.y, (size_t)ch.n * c.dim_model, c.dtype,
+                                 c.tp_int8, pdl, m->stream);
 }
 int o_gemm(zl_llama* m, int l, Chain& ch) { return row_parallel_gemm(m, l, kO, ch); }
 int down_gemm(zl_llama* m, int l, Chain& ch) { return row_parallel_gemm(m, l, kDown, ch); }
-
-// One non-W4 Linear of the decode chain: dense (NormalLinear), or W8A8 = activation quant + fused 8-bit GEMM
-// (Int8Linear::forward / Fp8Linear::forward in two launches instead of three).
-int dense_or_w8(zl_llama* m, const void* x, const DenseLin& L, void* y, int B, int pdl) {
-    const auto& c = m->cfg;
-    cudaStream_t st = m->stream;
-    if (!L.w8) return zl_dense_gemm_skinny(x, L.K, L.w.get(), L.bias.get(), y, B, L.N, L.K, c.dtype, c.dtype, pdl, st);
-    if (L.w8_kind == ZL_W8_INT8) {
-        RCHECK(zl_int8_quant_per_token(x, L.K, m->xq.get(), m->xs.get(), B, L.K, c.dtype, pdl, st));
-        return zl_w8a8_gemm(m->xq.get(), m->xs.get(), L.w8.get(), L.w_scale.get(), c.dtype, L.bias.get(), y, B, L.N, L.K,
-                            ZL_W8_INT8, c.dtype, pdl, st);
-    }
-    if (L.w8_kind == kW8Block) {   // Fp8Block::forward: per_token_cast_to_fp8 + the block-scaled GEMM
-        const int ld = (B + 3) / 4 * 4;
-        RCHECK(zl_fp8_quant_per_token_group(x, L.K, m->xq.get(), m->xs.get(), ld, B, L.K, c.dtype, pdl, st));
-        return zl_fp8_block_gemm(m->xq.get(), m->xs.get(), ld, L.w8.get(), static_cast<const float*>(L.w_scale.get()), y,
-                                 B, L.N, L.K, c.dtype, pdl, st);
-    }
-    RCHECK(zl_fp8_quant_per_tensor(x, m->xq.get(), m->xs.get(), (size_t)B * L.K, c.dtype, pdl, st));
-    return zl_w8a8_gemm(m->xq.get(), m->xs.get(), L.w8.get(), L.w_scale.get(), ZL_F32, L.bias.get(), y, B, L.N, L.K,
-                        ZL_W8_FP8_ROWS, c.dtype, pdl, st);
-}
 
 // pf != nullptr: a list of segments -- rows of one task at consecutive positions -- instead of one token per task.  Their
 // tokens, positions and token -> task map are staged in d_pf_tokens / d_pf_pos / d_tb.
@@ -1331,7 +1369,7 @@ static bool prefill_dual_enabled(const zl_llama* m, int n) {
     const char* e = getenv("ZL_PREFILL_DUAL");
     const int force = e ? atoi(e) : 2;
     const auto& c = m->cfg;
-    if (!(c.quant_type == 5 || c.quant_type == 6) || c.fuse < 1 || n < 16) return false;
+    if (lin_format(c) != kW4 || c.fuse < 1 || n < 16) return false;
     return force == 1 || (force == 2 && c.tp_size > 1);
 }
 
@@ -1423,12 +1461,12 @@ Pick pick_of(const zl_llama* m, int first, int n) {
 }
 
 // The final RMSNorm of rows row0 .. row0 + n - 1 of the residual stream h into xn.  W4: the down epilogue already added
-// the residual; dense: the last down's output (pend) is added here.
+// the residual; dense and W8A8: the last down's output (pend) is added here.
 int final_norm(zl_llama* m, void* h, int row0, int n, int pdl) {
     const auto& c = m->cfg;
     const int D = c.dim_model;
     void* hr = rows(h, row0, D);
-    if (c.quant_type == 5 || c.quant_type == 6)
+    if (m->layers.back().down.fmt == kW4)
         return zl_rmsnorm(hr, m->ln_f.get(), m->xn.get(), n, D, c.eps, 1.f, c.dtype, pdl, m->stream);
     return zl_add_rmsnorm(hr, rows(m->pend.get(), row0, D), m->ln_f.get(), hr, m->xn.get(), n, D, c.eps, 1.f, 0, c.dtype,
                           pdl, m->stream);
@@ -1439,7 +1477,6 @@ int enqueue_step(zl_llama* m, int n_tasks, int len_bucket, const Segments* pf, c
     const int B = pf ? pf->n : n_tasks;   // rows (tokens) of every activation matrix in this launch sequence
     const int D = c.dim_model, d = c.dim_head, dt = c.dtype, pdl = c.use_pdl;
     cudaStream_t st = m->stream;
-    const bool w4 = c.quant_type == 5 || c.quant_type == 6;
     const bool tp = c.tp_size > 1;
     const bool joined = pf && pf->joined;
     if (tp && !m->comm) return fail_state(__LINE__, "tp_size > 1 but zl_llama_set_comm was not called");
@@ -1473,32 +1510,18 @@ int enqueue_step(zl_llama* m, int n_tasks, int len_bucket, const Segments* pf, c
     ch.ho = m->h2.get();
     // Tensor parallel, decode-sized launches of a W4 model: the exchange rides inside the GEMMs (Chain).  ZL_TP_UNFUSED=1
     // keeps the separate exchange kernels everywhere (A/B).
-    ch.fused = tp && w4 && !pf && c.fuse >= 1 && !c.tp_int8 && dt == ZL_F16 && !getenv("ZL_TP_UNFUSED") &&
+    ch.fused = tp && lin_format(c) == kW4 && !pf && c.fuse >= 1 && !c.tp_int8 && dt == ZL_F16 && !getenv("ZL_TP_UNFUSED") &&
                (size_t)B * D * 2 <= zl_comm_slot_bytes(m->comm) && 2 * c.num_layers <= 512;
     if (ch.fused) {
         const Layer& L0 = m->layers[0];
-        for (const W4Lin* w : {&L0.q_qkv, &L0.q_o, &L0.q_gu, &L0.q_down})
+        for (const Lin* w : {&L0.qkv, &L0.o, &L0.gu, &L0.down})
             if (route_of(*w, B) != 3) ch.fused = false;
     }
     if (ch.fused) RCHECK(zl_comm_ll_begin_step(m->comm, st));   // the word tags of this step's exchanges
     ch.xodd = ((2 * c.num_layers - 1) & 1) << 9;
     for (int l = 0; l < (dual ? 0 : c.num_layers); ++l) {
-        Layer& L = m->layers[l];
-        if (w4) {
-            RCHECK(qkv_gemm(m, l, ch));
-        } else {
-            // residual of the previous layer's FFN is folded into this norm (block.cpp:139-141 + 131)
-            RCHECK(zl_add_rmsnorm(m->h.get(), l == 0 ? nullptr : m->pend.get(), L.ln_attn.get(), m->h.get(), m->xn.get(),
-                                  B, D, c.eps, 1.f, 0, dt, pdl, st));
-            RCHECK(dense_or_w8(m, m->xn.get(), L.d_qkv, m->qkv.get(), B, pdl));
-            if (c.kv_int8) {
-                RCHECK(kv8_rope_append(m, l, ch, m->qkv.get(), m->q.get(), pdl));
-            } else {
-                RCHECK(zl_qkv_rope_append(m->cosb.get(), m->sinb.get(), m->qkv.get(), m->q.get(), ch.tb, ch.pos,
-                                          L.k_addrs.get(), L.v_addrs.get(), B, m->hq, m->hkv, d, 1, 1, m->d_lens.get(), dt,
-                                          pdl, st));
-            }
-        }
+        const Layer& L = m->layers[l];
+        RCHECK(qkv_gemm(m, l, ch));
         if (joined) {
             // every segment causally over its own task's cache, one launch (attention.cpp:924-961)
             RCHECK(zl_varlen_attention(m->q.get(), j_seg, pf->nseg, B, L.k_addrs.get(), L.v_addrs.get(),
@@ -1510,25 +1533,9 @@ int enqueue_step(zl_llama* m, int n_tasks, int len_bucket, const Segments* pf, c
         } else {
             RCHECK(attention(m, l, m->q.get(), 0, nullptr, len_bucket, m->ao.get(), B, 1, stage_pdl(m, kAttn), st));
         }
-        if (w4) {
-            RCHECK(o_gemm(m, l, ch));
-            RCHECK(gate_up_gemm(m, l, ch));
-            RCHECK(down_gemm(m, l, ch));
-        } else {
-            RCHECK(dense_or_w8(m, m->ao.get(), L.d_o, m->pend.get(), B, pdl));
-            if (tp)
-                RCHECK(zl_allreduce_one_shot(m->comm, m->pend.get(), nullptr, m->pend.get(), (size_t)B * D, dt, c.tp_int8,
-                                             pdl, st));
-            RCHECK(zl_add_rmsnorm(m->h.get(), m->pend.get(), L.ln_ff.get(), m->h.get(), m->xn.get(), B, D, c.eps, 1.f, 0,
-                                  dt, pdl, st));
-            RCHECK(dense_or_w8(m, m->xn.get(), L.d_gu, m->gu.get(), B, pdl));
-            RCHECK(zl_gate_mul(m->gu.get(), 2 * m->ff, (char*)m->gu.get() + (size_t)m->ff * 2, 2 * m->ff, m->act.get(),
-                               m->ff, B, m->ff, 0, dt, st));
-            RCHECK(dense_or_w8(m, m->act.get(), L.d_down, m->pend.get(), B, pdl));
-            if (tp)
-                RCHECK(zl_allreduce_one_shot(m->comm, m->pend.get(), nullptr, m->pend.get(), (size_t)B * D, dt, c.tp_int8,
-                                             pdl, st));
-        }
+        RCHECK(o_gemm(m, l, ch));
+        RCHECK(gate_up_gemm(m, l, ch));
+        RCHECK(down_gemm(m, l, ch));
     }
     const void* head_x = m->xn.get();   // rows that reach lm_head
     if (joined) {
@@ -1657,13 +1664,13 @@ extern "C" int zl_llama_create(const zl_llama_config_t* cfg, zl_llama_t** out) {
     ZL_CHECK_SUPPORTED(cfg->quant_type != 10 ||
                        (cfg->dim_model % 128 == 0 && (cfg->num_heads * cfg->dim_head) % 128 == 0 &&
                         (cfg->num_kv_heads * cfg->dim_head) % 128 == 0 && cfg->dim_ff % 128 == 0));
-    ZL_CHECK_SUPPORTED(!(cfg->quant_type == 5 || cfg->quant_type == 6) || cfg->dtype == ZL_F16);
+    ZL_CHECK_SUPPORTED(lin_format(*cfg) != kW4 || cfg->dtype == ZL_F16);
     ZL_CHECK_SUPPORTED(!(cfg->quant_type == 2 || cfg->quant_type == 7) || cfg->tp_size == 1);   // "A must be half" q_gemm_k_major.cu:989
     ZL_CHECK_SUPPORTED(cfg->dtype == ZL_F16 || cfg->dtype == ZL_BF16);
     ZL_CHECK_SUPPORTED(cfg->tp_size >= 1 && cfg->tp_rank >= 0 && cfg->tp_rank < cfg->tp_size);
     ZL_CHECK_SUPPORTED(cfg->num_heads % cfg->tp_size == 0 && cfg->num_kv_heads % cfg->tp_size == 0 &&
                        cfg->dim_ff % cfg->tp_size == 0 && cfg->vocab_size % cfg->tp_size == 0);
-    ZL_CHECK_SUPPORTED(!(cfg->quant_type == 5 || cfg->quant_type == 6) || cfg->group_size == zl::kW4GroupK);
+    ZL_CHECK_SUPPORTED(lin_format(*cfg) != kW4 || cfg->group_size == zl::kW4GroupK);
     ZL_CHECK_ARG(cfg->fuse >= 0 && cfg->fuse <= 3);
     ZL_CHECK_ARG(cfg->prefill_chunk >= 0 && cfg->prefill_chunk <= 2048);
     ZL_CHECK_SUPPORTED(cfg->fuse < 2 || cfg->dim_head % 32 == 0);
@@ -1907,12 +1914,11 @@ extern "C" int zl_llama_get_logits(zl_llama_t* m, float* logits_host, int B) {
 extern "C" int zl_llama_bench_gemms(zl_llama_t* m, int B, int iters, float* ms, int* launches, double* bytes) {
     ZL_CHECK_ARG(m && B > 0 && B <= m->cfg.max_batch && iters > 0 && ms);
     const auto& c = m->cfg;
-    const int D = c.dim_model, d = c.dim_head, pdl = c.use_pdl;
-    const bool w4 = c.quant_type == 5 || c.quant_type == 6;
+    const int D = c.dim_model, d = c.dim_head;
     cudaStream_t st = m->stream;
-    // the decode step's W4 GEMMs, launched by the same functions (fused RMSNorm, qkv RoPE + KV append, SwiGLU and residual
-    // epilogues, PDL policy).  Rewrites the KV rows of the current positions and the residual stream: call it after the
-    // measurements that need the decode state.
+    // the decode step's layer GEMMs, launched by the same stage functions (W4: fused RMSNorm, qkv RoPE + KV append, SwiGLU
+    // and residual epilogues, PDL policy; W8A8: with the activation quantisation).  Rewrites the KV rows of the current
+    // positions and the residual stream: call it after the measurements that need the decode state.
     Chain ch;
     ch.n = B;
     ch.gemm_only = true;
@@ -1927,33 +1933,26 @@ extern "C" int zl_llama_bench_gemms(zl_llama_t* m, int B, int iters, float* ms, 
     for (int it = -1; it < iters; ++it) {   // it == -1: warm-up pass
         if (it == 0) ZL_CHECK_CUDA(cudaEventRecord(e0, st));
         for (int l = 0; l < c.num_layers; ++l) {
-            Layer& L = m->layers[l];
-            if (w4) {
-                RCHECK(qkv_gemm(m, l, ch));
-                RCHECK(o_gemm(m, l, ch));
-                RCHECK(gate_up_gemm(m, l, ch));
-                RCHECK(down_gemm(m, l, ch));
-                if (it == 0) {
-                    nbytes += (double)zl_w4_packed_bytes(L.q_qkv.N, D, c.group_size) +
-                              (double)zl_w4_packed_bytes(D, m->hq * d, c.group_size) +
-                              (double)zl_w4_packed_bytes(L.q_gu.N, D, c.group_size) +
-                              (double)zl_w4_packed_bytes(D, m->ff, c.group_size);
-                    // activations in/out (fp16)
-                    nbytes += 2.0 * B * (D + L.q_qkv.N + m->hq * d + 2 * D + D + m->ff + m->ff + 2 * D);
-                }
+            RCHECK(qkv_gemm(m, l, ch));
+            RCHECK(o_gemm(m, l, ch));
+            RCHECK(gate_up_gemm(m, l, ch));
+            RCHECK(down_gemm(m, l, ch));
+            if (it != 0) continue;
+            const Layer& L = m->layers[l];
+            n_launch += 4;
+            if (L.qkv.fmt == kW4) {
+                nbytes += (double)zl_w4_packed_bytes(L.qkv.N, D, c.group_size) +
+                          (double)zl_w4_packed_bytes(D, m->hq * d, c.group_size) +
+                          (double)zl_w4_packed_bytes(L.gu.N, D, c.group_size) +
+                          (double)zl_w4_packed_bytes(D, m->ff, c.group_size);
+                // activations in/out (fp16)
+                nbytes += 2.0 * B * (D + L.qkv.N + m->hq * d + 2 * D + D + m->ff + m->ff + 2 * D);
             } else {
-                RCHECK(dense_or_w8(m, m->xn.get(), L.d_qkv, m->qkv.get(), B, pdl));
-                RCHECK(dense_or_w8(m, m->ao.get(), L.d_o, m->pend.get(), B, pdl));
-                RCHECK(dense_or_w8(m, m->xn.get(), L.d_gu, m->gu.get(), B, pdl));
-                RCHECK(dense_or_w8(m, m->act.get(), L.d_down, m->pend.get(), B, pdl));
-                if (it == 0) {
-                    // weight bytes: 2 per element dense, 1 (+ per-row scale) for W8A8 (SURVEY 8d)
-                    const double wb = L.d_qkv.w8 ? 1.0 : 2.0;
-                    nbytes += wb * ((double)L.d_qkv.N * D + (double)D * m->hq * d + 2.0 * m->ff * D + (double)D * m->ff) +
-                              2.0 * B * (D + L.d_qkv.N + m->hq * d + D + D + 2 * m->ff + m->ff + D);
-                }
+                // weight bytes: 2 per element dense, 1 (+ per-row scale) for W8A8 (SURVEY 8d)
+                const double wb = L.qkv.fmt == kDense ? 2.0 : 1.0;
+                nbytes += wb * ((double)L.qkv.N * D + (double)D * m->hq * d + 2.0 * m->ff * D + (double)D * m->ff) +
+                          2.0 * B * (D + L.qkv.N + m->hq * d + D + D + 2 * m->ff + m->ff + D);
             }
-            if (it == 0) n_launch += 4;
         }
     }
     ZL_CHECK_CUDA(cudaEventRecord(e1, st));

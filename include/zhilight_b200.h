@@ -471,6 +471,26 @@ int zl_allreduce_one_shot(zl_comm_t* c, const void* partial, const void* residua
                           int int8_payload, int pdl, zl_stream_t stream);
 /* out[r*bytes ..] = `in` of rank r (bytes % 16 == 0, small: one CTA). */
 int zl_allgather_small(zl_comm_t* c, const void* in, void* out, size_t bytes, int pdl, zl_stream_t stream);
+/* Vocabulary all-gather for the full-vocabulary picks under tensor parallelism (the NCCLAllGather of the logit shards in
+ * src/nn/embedding/embedding.cu:353-390).  Each rank owns a (max_rows, vocab) fp32 row-major buffer, mapped into the
+ * peers with CUDA IPC like zl_comm's (handles of zl_comm_ipc_handle_bytes() bytes, index = rank); world_size 1 needs no
+ * peers.  zl_vocab_allgather writes rows 0 .. rows-1 of this rank's (rows, vocab / world_size) shard (row stride ld floats,
+ * 16-byte aligned) into columns [rank * vshard, (rank + 1) * vshard) of every rank's buffer, this one's included, and
+ * returns on the device once every rank's shard has arrived here: one launch, a collective that every rank must enqueue
+ * with the same rows.  A rank's next gather may overwrite the buffer as soon as every rank has enqueued its own, so a
+ * reader must finish before an exchange that all ranks reach before their next gather (the decode driver's all-reduces).
+ * create: vocab % world_size != 0, max_rows < 1 or max_rows * vocab >= 2^31: ZL_ERR_INVALID_ARG; (vocab / world_size) % 4
+ * != 0: ZL_ERR_UNSUPPORTED.  gather: rows outside [1, max_rows], ld < vshard, ld % 4 != 0 or a misaligned shard:
+ * ZL_ERR_INVALID_ARG; peers not opened: ZL_ERR_STATE; nothing is enqueued then. */
+typedef struct zl_vocab_gather zl_vocab_gather_t;
+int zl_vocab_gather_create(int rank, int world_size, int max_rows, int vocab, zl_vocab_gather_t** out);
+void zl_vocab_gather_destroy(zl_vocab_gather_t* g);
+int zl_vocab_gather_get_ipc_handle(zl_vocab_gather_t* g, void* handle_out);
+int zl_vocab_gather_open_peers(zl_vocab_gather_t* g, const void* handles_all);
+int zl_vocab_gather_info(zl_vocab_gather_t* g, int* rank, int* world_size, int* max_rows, int* vocab);
+/* the (max_rows, vocab) buffer of this rank (device pointer; NULL for g == NULL) */
+float* zl_vocab_gather_buffer(zl_vocab_gather_t* g);
+int zl_vocab_allgather(zl_vocab_gather_t* g, const float* shard, int rows, int ld, int pdl, zl_stream_t stream);
 /* int8_op::quant_group_32 / dequant_sum_quant_g32 / dequant_group_32 / dequant_group_fuse_add
  * (src/nn/quant/int8/quant_reduce_kernel.cu:14-38, 243-322, 105-140, 201-240); M = number of 32-groups. */
 int zl_quant_group_32(const void* in, int8_t* out_q, void* out_scale, size_t M, int dtype, zl_stream_t stream);
@@ -521,6 +541,15 @@ int zl_llama_config_layout(size_t* size, size_t* kv_int8_offset);
 int zl_llama_create(const zl_llama_config_t* cfg, zl_llama_t** out);
 /* tensor parallel: hand the driver its exchange object (zl_comm_create + open_peers) before the first step. */
 int zl_llama_set_comm(zl_llama_t* m, zl_comm_t* comm);
+/* tensor parallel: serve the full-vocabulary picks -- sampling, logits processors, beam steps and zl_llama_generate -- by
+ * gathering the lm_head shards into g (zl_vocab_gather_create with this rank and world size, max_rows >= max_batch,
+ * vocab == vocab_size, peers opened) before the sampler or zl_beam_topk, which then run on every rank over the same rows
+ * and pick the same tokens.  Greedy-only steps keep the candidate exchange.  Without it those entry points return
+ * ZL_ERR_UNSUPPORTED under tp_size > 1.  Every rank must make the same zl_llama_set_sampling, set_logits_processors,
+ * set_stop, beam_step and generate calls, as they make the same set_state and decode calls: ranks that disagree on
+ * whether a step samples wait on different exchanges.  g must outlive the model's steps.  Mismatched g:
+ * ZL_ERR_INVALID_ARG. */
+int zl_llama_set_vocab_gather(zl_llama_t* m, zl_vocab_gather_t* g);
 void zl_llama_destroy(zl_llama_t* m);
 /* Stage one checkpoint tensor (HOST pointer, row-major (rows, cols)); names as produced by
  * zhilight/loader.py:250-358 without the "llama." prefix, e.g. "layers.0.attn.project_q.qweight". */
@@ -565,8 +594,8 @@ int zl_llama_step_joined(zl_llama_t* m, const int32_t* tokens_host, const int32_
                          float* logits_host);
 /* Per-task sampling (zl_sample's contract) for the picks of zl_llama_decode / step_device / prefill.  Copies *p (HOST
  * pointer) to the device and clears the task's history and generated-token sequence; p == NULL returns the task to plain greedy.  Invalid values:
- * ZL_ERR_INVALID_ARG; anything but plain greedy under tp_size > 1: ZL_ERR_UNSUPPORTED (vocabulary shards would need a
- * global top-k / top-p threshold).  The decode step runs zl_sample instead of zl_argmax while a task in the batch
+ * ZL_ERR_INVALID_ARG; anything but plain greedy under tp_size > 1 without zl_llama_set_vocab_gather: ZL_ERR_UNSUPPORTED
+ * (vocabulary shards would need a global top-k / top-p threshold).  The decode step runs zl_sample instead of zl_argmax while a task in the batch
  * samples or has penalties (counter = the input token's position; prefill: pos0 + n - 1), so a task draws the same
  * tokens with host or device-resident stepping, with or without the graph.  The logits stay the raw lm_head output. */
 int zl_llama_set_sampling(zl_llama_t* m, int task, const zl_sample_params_t* p);
@@ -574,7 +603,8 @@ int zl_llama_set_sampling(zl_llama_t* m, int task, const zl_sample_params_t* p);
  * step_joined.  Stream-ordered after the steps already enqueued; the HOST arrays are staged before the call returns.
  * ngram_penalty finite and > 0 (<= 1: off, batch_generator.cpp:1664); n_bias in [0, ZL_MAX_LOGIT_BIAS] distinct tokens in
  * [0, vocab) with finite or -inf values (NaN and +inf are refused): ZL_ERR_INVALID_ARG otherwise.  n_bias = 0 with
- * ngram_penalty <= 1 returns the task to plain behaviour.  Anything on under tp_size > 1: ZL_ERR_UNSUPPORTED.  Every
+ * ngram_penalty <= 1 returns the task to plain behaviour.  Anything on under tp_size > 1 without zl_llama_set_vocab_gather:
+ * ZL_ERR_UNSUPPORTED.  Every
  * check runs before anything is enqueued.  A task with processors makes its batch's pick run the sampler, as a penalty
  * does.  The n-gram rule reads the task's generated-token sequence: the picks of the sampler route since
  * zl_llama_set_sampling last cleared it, up to max_seq tokens (later picks are not recorded). */
@@ -625,8 +655,8 @@ int zl_llama_kv_blocks_bench(zl_llama_t* m, int task, const int32_t* task_blocks
  * One beam step: the decode step over tasks 0 .. B-1 (tokens / positions HOST (B) as zl_llama_decode), with the pick
  * replaced by zl_beam_topk on the step's logits -- same CUDA graph, one per (B, G, K, length bucket), no argmax.  groups
  * (G, 2), cum (B) HOST; parent / token / score (G, K) HOST outputs as zl_beam_topk's; logits_host NULL or (B, vocab).
- * Synchronous.  Bad groups, K, cum (NaN or +inf), tokens or positions: ZL_ERR_INVALID_ARG; vocab > 262144 or tp_size > 1:
- * ZL_ERR_UNSUPPORTED; a task of the batch that samples or has penalties (zl_llama_set_sampling) or logits processors
+ * Synchronous.  Bad groups, K, cum (NaN or +inf), tokens or positions: ZL_ERR_INVALID_ARG; vocab > 262144, or tp_size > 1 without
+ * zl_llama_set_vocab_gather: ZL_ERR_UNSUPPORTED; a task of the batch that samples or has penalties (zl_llama_set_sampling) or logits processors
  * (zl_llama_set_logits_processors): ZL_ERR_STATE. */
 int zl_llama_beam_step(zl_llama_t* m, const int32_t* tokens, const int32_t* positions, int B, const int32_t* groups, int G,
                        const float* cum, int K, int32_t* parent, int32_t* token, float* score, float* logits_host);
@@ -651,8 +681,8 @@ int zl_llama_kv_copy_rows(zl_llama_t* m, const int32_t* ranges_host, int n);
  * until zl_llama_set_state moves it.  A task without a stop rule has no stop ids and no budget.
  * Per-task stop rule for zl_llama_generate: up to ZL_MAX_STOP_IDS distinct ids in [0, vocab); max_new_tokens >= 1, or 0
  * for no budget.  Re-arms a finished task and resets its emitted count.  Stream-ordered; host arrays staged before return.
- * Bad task or ids, a repeated id, n_stop > ZL_MAX_STOP_IDS or max_new_tokens < 0: ZL_ERR_INVALID_ARG; tp_size > 1:
- * ZL_ERR_UNSUPPORTED; a model not finalized: ZL_ERR_STATE. */
+ * Bad task or ids, a repeated id, n_stop > ZL_MAX_STOP_IDS or max_new_tokens < 0: ZL_ERR_INVALID_ARG; tp_size > 1 without
+ * zl_llama_set_vocab_gather: ZL_ERR_UNSUPPORTED; a model not finalized: ZL_ERR_STATE. */
 #define ZL_MAX_STOP_IDS 8
 int zl_llama_set_stop(zl_llama_t* m, int task, const int32_t* stop_ids_host, int n_stop, int max_new_tokens);
 /* Up to max_steps (1 .. max_seq) device-resident decode steps of rows 0..B-1, stopping early when all have finished.
@@ -663,7 +693,7 @@ int zl_llama_set_stop(zl_llama_t* m, int task, const int32_t* stop_ids_host, int
  * bucket): a head kernel and a while-loop conditional node whose body is the decode step plus the stop rules; a call
  * crosses buckets with one graph launch per bucket, without a host sync in between, and syncs once at the end.  A call
  * whose tasks have all finished runs 0 steps and enqueues nothing.  Bad B, max_steps or output pointers:
- * ZL_ERR_INVALID_ARG; tp_size > 1 or use_graph == 0: ZL_ERR_UNSUPPORTED; a model not finalized: ZL_ERR_STATE.  Every
+ * ZL_ERR_INVALID_ARG; tp_size > 1 without zl_llama_set_vocab_gather, or use_graph == 0: ZL_ERR_UNSUPPORTED; a model not finalized: ZL_ERR_STATE.  Every
  * check runs before anything is enqueued. */
 int zl_llama_generate(zl_llama_t* m, int B, int max_steps, int32_t* tokens_host, int32_t* n_out_host,
                       int32_t* finish_host, int* steps_host);

@@ -184,6 +184,9 @@ struct zl_llama {
     dev_ptr<int32_t> d_pf_tokens, d_pf_pos;
     zl_comm_t* comm = nullptr;            // TP exchange (set by zl_llama_set_comm when tp_size > 1)
     int vshard = 0;                       // vocabulary rows of lm_head held by this rank
+    // tensor parallel: the vocabulary all-gather that gives the sampler and the beam selection whole rows
+    // (zl_llama_set_vocab_gather); NULL keeps them refused under tp_size > 1
+    zl_vocab_gather_t* vgather = nullptr;
     dev_ptr<> cand;                       // [B] {float value, int index} local argmax candidates
     dev_ptr<> cand_all;                   // [tp][B] gathered candidates
     GraphCache graphs;                    // decode-step graphs, by graph_key (+ the beam bits)
@@ -960,7 +963,7 @@ int alloc_runtime(zl_llama* m) {
     }
     RCHECK(dmalloc(&m->attn_ws, m->attn_ws_bytes));
     RCHECK(dmalloc(&m->argmax_ws, zl_argmax_workspace_bytes(B)));
-    m->hwords = cdiv(m->vshard, 32);
+    m->hwords = cdiv(c.vocab_size, 32);   // the sampler reads whole rows: the gathered ones under tensor parallelism
     RCHECK(dmalloc(&m->d_hist, (size_t)B * m->hwords * 4));
     ZL_CHECK_CUDA(cudaMemsetAsync(m->d_hist.get(), 0, (size_t)B * m->hwords * 4, m->stream));
     RCHECK(dmalloc(&m->d_sparams, sizeof(zl_sample_params_t) * B));
@@ -1453,6 +1456,9 @@ struct Pick {
     }
 };
 
+// the sampler and the beam selection can see whole vocabulary rows: a single rank, or the vocabulary all-gather
+bool full_rows(const zl_llama* m) { return m->cfg.tp_size == 1 || m->vgather; }
+
 // the pick of tasks first .. first + n - 1
 Pick pick_of(const zl_llama* m, int first, int n) {
     Pick pk;
@@ -1559,18 +1565,25 @@ int enqueue_step(zl_llama* m, int n_tasks, int len_bucket, const Segments* pf, c
     // vocab-parallel lm_head (embedding.cu:353-392): each rank owns vshard rows
     RCHECK(zl_dense_gemm_skinny(head_x, D, m->lm_head, nullptr, m->logits.get(), HB, m->vshard, D, dt, ZL_F32,
                                 stage_pdl(m, kLmHead), st));
+    // the sampler and the beam selection read whole rows: under tensor parallelism every rank gathers the shards and
+    // picks the same tokens from the same rows (both are deterministic), so no pick is broadcast
+    const float* rows_v = m->logits.get();
+    if (tp && (pk.beam || pk.sampler)) {
+        if (!m->vgather) return fail_state(__LINE__, "a sampled or beam pick under tp_size > 1 needs zl_llama_set_vocab_gather");
+        RCHECK(zl_vocab_allgather(m->vgather, m->logits.get(), HB, m->vshard, pdl, st));
+        rows_v = zl_vocab_gather_buffer(m->vgather);
+    }
     if (const BeamPick* beam = pk.beam) {
-        // decode rows only, single rank, no sampling (zl_llama_beam_step checks)
-        RCHECK(beam_topk_launch(m->logits.get(), HB, m->vshard, beam->cum, beam->groups, beam->G, beam->K, beam->parent,
+        // decode rows only, no sampling (zl_llama_beam_step checks)
+        RCHECK(beam_topk_launch(rows_v, HB, c.vocab_size, beam->cum, beam->groups, beam->G, beam->K, beam->parent,
                                 beam->token, beam->score, beam->ws, stage_pdl(m, kPick), st));
     } else if (pk.sampler) {
         // one row per task at decode (row b = task b, counter = its input position); prefill: the task's last prompt
-        // position; joined: each emitting segment's task and last position.  set_sampling keeps this off under tensor
-        // parallelism.
+        // position; joined: each emitting segment's task and last position
         const int32_t* row_task = joined ? j_task : pf ? m->d_iota.get() + pf->task : m->d_iota.get();
         const int32_t* counter = joined ? j_pos : pf ? m->d_pf_pos.get() + (pf->n - 1) : m->d_pos.get();
         // k_ngram_levels runs only when a task of the step has the n-gram rule on (`pk.ngram`, a bit of the graph key)
-        RCHECK(sample_processed_launch(m->logits.get(), HB, m->vshard, m->d_sparams.get(), row_task, counter,
+        RCHECK(sample_processed_launch(rows_v, HB, c.vocab_size, m->d_sparams.get(), row_task, counter,
                                        m->d_hist.get(), m->hwords, pk.ngram ? m->d_ngram.get() : nullptr, m->d_seq.get(),
                                        m->d_seq_len.get(), c.max_seq, m->d_bias_tok.get(), m->d_bias_val.get(),
                                        m->d_bias_cnt.get(), ZL_MAX_LOGIT_BIAS, pk.frozen, m->d_next.get(),
@@ -1702,6 +1715,18 @@ extern "C" int zl_llama_set_comm(zl_llama_t* m, zl_comm_t* comm) {
     ZL_CHECK_ARG(m && comm);
     ZL_CHECK_ARG(zl_comm_world_size(comm) == m->cfg.tp_size && zl_comm_rank(comm) == m->cfg.tp_rank);
     m->comm = comm;
+    return ZL_OK;
+}
+
+extern "C" int zl_llama_set_vocab_gather(zl_llama_t* m, zl_vocab_gather_t* g) {
+    ZL_CHECK_ARG(m && g);
+    int rank = 0, ws = 0, max_rows = 0, vocab = 0;
+    RCHECK(zl_vocab_gather_info(g, &rank, &ws, &max_rows, &vocab));
+    // at most max_batch rows reach lm_head: a decode or beam step's tasks, a prefill's last position, a joined step's
+    // emitting segments
+    ZL_CHECK_ARG(ws == m->cfg.tp_size && rank == m->cfg.tp_rank && max_rows >= m->cfg.max_batch &&
+                 vocab == m->cfg.vocab_size);
+    m->vgather = g;
     return ZL_OK;
 }
 
@@ -2078,7 +2103,7 @@ extern "C" int zl_llama_set_sampling(zl_llama_t* m, int task, const zl_sample_pa
     ZL_CHECK_ARG(m && task >= 0 && task < m->cfg.max_batch);
     const bool on = p && ((p->temperature > 0.f && p->top_k != 1) || p->repetition_penalty != 1.f ||
                           p->presence_penalty != 0.f);
-    ZL_CHECK_SUPPORTED(!on || m->cfg.tp_size == 1);
+    ZL_CHECK_SUPPORTED(!on || full_rows(m));
     if (!m->finalized) return fail_state(__LINE__, "model not finalized");
     const zl_sample_params_t q = p ? *p : zl_sample_params_t{0.f, 1.f, 1.f, 0.f, 0, 0};
     // stream-ordered after every step already enqueued; the pageable source is staged before the call returns
@@ -2104,7 +2129,7 @@ extern "C" int zl_llama_set_logits_processors(zl_llama_t* m, int task, float ngr
     std::sort(sorted.begin(), sorted.end());
     ZL_CHECK_ARG(std::adjacent_find(sorted.begin(), sorted.end()) == sorted.end());
     const bool ngram = ngram_penalty > 1.f, on = ngram || n_bias > 0;
-    ZL_CHECK_SUPPORTED(!on || m->cfg.tp_size == 1);
+    ZL_CHECK_SUPPORTED(!on || full_rows(m));
     if (!m->finalized) return fail_state(__LINE__, "model not finalized");
     if (ngram && !m->ngram_ws) {
         m->ngram_ws_bytes = zl_sample_processed_workspace_bytes(m->cfg.max_batch, m->cfg.max_seq);
@@ -2343,7 +2368,7 @@ int ensure_beam(zl_llama* m) {
     const int MB = m->cfg.max_batch;
     size_t ws = 0;   // the workspace of the largest R <= max_batch
     for (int r = 1; r <= MB; ++r) {
-        const size_t b = zl_beam_topk_workspace_bytes(r, m->vshard, kBeamK);
+        const size_t b = zl_beam_topk_workspace_bytes(r, m->cfg.vocab_size, kBeamK);
         if (b > ws) ws = b;
     }
     const size_t words = (size_t)MB * (3 + 3 * kBeamK);
@@ -2365,10 +2390,10 @@ extern "C" int zl_llama_beam_step(zl_llama_t* m, const int32_t* tokens, const in
                                   float* score, float* logits_host) {
     ZL_CHECK_ARG(m && tokens && positions && groups && cum && parent && token && score);
     ZL_CHECK_ARG(B > 0 && B <= m->cfg.max_batch);
-    RCHECK(beam_topk_check(B, m->vshard, groups, G, K));
+    RCHECK(beam_topk_check(B, full_rows(m) ? m->cfg.vocab_size : m->vshard, groups, G, K));
     for (int i = 0; i < B; ++i) ZL_CHECK_ARG(cum[i] < INFINITY);   // -inf: a dead row; NaN and +inf are refused
-    if (m->cfg.tp_size > 1)
-        return fail_state(__LINE__, "beam steps need the whole vocabulary on one rank (tp_size 1)", ZL_ERR_UNSUPPORTED);
+    if (!full_rows(m))
+        return fail_state(__LINE__, "beam steps under tensor parallelism need zl_llama_set_vocab_gather", ZL_ERR_UNSUPPORTED);
     ZL_CHECK_SUPPORTED(B < 2048);   // the graph key holds B and G in 11 bits
     if (!m->finalized) return fail_state(__LINE__, "model not finalized");
     if (pick_of(m, 0, B).sampler)
@@ -2621,7 +2646,8 @@ extern "C" int zl_llama_set_stop(zl_llama_t* m, int task, const int32_t* stop_id
     }
     r.n = n_stop;
     r.budget = max_new_tokens;
-    if (m->cfg.tp_size > 1) return fail_state(__LINE__, "zl_llama_set_stop: tensor parallelism is not served", ZL_ERR_UNSUPPORTED);
+    if (!full_rows(m))
+        return fail_state(__LINE__, "zl_llama_set_stop: tensor parallelism needs zl_llama_set_vocab_gather", ZL_ERR_UNSUPPORTED);
     if (!m->finalized) return fail_state(__LINE__, "model not finalized");
     // stream-ordered after every step already enqueued; the rule travels as a kernel argument
     k_gen_arm<<<1, 1, 0, m->stream>>>(gen_state(m), task, r);
@@ -2635,7 +2661,8 @@ extern "C" int zl_llama_generate(zl_llama_t* m, int B, int max_steps, int32_t* t
     ZL_CHECK_ARG(m && tokens_host && n_out_host && finish_host && steps_host);
     const auto& c = m->cfg;
     ZL_CHECK_ARG(B > 0 && B <= c.max_batch && max_steps >= 1 && max_steps <= c.max_seq);
-    if (c.tp_size > 1) return fail_state(__LINE__, "zl_llama_generate: tensor parallelism is not served", ZL_ERR_UNSUPPORTED);
+    if (!full_rows(m))
+        return fail_state(__LINE__, "zl_llama_generate: tensor parallelism needs zl_llama_set_vocab_gather", ZL_ERR_UNSUPPORTED);
     if (!c.use_graph) return fail_state(__LINE__, "zl_llama_generate runs as a CUDA graph (use_graph = 0)", ZL_ERR_UNSUPPORTED);
     if (!m->finalized) return fail_state(__LINE__, "model not finalized");
     const int MB = c.max_batch;

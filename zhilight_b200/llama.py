@@ -141,10 +141,25 @@ class LlamaDecoder:
         self._comm = comm
         _lib.check(self.lib.zl_llama_set_comm(self.h, comm.handle))
 
+    def enable_tp_picks(self, group=None):
+        """Serve sampling, logits processors, beam_search, set_stop and generate under tensor parallelism: every rank
+        gathers the lm_head shards of a sampled or beam step over NVLink and picks from the whole rows
+        (zl_llama_set_vocab_gather).  Collective: every rank calls it, and from then on every rank must make the same
+        set_sampling, set_stop, beam_step and generate calls, as it makes the same decode calls.  A no-op at tp_size 1."""
+        if self.cfg.tp_size == 1 or getattr(self, "_vgather", None) is not None:
+            return
+        from .dist import VocabGather
+        g = VocabGather(self.max_batch, self.vocab_size, self.cfg.tp_rank, self.cfg.tp_size, group)
+        _lib.check(self.lib.zl_llama_set_vocab_gather(self.h, g.handle))
+        self._vgather = g   # released after the model (close)
+
     def close(self):
         if getattr(self, "h", None):
             self.lib.zl_llama_destroy(self.h)
             self.h = None
+        if getattr(self, "_vgather", None) is not None:
+            self._vgather.close()
+            self._vgather = None
 
     def __del__(self):
         try:
@@ -309,9 +324,9 @@ class LlamaDecoder:
         check_ngram_penalty(ngram_penalty)
         ngram = 1.0 if presence_penalty else float(ngram_penalty)
         toks, vals = logit_bias_arrays(logit_bias, self.cfg.vocab_size)
-        if self.cfg.tp_size > 1 and (ngram > 1 or toks.size):
-            # refused here so that neither the sampling nor the processors change
-            raise _lib.ZLError(-2, "logits processors are not served under tensor parallelism")
+        if self.cfg.tp_size > 1 and getattr(self, "_vgather", None) is None and (ngram > 1 or toks.size):
+            # refused here so that neither the sampling nor the processors change (enable_tp_picks serves them)
+            raise _lib.ZLError(-2, "logits processors under tensor parallelism need enable_tp_picks()")
         p = _lib.sample_params(temperature, top_p, top_k, repetition_penalty, presence_penalty, seed)
         _lib.check(self.lib.zl_llama_set_sampling(self.h, int(task), ctypes.byref(p)))
         _lib.check(self.lib.zl_llama_set_logits_processors(self.h, int(task), ngram, toks.ctypes.data_as(ctypes.c_void_p),

@@ -428,6 +428,21 @@ int zl_sample_processed(const float* logits, int T, int V, const zl_sample_param
                         int32_t* seq, int32_t* seq_len, int seq_stride, const int32_t* bias_tokens,
                         const float* bias_values, const int32_t* bias_count, int bias_stride, int32_t* out, void* ws,
                         size_t ws_bytes, int pdl, zl_stream_t stream);
+/* Allowed-token masks on top of zl_sample_processed (structured output: a token automaton's allowed set, or a grammar
+ * engine's per-step bitmask).  masks (rows, mask_words >= ceil(V/32)) u32: bit j of word i allows token 32 i + j.
+ * mask_row (tasks) int32 or NULL: task t is masked by row mask_row[t] (< rows, not checked on the device), or not at all
+ * when mask_row[t] < 0; NULL masks task t by row t.  For a masked row, with A its allowed set:
+ *   0. every token outside A is removed before anything else: it is never picked, gets no mass and does not count for
+ *      top_k (as a NaN logit); an allowed NaN logit counts as -inf;
+ *   1.-3. zl_sample_processed's contract, unchanged, on the tokens of A: penalties, n-gram rule, bias, temperature, top-k,
+ *      top-p and the Philox draw; greedy rows (temperature 0 or top_k 1) take the lowest-index maximum over A;
+ *   4. when every token of A ends at -inf after the bias, the pick is the smallest token of A.
+ * A is expected non-empty (an empty row picks token 0).  Unmasked rows get exactly zl_sample_processed's token. */
+int zl_sample_masked(const float* logits, int T, int V, const zl_sample_params_t* params, const int32_t* row_task,
+                     const int32_t* counter, uint32_t* history, int history_words, const float* ngram_penalty,
+                     int32_t* seq, int32_t* seq_len, int seq_stride, const int32_t* bias_tokens, const float* bias_values,
+                     const int32_t* bias_count, int bias_stride, const uint32_t* masks, int mask_words,
+                     const int32_t* mask_row, int32_t* out, void* ws, size_t ws_bytes, int pdl, zl_stream_t stream);
 /* Beam-search selection (beam_utility::log_softmax_bias, generator/beam_util.cu:20-130, then topk_all.get_top_k over each
  * task's flattened (beam x vocab) scores, generator/batch_generator.cpp:1770-1778), without writing an (R, V) tensor.
  * logits (R, V) fp32 and cum (R) fp32 on the device; groups (G, 2) {row0, width} a HOST array whose groups tile rows
@@ -610,6 +625,38 @@ int zl_llama_set_sampling(zl_llama_t* m, int task, const zl_sample_params_t* p);
  * zl_llama_set_sampling last cleared it, up to max_seq tokens (later picks are not recorded). */
 int zl_llama_set_logits_processors(zl_llama_t* m, int task, float ngram_penalty, const int32_t* bias_tokens_host,
                                    const float* bias_values_host, int n_bias);
+/* Constrained decoding: a per-task token automaton whose state's allowed set masks the task's picks (zl_sample_masked's
+ * contract) and whose state moves on the device with every recorded pick.  An automaton has S >= 1 states; state s has
+ * a non-empty allowed set A(s), ceil(vocab/32) u32 words with no bit at or past vocab (bit j of word i = token 32 i + j),
+ * edges (token, next) with distinct tokens of A(s) in ascending order, and default_next[s].  Picking x in state s moves
+ * the task to the next state of x's edge, or to default_next[s] when x has none.  The state moves exactly where a pick is
+ * recorded: zl_llama_decode / step_device rows, the last chunk of zl_llama_prefill, the emitting segments of
+ * zl_llama_step_joined and the running tasks of zl_llama_generate (a finished task neither records nor moves).  The
+ * returned logits stay raw.  A one-state automaton whose default is itself is a plain mask; setting one before each
+ * zl_llama_decode is how a host grammar engine drives the engine step by step.
+ * zl_llama_enable_constraints allocates, per task, max_states masks, max_states + 1 row offsets, max_edges edges and
+ * max_states defaults on the device, once per model (a second call: ZL_ERR_STATE; before zl_llama_finalize:
+ * ZL_ERR_STATE; max_states < 1 or max_edges < 0: ZL_ERR_INVALID_ARG).  Graphs captured before it are dropped. */
+int zl_llama_enable_constraints(zl_llama_t* m, int max_states, int max_edges);
+/* Host check of one automaton over a vocabulary of `vocab` tokens (HOST arrays, as zl_llama_set_constraint takes them,
+ * n_states >= 1): ZL_ERR_INVALID_ARG for every malformation listed there, else ZL_OK.  Needs no device. */
+int zl_token_automaton_check(int vocab, int n_states, const uint32_t* masks, const int32_t* row_ptr, int n_edges,
+                             const int32_t* edge_tok, const int32_t* edge_next, const int32_t* default_next, int start);
+/* The automaton of `task` from HOST arrays, staged before the call returns; stream-ordered after the steps already
+ * enqueued.  masks (n_states, ceil(vocab/32)); row_ptr (n_states + 1) CSR offsets of each state's edges in edge_tok /
+ * edge_next (n_edges); default_next (n_states); the task starts in `start`.  n_states = 0 clears the task's automaton (the
+ * other arrays are ignored).  Every check runs before anything is enqueued, in this order: a bad task or n_states < 0:
+ * ZL_ERR_INVALID_ARG; an automaton under tp_size > 1 without zl_llama_set_vocab_gather: ZL_ERR_UNSUPPORTED (with it,
+ * every rank moves the same states from the same rows); constraints not enabled: ZL_ERR_STATE; n_states or n_edges
+ * above the caps, an empty mask, a bit at or past vocab, row_ptr not starting at 0, decreasing or not ending at
+ * n_edges, edge tokens out of order, repeated or outside their state's mask, or a state out of range:
+ * ZL_ERR_INVALID_ARG.  A constrained task makes its batch's pick run the sampler, as a
+ * logits processor does, and a beam step over it is refused (ZL_ERR_STATE).  zl_llama_set_sampling leaves it alone. */
+int zl_llama_set_constraint(zl_llama_t* m, int task, int n_states, const uint32_t* masks_host, const int32_t* row_ptr_host,
+                            int n_edges, const int32_t* edge_tok_host, const int32_t* edge_next_host,
+                            const int32_t* default_next_host, int start);
+/* The current automaton state of tasks 0 .. B-1 (-1: none) into states_host, once every step enqueued has executed. */
+int zl_llama_get_constraint_state(zl_llama_t* m, int32_t* states_host, int B);
 /* Copy rows row0 .. row0 + n of task `task`'s layer-`layer` KV cache to the host (the reference's dump_task_buf,
  * rag_buffer_context.h:199-233).  Synchronous.  Plain cache: k_host / v_host get (n, H_kv, d) activation-dtype values and
  * sk_host / sv_host must be NULL.  kv_int8: k_host / v_host get (n, H_kv, d) uint8 codes and sk_host / sv_host (n, H_kv)
@@ -657,7 +704,7 @@ int zl_llama_kv_blocks_bench(zl_llama_t* m, int task, const int32_t* task_blocks
  * (G, 2), cum (B) HOST; parent / token / score (G, K) HOST outputs as zl_beam_topk's; logits_host NULL or (B, vocab).
  * Synchronous.  Bad groups, K, cum (NaN or +inf), tokens or positions: ZL_ERR_INVALID_ARG; vocab > 262144, or tp_size > 1 without
  * zl_llama_set_vocab_gather: ZL_ERR_UNSUPPORTED; a task of the batch that samples or has penalties (zl_llama_set_sampling) or logits processors
- * (zl_llama_set_logits_processors): ZL_ERR_STATE. */
+ * (zl_llama_set_logits_processors) or a constraint (zl_llama_set_constraint): ZL_ERR_STATE. */
 int zl_llama_beam_step(zl_llama_t* m, const int32_t* tokens, const int32_t* positions, int B, const int32_t* groups, int G,
                        const float* cum, int K, int32_t* parent, int32_t* token, float* score, float* logits_host);
 /* Beam forks: one launch copies rows [row0, row1) of task src into task dst for every range ranges_host[i] = {src task,

@@ -127,8 +127,10 @@ struct GraphCache {
     GraphCache() = default;
     GraphCache(const GraphCache&) = delete;
     GraphCache& operator=(const GraphCache&) = delete;
-    ~GraphCache() {
+    ~GraphCache() { clear(); }
+    void clear() {
         for (auto& g : execs) cudaGraphExecDestroy(g.second);
+        execs.clear();
     }
     template <typename Build>
     int get(long long key, Build&& build, cudaGraphExec_t* out, int* nodes = nullptr) {
@@ -214,7 +216,7 @@ struct zl_llama {
     dev_ptr<zl_sample_params_t> d_sparams;   // (max_batch)
     dev_ptr<uint32_t> d_hist;                // (max_batch, hwords)
     int hwords = 0;
-    std::vector<char> samp_on;               // pen_on[t] || proc_on[t]
+    std::vector<char> samp_on;               // pen_on[t] || proc_on[t] || cons_on[t]
     std::vector<char> pen_on;                // set by zl_llama_set_sampling: samples or has penalties
     // logits processors (zl_llama_set_logits_processors): per-task n-gram penalty and bias lists, and every task's
     // generated-token sequence (appended by the sampler where it sets the history bit, cleared with it); the n-gram
@@ -226,6 +228,13 @@ struct zl_llama {
     dev_ptr<> ngram_ws;
     size_t ngram_ws_bytes = 0;
     std::vector<char> proc_on, ngram_on;
+    // token automata (zl_llama_enable_constraints / zl_llama_set_constraint): per task, cons_max_states mask rows of
+    // hwords words, CSR edges (row offsets, tokens, next states), the default next states and the current state (-1:
+    // unconstrained), laid out as SampleAutomata reads them; cons_on[t] while task t has an automaton
+    dev_ptr<uint32_t> d_cmask;
+    dev_ptr<int32_t> d_crow, d_cedge_tok, d_cedge_next, d_cdflt, d_cstate;
+    int cons_max_states = 0, cons_max_edges = 0;
+    std::vector<char> cons_on;
     // int8 KV cache: the rotated fp16 K / V rows of the launch sequence are staged in kv_stage (k: tok_cap x Hkv x d, then
     // v) and quantised into the cache from there.  A qkv GEMM with the RoPE / KV-append epilogue appends into the staging
     // rows as into the cache of one task: stage_addrs = {k rows, v rows}, token -> task map d_zeros, placement d_rowidx.
@@ -978,6 +987,7 @@ int alloc_runtime(zl_llama* m) {
     m->pen_on.assign(B, 0);
     m->proc_on.assign(B, 0);
     m->ngram_on.assign(B, 0);
+    m->cons_on.assign(B, 0);
     RCHECK(dmalloc(&m->d_ngram, (size_t)B * 4));
     RCHECK(dmalloc(&m->d_seq, (size_t)B * c.max_seq * 4));
     RCHECK(dmalloc(&m->d_seq_len, (size_t)B * 4));
@@ -1449,7 +1459,7 @@ struct Pick {
     const BeamPick* beam = nullptr;
     const int32_t* frozen = nullptr;
 
-    // task t samples (or has penalties or logits processors), and has the n-gram rule on
+    // task t samples (or has penalties, logits processors or an automaton), and has the n-gram rule on
     void add(const zl_llama* m, int t) {
         sampler |= m->samp_on[t] != 0;
         ngram |= m->ngram_on[t] != 0;
@@ -1583,10 +1593,22 @@ int enqueue_step(zl_llama* m, int n_tasks, int len_bucket, const Segments* pf, c
         const int32_t* row_task = joined ? j_task : pf ? m->d_iota.get() + pf->task : m->d_iota.get();
         const int32_t* counter = joined ? j_pos : pf ? m->d_pf_pos.get() + (pf->n - 1) : m->d_pos.get();
         // k_ngram_levels runs only when a task of the step has the n-gram rule on (`pk.ngram`, a bit of the graph key)
+        // with automata enabled every sampler launch reads the tasks' states (-1: unconstrained), so no key bit is needed
+        SampleAutomata au{};
+        au.mask = m->d_cmask.get();
+        au.state = m->d_cstate.get();
+        au.words = m->hwords;
+        au.states = m->cons_max_states;
+        au.max_edges = m->cons_max_edges;
+        au.row_ptr = m->d_crow.get();
+        au.edge_tok = m->d_cedge_tok.get();
+        au.next = m->d_cedge_next.get();
+        au.dflt = m->d_cdflt.get();
         RCHECK(sample_processed_launch(rows_v, HB, c.vocab_size, m->d_sparams.get(), row_task, counter,
                                        m->d_hist.get(), m->hwords, pk.ngram ? m->d_ngram.get() : nullptr, m->d_seq.get(),
                                        m->d_seq_len.get(), c.max_seq, m->d_bias_tok.get(), m->d_bias_val.get(),
-                                       m->d_bias_cnt.get(), ZL_MAX_LOGIT_BIAS, pk.frozen, m->d_next.get(),
+                                       m->d_bias_cnt.get(), ZL_MAX_LOGIT_BIAS, pk.frozen, m->d_cmask ? &au : nullptr,
+                                       m->d_next.get(),
                                        pk.ngram ? m->ngram_ws.get() : nullptr, m->ngram_ws_bytes, stage_pdl(m, kPick), st));
     } else if (!tp) {
         RCHECK(zl_argmax(m->logits.get(), m->d_next.get(), HB, m->vshard, m->argmax_ws.get(), zl_argmax_workspace_bytes(HB),
@@ -2111,7 +2133,7 @@ extern "C" int zl_llama_set_sampling(zl_llama_t* m, int task, const zl_sample_pa
     ZL_CHECK_CUDA(cudaMemsetAsync(m->d_hist.get() + (size_t)task * m->hwords, 0, (size_t)m->hwords * 4, m->stream));
     ZL_CHECK_CUDA(cudaMemsetAsync(m->d_seq_len.get() + task, 0, 4, m->stream));
     m->pen_on[task] = on ? 1 : 0;
-    m->samp_on[task] = m->pen_on[task] || m->proc_on[task];
+    m->samp_on[task] = m->pen_on[task] || m->proc_on[task] || m->cons_on[task];
     return ZL_OK;
 }
 
@@ -2147,7 +2169,75 @@ extern "C" int zl_llama_set_logits_processors(zl_llama_t* m, int task, float ngr
     ZL_CHECK_CUDA(cudaMemcpyAsync(m->d_bias_cnt.get() + task, &n_bias, 4, cudaMemcpyHostToDevice, st));
     m->proc_on[task] = on ? 1 : 0;
     m->ngram_on[task] = ngram ? 1 : 0;
-    m->samp_on[task] = m->pen_on[task] || m->proc_on[task];
+    m->samp_on[task] = m->pen_on[task] || m->proc_on[task] || m->cons_on[task];
+    return ZL_OK;
+}
+
+extern "C" int zl_llama_enable_constraints(zl_llama_t* m, int max_states, int max_edges) {
+    ZL_CHECK_ARG(m && max_states >= 1 && max_edges >= 0);
+    if (!m->finalized) return fail_state(__LINE__, "model not finalized");
+    if (m->d_cmask) return fail_state(__LINE__, "zl_llama_enable_constraints was already called");
+    const size_t B = m->cfg.max_batch, S = max_states;
+    RCHECK(dmalloc(&m->d_cmask, B * S * m->hwords * 4));
+    RCHECK(dmalloc(&m->d_crow, B * (S + 1) * 4));
+    RCHECK(dmalloc(&m->d_cedge_tok, B * max_edges * 4));
+    RCHECK(dmalloc(&m->d_cedge_next, B * max_edges * 4));
+    RCHECK(dmalloc(&m->d_cdflt, B * S * 4));
+    RCHECK(dmalloc(&m->d_cstate, B * 4));
+    ZL_CHECK_CUDA(cudaMemsetAsync(m->d_cstate.get(), 0xff, B * 4, m->stream));   // -1: unconstrained
+    ZL_CHECK_CUDA(cudaStreamSynchronize(m->stream));
+    m->cons_max_states = max_states;
+    m->cons_max_edges = max_edges;
+    // the sampler launches captured so far carry no automata
+    m->graphs.clear();
+    m->gen_graphs.clear();
+    return ZL_OK;
+}
+
+extern "C" int zl_llama_set_constraint(zl_llama_t* m, int task, int n_states, const uint32_t* masks_host,
+                                       const int32_t* row_ptr_host, int n_edges, const int32_t* edge_tok_host,
+                                       const int32_t* edge_next_host, const int32_t* default_next_host, int start) {
+    ZL_CHECK_ARG(m && task >= 0 && task < m->cfg.max_batch && n_states >= 0);
+    const int W = m->hwords, S = n_states;
+    if (S > 0 && !full_rows(m))
+        return fail_state(__LINE__, "zl_llama_set_constraint: tensor parallelism needs zl_llama_set_vocab_gather",
+                          ZL_ERR_UNSUPPORTED);
+    if (!m->d_cmask) return fail_state(__LINE__, "zl_llama_set_constraint needs zl_llama_enable_constraints");
+    if (S > 0) {
+        ZL_CHECK_ARG(S <= m->cons_max_states && n_edges >= 0 && n_edges <= m->cons_max_edges);
+        RCHECK(zl_token_automaton_check(m->cfg.vocab_size, S, masks_host, row_ptr_host, n_edges, edge_tok_host,
+                                        edge_next_host, default_next_host, start));
+    }
+    // stream-ordered after every step already enqueued; pageable sources are staged before the copies return
+    cudaStream_t st = m->stream;
+    const size_t MS = m->cons_max_states, ME = m->cons_max_edges;
+    const int32_t state = S > 0 ? start : -1;
+    if (S > 0) {
+        ZL_CHECK_CUDA(cudaMemcpyAsync(m->d_cmask.get() + task * MS * W, masks_host, (size_t)S * W * 4,
+                                      cudaMemcpyHostToDevice, st));
+        ZL_CHECK_CUDA(cudaMemcpyAsync(m->d_crow.get() + task * (MS + 1), row_ptr_host, (size_t)(S + 1) * 4,
+                                      cudaMemcpyHostToDevice, st));
+        ZL_CHECK_CUDA(cudaMemcpyAsync(m->d_cdflt.get() + task * MS, default_next_host, (size_t)S * 4,
+                                      cudaMemcpyHostToDevice, st));
+        if (n_edges > 0) {
+            ZL_CHECK_CUDA(cudaMemcpyAsync(m->d_cedge_tok.get() + task * ME, edge_tok_host, (size_t)n_edges * 4,
+                                          cudaMemcpyHostToDevice, st));
+            ZL_CHECK_CUDA(cudaMemcpyAsync(m->d_cedge_next.get() + task * ME, edge_next_host, (size_t)n_edges * 4,
+                                          cudaMemcpyHostToDevice, st));
+        }
+    }
+    ZL_CHECK_CUDA(cudaMemcpyAsync(m->d_cstate.get() + task, &state, 4, cudaMemcpyHostToDevice, st));
+    m->cons_on[task] = S > 0 ? 1 : 0;
+    m->samp_on[task] = m->pen_on[task] || m->proc_on[task] || m->cons_on[task];
+    return ZL_OK;
+}
+
+extern "C" int zl_llama_get_constraint_state(zl_llama_t* m, int32_t* states_host, int B) {
+    ZL_CHECK_ARG(m && states_host && B > 0 && B <= m->cfg.max_batch);
+    if (!m->d_cmask) return fail_state(__LINE__, "zl_llama_get_constraint_state needs zl_llama_enable_constraints");
+    ZL_CHECK_CUDA(cudaMemcpyAsync(m->h_stage.get(), m->d_cstate.get(), (size_t)B * 4, cudaMemcpyDeviceToHost, m->stream));
+    ZL_CHECK_CUDA(cudaStreamSynchronize(m->stream));
+    for (int i = 0; i < B; ++i) states_host[i] = m->h_stage.get()[i];
     return ZL_OK;
 }
 
@@ -2397,7 +2487,7 @@ extern "C" int zl_llama_beam_step(zl_llama_t* m, const int32_t* tokens, const in
     ZL_CHECK_SUPPORTED(B < 2048);   // the graph key holds B and G in 11 bits
     if (!m->finalized) return fail_state(__LINE__, "model not finalized");
     if (pick_of(m, 0, B).sampler)
-        return fail_state(__LINE__, "a task of the beam step samples, has penalties or has logits processors");
+        return fail_state(__LINE__, "a task of the beam step samples, has penalties, logits processors or a constraint");
     RCHECK(ensure_beam(m));
     const int MB = m->cfg.max_batch;
     int32_t* d = static_cast<int32_t*>(m->beam_d.get());

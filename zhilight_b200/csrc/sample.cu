@@ -19,6 +19,11 @@
 // apply_beam_repetition_penalty, src/generator/beam_util.cu:318-375) and logit_bias (SearcherImplV1::add_logit_bias,
 // batch_generator.cpp:1709-1728).  k_ngram_levels gives each distinct token of a task's generated sequence its largest
 // n-gram level, in a per-row hash table; k_sample then stages a processed copy of its slice in shared memory.
+//
+// Token automata (zl_sample_masked, zl_llama_set_constraint): a constrained row reads NaN for every token outside the
+// allowed set of its task's state (in the staging pass, or in pass 1 when no other processor stages the row) -- NaN is
+// never the greedy pick and has probability 0, exactly as a NaN logit -- and an allowed NaN logit as -inf, so that a row
+// whose allowed tokens all end at -inf picks the smallest allowed token.  The CTA that writes the pick moves the task's state along the automaton's edge of that token.
 #include "common.cuh"
 #include "sample.cuh"
 
@@ -215,6 +220,7 @@ struct SampleProc {
     int2* table;              // k_ngram_levels' output: per row, table_stride {token, level} slots
     int table_stride;
     const int32_t* frozen;    // (tasks) or NULL: a row whose task has frozen[task] != 0 records its pick nowhere
+    SampleAutomata au;        // au.mask NULL: no row is masked
 };
 
 constexpr int kNgramThreads = 1024;
@@ -322,17 +328,21 @@ __global__ void __cluster_dims__(kSampleCluster, 1, 1) __launch_bounds__(kSample
     const float* src = logits + (size_t)row * V + lo;
     const int nbias = pr.bias_tok ? min(pr.bias_cnt[task], pr.bias_stride) : 0;
     const float ngram = pr.ngram ? pr.ngram[task] : 1.f;
-    const bool proc = nbias > 0 || ngram > 1.f;
+    const int ast = pr.au.mask ? (pr.au.state ? pr.au.state[task] : task) : -1;
+    const uint32_t* amask = ast >= 0 ? pr.au.mask + ((size_t)task * pr.au.states + ast) * pr.au.words : nullptr;
+    const bool proc = nbias > 0 || ngram > 1.f;   // a row with only a mask applies it in pass 1, unstaged
     if (proc) {
         // this thread's first bias entry, loaded before the slice so that its latency overlaps the slice's
         const int32_t* bt = pr.bias_tok + (size_t)task * pr.bias_stride;
         const float* bv = pr.bias_val + (size_t)task * pr.bias_stride;
         const int g0 = tid < nbias ? bt[tid] : -1;
         const float b0 = tid < nbias ? bv[tid] : 0.f;
-        // the processed slice in shared memory: penalties (the n-gram rule replaces the bitmap rule), then the bias
+        // the processed slice in shared memory: the automaton's mask, penalties (the n-gram rule replaces the bitmap
+        // rule), then the bias
         for (int i = tid; i < n; i += kSampleThreads) {
             float l = src[i];
             const int g = lo + i;
+            if (amask) l = ((amask[g >> 5] >> (g & 31)) & 1u) ? (l == l ? l : -INFINITY) : NAN;
             if (!(ngram > 1.f) && pen && ((hist[g >> 5] >> (g & 31)) & 1u))
                 l = p.presence_penalty != 0.f ? l - p.presence_penalty
                                               : (l < 0.f ? l * p.repetition_penalty : l / p.repetition_penalty);
@@ -359,12 +369,14 @@ __global__ void __cluster_dims__(kSampleCluster, 1, 1) __launch_bounds__(kSample
         __syncthreads();
     }
 
-    // pass 1: penalties, the greedy pick of the penalised row (zl_argmax's rule: max, ties -> lowest index), max of x
+    // pass 1: the mask and penalties of an unstaged row, the greedy pick of the penalised row (zl_argmax's rule: max,
+    // ties -> lowest index), max of x
     float best = -INFINITY, xmax = -INFINITY;
     int bi = 0x7fffffff;
     for (int i = tid; i < n; i += kSampleThreads) {
         float l = proc ? xs[i] : src[i];
         const int g = lo + i;
+        if (!proc && amask) l = ((amask[g >> 5] >> (g & 31)) & 1u) ? (l == l ? l : -INFINITY) : NAN;
         if (!proc && pen && ((hist[g >> 5] >> (g & 31)) & 1u)) {   // beam_util.cu:212-219
             if (p.presence_penalty != 0.f)
                 l = l - p.presence_penalty;
@@ -547,6 +559,23 @@ __global__ void __cluster_dims__(kSampleCluster, 1, 1) __launch_bounds__(kSample
                 pr.seq_len[task] = len + 1;
             }
         }
+        // the automaton's move (every CTA of the cluster read the state before the first cluster barrier)
+        const int cur = pr.au.next ? pr.au.state[task] : -1;
+        if (cur >= 0 && record) {
+            const int32_t* rp = pr.au.row_ptr + (size_t)task * (pr.au.states + 1);
+            const int32_t* et = pr.au.edge_tok + (size_t)task * pr.au.max_edges;
+            int a = rp[cur], b = rp[cur + 1], nx = pr.au.dflt[(size_t)task * pr.au.states + cur];
+            while (a < b) {   // the state's edge tokens are sorted
+                const int mid = (a + b) >> 1, et_mid = et[mid];
+                if (et_mid == tok) {
+                    nx = pr.au.next[(size_t)task * pr.au.max_edges + mid];
+                    break;
+                }
+                if (et_mid < tok) a = mid + 1;
+                else b = mid;
+            }
+            pr.au.state[task] = nx;
+        }
     }
     cl.sync();   // no CTA leaves while another may still read its shared memory
 }
@@ -572,6 +601,31 @@ extern "C" int zl_sample_check_params(const zl_sample_params_t* p, int n) {
         ZL_CHECK_ARG(q.top_k >= 0);
         ZL_CHECK_ARG(q.repetition_penalty > 0.f && q.repetition_penalty < INFINITY);
         ZL_CHECK_ARG(q.presence_penalty > -INFINITY && q.presence_penalty < INFINITY);
+    }
+    return ZL_OK;
+}
+
+extern "C" int zl_token_automaton_check(int vocab, int n_states, const uint32_t* masks, const int32_t* row_ptr,
+                                        int n_edges, const int32_t* edge_tok, const int32_t* edge_next,
+                                        const int32_t* default_next, int start) {
+    ZL_CHECK_ARG(vocab > 0 && n_states >= 1 && n_edges >= 0);
+    ZL_CHECK_ARG(masks && row_ptr && default_next && (n_edges == 0 || (edge_tok && edge_next)));
+    ZL_CHECK_ARG(start >= 0 && start < n_states && row_ptr[0] == 0 && row_ptr[n_states] == n_edges);
+    for (int s = 0; s < n_states; ++s) ZL_CHECK_ARG(row_ptr[s] <= row_ptr[s + 1]);
+    const int W = cdiv(vocab, 32);
+    const uint32_t tail = vocab % 32 ? ~0u << (vocab % 32) : 0u;   // bits at or past vocab in the last word
+    for (int s = 0; s < n_states; ++s) {
+        const uint32_t* a = masks + (size_t)s * W;
+        uint32_t any = 0;
+        for (int i = 0; i < W; ++i) any |= a[i];
+        ZL_CHECK_ARG(any != 0 && (a[W - 1] & tail) == 0);
+        ZL_CHECK_ARG(default_next[s] >= 0 && default_next[s] < n_states);
+        for (int e = row_ptr[s]; e < row_ptr[s + 1]; ++e) {
+            const int x = edge_tok[e];
+            ZL_CHECK_ARG(x >= 0 && x < vocab && ((a[x >> 5] >> (x & 31)) & 1u));
+            ZL_CHECK_ARG(e == row_ptr[s] || edge_tok[e - 1] < x);
+            ZL_CHECK_ARG(edge_next[e] >= 0 && edge_next[e] < n_states);
+        }
     }
     return ZL_OK;
 }
@@ -622,8 +676,8 @@ int zl::sample_processed_launch(const float* logits, int T, int V, const zl_samp
                                 const int32_t* row_task, const int32_t* counter, uint32_t* history, int history_words,
                                 const float* ngram_penalty, int32_t* seq, int32_t* seq_len, int seq_stride,
                                 const int32_t* bias_tokens, const float* bias_values, const int32_t* bias_count,
-                                int bias_stride, const int32_t* frozen, int32_t* out, void* ws, size_t ws_bytes, int pdl,
-                                cudaStream_t stream) {
+                                int bias_stride, const int32_t* frozen, const SampleAutomata* au, int32_t* out, void* ws,
+                                size_t ws_bytes, int pdl, cudaStream_t stream) {
     ZL_CHECK_ARG(!seq || (seq_len && seq_stride > 0));
     ZL_CHECK_ARG(!ngram_penalty || (seq && ws && ws_bytes >= zl_sample_processed_workspace_bytes(T, seq_stride)));
     ZL_CHECK_ARG(!bias_tokens || (bias_values && bias_count && bias_stride > 0));
@@ -639,6 +693,11 @@ int zl::sample_processed_launch(const float* logits, int T, int V, const zl_samp
     pr.table = static_cast<int2*>(ws);
     pr.table_stride = seq_stride > 0 ? ngram_table_size(seq_stride) : 0;
     pr.frozen = frozen;
+    if (au) {
+        ZL_CHECK_ARG(au->mask && au->words >= cdiv(V, 32) && au->states >= 0);
+        ZL_CHECK_ARG(!au->next || (au->state && au->row_ptr && au->edge_tok && au->dflt && au->states > 0));
+        pr.au = *au;
+    }
     return sample_launch(logits, T, V, params, row_task, counter, history, history_words, pr, out, pdl, stream);
 }
 
@@ -648,6 +707,22 @@ extern "C" int zl_sample_processed(const float* logits, int T, int V, const zl_s
                                    const int32_t* bias_tokens, const float* bias_values, const int32_t* bias_count,
                                    int bias_stride, int32_t* out, void* ws, size_t ws_bytes, int pdl, zl_stream_t stream) {
     return sample_processed_launch(logits, T, V, params, row_task, counter, history, history_words, ngram_penalty, seq,
-                                   seq_len, seq_stride, bias_tokens, bias_values, bias_count, bias_stride, nullptr, out,
-                                   ws, ws_bytes, pdl, static_cast<cudaStream_t>(stream));
+                                   seq_len, seq_stride, bias_tokens, bias_values, bias_count, bias_stride, nullptr, nullptr,
+                                   out, ws, ws_bytes, pdl, static_cast<cudaStream_t>(stream));
+}
+
+extern "C" int zl_sample_masked(const float* logits, int T, int V, const zl_sample_params_t* params,
+                                const int32_t* row_task, const int32_t* counter, uint32_t* history, int history_words,
+                                const float* ngram_penalty, int32_t* seq, int32_t* seq_len, int seq_stride,
+                                const int32_t* bias_tokens, const float* bias_values, const int32_t* bias_count,
+                                int bias_stride, const uint32_t* masks, int mask_words, const int32_t* mask_row,
+                                int32_t* out, void* ws, size_t ws_bytes, int pdl, zl_stream_t stream) {
+    // mask row of task t: (t * 0 + mask_row[t]), or t when mask_row is NULL; no automaton moves
+    SampleAutomata au{};
+    au.mask = masks;
+    au.words = mask_words;
+    au.state = const_cast<int32_t*>(mask_row);   // read only: au.next is NULL
+    return sample_processed_launch(logits, T, V, params, row_task, counter, history, history_words, ngram_penalty, seq,
+                                   seq_len, seq_stride, bias_tokens, bias_values, bias_count, bias_stride, nullptr, &au,
+                                   out, ws, ws_bytes, pdl, static_cast<cudaStream_t>(stream));
 }

@@ -320,7 +320,7 @@ class LlamaDecoder:
         zl_llama_set_logits_processors); clears the task's penalty history and generated-token sequence.  Both are set on
         every call, so a reused task slot never keeps an earlier request's bias.  logit_bias: {token: bias} or None.
         As GeneratorArg (zhilight/dynamic_batch.py:110-111), ngram_penalty is 1 when presence_penalty != 0.
-        The defaults are plain greedy."""
+        The defaults are plain greedy.  A task's constraint (set_constraint) is left alone."""
         check_ngram_penalty(ngram_penalty)
         ngram = 1.0 if presence_penalty else float(ngram_penalty)
         toks, vals = logit_bias_arrays(logit_bias, self.cfg.vocab_size)
@@ -331,6 +331,31 @@ class LlamaDecoder:
         _lib.check(self.lib.zl_llama_set_sampling(self.h, int(task), ctypes.byref(p)))
         _lib.check(self.lib.zl_llama_set_logits_processors(self.h, int(task), ngram, toks.ctypes.data_as(ctypes.c_void_p),
                                                            vals.ctypes.data_as(ctypes.c_void_p), toks.size))
+
+    def enable_constraints(self, max_states, max_edges=0):
+        """Device storage for one token automaton per task of up to max_states states and max_edges edges
+        (zl_llama_enable_constraints); once per decoder."""
+        _lib.check(self.lib.zl_llama_enable_constraints(self.h, int(max_states), int(max_edges)))
+
+    def set_constraint(self, task, automaton):
+        """Constrain the picks of `task` by a constraints.TokenAutomaton from its start state, or clear its constraint
+        with None (zl_llama_set_constraint).  Every pick the task records is masked by its state's allowed set and moves
+        the state on the device, in decode, step_device, prefill, step_joined and generate alike."""
+        if automaton is None:
+            _lib.check(self.lib.zl_llama_set_constraint(self.h, int(task), 0, None, None, 0, None, None, None, 0))
+            return
+        a = automaton
+        if a.vocab_size != self.cfg.vocab_size:
+            raise ValueError("automaton over %d tokens for a %d-token model" % (a.vocab_size, self.cfg.vocab_size))
+        p = lambda x: x.ctypes.data_as(ctypes.c_void_p)
+        _lib.check(self.lib.zl_llama_set_constraint(self.h, int(task), a.n_states, p(a.masks), p(a.row_ptr), a.n_edges,
+                                                    p(a.edge_tok), p(a.edge_next), p(a.default_next), a.start))
+
+    def constraint_state(self, b):
+        """The automaton state of tasks 0 .. b-1 (-1: unconstrained), once every enqueued step has run."""
+        out = np.empty(int(b), np.int32)
+        _lib.check(self.lib.zl_llama_get_constraint_state(self.h, out.ctypes.data_as(ctypes.c_void_p), int(b)))
+        return out
 
     def read_kv(self, layer, task, row0, n):
         """Rows row0 .. row0 + n of a task's layer-`layer` KV cache (zl_llama_read_kv), each (n, H_kv, d).

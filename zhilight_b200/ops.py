@@ -571,6 +571,27 @@ def sample_processed(logits, params, seq, seq_len, ngram_penalty=None, bias_toke
     return out
 
 
+def sample_masked(logits, params, masks, mask_row=None, seq=None, seq_len=None, ngram_penalty=None, bias_tokens=None,
+                  bias_values=None, bias_count=None, row_task=None, counter=None, history=None, pdl=False):
+    """zl_sample_masked: ops.sample_processed with allowed-token masks.  masks (rows, ceil(V/32)) uint32 bitmasks as an
+    int32 CUDA tensor; mask_row (tasks) int32 (task t masked by row mask_row[t], unmasked when negative) or None (task t
+    by row t).  Without seq the tasks are the rows of masks (mask_row None) or of mask_row."""
+    t, v = logits.shape
+    n_tasks = seq.shape[0] if seq is not None else (mask_row.shape[0] if mask_row is not None else masks.shape[0])
+    stride = seq.shape[1] if seq is not None else 0
+    arr = sample_params_array(params, n_tasks)
+    dparams = torch.frombuffer(bytearray(bytes(arr)), dtype=torch.uint8).to(logits.device)
+    out = torch.empty(t, dtype=torch.int32, device=logits.device)
+    hw = history.shape[1] if history is not None else 0
+    nb = _lib.load().zl_sample_processed_workspace_bytes(t, stride) if ngram_penalty is not None else 0
+    ws = torch.empty(max(nb, 16), dtype=torch.uint8, device=logits.device) if nb else None
+    bstride = bias_tokens.shape[1] if bias_tokens is not None else 0
+    _lib.call("zl_sample_masked", _p(logits), t, v, _p(dparams), _p(row_task), _p(counter), _p(history), hw,
+              _p(ngram_penalty), _p(seq), _p(seq_len), stride, _p(bias_tokens), _p(bias_values), _p(bias_count), bstride,
+              _p(masks), masks.shape[1], _p(mask_row), _p(out), _p(ws), nb, int(pdl), _stream())
+    return out
+
+
 def beam_topk(logits, cum, groups, k, pdl=False):
     """zl_beam_topk: logits (R, V) fp32 and cum (R) fp32 CUDA tensors, groups (G, 2) {row0, width} host ints.
     -> (parent, token, score), each (G, k) on the device."""

@@ -154,6 +154,35 @@ struct GraphCache {
     }
 };
 
+// Every task's pick state: which parts of the sampler it uses and the sampler's device tables.
+//   sampling (zl_llama_set_sampling): parameters and generated-token bitmaps of hwords words
+//   logits processors (zl_llama_set_logits_processors): n-gram penalty, bias lists and the generated-token sequence
+//     (appended by the sampler where it sets the history bit, cleared with it); the n-gram workspace (k_ngram_levels'
+//     tables) is allocated by the first task that turns the n-gram rule on
+//   token automata (zl_llama_enable_constraints / zl_llama_set_constraint): au.states mask rows of hwords words, CSR
+//     edges (row offsets, tokens, next states), the default next states and the current state (-1: unconstrained)
+// `proc` points at the tables as k_sample reads them; a launch sets only its n-gram and frozen fields.
+struct TaskPicks {
+    enum : uint8_t { kSamples = 1, kProcessors = 2, kNgram = 4, kAutomaton = 8 };
+    std::vector<uint8_t> on;   // per task: kSamples (samples or has penalties), kProcessors, kNgram, kAutomaton
+    dev_ptr<zl_sample_params_t> params;   // (max_batch)
+    dev_ptr<uint32_t> hist;               // (max_batch, hwords)
+    int hwords = 0;
+    dev_ptr<float> ngram;                 // (max_batch)
+    dev_ptr<int32_t> seq, seq_len;        // (max_batch, max_seq), (max_batch)
+    dev_ptr<int32_t> bias_tok, bias_cnt;  // (max_batch, ZL_MAX_LOGIT_BIAS), (max_batch)
+    dev_ptr<float> bias_val;              // (max_batch, ZL_MAX_LOGIT_BIAS)
+    dev_ptr<> ngram_ws;
+    dev_ptr<uint32_t> mask;
+    dev_ptr<int32_t> row_ptr, edge_tok, edge_next, dflt, state;
+    zl::SampleProc proc{};
+
+    int alloc(int B, int vocab, int max_seq, cudaStream_t st);
+    int alloc_ngram(int B, int max_seq);
+    int alloc_automata(int B, int max_states, int max_edges, cudaStream_t st);
+    void set(int t, uint8_t bits, bool v) { on[t] = v ? on[t] | bits : on[t] & ~bits; }
+};
+
 }  // namespace
 
 struct zl_llama {
@@ -211,30 +240,8 @@ struct zl_llama {
     dev_ptr<int32_t> d_join;
     host_ptr<int32_t> h_join;
     dev_ptr<> xperm;           // act-order: activations permuted for the GEMM routes that cannot gather (tok_cap x max K)
-    // sampling (zl_llama_set_sampling): per-task parameters and generated-token bitmaps on the device; samp_on[t] is set
-    // while task t samples or has penalties, and the step then runs zl_sample instead of zl_argmax
-    dev_ptr<zl_sample_params_t> d_sparams;   // (max_batch)
-    dev_ptr<uint32_t> d_hist;                // (max_batch, hwords)
-    int hwords = 0;
-    std::vector<char> samp_on;               // pen_on[t] || proc_on[t] || cons_on[t]
-    std::vector<char> pen_on;                // set by zl_llama_set_sampling: samples or has penalties
-    // logits processors (zl_llama_set_logits_processors): per-task n-gram penalty and bias lists, and every task's
-    // generated-token sequence (appended by the sampler where it sets the history bit, cleared with it); the n-gram
-    // workspace (k_ngram_levels' tables, max_batch rows) is allocated by the first task that turns the n-gram rule on
-    dev_ptr<float> d_ngram;                  // (max_batch)
-    dev_ptr<int32_t> d_seq, d_seq_len;       // (max_batch, max_seq), (max_batch)
-    dev_ptr<int32_t> d_bias_tok, d_bias_cnt; // (max_batch, ZL_MAX_LOGIT_BIAS), (max_batch)
-    dev_ptr<float> d_bias_val;               // (max_batch, ZL_MAX_LOGIT_BIAS)
-    dev_ptr<> ngram_ws;
-    size_t ngram_ws_bytes = 0;
-    std::vector<char> proc_on, ngram_on;
-    // token automata (zl_llama_enable_constraints / zl_llama_set_constraint): per task, cons_max_states mask rows of
-    // hwords words, CSR edges (row offsets, tokens, next states), the default next states and the current state (-1:
-    // unconstrained), laid out as SampleAutomata reads them; cons_on[t] while task t has an automaton
-    dev_ptr<uint32_t> d_cmask;
-    dev_ptr<int32_t> d_crow, d_cedge_tok, d_cedge_next, d_cdflt, d_cstate;
-    int cons_max_states = 0, cons_max_edges = 0;
-    std::vector<char> cons_on;
+    // a step whose tasks use none of the sampler runs zl_argmax
+    TaskPicks picks;
     // int8 KV cache: the rotated fp16 K / V rows of the launch sequence are staged in kv_stage (k: tok_cap x Hkv x d, then
     // v) and quantised into the cache from there.  A qkv GEMM with the RoPE / KV-append epilogue appends into the staging
     // rows as into the cache of one task: stage_addrs = {k rows, v rows}, token -> task map d_zeros, placement d_rowidx.
@@ -304,6 +311,55 @@ int StageRing::acquire(int32_t** hs, int32_t** ds) {
 int StageRing::release(cudaStream_t st) {
     ZL_CHECK_CUDA(cudaEventRecord(ev[cur], st));
     used[cur] = true;
+    return ZL_OK;
+}
+
+// every task greedy, unpenalised, without processors
+int TaskPicks::alloc(int B, int vocab, int max_seq, cudaStream_t st) {
+    hwords = cdiv(vocab, 32);   // the sampler reads whole rows: the gathered ones under tensor parallelism
+    RCHECK(dmalloc(&hist, (size_t)B * hwords * 4));
+    ZL_CHECK_CUDA(cudaMemsetAsync(hist.get(), 0, (size_t)B * hwords * 4, st));
+    RCHECK(dmalloc(&params, sizeof(zl_sample_params_t) * B));
+    {
+        const zl_sample_params_t greedy{0.f, 1.f, 1.f, 0.f, 0, 0};
+        std::vector<zl_sample_params_t> init(B, greedy);
+        ZL_CHECK_CUDA(cudaMemcpyAsync(params.get(), init.data(), sizeof(zl_sample_params_t) * B, cudaMemcpyHostToDevice, st));
+        ZL_CHECK_CUDA(cudaStreamSynchronize(st));   // `init` is pageable and goes out of scope
+    }
+    on.assign(B, 0);
+    RCHECK(dmalloc(&ngram, (size_t)B * 4));
+    RCHECK(dmalloc(&seq, (size_t)B * max_seq * 4));
+    RCHECK(dmalloc(&seq_len, (size_t)B * 4));
+    RCHECK(dmalloc(&bias_tok, (size_t)B * ZL_MAX_LOGIT_BIAS * 4));
+    RCHECK(dmalloc(&bias_val, (size_t)B * ZL_MAX_LOGIT_BIAS * 4));
+    RCHECK(dmalloc(&bias_cnt, (size_t)B * 4));
+    ZL_CHECK_CUDA(cudaMemsetAsync(ngram.get(), 0, (size_t)B * 4, st));   // 0.0f: off
+    ZL_CHECK_CUDA(cudaMemsetAsync(seq_len.get(), 0, (size_t)B * 4, st));
+    ZL_CHECK_CUDA(cudaMemsetAsync(bias_cnt.get(), 0, (size_t)B * 4, st));
+    proc = SampleProc{ngram.get(), seq.get(), seq_len.get(), max_seq, bias_tok.get(), bias_val.get(), bias_cnt.get(),
+                      ZL_MAX_LOGIT_BIAS, nullptr, ngram_table_size(max_seq)};
+    return ZL_OK;
+}
+
+// B rows of tables: no launch has more rows than tasks
+int TaskPicks::alloc_ngram(int B, int max_seq) {
+    RCHECK(dmalloc(&ngram_ws, zl_sample_processed_workspace_bytes(B, max_seq)));
+    proc.table = static_cast<int2*>(ngram_ws.get());
+    return ZL_OK;
+}
+
+int TaskPicks::alloc_automata(int B, int max_states, int max_edges, cudaStream_t st) {
+    const size_t S = max_states;
+    RCHECK(dmalloc(&mask, B * S * hwords * 4));
+    RCHECK(dmalloc(&row_ptr, B * (S + 1) * 4));
+    RCHECK(dmalloc(&edge_tok, (size_t)B * max_edges * 4));
+    RCHECK(dmalloc(&edge_next, (size_t)B * max_edges * 4));
+    RCHECK(dmalloc(&dflt, B * S * 4));
+    RCHECK(dmalloc(&state, (size_t)B * 4));
+    ZL_CHECK_CUDA(cudaMemsetAsync(state.get(), 0xff, (size_t)B * 4, st));   // -1: unconstrained
+    ZL_CHECK_CUDA(cudaStreamSynchronize(st));
+    proc.au = SampleAutomata{mask.get(), state.get(), hwords, max_states, max_edges, row_ptr.get(), edge_tok.get(),
+                             edge_next.get(), dflt.get()};
     return ZL_OK;
 }
 
@@ -972,31 +1028,7 @@ int alloc_runtime(zl_llama* m) {
     }
     RCHECK(dmalloc(&m->attn_ws, m->attn_ws_bytes));
     RCHECK(dmalloc(&m->argmax_ws, zl_argmax_workspace_bytes(B)));
-    m->hwords = cdiv(c.vocab_size, 32);   // the sampler reads whole rows: the gathered ones under tensor parallelism
-    RCHECK(dmalloc(&m->d_hist, (size_t)B * m->hwords * 4));
-    ZL_CHECK_CUDA(cudaMemsetAsync(m->d_hist.get(), 0, (size_t)B * m->hwords * 4, m->stream));
-    RCHECK(dmalloc(&m->d_sparams, sizeof(zl_sample_params_t) * B));
-    {
-        const zl_sample_params_t greedy{0.f, 1.f, 1.f, 0.f, 0, 0};
-        std::vector<zl_sample_params_t> init(B, greedy);
-        ZL_CHECK_CUDA(cudaMemcpyAsync(m->d_sparams.get(), init.data(), sizeof(zl_sample_params_t) * B, cudaMemcpyHostToDevice,
-                                      m->stream));
-        ZL_CHECK_CUDA(cudaStreamSynchronize(m->stream));   // `init` is pageable and goes out of scope
-    }
-    m->samp_on.assign(B, 0);
-    m->pen_on.assign(B, 0);
-    m->proc_on.assign(B, 0);
-    m->ngram_on.assign(B, 0);
-    m->cons_on.assign(B, 0);
-    RCHECK(dmalloc(&m->d_ngram, (size_t)B * 4));
-    RCHECK(dmalloc(&m->d_seq, (size_t)B * c.max_seq * 4));
-    RCHECK(dmalloc(&m->d_seq_len, (size_t)B * 4));
-    RCHECK(dmalloc(&m->d_bias_tok, (size_t)B * ZL_MAX_LOGIT_BIAS * 4));
-    RCHECK(dmalloc(&m->d_bias_val, (size_t)B * ZL_MAX_LOGIT_BIAS * 4));
-    RCHECK(dmalloc(&m->d_bias_cnt, (size_t)B * 4));
-    ZL_CHECK_CUDA(cudaMemsetAsync(m->d_ngram.get(), 0, (size_t)B * 4, m->stream));   // 0.0f: off
-    ZL_CHECK_CUDA(cudaMemsetAsync(m->d_seq_len.get(), 0, (size_t)B * 4, m->stream));
-    ZL_CHECK_CUDA(cudaMemsetAsync(m->d_bias_cnt.get(), 0, (size_t)B * 4, m->stream));
+    RCHECK(m->picks.alloc(B, c.vocab_size, c.max_seq, m->stream));
     RCHECK(alloc_generate(m));
     int32_t* stage = nullptr;
     ZL_CHECK_CUDA(cudaMallocHost((void**)&stage, sizeof(int32_t) * (4 * B + 4 + T)));
@@ -1461,13 +1493,19 @@ struct Pick {
 
     // task t samples (or has penalties, logits processors or an automaton), and has the n-gram rule on
     void add(const zl_llama* m, int t) {
-        sampler |= m->samp_on[t] != 0;
-        ngram |= m->ngram_on[t] != 0;
+        sampler |= m->picks.on[t] != 0;
+        ngram |= (m->picks.on[t] & TaskPicks::kNgram) != 0;
     }
 };
 
 // the sampler and the beam selection can see whole vocabulary rows: a single rank, or the vocabulary all-gather
 bool full_rows(const zl_llama* m) { return m->cfg.tp_size == 1 || m->vgather; }
+
+// refuses `what` (with `code`) on a rank that holds only its shard of the vocabulary rows
+int need_full_rows(const zl_llama* m, const char* what, int code = ZL_ERR_UNSUPPORTED) {
+    if (full_rows(m)) return ZL_OK;
+    return fail_state(__LINE__, std::string(what) + " under tensor parallelism needs zl_llama_set_vocab_gather", code);
+}
 
 // the pick of tasks first .. first + n - 1
 Pick pick_of(const zl_llama* m, int first, int n) {
@@ -1579,7 +1617,7 @@ int enqueue_step(zl_llama* m, int n_tasks, int len_bucket, const Segments* pf, c
     // picks the same tokens from the same rows (both are deterministic), so no pick is broadcast
     const float* rows_v = m->logits.get();
     if (tp && (pk.beam || pk.sampler)) {
-        if (!m->vgather) return fail_state(__LINE__, "a sampled or beam pick under tp_size > 1 needs zl_llama_set_vocab_gather");
+        RCHECK(need_full_rows(m, "a sampled or beam pick", ZL_ERR_STATE));
         RCHECK(zl_vocab_allgather(m->vgather, m->logits.get(), HB, m->vshard, pdl, st));
         rows_v = zl_vocab_gather_buffer(m->vgather);
     }
@@ -1594,22 +1632,14 @@ int enqueue_step(zl_llama* m, int n_tasks, int len_bucket, const Segments* pf, c
         const int32_t* counter = joined ? j_pos : pf ? m->d_pf_pos.get() + (pf->n - 1) : m->d_pos.get();
         // k_ngram_levels runs only when a task of the step has the n-gram rule on (`pk.ngram`, a bit of the graph key)
         // with automata enabled every sampler launch reads the tasks' states (-1: unconstrained), so no key bit is needed
-        SampleAutomata au{};
-        au.mask = m->d_cmask.get();
-        au.state = m->d_cstate.get();
-        au.words = m->hwords;
-        au.states = m->cons_max_states;
-        au.max_edges = m->cons_max_edges;
-        au.row_ptr = m->d_crow.get();
-        au.edge_tok = m->d_cedge_tok.get();
-        au.next = m->d_cedge_next.get();
-        au.dflt = m->d_cdflt.get();
-        RCHECK(sample_processed_launch(rows_v, HB, c.vocab_size, m->d_sparams.get(), row_task, counter,
-                                       m->d_hist.get(), m->hwords, pk.ngram ? m->d_ngram.get() : nullptr, m->d_seq.get(),
-                                       m->d_seq_len.get(), c.max_seq, m->d_bias_tok.get(), m->d_bias_val.get(),
-                                       m->d_bias_cnt.get(), ZL_MAX_LOGIT_BIAS, pk.frozen, m->d_cmask ? &au : nullptr,
-                                       m->d_next.get(),
-                                       pk.ngram ? m->ngram_ws.get() : nullptr, m->ngram_ws_bytes, stage_pdl(m, kPick), st));
+        SampleProc pr = m->picks.proc;
+        if (!pk.ngram) {
+            pr.ngram = nullptr;
+            pr.table = nullptr;
+        }
+        pr.frozen = pk.frozen;
+        RCHECK(sample_launch(rows_v, HB, c.vocab_size, m->picks.params.get(), row_task, counter, m->picks.hist.get(),
+                             m->picks.hwords, pr, m->d_next.get(), stage_pdl(m, kPick), st));
     } else if (!tp) {
         RCHECK(zl_argmax(m->logits.get(), m->d_next.get(), HB, m->vshard, m->argmax_ws.get(), zl_argmax_workspace_bytes(HB),
                          stage_pdl(m, kPick), st));
@@ -2125,15 +2155,15 @@ extern "C" int zl_llama_set_sampling(zl_llama_t* m, int task, const zl_sample_pa
     ZL_CHECK_ARG(m && task >= 0 && task < m->cfg.max_batch);
     const bool on = p && ((p->temperature > 0.f && p->top_k != 1) || p->repetition_penalty != 1.f ||
                           p->presence_penalty != 0.f);
-    ZL_CHECK_SUPPORTED(!on || full_rows(m));
+    if (on) RCHECK(need_full_rows(m, "zl_llama_set_sampling"));
     if (!m->finalized) return fail_state(__LINE__, "model not finalized");
+    TaskPicks& picks = m->picks;
     const zl_sample_params_t q = p ? *p : zl_sample_params_t{0.f, 1.f, 1.f, 0.f, 0, 0};
     // stream-ordered after every step already enqueued; the pageable source is staged before the call returns
-    ZL_CHECK_CUDA(cudaMemcpyAsync(m->d_sparams.get() + task, &q, sizeof(q), cudaMemcpyHostToDevice, m->stream));
-    ZL_CHECK_CUDA(cudaMemsetAsync(m->d_hist.get() + (size_t)task * m->hwords, 0, (size_t)m->hwords * 4, m->stream));
-    ZL_CHECK_CUDA(cudaMemsetAsync(m->d_seq_len.get() + task, 0, 4, m->stream));
-    m->pen_on[task] = on ? 1 : 0;
-    m->samp_on[task] = m->pen_on[task] || m->proc_on[task] || m->cons_on[task];
+    ZL_CHECK_CUDA(cudaMemcpyAsync(picks.params.get() + task, &q, sizeof(q), cudaMemcpyHostToDevice, m->stream));
+    ZL_CHECK_CUDA(cudaMemsetAsync(picks.hist.get() + (size_t)task * picks.hwords, 0, (size_t)picks.hwords * 4, m->stream));
+    ZL_CHECK_CUDA(cudaMemsetAsync(picks.seq_len.get() + task, 0, 4, m->stream));
+    picks.set(task, TaskPicks::kSamples, on);
     return ZL_OK;
 }
 
@@ -2151,43 +2181,30 @@ extern "C" int zl_llama_set_logits_processors(zl_llama_t* m, int task, float ngr
     std::sort(sorted.begin(), sorted.end());
     ZL_CHECK_ARG(std::adjacent_find(sorted.begin(), sorted.end()) == sorted.end());
     const bool ngram = ngram_penalty > 1.f, on = ngram || n_bias > 0;
-    ZL_CHECK_SUPPORTED(!on || full_rows(m));
+    if (on) RCHECK(need_full_rows(m, "zl_llama_set_logits_processors"));
     if (!m->finalized) return fail_state(__LINE__, "model not finalized");
-    if (ngram && !m->ngram_ws) {
-        m->ngram_ws_bytes = zl_sample_processed_workspace_bytes(m->cfg.max_batch, m->cfg.max_seq);
-        RCHECK(dmalloc(&m->ngram_ws, m->ngram_ws_bytes));
-    }
+    TaskPicks& picks = m->picks;
+    if (ngram && !picks.ngram_ws) RCHECK(picks.alloc_ngram(m->cfg.max_batch, m->cfg.max_seq));
     // stream-ordered after every step already enqueued; pageable sources are staged before the copies return
     cudaStream_t st = m->stream;
-    ZL_CHECK_CUDA(cudaMemcpyAsync(m->d_ngram.get() + task, &ngram_penalty, 4, cudaMemcpyHostToDevice, st));
+    ZL_CHECK_CUDA(cudaMemcpyAsync(picks.ngram.get() + task, &ngram_penalty, 4, cudaMemcpyHostToDevice, st));
     if (n_bias > 0) {
-        ZL_CHECK_CUDA(cudaMemcpyAsync(m->d_bias_tok.get() + (size_t)task * ZL_MAX_LOGIT_BIAS, bias_tokens_host,
+        ZL_CHECK_CUDA(cudaMemcpyAsync(picks.bias_tok.get() + (size_t)task * ZL_MAX_LOGIT_BIAS, bias_tokens_host,
                                       (size_t)n_bias * 4, cudaMemcpyHostToDevice, st));
-        ZL_CHECK_CUDA(cudaMemcpyAsync(m->d_bias_val.get() + (size_t)task * ZL_MAX_LOGIT_BIAS, bias_values_host,
+        ZL_CHECK_CUDA(cudaMemcpyAsync(picks.bias_val.get() + (size_t)task * ZL_MAX_LOGIT_BIAS, bias_values_host,
                                       (size_t)n_bias * 4, cudaMemcpyHostToDevice, st));
     }
-    ZL_CHECK_CUDA(cudaMemcpyAsync(m->d_bias_cnt.get() + task, &n_bias, 4, cudaMemcpyHostToDevice, st));
-    m->proc_on[task] = on ? 1 : 0;
-    m->ngram_on[task] = ngram ? 1 : 0;
-    m->samp_on[task] = m->pen_on[task] || m->proc_on[task] || m->cons_on[task];
+    ZL_CHECK_CUDA(cudaMemcpyAsync(picks.bias_cnt.get() + task, &n_bias, 4, cudaMemcpyHostToDevice, st));
+    picks.set(task, TaskPicks::kProcessors, on);
+    picks.set(task, TaskPicks::kNgram, ngram);
     return ZL_OK;
 }
 
 extern "C" int zl_llama_enable_constraints(zl_llama_t* m, int max_states, int max_edges) {
     ZL_CHECK_ARG(m && max_states >= 1 && max_edges >= 0);
     if (!m->finalized) return fail_state(__LINE__, "model not finalized");
-    if (m->d_cmask) return fail_state(__LINE__, "zl_llama_enable_constraints was already called");
-    const size_t B = m->cfg.max_batch, S = max_states;
-    RCHECK(dmalloc(&m->d_cmask, B * S * m->hwords * 4));
-    RCHECK(dmalloc(&m->d_crow, B * (S + 1) * 4));
-    RCHECK(dmalloc(&m->d_cedge_tok, B * max_edges * 4));
-    RCHECK(dmalloc(&m->d_cedge_next, B * max_edges * 4));
-    RCHECK(dmalloc(&m->d_cdflt, B * S * 4));
-    RCHECK(dmalloc(&m->d_cstate, B * 4));
-    ZL_CHECK_CUDA(cudaMemsetAsync(m->d_cstate.get(), 0xff, B * 4, m->stream));   // -1: unconstrained
-    ZL_CHECK_CUDA(cudaStreamSynchronize(m->stream));
-    m->cons_max_states = max_states;
-    m->cons_max_edges = max_edges;
+    if (m->picks.mask) return fail_state(__LINE__, "zl_llama_enable_constraints was already called");
+    RCHECK(m->picks.alloc_automata(m->cfg.max_batch, max_states, max_edges, m->stream));
     // the sampler launches captured so far carry no automata
     m->graphs.clear();
     m->gen_graphs.clear();
@@ -2198,44 +2215,42 @@ extern "C" int zl_llama_set_constraint(zl_llama_t* m, int task, int n_states, co
                                        const int32_t* row_ptr_host, int n_edges, const int32_t* edge_tok_host,
                                        const int32_t* edge_next_host, const int32_t* default_next_host, int start) {
     ZL_CHECK_ARG(m && task >= 0 && task < m->cfg.max_batch && n_states >= 0);
-    const int W = m->hwords, S = n_states;
-    if (S > 0 && !full_rows(m))
-        return fail_state(__LINE__, "zl_llama_set_constraint: tensor parallelism needs zl_llama_set_vocab_gather",
-                          ZL_ERR_UNSUPPORTED);
-    if (!m->d_cmask) return fail_state(__LINE__, "zl_llama_set_constraint needs zl_llama_enable_constraints");
+    TaskPicks& picks = m->picks;
+    const int W = picks.hwords, S = n_states;
+    if (S > 0) RCHECK(need_full_rows(m, "zl_llama_set_constraint"));
+    if (!picks.mask) return fail_state(__LINE__, "zl_llama_set_constraint needs zl_llama_enable_constraints");
     if (S > 0) {
-        ZL_CHECK_ARG(S <= m->cons_max_states && n_edges >= 0 && n_edges <= m->cons_max_edges);
+        ZL_CHECK_ARG(S <= picks.proc.au.states && n_edges >= 0 && n_edges <= picks.proc.au.max_edges);
         RCHECK(zl_token_automaton_check(m->cfg.vocab_size, S, masks_host, row_ptr_host, n_edges, edge_tok_host,
                                         edge_next_host, default_next_host, start));
     }
     // stream-ordered after every step already enqueued; pageable sources are staged before the copies return
     cudaStream_t st = m->stream;
-    const size_t MS = m->cons_max_states, ME = m->cons_max_edges;
+    const size_t MS = picks.proc.au.states, ME = picks.proc.au.max_edges;
     const int32_t state = S > 0 ? start : -1;
     if (S > 0) {
-        ZL_CHECK_CUDA(cudaMemcpyAsync(m->d_cmask.get() + task * MS * W, masks_host, (size_t)S * W * 4,
+        ZL_CHECK_CUDA(cudaMemcpyAsync(picks.mask.get() + task * MS * W, masks_host, (size_t)S * W * 4,
                                       cudaMemcpyHostToDevice, st));
-        ZL_CHECK_CUDA(cudaMemcpyAsync(m->d_crow.get() + task * (MS + 1), row_ptr_host, (size_t)(S + 1) * 4,
+        ZL_CHECK_CUDA(cudaMemcpyAsync(picks.row_ptr.get() + task * (MS + 1), row_ptr_host, (size_t)(S + 1) * 4,
                                       cudaMemcpyHostToDevice, st));
-        ZL_CHECK_CUDA(cudaMemcpyAsync(m->d_cdflt.get() + task * MS, default_next_host, (size_t)S * 4,
+        ZL_CHECK_CUDA(cudaMemcpyAsync(picks.dflt.get() + task * MS, default_next_host, (size_t)S * 4,
                                       cudaMemcpyHostToDevice, st));
         if (n_edges > 0) {
-            ZL_CHECK_CUDA(cudaMemcpyAsync(m->d_cedge_tok.get() + task * ME, edge_tok_host, (size_t)n_edges * 4,
+            ZL_CHECK_CUDA(cudaMemcpyAsync(picks.edge_tok.get() + task * ME, edge_tok_host, (size_t)n_edges * 4,
                                           cudaMemcpyHostToDevice, st));
-            ZL_CHECK_CUDA(cudaMemcpyAsync(m->d_cedge_next.get() + task * ME, edge_next_host, (size_t)n_edges * 4,
+            ZL_CHECK_CUDA(cudaMemcpyAsync(picks.edge_next.get() + task * ME, edge_next_host, (size_t)n_edges * 4,
                                           cudaMemcpyHostToDevice, st));
         }
     }
-    ZL_CHECK_CUDA(cudaMemcpyAsync(m->d_cstate.get() + task, &state, 4, cudaMemcpyHostToDevice, st));
-    m->cons_on[task] = S > 0 ? 1 : 0;
-    m->samp_on[task] = m->pen_on[task] || m->proc_on[task] || m->cons_on[task];
+    ZL_CHECK_CUDA(cudaMemcpyAsync(picks.state.get() + task, &state, 4, cudaMemcpyHostToDevice, st));
+    picks.set(task, TaskPicks::kAutomaton, S > 0);
     return ZL_OK;
 }
 
 extern "C" int zl_llama_get_constraint_state(zl_llama_t* m, int32_t* states_host, int B) {
     ZL_CHECK_ARG(m && states_host && B > 0 && B <= m->cfg.max_batch);
-    if (!m->d_cmask) return fail_state(__LINE__, "zl_llama_get_constraint_state needs zl_llama_enable_constraints");
-    ZL_CHECK_CUDA(cudaMemcpyAsync(m->h_stage.get(), m->d_cstate.get(), (size_t)B * 4, cudaMemcpyDeviceToHost, m->stream));
+    if (!m->picks.mask) return fail_state(__LINE__, "zl_llama_get_constraint_state needs zl_llama_enable_constraints");
+    ZL_CHECK_CUDA(cudaMemcpyAsync(m->h_stage.get(), m->picks.state.get(), (size_t)B * 4, cudaMemcpyDeviceToHost, m->stream));
     ZL_CHECK_CUDA(cudaStreamSynchronize(m->stream));
     for (int i = 0; i < B; ++i) states_host[i] = m->h_stage.get()[i];
     return ZL_OK;
@@ -2482,8 +2497,7 @@ extern "C" int zl_llama_beam_step(zl_llama_t* m, const int32_t* tokens, const in
     ZL_CHECK_ARG(B > 0 && B <= m->cfg.max_batch);
     RCHECK(beam_topk_check(B, full_rows(m) ? m->cfg.vocab_size : m->vshard, groups, G, K));
     for (int i = 0; i < B; ++i) ZL_CHECK_ARG(cum[i] < INFINITY);   // -inf: a dead row; NaN and +inf are refused
-    if (!full_rows(m))
-        return fail_state(__LINE__, "beam steps under tensor parallelism need zl_llama_set_vocab_gather", ZL_ERR_UNSUPPORTED);
+    RCHECK(need_full_rows(m, "zl_llama_beam_step"));
     ZL_CHECK_SUPPORTED(B < 2048);   // the graph key holds B and G in 11 bits
     if (!m->finalized) return fail_state(__LINE__, "model not finalized");
     if (pick_of(m, 0, B).sampler)
@@ -2736,8 +2750,7 @@ extern "C" int zl_llama_set_stop(zl_llama_t* m, int task, const int32_t* stop_id
     }
     r.n = n_stop;
     r.budget = max_new_tokens;
-    if (!full_rows(m))
-        return fail_state(__LINE__, "zl_llama_set_stop: tensor parallelism needs zl_llama_set_vocab_gather", ZL_ERR_UNSUPPORTED);
+    RCHECK(need_full_rows(m, "zl_llama_set_stop"));
     if (!m->finalized) return fail_state(__LINE__, "model not finalized");
     // stream-ordered after every step already enqueued; the rule travels as a kernel argument
     k_gen_arm<<<1, 1, 0, m->stream>>>(gen_state(m), task, r);
@@ -2751,8 +2764,7 @@ extern "C" int zl_llama_generate(zl_llama_t* m, int B, int max_steps, int32_t* t
     ZL_CHECK_ARG(m && tokens_host && n_out_host && finish_host && steps_host);
     const auto& c = m->cfg;
     ZL_CHECK_ARG(B > 0 && B <= c.max_batch && max_steps >= 1 && max_steps <= c.max_seq);
-    if (!full_rows(m))
-        return fail_state(__LINE__, "zl_llama_generate: tensor parallelism needs zl_llama_set_vocab_gather", ZL_ERR_UNSUPPORTED);
+    RCHECK(need_full_rows(m, "zl_llama_generate"));
     if (!c.use_graph) return fail_state(__LINE__, "zl_llama_generate runs as a CUDA graph (use_graph = 0)", ZL_ERR_UNSUPPORTED);
     if (!m->finalized) return fail_state(__LINE__, "model not finalized");
     const int MB = c.max_batch;

@@ -207,31 +207,8 @@ __device__ SelResult cluster_select(SampleShared& s, cg::cluster_group& cl, cons
     return r;
 }
 
-// The processors' device arguments (zl_sample_processed); all NULL for zl_sample.
-struct SampleProc {
-    const float* ngram;       // (tasks) or NULL: no n-gram rule
-    int32_t* seq;             // (tasks, seq_stride) generated tokens, oldest first, or NULL
-    int32_t* seq_len;         // (tasks)
-    int seq_stride;
-    const int32_t* bias_tok;  // (tasks, bias_stride) or NULL
-    const float* bias_val;
-    const int32_t* bias_cnt;  // (tasks)
-    int bias_stride;
-    int2* table;              // k_ngram_levels' output: per row, table_stride {token, level} slots
-    int table_stride;
-    const int32_t* frozen;    // (tasks) or NULL: a row whose task has frozen[task] != 0 records its pick nowhere
-    SampleAutomata au;        // au.mask NULL: no row is masked
-};
-
 constexpr int kNgramThreads = 1024;
 constexpr int kNgramSmem = 12032;   // sequence elements staged in shared memory; the rest is read from global memory
-
-// hash table slots for n distinct tokens at most: a power of two >= 2n, so an insert always finds a free slot
-__host__ __device__ inline int ngram_table_size(int n) {
-    int h = 2;
-    while (h < 2 * n) h <<= 1;
-    return h;
-}
 
 // Fibonacci hashing: the top log2(h) bits of tok * 2^32 / phi (h is a power of two >= 2)
 __device__ __forceinline__ int ngram_slot(int tok, int h) {
@@ -641,10 +618,15 @@ int prepare_sample() {
     return ZL_OK;
 }
 
-// the one launcher behind zl_sample and zl_sample_processed
-static int sample_launch(const float* logits, int T, int V, const zl_sample_params_t* params, const int32_t* row_task,
-                  const int32_t* counter, uint32_t* history, int history_words, const SampleProc& pr, int32_t* out,
-                  int pdl, cudaStream_t stream) {
+int zl::sample_launch(const float* logits, int T, int V, const zl_sample_params_t* params, const int32_t* row_task,
+                      const int32_t* counter, uint32_t* history, int history_words, const SampleProc& pr, int32_t* out,
+                      int pdl, cudaStream_t stream) {
+    ZL_CHECK_ARG(!pr.seq || (pr.seq_len && pr.seq_stride > 0));
+    ZL_CHECK_ARG(!pr.ngram || (pr.seq && pr.table));
+    ZL_CHECK_ARG(!pr.bias_tok || (pr.bias_val && pr.bias_cnt && pr.bias_stride > 0));
+    ZL_CHECK_ARG(!pr.au.mask || (pr.au.words >= cdiv(V, 32) && pr.au.states >= 0));
+    ZL_CHECK_ARG(!pr.au.next || (pr.au.mask && pr.au.state && pr.au.row_ptr && pr.au.edge_tok && pr.au.dflt &&
+                                 pr.au.states > 0));
     ZL_CHECK_ARG(logits && params && out && T > 0 && V > 0);
     ZL_CHECK_SUPPORTED(V <= kSampleMaxVocab);
     ZL_CHECK_ARG(!history || history_words >= cdiv(V, 32));
@@ -672,43 +654,16 @@ extern "C" size_t zl_sample_processed_workspace_bytes(int T, int seq_stride) {
     return (size_t)T * ngram_table_size(seq_stride) * sizeof(int2);
 }
 
-int zl::sample_processed_launch(const float* logits, int T, int V, const zl_sample_params_t* params,
-                                const int32_t* row_task, const int32_t* counter, uint32_t* history, int history_words,
-                                const float* ngram_penalty, int32_t* seq, int32_t* seq_len, int seq_stride,
-                                const int32_t* bias_tokens, const float* bias_values, const int32_t* bias_count,
-                                int bias_stride, const int32_t* frozen, const SampleAutomata* au, int32_t* out, void* ws,
-                                size_t ws_bytes, int pdl, cudaStream_t stream) {
-    ZL_CHECK_ARG(!seq || (seq_len && seq_stride > 0));
-    ZL_CHECK_ARG(!ngram_penalty || (seq && ws && ws_bytes >= zl_sample_processed_workspace_bytes(T, seq_stride)));
-    ZL_CHECK_ARG(!bias_tokens || (bias_values && bias_count && bias_stride > 0));
-    SampleProc pr{};
-    pr.ngram = ngram_penalty;
-    pr.seq = seq;
-    pr.seq_len = seq_len;
-    pr.seq_stride = seq_stride;
-    pr.bias_tok = bias_tokens;
-    pr.bias_val = bias_values;
-    pr.bias_cnt = bias_count;
-    pr.bias_stride = bias_stride;
-    pr.table = static_cast<int2*>(ws);
-    pr.table_stride = seq_stride > 0 ? ngram_table_size(seq_stride) : 0;
-    pr.frozen = frozen;
-    if (au) {
-        ZL_CHECK_ARG(au->mask && au->words >= cdiv(V, 32) && au->states >= 0);
-        ZL_CHECK_ARG(!au->next || (au->state && au->row_ptr && au->edge_tok && au->dflt && au->states > 0));
-        pr.au = *au;
-    }
-    return sample_launch(logits, T, V, params, row_task, counter, history, history_words, pr, out, pdl, stream);
-}
-
 extern "C" int zl_sample_processed(const float* logits, int T, int V, const zl_sample_params_t* params,
                                    const int32_t* row_task, const int32_t* counter, uint32_t* history, int history_words,
                                    const float* ngram_penalty, int32_t* seq, int32_t* seq_len, int seq_stride,
                                    const int32_t* bias_tokens, const float* bias_values, const int32_t* bias_count,
                                    int bias_stride, int32_t* out, void* ws, size_t ws_bytes, int pdl, zl_stream_t stream) {
-    return sample_processed_launch(logits, T, V, params, row_task, counter, history, history_words, ngram_penalty, seq,
-                                   seq_len, seq_stride, bias_tokens, bias_values, bias_count, bias_stride, nullptr, nullptr,
-                                   out, ws, ws_bytes, pdl, static_cast<cudaStream_t>(stream));
+    ZL_CHECK_ARG(!ngram_penalty || ws_bytes >= zl_sample_processed_workspace_bytes(T, seq_stride));
+    const SampleProc pr{ngram_penalty, seq, seq_len, seq_stride, bias_tokens, bias_values, bias_count, bias_stride,
+                        static_cast<int2*>(ws), seq_stride > 0 ? ngram_table_size(seq_stride) : 0};
+    return sample_launch(logits, T, V, params, row_task, counter, history, history_words, pr, out, pdl,
+                         static_cast<cudaStream_t>(stream));
 }
 
 extern "C" int zl_sample_masked(const float* logits, int T, int V, const zl_sample_params_t* params,
@@ -717,12 +672,14 @@ extern "C" int zl_sample_masked(const float* logits, int T, int V, const zl_samp
                                 const int32_t* bias_tokens, const float* bias_values, const int32_t* bias_count,
                                 int bias_stride, const uint32_t* masks, int mask_words, const int32_t* mask_row,
                                 int32_t* out, void* ws, size_t ws_bytes, int pdl, zl_stream_t stream) {
+    ZL_CHECK_ARG(!ngram_penalty || ws_bytes >= zl_sample_processed_workspace_bytes(T, seq_stride));
+    ZL_CHECK_ARG(masks);
+    SampleProc pr{ngram_penalty, seq, seq_len, seq_stride, bias_tokens, bias_values, bias_count, bias_stride,
+                  static_cast<int2*>(ws), seq_stride > 0 ? ngram_table_size(seq_stride) : 0};
     // mask row of task t: (t * 0 + mask_row[t]), or t when mask_row is NULL; no automaton moves
-    SampleAutomata au{};
-    au.mask = masks;
-    au.words = mask_words;
-    au.state = const_cast<int32_t*>(mask_row);   // read only: au.next is NULL
-    return sample_processed_launch(logits, T, V, params, row_task, counter, history, history_words, ngram_penalty, seq,
-                                   seq_len, seq_stride, bias_tokens, bias_values, bias_count, bias_stride, nullptr, &au,
-                                   out, ws, ws_bytes, pdl, static_cast<cudaStream_t>(stream));
+    pr.au.mask = masks;
+    pr.au.words = mask_words;
+    pr.au.state = const_cast<int32_t*>(mask_row);   // read only: au.next is NULL
+    return sample_launch(logits, T, V, params, row_task, counter, history, history_words, pr, out, pdl,
+                         static_cast<cudaStream_t>(stream));
 }

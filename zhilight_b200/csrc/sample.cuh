@@ -21,13 +21,34 @@ struct SampleAutomata {
     const int32_t *row_ptr = nullptr, *edge_tok = nullptr, *next = nullptr, *dflt = nullptr;
 };
 
-// zl_sample_processed, plus frozen (tasks) or NULL: a row whose task has frozen[task] != 0 is picked as usual but its
-// pick is recorded in neither the history bitmap nor the sequence, and moves no automaton (zl_llama_generate's finished
-// tasks); au NULL or the tasks' automata (zl_sample_masked's contract for the mask)
-int sample_processed_launch(const float* logits, int T, int V, const zl_sample_params_t* params, const int32_t* row_task,
-                            const int32_t* counter, uint32_t* history, int history_words, const float* ngram_penalty,
-                            int32_t* seq, int32_t* seq_len, int seq_stride, const int32_t* bias_tokens,
-                            const float* bias_values, const int32_t* bias_count, int bias_stride, const int32_t* frozen,
-                            const SampleAutomata* au, int32_t* out, void* ws, size_t ws_bytes, int pdl, cudaStream_t stream);
+// The processors' device arguments (zl_sample_processed); all NULL for zl_sample.
+struct SampleProc {
+    const float* ngram;       // (tasks) or NULL: no n-gram rule
+    int32_t* seq;             // (tasks, seq_stride) generated tokens, oldest first, or NULL
+    int32_t* seq_len;         // (tasks)
+    int seq_stride;
+    const int32_t* bias_tok;  // (tasks, bias_stride) or NULL
+    const float* bias_val;
+    const int32_t* bias_cnt;  // (tasks)
+    int bias_stride;
+    int2* table;              // k_ngram_levels' output: per row, table_stride {token, level} slots
+    int table_stride;
+    const int32_t* frozen;    // (tasks) or NULL: a row whose task has frozen[task] != 0 records its pick nowhere
+    SampleAutomata au;        // au.mask NULL: no row is masked
+};
+
+// hash table slots for n distinct tokens at most: a power of two >= 2n, so an insert always finds a free slot
+__host__ __device__ inline int ngram_table_size(int n) {
+    int h = 2;
+    while (h < 2 * n) h <<= 1;
+    return h;
+}
+
+// zl_sample over the processors of pr: zl_sample_processed's contract, plus pr.frozen (zl_llama_generate's finished
+// tasks: a frozen task's pick is recorded in neither the history bitmap nor the sequence, and moves no automaton) and
+// pr.au (zl_sample_masked's contract for the mask).  pr.table must hold T rows.
+int sample_launch(const float* logits, int T, int V, const zl_sample_params_t* params, const int32_t* row_task,
+                  const int32_t* counter, uint32_t* history, int history_words, const SampleProc& pr, int32_t* out,
+                  int pdl, cudaStream_t stream);
 
 }  // namespace zl

@@ -164,5 +164,30 @@ def test_strided_activations_and_fused_norm_is_rejected(lib, cuda):
     x = big[:, :k]                                                # ldx = k + 64
     y = ops.w4a16_gemm_fused(x, packed, n, k, variant=1).float().cpu().numpy()
     assert rel_l2(y, gptq.gemm_f32(x.cpu().numpy(), w)) <= TOL
-    with pytest.raises(_lib.ZLError):
+    with pytest.raises(_lib.ZLError) as e:
         ops.w4a16_gemm_fused(x, packed, n, k, variant=1, ln_weight=torch.ones(k, dtype=torch.float16, device=cuda))
+    assert e.value.code == -2
+
+
+@pytest.mark.parametrize("m", [17, 32])
+@pytest.mark.parametrize("tp_mode", [1, 2])
+def test_tp_exchange_is_rejected_on_the_wgmma_route(lib, cuda, m, tp_mode):
+    """Only the exact-integer kernel (M <= 16) carries the tensor-parallel exchange: a one-rank comm with opened state
+    gets as far as that check."""
+    import ctypes
+    from zhilight_b200 import _lib, dist
+    k, n = 512, 256
+    _, packed = _setup(cuda, k, n, False, 21)
+    assert lib.zl_w4_int_layout_route(m, n, k) == 4
+    x = torch.randn(m, k, generator=torch.Generator().manual_seed(3)).half().to(cuda)
+    y = torch.empty(m, n, dtype=torch.float16, device=cuda)
+    h_out = torch.empty_like(x)
+    comm = dist.TPComm(m * n, 0, 1)
+    try:
+        a = _lib.W4FusedArgs()
+        a.x, a.ldx, a.packed, a.y, a.M, a.N, a.K, a.group_size, a.variant = (x.data_ptr(), k, packed.data_ptr(),
+                                                                              y.data_ptr(), m, n, k, 128, 1)
+        a.tp_mode, a.tp_comm, a.tp_h_out = tp_mode, comm.handle.value, h_out.data_ptr()
+        assert lib.zl_w4a16_gemm_fused(ctypes.byref(a), None) == -2
+    finally:
+        comm.close()

@@ -43,6 +43,10 @@ constexpr int kWarp = 32;
 
 __host__ __device__ inline int cdiv(int a, int b) { return (a + b - 1) / b; }
 
+// zl_prepare() on the CURRENT device unless it already ran there (w4a16_api.cu).  Called lazily before the first launch
+// that needs it: opt-in shared memory must be set outside of stream capture.
+int prepare_once();
+
 // SM count of the CURRENT device, cached per device id (one process may drive several devices: one host thread per
 // GPU in the reference engine, engine.cpp:115-117).  A benign race only repeats the query.
 inline int device_sm_count() {

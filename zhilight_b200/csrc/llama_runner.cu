@@ -565,8 +565,8 @@ int to_k_major(zl_llama* m, const std::string& prefix, int K, int N, uint32_t* q
     return ZL_OK;
 }
 
-// The kernel that serves a W4 Linear at B rows: 3 exact-integer, 4 wgmma, 0 fp16 mma.sync.
-int route_of(const Lin& w, int B) { return w.packed_i ? zl_w4_int_layout_route(B, w.N, w.K) : 0; }
+// The kernel that serves a W4 Linear at B rows, and what it fuses.
+W4Route route_of(const Lin& w, int B) { return w4_route(B, w.N, w.K, 0); }
 
 // The (N) fp16 bias of Linears fused along N: zeros, with each present `prefix.bias` at its row offset.  *out stays
 // empty when none has one.  Every staged bias is checked before the first copy.
@@ -659,7 +659,7 @@ int build_w4(zl_llama* m, const std::vector<std::string>& prefixes, const std::v
     const int m_max = m->cfg.prefill_chunk > m->cfg.max_batch ? m->cfg.prefill_chunk : m->cfg.max_batch;
     bool need_half = false;
     for (int mm = 1; mm <= (m_max < 17 ? m_max : 17); ++mm)
-        if (!zl_w4_int_layout_route(mm, N, K)) need_half = true;
+        if (w4_route(mm, N, K, 0).kernel == W4Kernel::V2) need_half = true;
     RCHECK(dmalloc(&out->packed_i, pbytes));
     RCHECK(zl_w4_pack_v(qw_km.get(), qz_km.get(), sc_km.get(), row_map.get(), out->packed_i.get(), N, K,
                         m->cfg.group_size, m->cfg.sym, 1, m->stream));
@@ -1150,12 +1150,13 @@ struct Chain {
 // head of the successor.
 int w4_gemm(zl_llama* m, int l, Stage s, const Chain& ch, const Lin& w, const void* ln_w, zl_w4_fused_args_t a) {
     const auto& c = m->cfg;
-    const int route = route_of(w, ch.n);
-    a.packed = route ? w.packed_i.get() : w.packed.get();
-    a.variant = route ? 1 : 0;
+    const W4Route route = route_of(w, ch.n);
+    const bool half = route.kernel == W4Kernel::V2;   // the fp16 kernel reads the ZLW4 layout
+    a.packed = half ? w.packed.get() : w.packed_i.get();
+    a.variant = half ? kW4VariantHalf : kW4VariantInt;
     if (!a.packed) return fail_state(__LINE__, "no packed weight variant for this batch size");
     const int pdl = ch.no_pdl ? 0 : c.use_pdl;
-    if (ln_w && (c.fuse == 0 || route == 4 || (w.k_perm && route != 3))) {
+    if (ln_w && (c.fuse == 0 || !route.fuses_rmsnorm() || (w.k_perm && !route.gathers_k_perm()))) {
         // the RMSNorm runs as its own kernel (reference order, block.cpp:125,131) into the matching rows of xn: at fuse 0,
         // for the wgmma kernel, which reads x through the TMA engine, and for an act-order GEMM not gathered while staged
         void* xn = rows(m->xn.get(), ch.row0, w.K);
@@ -1164,7 +1165,7 @@ int w4_gemm(zl_llama* m, int l, Stage s, const Chain& ch, const Lin& w, const vo
         a.x = xn;
         ln_w = nullptr;
     }
-    if (w.k_perm && route == 3) {
+    if (w.k_perm && route.gathers_k_perm()) {
         a.k_perm = w.k_perm.get();   // gathered while the integer kernel stages x
     } else if (w.k_perm) {
         // the other routes read x in tiles: permute it first (permute_input, gptq/utils.cu:322-398)
@@ -1173,10 +1174,10 @@ int w4_gemm(zl_llama* m, int l, Stage s, const Chain& ch, const Lin& w, const vo
         a.ldx = w.K;
     }
     W4L2Head l2;
-    if (!ch.no_pdl && route == 3 && (l2_head_depth() > 0 || l2_whole_max() > 0)) {
+    if (!ch.no_pdl && route.kernel == W4Kernel::V3 && (l2_head_depth() > 0 || l2_whole_max() > 0)) {
         int succ_tp = 0;
         const Lin* nx = w4_successor(m, l, s, a.tp_mode, &succ_tp);
-        if (nx && route_of(*nx, ch.n) == 3)
+        if (nx && route_of(*nx, ch.n).kernel == W4Kernel::V3)
             w4_v3_l2_head(nx->packed_i.get(), ch.n, nx->N, nx->K, succ_tp, device_sm_count(), l2_head_depth(),
                           l2_whole_max(), &l2);
     }
@@ -1269,7 +1270,7 @@ int qkv_gemm(zl_llama* m, int l, Chain& ch) {
     const bool epi = L.qkv.fmt == kW4 && c.fuse >= 2;
     // int8 cache at fuse >= 2 on the exact-integer route (M <= 16): the epilogue quantises K / V into the cache.  The wgmma
     // and fp16 routes, and act-order qkv, append fp16 rows to the staging rows and kv8_append quantises them.
-    const bool fused_kv8 = c.kv_int8 && epi && !L.qkv.k_perm && route_of(L.qkv, ch.n) == 3;
+    const bool fused_kv8 = c.kv_int8 && epi && !L.qkv.k_perm && route_of(L.qkv, ch.n).fuses_kv_int8();
     if (epi) {
         a.epilogue = ZL_EPI_QKV_ROPE;
         a.cos = cos;
@@ -1569,7 +1570,7 @@ int enqueue_step(zl_llama* m, int n_tasks, int len_bucket, const Segments* pf, c
     if (ch.fused) {
         const Layer& L0 = m->layers[0];
         for (const Lin* w : {&L0.qkv, &L0.o, &L0.gu, &L0.down})
-            if (route_of(*w, B) != 3) ch.fused = false;
+            if (!route_of(*w, B).exchanges_tp()) ch.fused = false;
     }
     if (ch.fused) RCHECK(zl_comm_ll_begin_step(m->comm, st));   // the word tags of this step's exchanges
     ch.xodd = ((2 * c.num_layers - 1) & 1) << 9;

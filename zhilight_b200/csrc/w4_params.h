@@ -66,16 +66,32 @@ struct W4Params {
 // zl_w4a16_gemm_fused with the L2 head of the successor GEMM as a descriptor (l2 == nullptr: the public whole-range
 // prefetch_ptr / prefetch_bytes).  Only the exact-integer kernel issues it, at the tail of its weight stream.
 int w4a16_gemm_fused_l2(const zl_w4_fused_args_t* a, const W4L2Head* l2, zl_stream_t stream);
-cudaError_t launch_w4_v2(const W4Params& p, bool pdl, cudaStream_t stream);
-cudaError_t prepare_w4_v2();
-// exact-integer kernel on the ZLW4I layout; false = staged activations do not fit shared memory
-bool launch_w4_v3(const W4Params& p, bool pdl, cudaStream_t stream, cudaError_t* err);
-bool w4_v3_fits(int mc, int N, int K);
 // the variant launch_w4_v3 runs for (mc, N, K, tp_mode) on sm_count SMs; false = none fits
 struct V3Plan {
     int nt, warps, subs, stages, rt, pack, grid, smem, sub_major;
 };
 bool w4_v3_plan(int mc, int N, int K, int tp_mode, int sm_count, V3Plan* plan);
+
+// The kernel that serves M rows of an (N, K) W4 weight, and what it fuses: v3 (exact-integer mma.sync, ZLW4I layout)
+// wherever w4_v3_plan finds a variant, else tc (wgmma, ZLW4I layout) where w4_tc_supports, else v2 (fp16 mma.sync, ZLW4
+// layout).  None: no W4 kernel takes the shape.  tp_mode and the SM count only choose among v3 variants, never the kernel.
+enum class W4Kernel { None, V2, V3, Tc };
+struct W4Route {
+    W4Kernel kernel = W4Kernel::None;
+    int rows = 32;   // rows per launch: up to 256 tokens on the wgmma kernel, 32 on the mma.sync kernels
+    V3Plan v3{};     // kernel == V3: the variant launch_w4_v3 runs
+    // the wgmma kernel reads x through the TMA engine, so it neither normalises nor gathers it while staging
+    bool fuses_rmsnorm() const { return kernel != W4Kernel::Tc; }
+    bool gathers_k_perm() const { return kernel == W4Kernel::V3; }
+    bool fuses_kv_int8() const { return kernel == W4Kernel::V3; }
+    bool exchanges_tp() const { return kernel == W4Kernel::V3; }
+};
+W4Route w4_route(int M, int N, int K, int tp_mode);
+
+cudaError_t launch_w4_v2(const W4Params& p, bool pdl, cudaStream_t stream);
+cudaError_t prepare_w4_v2();
+// exact-integer kernel on the ZLW4I layout: the variant w4_route planned for p
+cudaError_t launch_w4_v3(const W4Params& p, const V3Plan& plan, bool pdl, cudaStream_t stream);
 // descriptor of the L2 head of a successor v3 launch with weights `packed`: its first h ring items per warp, or the
 // whole blob when it is at most whole_max bytes; false = the successor does not run the v3 kernel
 bool w4_v3_l2_head(const void* packed, int mc, int N, int K, int tp_mode, int sm_count, int h, size_t whole_max,

@@ -26,11 +26,28 @@ extern "C" int zl_prepare(void) {
     return prepare_sample();
 }
 
-// which kernel serves (M, N, K) on the ZLW4I layout: 3 = exact-integer mma.sync, 4 = wgmma, 0 = neither
-static int int_layout_route(int M, int N, int K) {
-    if (M <= 16 && w4_v3_fits(M, N, K)) return 3;
-    if (w4_tc_supports(M < 256 ? M : 256, N, K)) return 4;
-    return 0;
+int zl::prepare_once() {
+    static bool prepared[64] = {};
+    int dev = 0;
+    cudaGetDevice(&dev);
+    if (dev >= 0 && dev < 64 && prepared[dev]) return ZL_OK;
+    const int rc = zl_prepare();
+    if (rc == ZL_OK && dev >= 0 && dev < 64) prepared[dev] = true;
+    return rc;
+}
+
+W4Route zl::w4_route(int M, int N, int K, int tp_mode) {
+    W4Route r;
+    if (M <= 0 || N <= 0 || K <= 0 || N % 32 || K % kW4GroupK) return r;
+    if (w4_v3_plan(M, N, K, tp_mode, device_sm_count(), &r.v3)) {
+        r.kernel = W4Kernel::V3;
+    } else if (w4_tc_supports(M < 256 ? M : 256, N, K)) {
+        r.kernel = W4Kernel::Tc;
+        r.rows = 256;
+    } else {
+        r.kernel = W4Kernel::V2;
+    }
+    return r;
 }
 
 namespace zl {
@@ -56,14 +73,11 @@ extern "C" int zl_w4_set_trace(void* buf) {
     return ZL_OK;
 }
 
-extern "C" int zl_w4_int_kernel_fits(int M, int N, int K) {
-    if (M <= 0 || N <= 0 || K <= 0 || N % 32 || K % kW4GroupK) return 0;
-    return (M <= 16 && w4_v3_fits(M, N, K)) ? 1 : 0;
-}
+extern "C" int zl_w4_int_kernel_fits(int M, int N, int K) { return w4_route(M, N, K, 0).kernel == W4Kernel::V3; }
 
 extern "C" int zl_w4_int_layout_route(int M, int N, int K) {
-    if (M <= 0 || N <= 0 || K <= 0 || N % 32 || K % kW4GroupK) return 0;
-    return int_layout_route(M, N, K);
+    const W4Kernel k = w4_route(M, N, K, 0).kernel;
+    return k == W4Kernel::V3 ? 3 : k == W4Kernel::Tc ? 4 : 0;
 }
 
 extern "C" int zl_qkv_rope_row_map(int32_t* row_map, int n_heads_total, int dim_head, zl_stream_t stream) {
@@ -94,16 +108,7 @@ extern "C" int zl_w4_fused_args_layout(size_t* size, size_t* k_perm_offset) {
 }
 
 int zl::w4a16_gemm_fused_l2(const zl_w4_fused_args_t* a, const W4L2Head* l2, zl_stream_t stream) {
-    {
-        static bool prepared[64] = {};
-        int dev = 0;
-        cudaGetDevice(&dev);
-        if (dev < 0 || dev >= 64 || !prepared[dev]) {
-            int rc = zl_prepare();
-            if (rc != ZL_OK) return rc;
-            if (dev >= 0 && dev < 64) prepared[dev] = true;
-        }
-    }
+    if (const int rc = prepare_once()) return rc;
     ZL_CHECK_ARG(a && a->x && a->packed && a->M > 0 && a->N > 0 && a->K > 0);
     ZL_CHECK_SUPPORTED(a->group_size == kW4GroupK);
     ZL_CHECK_SUPPORTED(a->N % 32 == 0 && a->K % kW4GroupK == 0);
@@ -128,6 +133,8 @@ int zl::w4a16_gemm_fused_l2(const zl_w4_fused_args_t* a, const W4L2Head* l2, zl_
                      a->kv8_counters);
         ZL_CHECK_SUPPORTED(!a->k_perm && "the int8-cache epilogue is not combined with k_perm");
     }
+    // variant 0 packs the ZLW4 layout, which only the fp16 kernel reads
+    const W4Route route = a->variant == kW4VariantInt ? w4_route(a->M, a->N, a->K, a->tp_mode) : W4Route{W4Kernel::V2};
     const void* tp_cd = nullptr;
     if (a->tp_mode != 0) {
         ZL_CHECK_ARG(a->tp_mode == 1 || a->tp_mode == 2);
@@ -138,7 +145,7 @@ int zl::w4a16_gemm_fused_l2(const zl_w4_fused_args_t* a, const W4L2Head* l2, zl_
             zl_set_last_error(__FILE__, __LINE__, "tp_comm: peers not opened");
             return ZL_ERR_STATE;
         }
-        ZL_CHECK_SUPPORTED(a->M <= 16 && w4_v3_fits(a->M, a->N, a->K) && "tp_mode needs the integer kernel (M <= 16)");
+        ZL_CHECK_SUPPORTED(route.exchanges_tp() && "tp_mode needs the integer kernel (M <= 16)");
         if (a->tp_mode == 1) {
             ZL_CHECK_ARG(a->tp_h_out != nullptr && a->tp_h_out != a->x && a->ldx == a->K);
             ZL_CHECK_ARG((size_t)a->M * a->K * 2 <= zl_comm_slot_bytes(a->tp_comm));
@@ -148,15 +155,15 @@ int zl::w4a16_gemm_fused_l2(const zl_w4_fused_args_t* a, const W4L2Head* l2, zl_
         }
     }
     const int n_out = a->epilogue == ZL_EPI_SWIGLU ? a->N / 2 : a->N;
-    // rows per pass: the wgmma kernel takes up to 256 tokens at once, the mma.sync kernels 32 (v2) / 16 (v3)
-    const int route = a->variant == kW4VariantInt ? int_layout_route(a->M, a->N, a->K) : 2;
-    ZL_CHECK_SUPPORTED(route != 0 && "ZLW4I layout: M > 16 (or staged activations too large) and N % 128 != 0: use variant 0");
-    ZL_CHECK_SUPPORTED(!(route == 4 && a->ln_weight) && "the wgmma kernel has no fused RMSNorm prologue: run zl_rmsnorm first");
-    ZL_CHECK_SUPPORTED(!(route != 3 && a->k_perm) &&
+    ZL_CHECK_SUPPORTED((a->variant == kW4VariantHalf || route.kernel != W4Kernel::V2) &&
+                       "ZLW4I layout: M > 16 (or staged activations too large) and N % 128 != 0: use variant 0");
+    ZL_CHECK_SUPPORTED(!(a->ln_weight && !route.fuses_rmsnorm()) &&
+                       "the wgmma kernel has no fused RMSNorm prologue: run zl_rmsnorm first");
+    ZL_CHECK_SUPPORTED(!(a->k_perm && !route.gathers_k_perm()) &&
                        "only the exact-integer kernel gathers k_perm: permute x with zl_gather_cols_16 first");
-    ZL_CHECK_SUPPORTED(!(route != 3 && a->kv_int8) &&
+    ZL_CHECK_SUPPORTED(!(a->kv_int8 && !route.fuses_kv_int8()) &&
                        "only the exact-integer kernel (M <= 16) quantises an int8 KV cache: use zl_kv_int8_quant_append");
-    const int step = route == 4 ? 256 : 32;
+    const int step = route.rows;
     for (int m0 = 0; m0 < a->M; m0 += step) {
         W4Params p;
         p.mc = (a->M - m0) < step ? (a->M - m0) : step;
@@ -196,7 +203,7 @@ int zl::w4a16_gemm_fused_l2(const zl_w4_fused_args_t* a, const W4L2Head* l2, zl_
         p.tp_index = a->tp_index;
         p.tp_h_out = static_cast<__half*>(a->tp_h_out);
         p.k_perm = a->k_perm;
-        if (a->kv_int8) {   // route 3: M <= 16, one pass
+        if (a->kv_int8) {   // the v3 route
             p.kv8 = 1;
             p.kv8_sk = reinterpret_cast<float* const*>(a->scale_k_addrs);
             p.kv8_sv = reinterpret_cast<float* const*>(a->scale_v_addrs);
@@ -209,15 +216,13 @@ int zl::w4a16_gemm_fused_l2(const zl_w4_fused_args_t* a, const W4L2Head* l2, zl_
             p.l2.base = static_cast<const uint8_t*>(a->prefetch_ptr);
             p.l2.whole_bytes = a->prefetch_bytes;
         }
-        if (route == 4) {
-            ZL_CHECK_CUDA(launch_w4_tc(p, a->pdl != 0 && m0 == 0, stream));
-        } else if (route == 3) {
-            cudaError_t ce = cudaSuccess;
-            const bool ok = launch_w4_v3(p, a->pdl != 0 && m0 == 0, stream, &ce);
-            ZL_CHECK_SUPPORTED(ok && "ZLW4I kernel: staged activations do not fit shared memory (use variant 0)");
-            ZL_CHECK_CUDA(ce);
+        const bool pdl = a->pdl != 0 && m0 == 0;
+        if (route.kernel == W4Kernel::Tc) {
+            ZL_CHECK_CUDA(launch_w4_tc(p, pdl, stream));
+        } else if (route.kernel == W4Kernel::V3) {   // M <= 16: one pass
+            ZL_CHECK_CUDA(launch_w4_v3(p, route.v3, pdl, stream));
         } else {
-            ZL_CHECK_CUDA(launch_w4_v2(p, a->pdl != 0 && m0 == 0, stream));
+            ZL_CHECK_CUDA(launch_w4_v2(p, pdl, stream));
         }
     }
     return ZL_OK;

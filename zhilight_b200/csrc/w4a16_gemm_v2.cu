@@ -390,54 +390,48 @@ __global__ void __launch_bounds__(WARPS * 32, ((NT <= 2 && WARPS == 8) ? 2 : 1))
     }
 }
 
-static int v2_num_sms() { return device_sm_count(); }
-
-template <int NT, bool NORM, bool XC, int WARPS, int STAGES>
-static cudaError_t launch_v2_t(const W4Params& p, bool pdl, cudaStream_t stream) {
-    using S = V2Smem<NT, WARPS, STAGES>;
-    const int smem = S::kBytes + (XC ? p.mc * x_row_bytes(p.K) : 0);
-    const int tiles = p.N / 32;
-    const int max_ctas = v2_num_sms() * (WARPS == 8 ? 2 : 1);
-    const int grid = tiles < max_ctas ? tiles : max_ctas;
-    return launch(k_w4a16_v2<NT, NORM, XC, WARPS, STAGES>, dim3(grid), dim3(WARPS * 32), (size_t)smem, stream, pdl, p);
+// The kernels of one ring shape, by fused RMSNorm prologue and by staging x in shared memory (XC).  NT token tiles of 8:
+// 16 warps (tall: one CTA per SM, k split 16 ways) for NT <= 2, 8 warps (two CTAs per SM) otherwise.
+using V2Kernel = void (*)(W4Params);
+struct V2Variant {
+    int nt, warps, ring_bytes;   // ring_bytes: shared memory without the staged x
+    V2Kernel k[2][2];            // [NORM][XC]
+};
+template <int NT, int W, int ST>
+static V2Variant v2_variant() {
+    return {NT, W, V2Smem<NT, W, ST>::kBytes,
+            {{k_w4a16_v2<NT, false, false, W, ST>, k_w4a16_v2<NT, false, true, W, ST>},
+             {k_w4a16_v2<NT, true, false, W, ST>, k_w4a16_v2<NT, true, true, W, ST>}}};
 }
-
-template <int NT, int WARPS, int STAGES>
-static cudaError_t launch_v2_shape(const W4Params& p, bool pdl, cudaStream_t stream) {
-    const bool norm = p.ln_w != nullptr;
-    // stage x in shared memory when the CTA budget allows (always true for M = 1 at the Llama shapes)
-    const int budget = WARPS == 8 ? kV2TwoCtaBudget : kV2OneCtaBudget;
-    const bool xc = V2Smem<NT, WARPS, STAGES>::kBytes + p.mc * x_row_bytes(p.K) <= budget;
-    if (xc)
-        return norm ? launch_v2_t<NT, true, true, WARPS, STAGES>(p, pdl, stream)
-                    : launch_v2_t<NT, false, true, WARPS, STAGES>(p, pdl, stream);
-    return norm ? launch_v2_t<NT, true, false, WARPS, STAGES>(p, pdl, stream)
-                : launch_v2_t<NT, false, false, WARPS, STAGES>(p, pdl, stream);
-}
-
-template <int NT>
-static cudaError_t launch_v2_nt(const W4Params& p, bool pdl, cudaStream_t stream) {
-    const bool tall = NT <= 2 && p.N / 32 <= v2_num_sms() && p.K / kW4GroupK >= 32;
-    if (tall) return launch_v2_shape<(NT <= 2 ? NT : 1), 16, 4>(p, pdl, stream);
-    return launch_v2_shape<NT, 8, (NT == 1 ? 5 : 4)>(p, pdl, stream);
-}
+// Every v2 kernel: launch_w4_v2 runs one of these and prepare_w4_v2 opts all of them in
+static const V2Variant kV2Variants[] = {v2_variant<1, 8, 5>(), v2_variant<2, 8, 4>(), v2_variant<4, 8, 4>(),
+                                        v2_variant<1, 16, 4>(), v2_variant<2, 16, 4>()};
+static int v2_budget(const V2Variant& v) { return v.warps == 8 ? kV2TwoCtaBudget : kV2OneCtaBudget; }
 
 cudaError_t launch_w4_v2(const W4Params& p, bool pdl, cudaStream_t stream) {
-    if (p.mc <= 8) return launch_v2_nt<1>(p, pdl, stream);
-    if (p.mc <= 16) return launch_v2_nt<2>(p, pdl, stream);
-    return launch_v2_nt<4>(p, pdl, stream);
+    const int sms = device_sm_count();
+    const int nt = p.mc <= 8 ? 1 : p.mc <= 16 ? 2 : 4;
+    const bool tall = nt <= 2 && p.N / 32 <= sms && p.K / kW4GroupK >= 32;
+    for (const V2Variant& v : kV2Variants) {
+        if (v.nt != nt || v.warps != (tall ? 16 : 8)) continue;
+        // stage x in shared memory when the CTA budget allows (always true for M = 1 at the Llama shapes)
+        const int x_bytes = p.mc * x_row_bytes(p.K);
+        const bool xc = v.ring_bytes + x_bytes <= v2_budget(v);
+        const int tiles = p.N / 32, max_ctas = sms * (v.warps == 8 ? 2 : 1);
+        return launch(v.k[p.ln_w != nullptr][xc], dim3(tiles < max_ctas ? tiles : max_ctas), dim3(v.warps * 32),
+                      (size_t)(v.ring_bytes + (xc ? x_bytes : 0)), stream, pdl, p);
+    }
+    return cudaErrorNotSupported;
 }
 
 cudaError_t prepare_w4_v2() {
-    cudaError_t e;
-#define ZL_SET(NT, NORM, XC, W, ST)                                                                                \
-    e = cudaFuncSetAttribute(k_w4a16_v2<NT, NORM, XC, W, ST>, cudaFuncAttributeMaxDynamicSharedMemorySize,         \
-                             XC ? (W == 8 ? kV2TwoCtaBudget : kV2OneCtaBudget) : V2Smem<NT, W, ST>::kBytes);        \
-    if (e != cudaSuccess) return e;
-#define ZL_SET4(NT, W, ST) ZL_SET(NT, false, false, W, ST) ZL_SET(NT, true, false, W, ST) ZL_SET(NT, false, true, W, ST) ZL_SET(NT, true, true, W, ST)
-    ZL_SET4(1, 8, 5) ZL_SET4(2, 8, 4) ZL_SET4(4, 8, 4) ZL_SET4(1, 16, 4) ZL_SET4(2, 16, 4)
-#undef ZL_SET4
-#undef ZL_SET
+    for (const V2Variant& v : kV2Variants)
+        for (const auto& by_xc : v.k)
+            for (int xc = 0; xc < 2; ++xc) {
+                const cudaError_t e = cudaFuncSetAttribute(by_xc[xc], cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                                           xc ? v2_budget(v) : v.ring_bytes);
+                if (e != cudaSuccess) return e;
+            }
     return cudaSuccess;
 }
 

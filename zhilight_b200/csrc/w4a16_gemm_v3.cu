@@ -809,48 +809,45 @@ __global__ void __launch_bounds__(WARPS * SUBS * 32, 1) k_w4a16_v3(const W4Param
     }
 }
 
-static int v3_num_sms() { return device_sm_count(); }
-
 constexpr int kV3Budget = 231000;   // one CTA per SM (227 KB usable + 1 KB reserved)
 
-template <int NT, bool NORM, int WARPS, int SUBS, int STAGES, int RT, bool PACK>
-static cudaError_t launch_v3_t(const W4Params& params, const V3Plan& pl, bool pdl, cudaStream_t stream) {
-    const dim3 grid(pl.grid), block(WARPS * SUBS * 32);
-    W4Params p = params;
-    p.sub_major = pl.sub_major;
-    if (p.tp_mode != 0) {
-        // exchange variants exist for the 4-stage rings only (w4_v3_plan routes tensor-parallel launches there)
-        if constexpr (STAGES == 4 && RT == NT * 8) {
-            if (p.tp_mode == 1 && p.kv8)   // reduce-in on the qkv GEMM of an int8-cache model
-                return launch(k_w4a16_v3<NT, NORM, WARPS, SUBS, STAGES, RT, PACK, 1, false, true>, grid, block,
-                              (size_t)pl.smem, stream, pdl, p);
-            if (p.tp_mode == 1)
-                return launch(k_w4a16_v3<NT, NORM, WARPS, SUBS, STAGES, RT, PACK, 1>, grid, block, (size_t)pl.smem, stream,
-                              pdl, p);
-            return launch(k_w4a16_v3<NT, NORM, WARPS, SUBS, STAGES, RT, PACK, 2>, grid, block, (size_t)pl.smem, stream, pdl,
-                          p);
-        } else {
-            return cudaErrorNotSupported;
-        }
+// The kernels of one plan shape, by fused RMSNorm prologue and by fusion: plain, act-order gather (k_perm), int8-cache
+// epilogue, tensor-parallel reduce-in, reduce-in on the qkv GEMM of an int8-cache model, push.  The exchange variants
+// exist for the 4-stage rings only (w4_v3_plan routes tensor-parallel launches there).
+using V3Kernel = void (*)(W4Params);
+struct V3Variant {
+    int nt, warps, subs, stages;
+    bool pack;
+    V3Kernel k[2][6];   // [NORM][fusion]
+};
+static int v3_fusion(const W4Params& p) {
+    if (p.tp_mode != 0) return p.tp_mode == 2 ? 5 : p.kv8 ? 4 : 3;
+    return p.k_perm ? 1 : p.kv8 ? 2 : 0;   // the front end rejects k_perm with tp_mode and with kv8
+}
+template <int NT, bool NORM, int W, int SB, int ST, bool PK>
+static void v3_fusions(V3Kernel (&k)[6]) {
+    k[0] = k_w4a16_v3<NT, NORM, W, SB, ST, NT * 8, PK>;
+    k[1] = k_w4a16_v3<NT, NORM, W, SB, ST, NT * 8, PK, 0, true>;
+    k[2] = k_w4a16_v3<NT, NORM, W, SB, ST, NT * 8, PK, 0, false, true>;
+    if constexpr (ST == 4) {
+        k[3] = k_w4a16_v3<NT, NORM, W, SB, ST, NT * 8, PK, 1>;
+        k[4] = k_w4a16_v3<NT, NORM, W, SB, ST, NT * 8, PK, 1, false, true>;
+        k[5] = k_w4a16_v3<NT, NORM, W, SB, ST, NT * 8, PK, 2>;
     }
-    if (p.k_perm)   // act-order (the front end rejects k_perm with tp_mode and with kv8)
-        return launch(k_w4a16_v3<NT, NORM, WARPS, SUBS, STAGES, RT, PACK, 0, true>, grid, block, (size_t)pl.smem, stream, pdl,
-                      p);
-    if (p.kv8)
-        return launch(k_w4a16_v3<NT, NORM, WARPS, SUBS, STAGES, RT, PACK, 0, false, true>, grid, block, (size_t)pl.smem,
-                      stream, pdl, p);
-    return launch(k_w4a16_v3<NT, NORM, WARPS, SUBS, STAGES, RT, PACK>, grid, block, (size_t)pl.smem, stream, pdl, p);
 }
-
-template <int NT, int WARPS, int SUBS, int STAGES, int RT>
-static cudaError_t v3_run(const W4Params& p, const V3Plan& pl, bool pdl, cudaStream_t stream) {
-    constexpr bool kPack = NT == 1 && RT == NT * 8;
-    if (kPack && pl.pack)
-        return p.ln_w ? launch_v3_t<NT, true, WARPS, SUBS, STAGES, RT, kPack>(p, pl, pdl, stream)
-                      : launch_v3_t<NT, false, WARPS, SUBS, STAGES, RT, kPack>(p, pl, pdl, stream);
-    return p.ln_w ? launch_v3_t<NT, true, WARPS, SUBS, STAGES, RT, false>(p, pl, pdl, stream)
-                  : launch_v3_t<NT, false, WARPS, SUBS, STAGES, RT, false>(p, pl, pdl, stream);
+template <int NT, int W, int SB, int ST, bool PK>
+static V3Variant v3_variant() {
+    V3Variant v{NT, W, SB, ST, PK, {}};
+    v3_fusions<NT, false, W, SB, ST, PK>(v.k[0]);
+    v3_fusions<NT, true, W, SB, ST, PK>(v.k[1]);
+    return v;
 }
+// Every v3 kernel: launch_w4_v3 runs one of these and prepare_w4_v3 opts all of them into kV3Budget.  The shapes are
+// those w4_v3_plan picks from; PACK only with NT = 1.
+static const V3Variant kV3Variants[] = {
+    v3_variant<1, 16, 1, 4, false>(), v3_variant<1, 16, 1, 4, true>(), v3_variant<1, 8, 2, 5, false>(),
+    v3_variant<1, 8, 2, 5, true>(),   v3_variant<1, 8, 2, 4, false>(), v3_variant<1, 8, 2, 4, true>(),
+    v3_variant<2, 16, 1, 4, false>(), v3_variant<2, 8, 2, 4, false>()};
 
 // The one place that picks the v3 variant: launch_w4_v3 runs exactly this plan, and the L2 head of a successor launch
 // (w4_v3_l2_head) is computed from it.
@@ -878,19 +875,18 @@ bool w4_v3_plan(int mc, int N, int K, int tp_mode, int sm_count, V3Plan* plan) {
     return false;
 }
 
-// returns false when the staged activations do not fit shared memory (caller falls back to the fp16 kernels)
-bool launch_w4_v3(const W4Params& p, bool pdl, cudaStream_t stream, cudaError_t* err) {
-    V3Plan pl;
-    if (!w4_v3_plan(p.mc, p.N, p.K, p.tp_mode, v3_num_sms(), &pl)) return false;
-#define ZL_V3(NT, W, SB, ST, RT)                                                                               \
-    if (pl.nt == NT && pl.warps == W && pl.subs == SB && pl.stages == ST && pl.rt == RT) {                     \
-        *err = v3_run<NT, W, SB, ST, RT>(p, pl, pdl, stream);                                                  \
-        return true;                                                                                           \
+cudaError_t launch_w4_v3(const W4Params& params, const V3Plan& pl, bool pdl, cudaStream_t stream) {
+    for (const V3Variant& v : kV3Variants) {
+        if (v.nt != pl.nt || v.warps != pl.warps || v.subs != pl.subs || v.stages != pl.stages || v.nt * 8 != pl.rt ||
+            v.pack != (pl.pack != 0))
+            continue;
+        const V3Kernel k = v.k[params.ln_w != nullptr][v3_fusion(params)];
+        if (!k) return cudaErrorNotSupported;
+        W4Params p = params;
+        p.sub_major = pl.sub_major;
+        return launch(k, dim3(pl.grid), dim3(pl.warps * pl.subs * 32), (size_t)pl.smem, stream, pdl, p);
     }
-    ZL_V3(1, 16, 1, 4, 8) ZL_V3(1, 8, 2, 5, 8) ZL_V3(1, 8, 2, 4, 8)
-    ZL_V3(2, 16, 1, 4, 16) ZL_V3(2, 8, 2, 4, 16)
-#undef ZL_V3
-    return false;
+    return cudaErrorNotSupported;
 }
 
 bool w4_v3_l2_head(const void* packed, int mc, int N, int K, int tp_mode, int sm_count, int h, size_t whole_max,
@@ -953,58 +949,14 @@ extern "C" int zl_w4_v3_l2_head(int mc, int N, int K, int tp_mode, int sm_count,
 
 namespace zl {
 
-bool w4_v3_fits(int mc, int N, int K) {
-    const int G = K / kW4GroupK;
-    if (G > 8 * 16) return false;
-    const int stage = v3_stage_bytes(mc, K);
-    if (mc <= 8) return V3Smem<1, 8, 2, 4>::kBytes + stage <= kV3Budget;
-    if (mc <= 16) return V3Smem<2, 8, 2, 4>::kBytes + stage <= kV3Budget;
-    (void)N;
-    return false;
-}
-
-// opt-in shared memory of one single-GPU variant, with and without the act-order gather, and with the int8-cache epilogue
-template <int NT, bool NORM, int W, int SB, int ST, int RT = NT * 8, bool PK = false>
-static cudaError_t v3_set_smem() {
-    cudaError_t e = cudaFuncSetAttribute(k_w4a16_v3<NT, NORM, W, SB, ST, RT, PK>,
-                                         cudaFuncAttributeMaxDynamicSharedMemorySize, kV3Budget);
-    if (e != cudaSuccess) return e;
-    e = cudaFuncSetAttribute(k_w4a16_v3<NT, NORM, W, SB, ST, RT, PK, 0, true>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                             kV3Budget);
-    if (e != cudaSuccess) return e;
-    return cudaFuncSetAttribute(k_w4a16_v3<NT, NORM, W, SB, ST, RT, PK, 0, false, true>,
-                                cudaFuncAttributeMaxDynamicSharedMemorySize, kV3Budget);
-}
-
 cudaError_t prepare_w4_v3() {
-    cudaError_t e;
-#define ZL_SET(NT, NORM, W, SB, ST)                                                                            \
-    e = v3_set_smem<NT, NORM, W, SB, ST>();                                                                    \
-    if (e != cudaSuccess) return e;
-#define ZL_SET1(NORM, W, SB, ST)                                                                               \
-    e = v3_set_smem<1, NORM, W, SB, ST, 8, true>();                                                            \
-    if (e != cudaSuccess) return e;
-    ZL_SET1(false, 8, 2, 5) ZL_SET1(true, 8, 2, 5) ZL_SET1(false, 8, 2, 4) ZL_SET1(true, 8, 2, 4)
-    ZL_SET1(false, 16, 1, 4) ZL_SET1(true, 16, 1, 4)
-#undef ZL_SET1
-    ZL_SET(1, false, 8, 2, 5) ZL_SET(1, true, 8, 2, 5) ZL_SET(1, false, 8, 2, 4) ZL_SET(1, true, 8, 2, 4)
-    ZL_SET(1, false, 16, 1, 4) ZL_SET(1, true, 16, 1, 4)
-    ZL_SET(2, false, 8, 2, 4) ZL_SET(2, true, 8, 2, 4) ZL_SET(2, false, 16, 1, 4) ZL_SET(2, true, 16, 1, 4)
-#undef ZL_SET
-#define ZL_SETX(NT, NORM, W, SB, PK)                                                                            \
-    e = cudaFuncSetAttribute(k_w4a16_v3<NT, NORM, W, SB, 4, NT * 8, PK, 1>,                                     \
-                             cudaFuncAttributeMaxDynamicSharedMemorySize, kV3Budget);                           \
-    if (e != cudaSuccess) return e;                                                                             \
-    e = cudaFuncSetAttribute(k_w4a16_v3<NT, NORM, W, SB, 4, NT * 8, PK, 2>,                                     \
-                             cudaFuncAttributeMaxDynamicSharedMemorySize, kV3Budget);                           \
-    if (e != cudaSuccess) return e;                                                                             \
-    e = cudaFuncSetAttribute(k_w4a16_v3<NT, NORM, W, SB, 4, NT * 8, PK, 1, false, true>,                        \
-                             cudaFuncAttributeMaxDynamicSharedMemorySize, kV3Budget);                           \
-    if (e != cudaSuccess) return e;
-    ZL_SETX(1, false, 8, 2, false) ZL_SETX(1, true, 8, 2, false) ZL_SETX(1, false, 16, 1, false) ZL_SETX(1, true, 16, 1, false)
-    ZL_SETX(1, false, 8, 2, true) ZL_SETX(1, true, 8, 2, true) ZL_SETX(1, false, 16, 1, true) ZL_SETX(1, true, 16, 1, true)
-    ZL_SETX(2, false, 8, 2, false) ZL_SETX(2, true, 8, 2, false) ZL_SETX(2, false, 16, 1, false) ZL_SETX(2, true, 16, 1, false)
-#undef ZL_SETX
+    for (const V3Variant& v : kV3Variants)
+        for (const auto& by_fusion : v.k)
+            for (V3Kernel k : by_fusion) {
+                if (!k) continue;
+                const cudaError_t e = cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, kV3Budget);
+                if (e != cudaSuccess) return e;
+            }
     return cudaSuccess;
 }
 

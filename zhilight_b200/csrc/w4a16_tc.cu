@@ -366,6 +366,13 @@ TcDeviceState* tc_state() {
     return (dev >= 0 && dev < 64) ? &g_tc_state[dev] : nullptr;
 }
 
+// Every wgmma kernel, one per token tile: launch_w4_tc runs the smallest tile that holds the launch's rows, and
+// prepare_w4_tc opts all of them in
+struct TsVariant { int ntok, threads, smem; void (*k)(W4TcParams); };
+template <int NTOK>
+static TsVariant ts_variant() { return {NTOK, TsCfg<NTOK>::kThreads, TsCfg<NTOK>::kBytes, k_w4a16_ts<NTOK>}; }
+static const TsVariant kTsVariants[] = {ts_variant<32>(), ts_variant<64>(), ts_variant<128>(), ts_variant<256>()};
+
 // allocates the per-device partial-tile workspace and sets the opt-in shared-memory sizes; must run outside stream capture
 cudaError_t prepare_w4_tc() {
     TcDeviceState* st = tc_state();
@@ -381,12 +388,8 @@ cudaError_t prepare_w4_tc() {
         if ((e = cudaMemset(st->ws_ll, 0, kTcWsLlBytes)) != cudaSuccess) return e;
         st->ws_ll_bytes = kTcWsLlBytes;
     }
-#define ZL_TS_SET(NT)                                                                                             \
-    if ((e = cudaFuncSetAttribute(k_w4a16_ts<NT>, cudaFuncAttributeMaxDynamicSharedMemorySize,                     \
-                                  TsCfg<NT>::kBytes)) != cudaSuccess)                                              \
-        return e;
-    ZL_TS_SET(32) ZL_TS_SET(64) ZL_TS_SET(128) ZL_TS_SET(256)
-#undef ZL_TS_SET
+    for (const TsVariant& v : kTsVariants)
+        if ((e = cudaFuncSetAttribute(v.k, cudaFuncAttributeMaxDynamicSharedMemorySize, v.smem)) != cudaSuccess) return e;
     return cudaSuccess;
 }
 
@@ -452,11 +455,12 @@ static int tc_pick_ctas(int n_tiles, int G) {
 cudaError_t launch_w4_tc(const W4Params& p, bool pdl, cudaStream_t stream) {
     TcDeviceState* st = tc_state();
     if (!st || !st->ws) return cudaErrorNotSupported;
-    const int ntok = p.mc <= 32 ? 32 : p.mc <= 64 ? 64 : p.mc <= 128 ? 128 : 256;
+    const TsVariant* v = kTsVariants;
+    while (v->ntok < p.mc && v + 1 != std::end(kTsVariants)) ++v;
     const int n_tiles = p.N / kTcRows, G = p.K / kW4GroupK;
     W4TcParams q;
     if (!tc_make_map_2d(&q.xmap, p.x, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 2, (uint64_t)p.mc, (uint64_t)p.K, (uint64_t)p.ldx * 2,
-                        (uint32_t)ntok))
+                        (uint32_t)v->ntok))
         return cudaErrorInvalidValue;
     {
         // the weight maps depend only on (address, N, K): encode once per weight matrix (cuTensorMapEncodeTiled costs
@@ -509,12 +513,7 @@ cudaError_t launch_w4_tc(const W4Params& p, bool pdl, cudaStream_t stream) {
     const int ctas = tc_pick_ctas(n_tiles, G);
     if ((size_t)2 * ctas * p.mc * kTcRows * 8 > st->ws_ll_bytes) return cudaErrorInvalidValue;
     const dim3 grid(ctas);
-    switch (ntok) {
-        case 32: return launch(k_w4a16_ts<32>, grid, dim3(TsCfg<32>::kThreads), (size_t)TsCfg<32>::kBytes, stream, pdl, q);
-        case 64: return launch(k_w4a16_ts<64>, grid, dim3(TsCfg<64>::kThreads), (size_t)TsCfg<64>::kBytes, stream, pdl, q);
-        case 128: return launch(k_w4a16_ts<128>, grid, dim3(TsCfg<128>::kThreads), (size_t)TsCfg<128>::kBytes, stream, pdl, q);
-        default: return launch(k_w4a16_ts<256>, grid, dim3(TsCfg<256>::kThreads), (size_t)TsCfg<256>::kBytes, stream, pdl, q);
-    }
+    return launch(v->k, grid, dim3(v->threads), (size_t)v->smem, stream, pdl, q);
 }
 
 }  // namespace zl

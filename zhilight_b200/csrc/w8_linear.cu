@@ -439,14 +439,7 @@ static cudaError_t launch_w8(const uint8_t* xq, const float* sx, const uint8_t* 
 template <typename TcFn, typename SkinnyFn>
 static int w8_route(int M, int N, int K, int pdl, TcFn tc, SkinnyFn skinny) {
     if (M > 32 && w8_tc_supports(N, K)) {
-        static bool prepared[64] = {};   // zl_prepare() once per device: split-k workspace, opt-in shared memory
-        int dev = 0;
-        cudaGetDevice(&dev);
-        if (dev < 0 || dev >= 64 || !prepared[dev]) {
-            int rc = zl_prepare();
-            if (rc != ZL_OK) return rc;
-            if (dev >= 0 && dev < 64) prepared[dev] = true;
-        }
+        if (const int rc = prepare_once()) return rc;   // split-k workspace, opt-in shared memory
         for (int m0 = 0; m0 < M; m0 += 256) {
             const int mc = (M - m0) < 256 ? (M - m0) : 256;
             ZL_CHECK_CUDA(tc(m0, mc, pdl != 0 && m0 == 0));

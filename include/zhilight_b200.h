@@ -479,6 +479,8 @@ int zl_comm_open_peers(zl_comm_t* c, const void* handles_all);
 /* once per decode step that uses the exchange fused into the W4 GEMMs (tp_mode of zl_w4a16_gemm_fused), before the first
  * such GEMM of the step and on every rank: advances the step counter the word tags are derived from. */
 int zl_comm_ll_begin_step(zl_comm_t* c, zl_stream_t stream);
+/* tests: this rank's symmetric buffer (device pointer) and its size in bytes. */
+int zl_comm_local_buffer(zl_comm_t* c, void** base, size_t* bytes);
 /* out = T(T(sum over ranks of partial) + residual); n % 32 == 0; residual may be NULL; out may alias residual.
  * int8_payload != 0: peers' contributions travel as int8 + one T scale per 32 values (the reference's group-32
  * format, int8/quant_reduce_kernel.cu:14-38); deterministic rank-ordered fp32 reduction either way. */

@@ -331,6 +331,12 @@ extern "C" int zl_comm_ll_begin_step(zl_comm_t* c, zl_stream_t stream) {
     return ZL_OK;
 }
 extern "C" int zl_comm_world_size(zl_comm_t* c) { return c ? c->ws : -1; }
+extern "C" int zl_comm_local_buffer(zl_comm_t* c, void** base, size_t* bytes) {
+    ZL_CHECK_ARG(c && base && bytes);
+    *base = c->local;
+    *bytes = comm_total_bytes(c->ws, c->slot_bytes);
+    return ZL_OK;
+}
 
 extern "C" int zl_allreduce_one_shot(zl_comm_t* c, const void* partial, const void* residual, void* out, size_t n,
                                      int dtype, int int8_payload, int pdl, zl_stream_t stream) {

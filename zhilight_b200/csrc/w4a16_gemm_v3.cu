@@ -843,11 +843,12 @@ static V3Variant v3_variant() {
     return v;
 }
 // Every v3 kernel: launch_w4_v3 runs one of these and prepare_w4_v3 opts all of them into kV3Budget.  The shapes are
-// those w4_v3_plan picks from; PACK only with NT = 1.
+// those w4_v3_plan picks from; PACK only with NT = 1.  There is no tall NT = 2 shape (1 x 16 warps for 9..16 tokens):
+// tall needs K >= 4096, where its fixed shared memory plus 9 staged rows already exceed kV3Budget.
 static const V3Variant kV3Variants[] = {
     v3_variant<1, 16, 1, 4, false>(), v3_variant<1, 16, 1, 4, true>(), v3_variant<1, 8, 2, 5, false>(),
     v3_variant<1, 8, 2, 5, true>(),   v3_variant<1, 8, 2, 4, false>(), v3_variant<1, 8, 2, 4, true>(),
-    v3_variant<2, 16, 1, 4, false>(), v3_variant<2, 8, 2, 4, false>()};
+    v3_variant<2, 8, 2, 4, false>()};
 
 // The one place that picks the v3 variant: launch_w4_v3 runs exactly this plan, and the L2 head of a successor launch
 // (w4_v3_l2_head) is computed from it.
@@ -867,11 +868,11 @@ bool w4_v3_plan(int mc, int N, int K, int tp_mode, int sm_count, V3Plan* plan) {
     };
     if (tp_mode != 0) {   // fused tensor-parallel exchange: 4-stage variants
         if (mc <= 8) return (tall && fits(1, 16, 1, 4, 8)) || fits(1, 8, 2, 4, 8);
-        if (mc <= 16) return (tall && fits(2, 16, 1, 4, 16)) || fits(2, 8, 2, 4, 16);
+        if (mc <= 16) return fits(2, 8, 2, 4, 16);
         return false;
     }
     if (mc <= 8) return (tall && fits(1, 16, 1, 4, 8)) || fits(1, 8, 2, 5, 8) || fits(1, 8, 2, 4, 8);
-    if (mc <= 16) return (tall && fits(2, 16, 1, 4, 16)) || fits(2, 8, 2, 4, 16);
+    if (mc <= 16) return fits(2, 8, 2, 4, 16);
     return false;
 }
 

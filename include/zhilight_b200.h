@@ -33,7 +33,10 @@ enum {
     ZL_ERR_INVALID_ARG = -1,
     ZL_ERR_UNSUPPORTED = -2,
     ZL_ERR_CUDA = -3,
-    ZL_ERR_STATE = -4
+    ZL_ERR_STATE = -4,
+    /* the KV arena (zl_llama_config_t.kv_rows > 0) cannot give a call the rows it writes, even after compaction: nothing
+     * was enqueued and the model keeps running, so the caller can release a task (zl_llama_kv_release) and retry */
+    ZL_ERR_KV_FULL = -5
 };
 
 enum { ZL_F16 = 0, ZL_BF16 = 1, ZL_F32 = 2 };
@@ -551,6 +554,12 @@ typedef struct zl_llama_config {
                   * (token, kv head) and decode, chunked prefill and the dual-stream prefill attend over the quantised
                   * cache with zl_decode_attention_kv8 (the reference attends a prompt over an fp16 copy of its own K/V).
                   * fp16 only, dim_head 64 or 128, max_seq <= 65536: other configurations return ZL_ERR_UNSUPPORTED */
+    int kv_rows; /* 0: fixed KV layout, task t owns rows [t max_seq, (t + 1) max_seq) of every layer for good.  1 ..
+                  * max_batch * max_seq (else ZL_ERR_INVALID_ARG): a KV arena of this many rows per layer (rounded up to
+                  * 64), shared by every task slot.  Tasks start with no rows; before a call writes rows up to r of a task,
+                  * the task is granted at least r + 1 (geometric growth, a move or a compaction of the other tasks, the new
+                  * rows zero-filled).  Each entry point that writes rows returns ZL_ERR_KV_FULL when they cannot be
+                  * granted.  zl_llama_kv_release returns a task's rows. */
 } zl_llama_config_t;
 /* sizeof(zl_llama_config_t) and offsetof(zl_llama_config_t, kv_int8), so that bindings can check their mirror. */
 int zl_llama_config_layout(size_t* size, size_t* kv_int8_offset);
@@ -578,11 +587,13 @@ int zl_llama_init_synthetic(zl_llama_t* m, uint64_t seed);
 /* Run the load pipeline (Int4GPTQ::preprocess_weight + fusion + ZLW4 pack) on the staged tensors. */
 int zl_llama_finalize(zl_llama_t* m);
 /* One decode step for B tasks.  tokens_host/positions_host (B) int32; task b owns KV slot b.
- * next_tokens_host (B) int32 greedy picks; logits_host NULL or (B, vocab) fp32.  Synchronous. */
+ * next_tokens_host (B) int32 greedy picks; logits_host NULL or (B, vocab) fp32.  Synchronous.
+ * KV arena: ZL_ERR_KV_FULL when a task's row at its position cannot be granted (also zl_llama_step_device). */
 int zl_llama_decode(zl_llama_t* m, const int32_t* tokens_host, const int32_t* positions_host, int B,
                     int32_t* next_tokens_host, float* logits_host);
 /* Device-resident variant: stage tokens/positions once, then each call replays the step, feeds the picked
- * tokens back and advances positions on the device; no host sync. */
+ * tokens back and advances positions on the device; no host sync.  The host mirrors the positions, so a KV arena grants
+ * each step's rows before the step is enqueued (ZL_ERR_KV_FULL when it cannot). */
 int zl_llama_set_state(zl_llama_t* m, const int32_t* tokens_host, const int32_t* positions_host, int B);
 int zl_llama_step_device(zl_llama_t* m, int B);
 /* read back the device-resident (token, position) state; synchronous. */
@@ -592,7 +603,8 @@ int zl_llama_get_logits(zl_llama_t* m, float* logits_host, int B);
 int zl_llama_sync(zl_llama_t* m);
 /* Chunked prefill of ONE task (SearchTask prompt, src/generator/batch_generator.cpp:1576): appends tokens_host[0..n) at
  * positions pos0.. to the task's KV buffers through the same kernels (M = chunk GEMMs, causal len_q = chunk attention)
- * and returns the greedy next token (and optionally the last position's logits, vocab/tp floats).  Synchronous. */
+ * and returns the greedy next token (and optionally the last position's logits, vocab/tp floats).  Synchronous.
+ * KV arena: rows up to pos0 + n are granted before the first chunk, or ZL_ERR_KV_FULL with nothing enqueued. */
 /* Prefill keeps its own token / position staging on the device: the (token, position) state of the decode tasks set by
  * zl_llama_set_state survives a prefill issued between two zl_llama_step_device calls (continuous batching).  It
  * overwrites the next-token / logits row 0 outputs, which zl_llama_step_device consumes before it returns. */
@@ -606,7 +618,8 @@ int zl_llama_prefill(zl_llama_t* m, int task, const int32_t* tokens_host, int n,
  * norm, lm_head and the pick (greedy, or per-task sampling with counter = that row's position, recorded in the task's
  * history); next_host (nseg) gets the pick or -1, logits_host (n_emit x vocab, segment order) may be NULL.  The
  * device-resident decode state (zl_llama_set_state) survives the call, as it survives a prefill.  Synchronous, no graph.
- * prefill_chunk == 0: ZL_ERR_STATE; malformed segments: ZL_ERR_INVALID_ARG; kv_int8 or tp_size > 1: ZL_ERR_UNSUPPORTED. */
+ * prefill_chunk == 0: ZL_ERR_STATE; malformed segments: ZL_ERR_INVALID_ARG; kv_int8 or tp_size > 1: ZL_ERR_UNSUPPORTED;
+ * a KV arena that cannot grant every segment's rows: ZL_ERR_KV_FULL. */
 int zl_llama_step_joined(zl_llama_t* m, const int32_t* tokens_host, const int32_t* seg_host, int nseg, int32_t* next_host,
                          float* logits_host);
 /* Per-task sampling (zl_sample's contract) for the picks of zl_llama_decode / step_device / prefill.  Copies *p (HOST
@@ -662,7 +675,8 @@ int zl_llama_get_constraint_state(zl_llama_t* m, int32_t* states_host, int B);
 /* Copy rows row0 .. row0 + n of task `task`'s layer-`layer` KV cache to the host (the reference's dump_task_buf,
  * rag_buffer_context.h:199-233).  Synchronous.  Plain cache: k_host / v_host get (n, H_kv, d) activation-dtype values and
  * sk_host / sv_host must be NULL.  kv_int8: k_host / v_host get (n, H_kv, d) uint8 codes and sk_host / sv_host (n, H_kv)
- * fp32 scales (either may be NULL to skip it).  H_kv is this rank's kv heads. */
+ * fp32 scales (either may be NULL to skip it).  H_kv is this rank's kv heads.  Rows past the task's capacity
+ * (zl_llama_kv_capacity): ZL_ERR_INVALID_ARG. */
 int zl_llama_read_kv(zl_llama_t* m, int layer, int task, int row0, int n, void* k_host, void* v_host, float* sk_host,
                      float* sv_host);
 zl_stream_t zl_llama_stream(zl_llama_t* m);
@@ -689,7 +703,8 @@ int zl_llama_kv_pool_create(zl_llama_t* m, int num_blocks, int block_tokens);
  * before the call returns; stream-ordered after every step already enqueued, no device sync.  Loading writes KV rows
  * only: the positions stay with the caller (zl_llama_prefill with pos0 = the loaded length, or a joined segment).
  * Every check runs before anything is enqueued: no pool -> ZL_ERR_STATE; task out of range, a block out of range or past
- * max_seq ((j + 1) bt > max_seq), or a destination block named twice -> ZL_ERR_INVALID_ARG. */
+ * max_seq ((j + 1) bt > max_seq), or a destination block named twice -> ZL_ERR_INVALID_ARG.  A KV arena grants the task
+ * the rows the blocks cover first (a save too: it reads them through the task's table); ZL_ERR_KV_FULL when it cannot. */
 int zl_llama_kv_blocks_save(zl_llama_t* m, int task, const int32_t* task_blocks, const int32_t* pool_blocks, int n);
 int zl_llama_kv_blocks_load(zl_llama_t* m, int task, const int32_t* task_blocks, const int32_t* pool_blocks, int n);
 /* Bandwidth probe of the block copy: one warm-up pass, then `iters` passes of the same save (load = 0) or load between
@@ -706,14 +721,16 @@ int zl_llama_kv_blocks_bench(zl_llama_t* m, int task, const int32_t* task_blocks
  * (G, 2), cum (B) HOST; parent / token / score (G, K) HOST outputs as zl_beam_topk's; logits_host NULL or (B, vocab).
  * Synchronous.  Bad groups, K, cum (NaN or +inf), tokens or positions: ZL_ERR_INVALID_ARG; vocab > 262144, or tp_size > 1 without
  * zl_llama_set_vocab_gather: ZL_ERR_UNSUPPORTED; a task of the batch that samples or has penalties (zl_llama_set_sampling) or logits processors
- * (zl_llama_set_logits_processors) or a constraint (zl_llama_set_constraint): ZL_ERR_STATE. */
+ * (zl_llama_set_logits_processors) or a constraint (zl_llama_set_constraint): ZL_ERR_STATE; a KV arena that cannot grant
+ * the step's rows: ZL_ERR_KV_FULL. */
 int zl_llama_beam_step(zl_llama_t* m, const int32_t* tokens, const int32_t* positions, int B, const int32_t* groups, int G,
                        const float* cum, int K, int32_t* parent, int32_t* token, float* score, float* logits_host);
 /* Beam forks: one launch copies rows [row0, row1) of task src into task dst for every range ranges_host[i] = {src task,
  * dst task, row0, row1} (HOST (n, 4)), every layer, K and V, and with kv_int8 the fp32 scales.  Staged before the call
  * returns; stream-ordered after the steps already issued, no device sync.  Every check runs before anything is enqueued:
  * a task out of range, rows outside [0, max_seq) or an empty range, a destination named twice, or a task that is both a
- * source and a destination: ZL_ERR_INVALID_ARG. */
+ * source and a destination: ZL_ERR_INVALID_ARG.  A KV arena grants every source and destination rows [0, row1) first;
+ * ZL_ERR_KV_FULL when it cannot. */
 int zl_llama_kv_copy_rows(zl_llama_t* m, const int32_t* ranges_host, int n);
 
 /* Generate until stop on the device (the reference stops a task at eos_id or max_length,
@@ -742,10 +759,36 @@ int zl_llama_set_stop(zl_llama_t* m, int task, const int32_t* stop_ids_host, int
  * bucket): a head kernel and a while-loop conditional node whose body is the decode step plus the stop rules; a call
  * crosses buckets with one graph launch per bucket, without a host sync in between, and syncs once at the end.  A call
  * whose tasks have all finished runs 0 steps and enqueues nothing.  Bad B, max_steps or output pointers:
- * ZL_ERR_INVALID_ARG; tp_size > 1 without zl_llama_set_vocab_gather, or use_graph == 0: ZL_ERR_UNSUPPORTED; a model not finalized: ZL_ERR_STATE.  Every
+ * ZL_ERR_INVALID_ARG; tp_size > 1 without zl_llama_set_vocab_gather, or use_graph == 0: ZL_ERR_UNSUPPORTED; a model not finalized: ZL_ERR_STATE.
+ * A KV arena first grants each running task min(position + max_steps, max_seq) rows and each finished one the row of its
+ * state position: ZL_ERR_KV_FULL when it cannot (retry with a smaller max_steps, or release a task).  Every
  * check runs before anything is enqueued. */
 int zl_llama_generate(zl_llama_t* m, int B, int max_steps, int32_t* tokens_host, int32_t* n_out_host,
                       int32_t* finish_host, int* steps_host);
+
+/* KV arena (zl_llama_config_t.kv_rows > 0).  zl_llama_kv_release returns task's rows to the arena (stream order does not
+ * matter: no enqueued work is touched, and the rows are zero-filled when granted again); the task's next write is granted
+ * fresh rows.  A no-op in the fixed layout.  zl_llama_kv_capacity: the rows the task holds (max_seq in the fixed layout);
+ * zl_llama_kv_free_rows: the rows no task holds (0 in the fixed layout).  A bad task: ZL_ERR_INVALID_ARG. */
+int zl_llama_kv_release(zl_llama_t* m, int task);
+int zl_llama_kv_capacity(zl_llama_t* m, int task, int* rows);
+int zl_llama_kv_free_rows(zl_llama_t* m, int* rows);
+/* The arena's decisions without a device: replays n_ops operations ops (n_ops, 3) {call, task, rows} on an arena of
+ * kv_rows rows (as zl_llama_config_t.kv_rows).  Consecutive operations with the same call id form one call, planned as an
+ * entry point plans the rows it writes: rows >= 1 grants the task at least that many rows; rows == 0 releases the task
+ * (a call of its own).  Reports results (n_ops) ZL_OK or ZL_ERR_KV_FULL of each operation's call, extents (n_ops,
+ * max_batch, 2) {first row, capacity} of every task after it, and the relocation moves (max_moves, 6) {first operation of
+ * the call, launch, src row, dst row, rows copied, rows zero-filled} in launch order, *n_moves of them.  Bad arguments, or
+ * more than max_moves moves: ZL_ERR_INVALID_ARG. */
+int zl_kv_arena_replay(int kv_rows, int max_batch, int max_seq, const int32_t* ops, int n_ops, int32_t* results,
+                       int32_t* extents, int32_t* moves, int max_moves, int* n_moves);
+/* One k_kv_relocate launch on `stream`: moves (n, 4) {src row, dst row, rows to copy, rows to zero} (DEVICE int32) of the
+ * row spaces bases[4 l + t] (DEVICE table; t = 0 K, 1 V, 2 K scales, 3 V scales) of `layers` layers: rows [src, src +
+ * copy) to [dst, dst + copy), then rows [dst + copy, dst + copy + zero) zero-filled.  max_rows >= the largest copy + zero;
+ * row_bytes % 16 == 0; srow_bytes 0 (no scales) or a multiple of 4.  No move may overlap another's source or
+ * destination, and no destination its own source. */
+int zl_kv_relocate(void* const* bases, int layers, const int32_t* moves, int n, int max_rows, int row_bytes,
+                   int srow_bytes, zl_stream_t stream);
 
 #ifdef __cplusplus
 }

@@ -34,7 +34,7 @@ class LlamaConfig(ctypes.Structure):
         ("dtype", ctypes.c_int), ("max_batch", ctypes.c_int), ("max_seq", ctypes.c_int),
         ("tp_rank", ctypes.c_int), ("tp_size", ctypes.c_int),
         ("use_pdl", ctypes.c_int), ("use_graph", ctypes.c_int), ("tp_int8", ctypes.c_int), ("fuse", ctypes.c_int), ("prefill_chunk", ctypes.c_int),
-        ("qkv_bias", ctypes.c_int), ("kv_int8", ctypes.c_int),
+        ("qkv_bias", ctypes.c_int), ("kv_int8", ctypes.c_int), ("kv_rows", ctypes.c_int),
     ]
 
 

@@ -11,6 +11,7 @@
 #include "comm_dev.cuh"
 #include "w4_params.h"
 #include "kv_pool.cuh"
+#include "kv_arena.cuh"
 #include "beam.cuh"
 #include "sample.cuh"
 
@@ -83,11 +84,11 @@ struct Layer {
     dev_ptr<> ln_attn;
     dev_ptr<> ln_ff;
     Lin qkv, o, gu, down;
-    dev_ptr<> kbuf;   // (max_batch, max_seq, Hkv, d): activation dtype, or uint8 codes at kv_int8
+    dev_ptr<> kbuf;   // the row space (KvArena::rows, Hkv, d): activation dtype, or uint8 codes at kv_int8
     dev_ptr<> vbuf;
-    dev_ptr<void*> k_addrs;   // (max_batch)
+    dev_ptr<void*> k_addrs;   // (max_batch): each task's first row, written by the arena (k_kv_relocate)
     dev_ptr<void*> v_addrs;
-    dev_ptr<> skbuf;          // kv_int8: (max_batch, max_seq, Hkv) fp32 scales
+    dev_ptr<> skbuf;          // kv_int8: (KvArena::rows, Hkv) fp32 scales
     dev_ptr<> svbuf;
     dev_ptr<void*> sk_addrs;  // (max_batch)
     dev_ptr<void*> sv_addrs;
@@ -252,8 +253,14 @@ struct zl_llama {
     // between launches (every qkv GEMM of the model runs in stream order on the compute stream)
     dev_ptr<__half> kv8_rows;
     dev_ptr<uint32_t> kv8_cnt;
-    // the task buffers of every layer as a device table (4 per layer: kv_bases), built by the first block pool or row copy
-    dev_ptr<void*> kv_tab;
+    // where each task's KV rows live (the only owner of task placement), a host mirror of every task's decode position
+    // (zl_llama_set_state, step_device, generate) that tells which rows a step writes, and two device tables of 4 entries
+    // per layer (K, V, K scales, V scales): the row spaces (kv_bases) and the per-task pointer tables (kv_tabs).  The
+    // moves and table entries of a grant are staged in arena_ring slots of 4 * rows / kGrant + max_batch words.
+    zl::KvArena arena;
+    std::vector<int> pos_host;
+    dev_ptr<void*> kv_bases, kv_tabs;
+    StageRing arena_ring;
     // prompt prefix cache (zl_llama_kv_pool_create): the device block pool [layer][K|V][block][bt][H_kv][d] (+ fp32 scales
     // [layer][K|V][block][bt][H_kv] at kv_int8), and the block lists of zl_llama_kv_blocks_save / load, staged on the host
     // and the device in slots of 2 * pool_cap words
@@ -939,28 +946,43 @@ int alloc_generate(zl_llama* m) {
 int alloc_runtime(zl_llama* m) {
     const auto& c = m->cfg;
     const int B = c.max_batch, D = c.dim_model, d = c.dim_head;
-    // bytes per task: codes (1 byte per value) + one fp32 scale per (token, kv head) at kv_int8, else 2 bytes per value
-    const size_t kv_task = (size_t)c.max_seq * m->hkv * d * (c.kv_int8 ? 1 : 2);
-    const size_t sc_task = (size_t)c.max_seq * m->hkv * 4;
+    // bytes per row: codes (1 byte per value) + one fp32 scale per (token, kv head) at kv_int8, else 2 bytes per value
+    const size_t kv_row = (size_t)m->hkv * d * (c.kv_int8 ? 1 : 2);
+    const size_t sc_row = (size_t)m->hkv * 4;
+    const size_t rows = m->arena.rows;
     // never-written rows must be finite: masked keys still multiply their V rows by an exact 0, and with the dual-stream
     // prefill one half's attention sees the other half's rows before they are appended.  Zero codes with zero scales
-    // decode to 0.
-    auto cache = [&](dev_ptr<>* buf, dev_ptr<void*>* tab, size_t per_task) -> int {
-        RCHECK(dmalloc(buf, per_task * B));
-        ZL_CHECK_CUDA(cudaMemsetAsync(buf->get(), 0, per_task * B, m->stream));
+    // decode to 0 (the arena zero-fills every row it grants).  The fixed layout's tables point at task t's max_seq rows;
+    // an arena's tasks hold no rows yet.
+    auto cache = [&](dev_ptr<>* buf, dev_ptr<void*>* tab, size_t row) -> int {
+        RCHECK(dmalloc(buf, row * rows));
+        ZL_CHECK_CUDA(cudaMemsetAsync(buf->get(), 0, row * rows, m->stream));
         RCHECK(dmalloc(tab, sizeof(void*) * B));
-        k_ptr_table<<<cdiv(B, 256), 256, 0, m->stream>>>(tab->get(), (char*)buf->get(), per_task, B);
+        k_ptr_table<<<cdiv(B, 256), 256, 0, m->stream>>>(tab->get(), (char*)buf->get(),
+                                                         m->arena.fixed ? row * c.max_seq : 0, B);
         ZL_CHECK_LAUNCH();
         return ZL_OK;
     };
+    std::vector<void*> h_bases, h_tabs;
     for (auto& L : m->layers) {
-        RCHECK(cache(&L.kbuf, &L.k_addrs, kv_task));
-        RCHECK(cache(&L.vbuf, &L.v_addrs, kv_task));
+        RCHECK(cache(&L.kbuf, &L.k_addrs, kv_row));
+        RCHECK(cache(&L.vbuf, &L.v_addrs, kv_row));
         if (c.kv_int8) {
-            RCHECK(cache(&L.skbuf, &L.sk_addrs, sc_task));
-            RCHECK(cache(&L.svbuf, &L.sv_addrs, sc_task));
+            RCHECK(cache(&L.skbuf, &L.sk_addrs, sc_row));
+            RCHECK(cache(&L.svbuf, &L.sv_addrs, sc_row));
         }
+        for (void* p : {L.kbuf.get(), L.vbuf.get(), L.skbuf.get(), L.svbuf.get()}) h_bases.push_back(p);
+        for (void* p : {(void*)L.k_addrs.get(), (void*)L.v_addrs.get(), (void*)L.sk_addrs.get(), (void*)L.sv_addrs.get()})
+            h_tabs.push_back(p);
     }
+    RCHECK(dmalloc(&m->kv_bases, sizeof(void*) * h_bases.size()));
+    RCHECK(dmalloc(&m->kv_tabs, sizeof(void*) * h_tabs.size()));
+    ZL_CHECK_CUDA(cudaMemcpyAsync(m->kv_bases.get(), h_bases.data(), sizeof(void*) * h_bases.size(),
+                                  cudaMemcpyHostToDevice, m->stream));
+    ZL_CHECK_CUDA(cudaMemcpyAsync(m->kv_tabs.get(), h_tabs.data(), sizeof(void*) * h_tabs.size(), cudaMemcpyHostToDevice,
+                                  m->stream));
+    if (!m->arena.fixed) RCHECK(m->arena_ring.alloc((size_t)4 * (rows / KvArena::kGrant) + B, true));
+    m->pos_host.assign(B, 0);
     const int T = c.prefill_chunk > B ? c.prefill_chunk : B;   // tokens per launch: decode batch or prefill chunk
     m->tok_cap = T;
     if (c.kv_int8) {
@@ -1707,6 +1729,77 @@ int read_picks(zl_llama* m, int n, float* logits_host, const int32_t** picks) {
     return ZL_OK;
 }
 
+// Before work that writes (or reads) rows [0, rows) of each {task, rows} of `needs`: grants the rows the tasks lack from
+// the arena and enqueues the relocation -- k_kv_relocate launches in order, the last one rewriting the per-task tables.
+// ZL_ERR_KV_FULL when they cannot all be granted; then nothing is enqueued and no task moves.  The host arena takes the
+// new placement only once every launch is enqueued.  A CUDA error between the first launch and the last leaves rows
+// partly moved and the tables not yet rewritten: the model must then be destroyed, as after any CUDA error of a step.
+int kv_reserve(zl_llama* m, const std::vector<std::pair<int, int>>& needs) {
+    if (!m->finalized) return fail_state(__LINE__, "model not finalized");
+    std::vector<std::vector<KvMove>> launches;
+    KvArena next;
+    const int rc = m->arena.plan(needs, &next, &launches);
+    if (rc == ZL_ERR_KV_FULL)
+        return fail_state(__LINE__, "the KV arena cannot grant the rows this call writes (release a task, or a smaller call)",
+                          ZL_ERR_KV_FULL);
+    RCHECK(rc);
+    if (launches.empty()) return ZL_OK;
+    const auto& c = m->cfg;
+    const int MB = c.max_batch;
+    // a launch holds at most rows / kGrant moves (their destinations are disjoint multiples of kGrant rows)
+    for (const std::vector<KvMove>& mv : launches)
+        if (4 * mv.size() + MB > m->arena_ring.words) return fail_state(__LINE__, "KV arena move list overflows its slot");
+    for (size_t i = 0; i < launches.size(); ++i) {
+        const std::vector<KvMove>& mv = launches[i];
+        const bool last = i + 1 == launches.size();
+        int32_t *hs = nullptr, *ds = nullptr;
+        RCHECK(m->arena_ring.acquire(&hs, &ds));
+        int max_rows = 0;
+        for (size_t j = 0; j < mv.size(); ++j) {
+            std::memcpy(hs + 4 * j, &mv[j], sizeof(KvMove));
+            max_rows = std::max(max_rows, mv[j].copy + mv[j].zero);
+        }
+        if (last) std::memcpy(hs + 4 * mv.size(), next.first.data(), sizeof(int32_t) * MB);
+        ZL_CHECK_CUDA(cudaMemcpyAsync(ds, hs, sizeof(int32_t) * (4 * mv.size() + (last ? MB : 0)), cudaMemcpyHostToDevice,
+                                      m->stream));
+        KvRelocateArgs a{};
+        a.bases = m->kv_bases.get();
+        a.moves = ds;
+        a.n = (int)mv.size();
+        a.layers = c.num_layers;
+        a.max_rows = max_rows;
+        a.row_bytes = m->hkv * c.dim_head * (c.kv_int8 ? 1 : 2);
+        a.srow_bytes = c.kv_int8 ? m->hkv * 4 : 0;
+        if (last) {
+            a.tabs = reinterpret_cast<void** const*>(m->kv_tabs.get());
+            a.firsts = ds + 4 * mv.size();
+            a.n_tasks = MB;
+        }
+        RCHECK(kv_relocate(a, m->stream));
+        RCHECK(m->arena_ring.release(m->stream));
+    }
+    m->arena = std::move(next);
+    return ZL_OK;
+}
+
+// the rows a decode step of tasks 0 .. B-1 at `positions` writes: row p of each task
+int kv_reserve_step(zl_llama* m, const int* positions, int B) {
+    std::vector<std::pair<int, int>> needs(B);
+    for (int i = 0; i < B; ++i) needs[i] = {i, std::min(positions[i] + 1, m->cfg.max_seq)};
+    return kv_reserve(m, needs);
+}
+
+// every check of zl_llama_set_state's arguments
+int check_state(const zl_llama* m, const int32_t* tokens_host, const int32_t* positions_host, int B) {
+    ZL_CHECK_ARG(m && tokens_host && positions_host && B > 0 && B <= m->cfg.max_batch);
+    if (!m->finalized) return fail_state(__LINE__, "model not finalized");
+    for (int i = 0; i < B; ++i) {
+        ZL_CHECK_ARG(positions_host[i] >= 0 && positions_host[i] < m->cfg.max_seq);
+        ZL_CHECK_ARG(tokens_host[i] >= 0 && tokens_host[i] < m->cfg.vocab_size);
+    }
+    return ZL_OK;
+}
+
 }  // namespace
 
 extern "C" int zl_llama_create(const zl_llama_config_t* cfg, zl_llama_t** out) {
@@ -1747,9 +1840,13 @@ extern "C" int zl_llama_create(const zl_llama_config_t* cfg, zl_llama_t** out) {
             return fail_state(__LINE__, "kv_int8 needs dtype fp16, dim_head 64 or 128 and max_seq <= 65536",
                               ZL_ERR_UNSUPPORTED);
     }
+    zl::KvArena arena;
+    if (arena.init(cfg->kv_rows, cfg->max_batch, cfg->max_seq) != ZL_OK)
+        return fail_state(__LINE__, "kv_rows must be 0 (fixed layout) or 1 .. max_batch * max_seq", ZL_ERR_INVALID_ARG);
     RCHECK(zl_prepare());
     zl_llama* m = new zl_llama();
     m->cfg = *cfg;
+    m->arena = std::move(arena);
     m->hq = cfg->num_heads / cfg->tp_size;
     m->hkv = cfg->num_kv_heads / cfg->tp_size;
     m->ff = cfg->dim_ff / cfg->tp_size;
@@ -1931,16 +2028,14 @@ extern "C" int zl_llama_init_synthetic(zl_llama_t* m, uint64_t seed) {
 
 extern "C" int zl_llama_set_state(zl_llama_t* m, const int32_t* tokens_host, const int32_t* positions_host,
                                   int B) {
-    ZL_CHECK_ARG(m && tokens_host && positions_host && B > 0 && B <= m->cfg.max_batch);
-    if (!m->finalized) return fail_state(__LINE__, "model not finalized");
+    RCHECK(check_state(m, tokens_host, positions_host, B));
     int32_t* hs = nullptr;
     RCHECK(m->state_ring.acquire(&hs));
     int mx = 0;
     for (int i = 0; i < B; ++i) {
-        ZL_CHECK_ARG(positions_host[i] >= 0 && positions_host[i] < m->cfg.max_seq);
-        ZL_CHECK_ARG(tokens_host[i] >= 0 && tokens_host[i] < m->cfg.vocab_size);
         hs[i] = tokens_host[i];
         hs[B + i] = positions_host[i];
+        m->pos_host[i] = positions_host[i];
         if (positions_host[i] + 1 > mx) mx = positions_host[i] + 1;
     }
     m->cur_max_len = mx;
@@ -1952,9 +2047,12 @@ extern "C" int zl_llama_set_state(zl_llama_t* m, const int32_t* tokens_host, con
 extern "C" int zl_llama_step_device(zl_llama_t* m, int B) {
     ZL_CHECK_ARG(m && B > 0 && B <= m->cfg.max_batch);
     if (m->cur_max_len >= m->cfg.max_seq) return fail_state(__LINE__, "KV buffers full (max_seq reached)");
+    if (!m->finalized) return fail_state(__LINE__, "model not finalized");
+    RCHECK(kv_reserve_step(m, m->pos_host.data(), B));
     RCHECK(run_step(m, B));
     k_advance<<<cdiv(B, 64), 64, 0, m->stream>>>(m->d_tokens.get(), m->d_pos.get(), m->d_next.get(), B, g_w4_trace);
     ZL_CHECK_LAUNCH();
+    for (int i = 0; i < B; ++i) m->pos_host[i] += 1;
     m->cur_max_len += 1;
     return ZL_OK;
 }
@@ -1962,6 +2060,8 @@ extern "C" int zl_llama_step_device(zl_llama_t* m, int B) {
 extern "C" int zl_llama_decode(zl_llama_t* m, const int32_t* tokens_host, const int32_t* positions_host, int B,
                                int32_t* next_tokens_host, float* logits_host) {
     ZL_CHECK_ARG(next_tokens_host != nullptr);
+    RCHECK(check_state(m, tokens_host, positions_host, B));
+    RCHECK(kv_reserve_step(m, positions_host, B));
     RCHECK(zl_llama_set_state(m, tokens_host, positions_host, B));
     RCHECK(run_step(m, B));
     const int32_t* picks = nullptr;
@@ -1991,6 +2091,7 @@ extern "C" int zl_llama_get_logits(zl_llama_t* m, float* logits_host, int B) {
 
 extern "C" int zl_llama_bench_gemms(zl_llama_t* m, int B, int iters, float* ms, int* launches, double* bytes) {
     ZL_CHECK_ARG(m && B > 0 && B <= m->cfg.max_batch && iters > 0 && ms);
+    RCHECK(kv_reserve_step(m, m->pos_host.data(), B));
     const auto& c = m->cfg;
     const int D = c.dim_model, d = c.dim_head;
     cudaStream_t st = m->stream;
@@ -2056,6 +2157,8 @@ extern "C" int zl_llama_prefill(zl_llama_t* m, int task, const int32_t* tokens_h
     const int chunk = m->cfg.prefill_chunk;
     if (chunk <= 0) return fail_state(__LINE__, "zl_llama_prefill needs cfg.prefill_chunk > 0");
     if (pos0 + n > m->cfg.max_seq) return fail_state(__LINE__, "prompt does not fit the KV buffers (max_seq)");
+    for (int i = 0; i < n; ++i) ZL_CHECK_ARG(tokens_host[i] >= 0 && tokens_host[i] < m->cfg.vocab_size);
+    RCHECK(kv_reserve(m, {{task, pos0 + n}}));
     int32_t* h_tok = m->h_stage.get() + 4 * m->cfg.max_batch + 4;   // pinned staging for one chunk of token ids
     for (int c0 = 0; c0 < n; c0 += chunk) {
         const int cn = (n - c0) < chunk ? (n - c0) : chunk;
@@ -2102,6 +2205,9 @@ extern "C" int zl_llama_step_joined(zl_llama_t* m, const int32_t* tokens_host, c
         ZL_CHECK_ARG(rows <= m->tok_cap);
     }
     for (int i = 0; i < rows; ++i) ZL_CHECK_ARG(tokens_host[i] >= 0 && tokens_host[i] < c.vocab_size);
+    std::vector<std::pair<int, int>> needs(nseg);
+    for (int s = 0; s < nseg; ++s) needs[s] = {seg_host[4 * s], seg_host[4 * s + 1] + seg_host[4 * s + 2]};
+    RCHECK(kv_reserve(m, needs));
 
     // host staging: tokens | positions | token -> task (tok_cap each) | segments | emitting rows | tasks | positions
     const int T = m->tok_cap, MB = c.max_batch;
@@ -2260,13 +2366,14 @@ extern "C" int zl_llama_get_constraint_state(zl_llama_t* m, int32_t* states_host
 extern "C" int zl_llama_read_kv(zl_llama_t* m, int layer, int task, int row0, int n, void* k_host, void* v_host,
                                 float* sk_host, float* sv_host) {
     ZL_CHECK_ARG(m && m->finalized && layer >= 0 && layer < m->cfg.num_layers && task >= 0 && task < m->cfg.max_batch);
-    ZL_CHECK_ARG(row0 >= 0 && n > 0 && row0 + n <= m->cfg.max_seq);
+    ZL_CHECK_ARG(row0 >= 0 && n > 0 && row0 + n <= m->arena.cap[task]);
     ZL_CHECK_ARG(m->cfg.kv_int8 || (!sk_host && !sv_host));
     const Layer& L = m->layers[layer];
     const size_t row = (size_t)m->hkv * m->cfg.dim_head;   // values per token
     const size_t vb = m->cfg.kv_int8 ? 1 : 2;               // bytes per value
-    const size_t off = ((size_t)task * m->cfg.max_seq + row0) * row * vb;
-    const size_t soff = ((size_t)task * m->cfg.max_seq + row0) * m->hkv * 4;
+    const size_t r0 = (size_t)m->arena.first[task] + row0;
+    const size_t off = r0 * row * vb;
+    const size_t soff = r0 * m->hkv * 4;
     ZL_CHECK_CUDA(cudaStreamSynchronize(m->stream));   // the steps that wrote the rows
     if (k_host) ZL_CHECK_CUDA(cudaMemcpy(k_host, (char*)L.kbuf.get() + off, n * row * vb, cudaMemcpyDeviceToHost));
     if (v_host) ZL_CHECK_CUDA(cudaMemcpy(v_host, (char*)L.vbuf.get() + off, n * row * vb, cudaMemcpyDeviceToHost));
@@ -2296,28 +2403,6 @@ extern "C" int zl_llama_stats(zl_llama_t* m, int B, double* weight_bytes, int* k
 // Prompt prefix cache: the block pool and the block copies (PrefixCache, src/generator/prefix_cache.hpp:35-117).  Which
 // blocks to save and load is the caller's policy (zhilight_b200/prefix_cache.py); this owns the memory and the copies.
 // ------------------------------------------------------------------------------------------------------------------
-namespace {
-
-// layer L's task buffers: k, v, scale k, scale v (the scales are null without an int8 cache)
-std::array<void*, 4> kv_bases(const Layer& L) { return {L.kbuf.get(), L.vbuf.get(), L.skbuf.get(), L.svbuf.get()}; }
-
-// kv_tab, built by the first block pool or row copy
-int ensure_kv_tab(zl_llama* m) {
-    if (m->kv_tab) return ZL_OK;
-    std::vector<void*> h_tab;
-    for (const Layer& L : m->layers)
-        for (void* p : kv_bases(L)) h_tab.push_back(p);
-    dev_ptr<void*> tab;
-    RCHECK(dmalloc(&tab, sizeof(void*) * h_tab.size()));
-    ZL_CHECK_CUDA(cudaMemcpyAsync(tab.get(), h_tab.data(), sizeof(void*) * h_tab.size(), cudaMemcpyHostToDevice,
-                                  m->stream));
-    ZL_CHECK_CUDA(cudaStreamSynchronize(m->stream));   // h_tab is pageable and goes out of scope
-    m->kv_tab = std::move(tab);
-    return ZL_OK;
-}
-
-}  // namespace
-
 extern "C" int zl_llama_kv_pool_create(zl_llama_t* m, int num_blocks, int block_tokens) {
     ZL_CHECK_ARG(m && num_blocks > 0);
     ZL_CHECK_ARG(block_tokens == 16 || block_tokens == 32 || block_tokens == 64 || block_tokens == 128 ||
@@ -2328,7 +2413,7 @@ extern "C" int zl_llama_kv_pool_create(zl_llama_t* m, int num_blocks, int block_
     const int L = c.num_layers;
     const int row_bytes = m->hkv * c.dim_head * (c.kv_int8 ? 1 : 2);
     const int srow_bytes = c.kv_int8 ? m->hkv * 4 : 0;
-    if (!kv_block_copy_aligned(block_tokens, c.max_seq, row_bytes, srow_bytes))
+    if (!kv_block_copy_aligned(block_tokens, m->arena.unit(), row_bytes, srow_bytes))
         return fail_state(__LINE__, "KV block copies need max_seq * (bytes of one cached row) to be a multiple of 16",
                           ZL_ERR_UNSUPPORTED);
     const size_t blk = (size_t)block_tokens * row_bytes, sblk = (size_t)block_tokens * srow_bytes;
@@ -2336,7 +2421,6 @@ extern "C" int zl_llama_kv_pool_create(zl_llama_t* m, int num_blocks, int block_
     dev_ptr<> pool, scales;
     RCHECK(dmalloc(&pool, (size_t)L * 2 * num_blocks * blk));
     if (c.kv_int8) RCHECK(dmalloc(&scales, (size_t)L * 2 * num_blocks * sblk));
-    RCHECK(ensure_kv_tab(m));
     RCHECK(m->pool_ring.alloc((size_t)2 * cap, true));
     m->pool = std::move(pool);
     m->pool_scales = std::move(scales);
@@ -2369,7 +2453,7 @@ int check_kv_blocks(zl_llama* m, int task, const int32_t* task_blocks, const int
 KvBlockCopyArgs kv_copy_args(zl_llama* m, int task, const int32_t* d_pairs, int n, bool to_pool) {
     const auto& c = m->cfg;
     KvBlockCopyArgs a{};
-    a.task_bases = m->kv_tab.get();
+    a.task_tabs = reinterpret_cast<void* const* const*>(m->kv_tabs.get());
     a.pool = static_cast<char*>(m->pool.get());
     a.pool_scales = static_cast<char*>(m->pool_scales.get());
     a.pairs = d_pairs;
@@ -2378,7 +2462,6 @@ KvBlockCopyArgs kv_copy_args(zl_llama* m, int task, const int32_t* d_pairs, int 
     a.num_blocks = m->pool_blocks;
     a.bt = m->pool_bt;
     a.task = task;
-    a.task_rows = c.max_seq;
     a.row_bytes = m->hkv * c.dim_head * (c.kv_int8 ? 1 : 2);
     a.srow_bytes = c.kv_int8 ? m->hkv * 4 : 0;
     a.to_pool = to_pool ? 1 : 0;
@@ -2396,8 +2479,16 @@ int stage_kv_blocks(zl_llama* m, const int32_t* task_blocks, const int32_t* pool
     return ZL_OK;
 }
 
+// the task's rows the blocks cover, granted before a save reads or a load writes them
+int kv_reserve_blocks(zl_llama* m, int task, const int32_t* task_blocks, int n) {
+    int rows = 0;
+    for (int i = 0; i < n; ++i) rows = std::max(rows, (task_blocks[i] + 1) * m->pool_bt);
+    return kv_reserve(m, {{task, rows}});
+}
+
 int kv_blocks(zl_llama* m, int task, const int32_t* task_blocks, const int32_t* pool_blocks, int n, bool to_pool) {
     RCHECK(check_kv_blocks(m, task, task_blocks, pool_blocks, n, to_pool));
+    RCHECK(kv_reserve_blocks(m, task, task_blocks, n));
     const int32_t* d_pairs = nullptr;
     RCHECK(stage_kv_blocks(m, task_blocks, pool_blocks, n, &d_pairs));
     RCHECK(kv_block_copy(kv_copy_args(m, task, d_pairs, n, to_pool), m->stream));
@@ -2421,6 +2512,7 @@ extern "C" int zl_llama_kv_blocks_bench(zl_llama_t* m, int task, const int32_t* 
     ZL_CHECK_ARG(iters > 0 && ms);
     const bool to_pool = !load;
     RCHECK(check_kv_blocks(m, task, task_blocks, pool_blocks, n, to_pool));
+    RCHECK(kv_reserve_blocks(m, task, task_blocks, n));
     const auto& c = m->cfg;
     const KvBlockCopyArgs a0 = kv_copy_args(m, task, nullptr, 0, to_pool);
     const size_t blk = (size_t)a0.bt * a0.row_bytes, sblk = (size_t)a0.bt * a0.srow_bytes;
@@ -2431,11 +2523,13 @@ extern "C" int zl_llama_kv_blocks_bench(zl_llama_t* m, int task, const int32_t* 
         if (!per_range_memcpy) return kv_block_copy(a, m->stream);
         for (int i = 0; i < n; ++i)
             for (int l = 0; l < c.num_layers; ++l) {
-                const auto tbuf = kv_bases(m->layers[l]);
+                const Layer& L = m->layers[l];
+                const std::array<void*, 4> tbuf = {L.kbuf.get(), L.vbuf.get(), L.skbuf.get(), L.svbuf.get()};
                 for (int t = 0; t < (sblk ? 4 : 2); ++t) {
                     const bool sc = t >= 2;
                     const size_t rb = sc ? a.srow_bytes : a.row_bytes, bb = sc ? sblk : blk;
-                    char* tp = static_cast<char*>(tbuf[t]) + ((size_t)task * c.max_seq + (size_t)task_blocks[i] * a.bt) * rb;
+                    char* tp = static_cast<char*>(tbuf[t]) +
+                               ((size_t)m->arena.first[task] + (size_t)task_blocks[i] * a.bt) * rb;
                     char* pp = (sc ? a.pool_scales : a.pool) + ((size_t)(l * 2 + (t & 1)) * a.num_blocks + pool_blocks[i]) * bb;
                     ZL_CHECK_CUDA(cudaMemcpyAsync(to_pool ? pp : tp, to_pool ? tp : pp, bb, cudaMemcpyDeviceToDevice,
                                                   m->stream));
@@ -2503,7 +2597,9 @@ extern "C" int zl_llama_beam_step(zl_llama_t* m, const int32_t* tokens, const in
     if (!m->finalized) return fail_state(__LINE__, "model not finalized");
     if (pick_of(m, 0, B).sampler)
         return fail_state(__LINE__, "a task of the beam step samples, has penalties, logits processors or a constraint");
+    RCHECK(check_state(m, tokens, positions, B));
     RCHECK(ensure_beam(m));
+    RCHECK(kv_reserve_step(m, positions, B));
     const int MB = m->cfg.max_batch;
     int32_t* d = static_cast<int32_t*>(m->beam_d.get());
     int32_t* h = m->beam_h.get();
@@ -2517,7 +2613,7 @@ extern "C" int zl_llama_beam_step(zl_llama_t* m, const int32_t* tokens, const in
     bp.token = bp.parent + kBeamK * MB;
     bp.score = reinterpret_cast<float*>(bp.token + kBeamK * MB);
     bp.ws = m->beam_ws.get();
-    RCHECK(zl_llama_set_state(m, tokens, positions, B));   // checks tokens and positions before its copies
+    RCHECK(zl_llama_set_state(m, tokens, positions, B));
     std::memcpy(h, cum, sizeof(float) * B);
     std::memcpy(h + MB, groups, sizeof(int32_t) * 2 * G);
     cudaStream_t st = m->stream;
@@ -2560,18 +2656,21 @@ extern "C" int zl_llama_kv_copy_rows(zl_llama_t* m, const int32_t* ranges_host, 
     const int row_bytes = m->hkv * c.dim_head * (c.kv_int8 ? 1 : 2);
     if (row_bytes % 16 != 0)
         return fail_state(__LINE__, "KV row copies need 16-byte cached rows (H_kv * dim_head)", ZL_ERR_UNSUPPORTED);
-    RCHECK(ensure_kv_tab(m));
+    // the sources' rows are granted too: the copy reads them through the same tables
+    std::vector<std::pair<int, int>> needs;
+    for (int i = 0; i < n; ++i)
+        for (int t : {ranges_host[4 * i], ranges_host[4 * i + 1]}) needs.push_back({t, ranges_host[4 * i + 3]});
+    RCHECK(kv_reserve(m, needs));
     if (!m->rows_ring.h) RCHECK(m->rows_ring.alloc((size_t)4 * c.max_batch, true));
     int32_t *hs = nullptr, *ds = nullptr;
     RCHECK(m->rows_ring.acquire(&hs, &ds));
     std::memcpy(hs, ranges_host, sizeof(int32_t) * 4 * n);
     ZL_CHECK_CUDA(cudaMemcpyAsync(ds, hs, sizeof(int32_t) * 4 * n, cudaMemcpyHostToDevice, m->stream));
     KvRowCopyArgs a{};
-    a.task_bases = m->kv_tab.get();
+    a.task_tabs = reinterpret_cast<void* const* const*>(m->kv_tabs.get());
     a.ranges = ds;
     a.n = n;
     a.layers = c.num_layers;
-    a.task_rows = c.max_seq;
     a.max_rows = max_rows;
     a.row_bytes = row_bytes;
     a.srow_bytes = c.kv_int8 ? m->hkv * 4 : 0;
@@ -2780,6 +2879,12 @@ extern "C" int zl_llama_generate(zl_llama_t* m, int B, int max_steps, int32_t* t
         *steps_host = 0;
         return ZL_OK;
     }
+    // every row the call can write: min(pos + max_steps, max_seq) rows of a running task; a finished task re-runs its
+    // state position (max_seq - 1 at the end of its buffer)
+    std::vector<std::pair<int, int>> needs(B);
+    for (int i = 0; i < B; ++i)
+        needs[i] = {i, std::min(m->pos_host[i] + (m->gen_fin[i] ? 1 : max_steps), c.max_seq)};
+    RCHECK(kv_reserve(m, needs));
     const Pick pk = pick_of(m, 0, B);
     const GenState gs = gen_state(m);
     // attention lengths at step s are at most min(L0 + s, max_seq): one launch per length bucket crossed
@@ -2821,9 +2926,31 @@ extern "C" int zl_llama_generate(zl_llama_t* m, int B, int max_steps, int32_t* t
     for (int i = 0; i < B; ++i) {
         finish_host[i] = h_fin[i];
         m->gen_fin[i] = (char)h_fin[i];
+        m->pos_host[i] = h_pos[i];
         mx = std::max(mx, h_pos[i] + 1);
     }
     m->cur_max_len = mx;
     *steps_host = steps;
+    return ZL_OK;
+}
+
+// ------------------------------------------------------------------------------------------------------------------
+// KV arena (cfg.kv_rows > 0): each task's rows come from one shared row space as its writes reach them (KvArena).
+// ------------------------------------------------------------------------------------------------------------------
+extern "C" int zl_llama_kv_release(zl_llama_t* m, int task) {
+    ZL_CHECK_ARG(m && task >= 0 && task < m->cfg.max_batch);
+    m->arena.release(task);
+    return ZL_OK;
+}
+
+extern "C" int zl_llama_kv_capacity(zl_llama_t* m, int task, int* rows) {
+    ZL_CHECK_ARG(m && rows && task >= 0 && task < m->cfg.max_batch);
+    *rows = m->arena.cap[task];
+    return ZL_OK;
+}
+
+extern "C" int zl_llama_kv_free_rows(zl_llama_t* m, int* rows) {
+    ZL_CHECK_ARG(m && rows);
+    *rows = m->arena.free_rows();
     return ZL_OK;
 }

@@ -77,6 +77,32 @@ def stop_rule(stop_ids, max_new_tokens, vocab_size):
     return ids.astype(np.int32), int(max_new_tokens)
 
 
+KV_FULL = -5   # ZL_ERR_KV_FULL
+
+
+def kv_arena_replay(kv_rows, max_batch, max_seq, ops, max_moves=1 << 16):
+    """The KV arena's decisions without a device (zl_kv_arena_replay).  ops: a list of calls, each (task, rows) or a list
+    of (task, rows) granted together as one entry point's call; rows >= 1 grants the task at least that many rows, 0
+    releases it (alone in its call).  -> (results (n,) 0 or KV_FULL, extents (n, max_batch, 2) {first row, capacity}
+    after each call, moves (m, 6) {first op of the call, launch, src, dst, rows copied, rows zero-filled}), one entry of
+    results and extents per (task, rows) pair in call order."""
+    lib = _lib.load()
+    flat = []
+    for c, call in enumerate(ops):
+        pairs = [call] if np.ndim(call) == 1 else list(call)
+        flat += [(c, int(t), int(r)) for t, r in pairs]
+    o = np.ascontiguousarray(np.asarray(flat, dtype=np.int32).reshape(-1, 3))
+    n = o.shape[0]
+    res = np.empty(n, np.int32)
+    ext = np.empty((n, max_batch, 2), np.int32)
+    mv = np.empty((max_moves, 6), np.int32)
+    nm = ctypes.c_int()
+    p = lambda a: a.ctypes.data_as(ctypes.c_void_p)
+    _lib.check(lib.zl_kv_arena_replay(int(kv_rows), int(max_batch), int(max_seq), p(o), n, p(res), p(ext), p(mv),
+                                      int(max_moves), ctypes.byref(nm)))
+    return res, ext, mv[:nm.value].copy()
+
+
 QUANT_NONE, QUANT_AUTO_INT8, QUANT_GPTQ, QUANT_AWQ, QUANT_FP8, QUANT_FP8_BLOCK = 0, 2, 5, 6, 7, 10   # model_config.hpp:132-144
 
 
@@ -113,9 +139,12 @@ class LlamaDecoder:
     def __init__(self, num_layers, dim_model, num_heads, num_kv_heads, dim_head, dim_ff, vocab_size, eps=1e-5,
                  rope_theta=10000.0, rope_llama3=None, quant_type=QUANT_NONE, group_size=128, sym=False,
                  dtype="f16", max_batch=1, max_seq=512, use_pdl=True, use_graph=True, tp_rank=0, tp_size=1, fuse=2, tp_int8=False,
-                 prefill_chunk=0, qkv_bias=False, kv_cache_dtype=None):
+                 prefill_chunk=0, qkv_bias=False, kv_cache_dtype=None, kv_rows=None):
         """kv_cache_dtype: None keeps K/V in the activation dtype; "int8" stores them as per-(token, kv head) int8 codes
-        with fp32 scales (the reference's KV_CACHE_DTYPE=int8; fp16 models with dim_head 64 or 128)."""
+        with fp32 scales (the reference's KV_CACHE_DTYPE=int8; fp16 models with dim_head 64 or 128).
+        kv_rows: None (or 0) gives every task slot max_seq KV rows for good; 1 .. max_batch * max_seq allocates that many
+        rows per layer (rounded up to 64) shared by all slots, granted to each task as its writes reach them.  A call the
+        arena cannot serve raises ZLError with code KV_FULL and changes nothing: release a task (kv_release) and retry."""
         if kv_cache_dtype not in (None, "int8"):
             raise ValueError("kv_cache_dtype must be None or 'int8', not %r" % (kv_cache_dtype,))
         self.lib = _lib.load()
@@ -125,7 +154,7 @@ class LlamaDecoder:
             float(l3.get("factor", 0.0)), float(l3.get("low", 1.0)), float(l3.get("high", 4.0)),
             float(l3.get("orig", 8192.0)), quant_type, group_size, int(sym), {"f16": 0, "bf16": 1}[dtype],
             max_batch, max_seq, tp_rank, tp_size, int(use_pdl), int(use_graph), int(tp_int8), int(fuse), int(prefill_chunk), int(qkv_bias),
-            int(kv_cache_dtype == "int8"))
+            int(kv_cache_dtype == "int8"), int(kv_rows or 0))
         self.vocab_size = vocab_size
         self.vocab_shard = vocab_size // tp_size      # lm_head is vocab-parallel: logits come back per rank shard
         self.max_batch = max_batch
@@ -356,6 +385,23 @@ class LlamaDecoder:
         out = np.empty(int(b), np.int32)
         _lib.check(self.lib.zl_llama_get_constraint_state(self.h, out.ctypes.data_as(ctypes.c_void_p), int(b)))
         return out
+
+    def kv_release(self, task):
+        """Return the task's KV rows to the arena; its next write is granted fresh, zero-filled rows
+        (zl_llama_kv_release).  A no-op without kv_rows."""
+        _lib.check(self.lib.zl_llama_kv_release(self.h, int(task)))
+
+    def kv_capacity(self, task):
+        """KV rows the task holds now (max_seq without kv_rows)."""
+        r = ctypes.c_int()
+        _lib.check(self.lib.zl_llama_kv_capacity(self.h, int(task), ctypes.byref(r)))
+        return r.value
+
+    def kv_free_rows(self):
+        """KV rows of the arena no task holds (0 without kv_rows)."""
+        r = ctypes.c_int()
+        _lib.check(self.lib.zl_llama_kv_free_rows(self.h, ctypes.byref(r)))
+        return r.value
 
     def read_kv(self, layer, task, row0, n):
         """Rows row0 .. row0 + n of a task's layer-`layer` KV cache (zl_llama_read_kv), each (n, H_kv, d).
